@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- SDF+grad queries/s of the batched signed-distance query path on B200.
+"""bench.py -- SDF+grad queries/s of the batched signed-distance query path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload default|c4|c2|mesh10k|mesh50k|c3|c3cached|c5|c4readme]
-                    [--impl reference]
+                    [--impl reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of synthetic input.
 
@@ -17,11 +17,18 @@ DEFAULT (no --workload): the line the driver records.
     an NVLS multicast mapping), each timed the same way.
   * `workloads`: every other BASELINE config on the same GPUs in the same run -- mesh10k (the north-star
     single-GPU target: MeshSDF on a 10 000-triangle mesh, 10^7 queries), c2, c3, c3cached, c5 -- each with value,
-    ms_per_step, roofline{achieved, frac, traffic, kernel_ms}, e2e and (N=1) cpu_baseline.
+    ms_per_step, roofline{achieved, frac, kernel_ms}, e2e and (N=1) cpu_baseline.
 
 `roofline.kernel_ms` is an independent measurement: the library brackets the dominant kernel launch of one call with
 its own pair of CUDA events on the launch stream (pvb_timing_enable / pvb_timing_last_ms); median of 7 launches.
-`roofline.traffic` is the ncu dram__bytes_read+write of that kernel from the committed capture (profiles/ncu_traffic.json).
+
+`--steps K` sets the number of timed steps of every timed loop (headline, re-assembly variants, reconfigure, each
+workload, each e2e arm); only roofline.kernel_ms (7 single launches) and cpu_baseline (a time budget) are not steps.
+
+`--dump-outputs DIR` writes what the timed path returned in its last timed step -- the headline's in a default run,
+otherwise the one --workload's -- as DIR/<name>.npy (float32 / float64, at most 64 MB: larger results are sampled at
+fixed seeded rows, listed in DIR/sample_index.npy), so that two builds can be compared output for output on
+identical seeded inputs.  It is refused with --impl reference, which runs no GPU path.
 
 `--impl reference` times the CPU restatement of the reference (oracle/port.py, torch-cpu + OpenMP BVH, all host
 threads that help) on a bounded sample of the same workloads; the reference itself is pure Python over third-party
@@ -30,8 +37,10 @@ wheels that are not installable in this image (SURVEY.md section 0), so the orac
 Prints ONE JSON line (rank 0).
 """
 import argparse
+import atexit
 import json
 import os
+import shutil
 import statistics
 import sys
 import tempfile
@@ -52,39 +61,59 @@ OTHER_WORKLOADS = ("mesh10k", "c2", "c3", "c3cached", "c5")
 
 
 # ------------------------------------------------------------------------------------------------ helpers
+_SCRATCH = []
+
+
+def scratch_dir():
+    """This process's own temporary directory for table caches and generated meshes, removed at exit: fixed names in
+    the shared temporary directory collide with files another user's run left behind."""
+    if not _SCRATCH:
+        _SCRATCH.append(tempfile.mkdtemp(prefix="pvb_bench_"))
+        atexit.register(shutil.rmtree, _SCRATCH[0], True)
+    return _SCRATCH[0]
+
+
 def measured_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "the H100 SXM data sheet (HBM3, not a measured rate)"
 
 
-def ncu_traffic(workload):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu --set full capture (profiles/)."""
-    path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(path):
-        with open(path) as fh:
-            return json.load(fh).get(workload)
-    return None
+DUMP_MAX_BYTES = 64 << 20
+DUMP_MAX_ROWS = 1 << 20
 
 
-def ncu_limits(workload):
-    """Issue-slot / L1 data pipe / DRAM utilisation of the dominant kernel from the same committed capture: says what
-    bounds a kernel whose HBM fraction is small by nature (tree walks, the RobotSDF kernel)."""
-    path = os.path.join(ROOT, "profiles", "ncu_limits.json")
-    if os.path.exists(path):
-        with open(path) as fh:
-            return json.load(fh).get(workload)
-    return None
+def dump_outputs(out, dirname):
+    """Writes one step's result as dirname/<name>.npy: a (value, gradient) pair as value.npy / grad.npy, a single
+    tensor as value.npy.  Rows are the elements of the first output (a gradient row is its 3 components); beyond
+    DUMP_MAX_ROWS rows the same seeded sample of rows is taken from every output and its flat row indices are written
+    as sample_index.npy (float64: exact below 2^53)."""
+    outs = list(out) if isinstance(out, (tuple, list)) else [out]
+    names = ["value", "grad"] if len(outs) == 2 else [f"out{i}" for i in range(len(outs))]
+    rows = outs[0].numel()
+    flat = [t.detach().reshape(rows, -1) for t in outs]
+    row_bytes = 8 + sum(t.shape[1] * (8 if t.dtype == torch.float64 else 4) for t in flat)
+    k = min(rows, DUMP_MAX_ROWS, DUMP_MAX_BYTES // row_bytes)
+    os.makedirs(dirname, exist_ok=True)
+    if k < rows:
+        idx = np.sort(np.random.default_rng(0).choice(rows, size=k, replace=False))
+        sel = torch.from_numpy(idx).to(flat[0].device)
+        flat = [t[sel] for t in flat]
+        np.save(os.path.join(dirname, "sample_index.npy"), idx.astype(np.float64))
+    for name, t, full in zip(names, flat, outs):
+        a = t.cpu().numpy()
+        a = a.astype(np.float64 if a.dtype == np.float64 or a.dtype.kind in "iub" else np.float32, copy=False)
+        shape = tuple(full.shape) if k == rows else (k,) if a.shape[1] == 1 else a.shape
+        np.save(os.path.join(dirname, f"{name}.npy"), a.reshape(shape))
 
 
 class ClockSampler:
     """SM clock + throttle reasons sampled DURING the timed region through NVML (nvidia_ml_py).
 
-    Measured on this pool (gpurun_out/bisect.log, round 1): NVML queries and `nvidia-smi -lms` contend with kernel
-    launches for a driver lock -- a 2 ms sampling period doubled the host issue time per step (25 -> 55 us) and
-    made a 58 us/step kernel loop host-bound.  So: NVML is initialised before the warm-up, a background thread
+    NVML queries and `nvidia-smi -lms` contend with kernel launches for a driver lock -- a millisecond sampling
+    period can make a short-kernel loop host-bound.  So: NVML is initialised before the warm-up, a background thread
     samples every 100 ms (long runs), and one sample is always taken right after the last timed launch has been
     ENQUEUED, i.e. while the timed kernels are still executing on the GPU, where it cannot delay any launch."""
     REASONS = (("hw_slowdown", 0x8), ("hw_thermal_slowdown", 0x40), ("sw_thermal_slowdown", 0x20),
@@ -205,7 +234,7 @@ class C2(Workload):
         v, f = workloads.fixture_mesh("drill")
         self.obj = pv.MeshObjectFactory("drill", mesh=(v, f))
         gt = pv.MeshSDF(self.obj)
-        cache = os.path.join(cache_dir or tempfile.gettempdir(), f"pvb_bench_c2_{rank}.pkl")
+        cache = os.path.join(cache_dir or scratch_dir(), f"pvb_bench_c2_{rank}.pkl")
         self.sdf = pv.CachedSDF("drill", 0.005, self.obj.bounding_box(padding=0.1), gt, device="cuda",
                                 cache_path=cache, clean_cache=True)
         # same object for host callers: results come back as host tensors (tables still live on the GPU)
@@ -304,7 +333,7 @@ def c4_config(n_cfg=200, n_pts=100_000):
                         f"configurations x {n_pts} uniform points, value+gradient; configurations sharded over the "
                         f"ranks, full ({n_cfg}, {n_pts}) result on every rank inside the timed region",
             "n_cfg": n_cfg, "n_pts": n_pts, "units_per_step": n_cfg * n_pts,
-            "l2_policy": "output 320 MB/step > L2 (126 MB); 3 rotating point buffers",
+            "l2_policy": "output 320 MB/step > L2 (50 MB); 3 rotating point buffers",
             "result_reassembly": "full result on every rank; method = the fastest of NCCL all-gather / peer stores / "
                                  "multicast stores measured in this run (reassembly.chosen); no collective at N=1"}
 
@@ -325,7 +354,7 @@ class C4(Workload):
         self.mode = mode if world > 1 else "none"
         self.peer = None
         self.peer_error = None
-        d = os.path.join(cache_dir or tempfile.gettempdir(), f"pvb_bench_arm_{rank}")
+        d = os.path.join(cache_dir or scratch_dir(), f"pvb_bench_arm_{rank}")
         urdf, end = workloads.write_arm(d)
         chain = pv.build_serial_chain_from_urdf(open(urdf).read(), end).to(device="cuda")
         self.robot = pv.RobotSDF(chain, path_prefix=d,
@@ -426,8 +455,8 @@ class C5(Workload):
         begin, end = pd.shard_range(n_pts, rank, world)
         self.pts = world_pts[begin:end].contiguous()
         self.host_pts = self.pts.cpu().pin_memory()
-        # 60 MB cloud < L2: rotate 3 device copies (180 MB) so that no step finds its input in L2, instead of a flush
-        # memset inside the timed step
+        # the 60 MB cloud would be largely L2-resident (50 MB): rotate 3 device copies (180 MB) so that no step finds
+        # its input in L2, instead of a flush memset inside the timed step
         self.copies = [self.pts] + [self.pts.clone() for _ in range(2 if (end - begin) * 36 < 400e6 else 0)]
         pert = workloads.random_rigid(n_tf, seed=6, t_range=0.01).cuda()
         self.w2o = torch.linalg.inv(tf.unsqueeze(0)) @ pert
@@ -439,7 +468,7 @@ class C5(Workload):
         self.pv = pv
         self.desc = {"workload": f"C5 chamfer: {n_pts}-point cloud -> 50 000-triangle bumpy sphere, B={n_tf} "
                                  f"transform(s), cloud sharded over ranks", "points_this_rank": end - begin,
-                     "l2_policy": "60 MB cloud fits L2: 3 rotating device copies of the cloud (180 MB > L2)"}
+                     "l2_policy": "60 MB cloud, 50 MB L2: 3 rotating device copies of the cloud (180 MB > L2)"}
 
     def step(self, i):
         return self.pv.batch_chamfer_dist(self.w2o, self.copies[i % len(self.copies)], self.obj)
@@ -460,7 +489,7 @@ class C3(Workload):
         gt = pv.MeshSDF(obj)
         if cached:
             sub = pv.CachedSDF("drill", 0.005, obj.bounding_box(padding=0.1), gt, device="cuda",
-                               cache_path=os.path.join(cache_dir or tempfile.gettempdir(), f"pvb_c3_{rank}.pkl"))
+                               cache_path=os.path.join(cache_dir or scratch_dir(), f"pvb_c3_{rank}.pkl"))
         else:
             sub = gt
         tm = workloads.random_rigid(16, seed=1, t_range=0.5).cuda()
@@ -471,8 +500,8 @@ class C3(Workload):
         b, e = pd.shard_range(len(pts), rank, world)
         self.host_pts = pts[b:e].contiguous().pin_memory()
         self.pts = self.host_pts.cuda()
-        # 24 MB of points + 32 MB of results per step fit L2: rotate 6 device copies of the point set (144 MB > L2)
-        # instead of a flush memset inside the timed step
+        # 24 MB of points would stay largely L2-resident (50 MB) from step to step: rotate 6 device copies of the point
+        # set (144 MB > L2) instead of a flush memset inside the timed step
         self.copies = [self.pts] + [self.pts.clone() for _ in range(5)]
         self.units = e - b
         self.alg_bytes = 28 * self.units
@@ -484,7 +513,7 @@ class C3(Workload):
                      "l2_policy": "6 rotating device copies of the point set (144 MB > L2); results are fresh buffers"}
         if cached:
             self.kernel = "composed_query_kernel<false>"
-            self.name = "c3cached"          # its own entry in profiles/ncu_traffic.json
+            self.name = "c3cached"
 
     def step(self, i):
         return self.comp(self.copies[i % len(self.copies)])
@@ -564,7 +593,7 @@ def cpu_arm(name):
                       "(sdf.py:392-433 restated: per-SDF loop + argmin)",
                       f"C3 ComposedSDF of 16 drills ({'CachedSDF res=0.005' if name == 'c3cached' else 'MeshSDF'})")
     if name in ("c4", "c4readme"):
-        d = os.path.join(tempfile.gettempdir(), "pvb_bench_arm_cpu")
+        d = os.path.join(scratch_dir(), "arm_cpu")
         urdf, end = workloads.write_arm(d)
         chain = opk.build_serial_chain_from_urdf(open(urdf).read(), end)
         robot = port.RobotSDFPort(chain, path_prefix=d, link_sdf_factory=port.cache_link_sdf_factory_port(0.02, 1.0))
@@ -699,9 +728,10 @@ def sum_over_ranks(x, world):
     return x
 
 
-def timed_steps(step, steps, warmup, world, sampler=None):
+def timed_steps(step, steps, warmup, world, sampler=None, last=None):
     """`warmup` untimed steps, then exactly `steps` steps bracketed by barrier + synchronize on both sides, timed with
-    CUDA events on the launch stream; returns (max-over-ranks ms for all steps, this rank's ms, host issue us/step)."""
+    CUDA events on the launch stream; returns (max-over-ranks ms for all steps, this rank's ms, host issue us/step).
+    `last`, when given, is called with the result of the last timed step after the timing has ended."""
     out = None
     for i in range(warmup):             # same ownership pattern as the timed loop (the previous result stays alive
         out = step(i)                   # while the next one is allocated), so the allocator is in steady state
@@ -720,6 +750,8 @@ def timed_steps(step, steps, warmup, world, sampler=None):
         sampler.sample_now()            # the GPU is still executing the queued timed steps here
     barrier(world)
     mine = t_begin.elapsed_time(t_end)
+    if last is not None:
+        last(out)
     del out
     return max_over_ranks(mine, world), mine, issue_us
 
@@ -765,7 +797,7 @@ def roofline_of(wl, kernel_ms):
     peak, peak_kind = measured_peaks()
     achieved = wl.alg_bytes / (kernel_ms * 1e-3) / 1e9
     return {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": ncu_traffic(wl.name), "ncu": ncu_limits(wl.name), "kernel": wl.kernel, "kernel_ms": kernel_ms,
+            "kernel": wl.kernel, "kernel_ms": kernel_ms,
             "algorithmic_bytes_per_launch": wl.alg_bytes, "peak_source": f"of {peak_kind}"}
 
 
@@ -807,11 +839,11 @@ def cpu_baseline_of(name, wl=None, seconds=6.0):
     return {"value": done / dt, "unit": UNIT, "cores": cpu_threads, "kind": "port", "sample": sample}
 
 
-def run_workload(name, rank, world, steps, warmup, with_e2e, with_cpu, sampler=None, full_affinity=None):
+def run_workload(name, rank, world, steps, warmup, with_e2e, with_cpu, sampler=None, full_affinity=None, last=None):
     """One non-headline workload: device-resident value, independent kernel time + roofline, e2e, CPU baseline."""
     wl = make_workload(name, rank, world)
     torch.cuda.synchronize()
-    total_ms, _, issue_us = timed_steps(wl.step, steps, warmup, world, sampler)
+    total_ms, _, issue_us = timed_steps(wl.step, steps, warmup, world, sampler, last)
     units_all = max_over_ranks(float(wl.units), world) * world if name in WEAK_SCALED \
         else sum_over_ranks(float(wl.units), world)
     res = {"value": units_all * steps / (total_ms * 1e-3), "unit": UNIT, "ms_per_step": total_ms / steps,
@@ -819,7 +851,7 @@ def run_workload(name, rank, world, steps, warmup, with_e2e, with_cpu, sampler=N
            "gpu_launches": wl.launches_per_step * steps, "host_issue_us_per_step": issue_us}
     res["roofline"] = roofline_of(wl, kernel_time_ms(wl.step))
     if with_e2e:
-        res["e2e"] = e2e_arm(wl, units_all, world, max(3, min(steps, 10)))
+        res["e2e"] = e2e_arm(wl, units_all, world, steps)
     if with_cpu:
         with all_host_cpus(full_affinity):
             res["cpu_baseline"] = cpu_baseline_of(name, wl)
@@ -830,7 +862,11 @@ def run_workload(name, rank, world, steps, warmup, with_e2e, with_cpu, sampler=N
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--steps", type=int, default=50,
+                    help="timed steps of every timed loop: the headline, its re-assembly variants and "
+                         "reconfigure_and_query, each entry of `workloads`, and every e2e arm. Not governed: "
+                         "roofline.kernel_ms (median of 7 separately timed launches) and cpu_baseline (a fixed "
+                         "time budget on the host)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--workload", default="default")
     ap.add_argument("--impl", default="native", choices=["native", "reference"])
@@ -839,7 +875,12 @@ def main():
     ap.add_argument("--no-workloads", action="store_true", help="default run: headline only")
     ap.add_argument("--mode", default=None, choices=[None, "none", "nccl", "peer", "mc", "dma"],
                     help="C4 at N>1: force the re-assembly method of the headline instead of picking the faster one")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the result of the last timed step as DIR/<name>.npy: the headline's (C4, or "
+                         "c4readme) in a default run, otherwise the one --workload's; GPU path only")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the GPU path computed; it has no meaning with --impl reference")
     args.warmup = max(args.warmup, 3) if args.impl == "native" else args.warmup
     if args.impl == "reference":
         return run_reference(args)
@@ -855,11 +896,12 @@ def main():
     barrier(world)
     sampler = ClockSampler(local)
     with_cpu = rank == 0 and world == 1 and not args.no_cpu_baseline
+    last = (lambda out: dump_outputs(out, args.dump_outputs)) if args.dump_outputs and rank == 0 else None
 
     if args.workload != "default" and args.workload not in ("c4", "c4readme"):
         # ---- single-workload mode (tuning / profiling scripts) ----
         wl, res = run_workload(args.workload, rank, world, args.steps, args.warmup, not args.no_e2e, with_cpu,
-                               sampler, full_affinity)
+                               sampler, full_affinity, last)
         clocks = sampler.stop()
         if rank == 0:
             line = {"metric": METRIC, "value": res["value"], "unit": UNIT, "n_gpus": world, "steps": args.steps,
@@ -875,39 +917,38 @@ def main():
     wl = make_workload("c4" if args.workload == "default" else args.workload, rank, world)
     torch.cuda.synchronize()
     units_all = sum_over_ranks(float(wl.units), world)
-    sub_steps = max(5, min(args.steps, 20))
     reassembly = None
     if world > 1:
         reassembly = {}
         wl.set_mode("none")
-        ms, _, _ = timed_steps(wl.step, sub_steps, args.warmup, world)
-        reassembly["no_reassembly"] = {"ms_per_step": ms / sub_steps, "value": units_all * sub_steps / (ms * 1e-3)}
+        ms, _, _ = timed_steps(wl.step, args.steps, args.warmup, world)
+        reassembly["no_reassembly"] = {"ms_per_step": ms / args.steps, "value": units_all * args.steps / (ms * 1e-3)}
         wl.set_mode("nccl")
-        ms, _, _ = timed_steps(wl.step, sub_steps, args.warmup, world)
-        reassembly["nccl_all_gather"] = {"ms_per_step": ms / sub_steps, "value": units_all * sub_steps / (ms * 1e-3)}
+        ms, _, _ = timed_steps(wl.step, args.steps, args.warmup, world)
+        reassembly["nccl_all_gather"] = {"ms_per_step": ms / args.steps, "value": units_all * args.steps / (ms * 1e-3)}
         err = wl.enable_peer()
         if err is None:
             wl.set_mode("peer")
-            ms, _, _ = timed_steps(wl.step, sub_steps, args.warmup, world)
+            ms, _, _ = timed_steps(wl.step, args.steps, args.warmup, world)
             remote = 16.0 * wl.units * (world - 1)          # bytes this rank pushes to its peers per step
-            reassembly["peer_stores"] = {"ms_per_step": ms / sub_steps, "value": units_all * sub_steps / (ms * 1e-3),
-                                         "nvlink_out_GBps_per_rank": remote / (ms / sub_steps * 1e-3) / 1e9,
+            reassembly["peer_stores"] = {"ms_per_step": ms / args.steps, "value": units_all * args.steps / (ms * 1e-3),
+                                         "nvlink_out_GBps_per_rank": remote / (ms / args.steps * 1e-3) / 1e9,
                                          "nvlink_in_bytes_per_rank": remote, "buffers": wl.peer.backend}
             slab = wl.end - wl.begin
             for pieces in (1, 2, 4):         # copy-engine pushes: the slab at once, or in pieces that overlap the kernel
                 wl.peer.dma_chunk_cfgs = 0 if pieces == 1 else max(1, -(-slab // pieces))
                 wl.set_mode("dma")
-                ms, _, _ = timed_steps(wl.step, sub_steps, args.warmup, world)
+                ms, _, _ = timed_steps(wl.step, args.steps, args.warmup, world)
                 reassembly[f"dma_push_{pieces}"] = {
-                    "ms_per_step": ms / sub_steps, "value": units_all * sub_steps / (ms * 1e-3),
+                    "ms_per_step": ms / args.steps, "value": units_all * args.steps / (ms * 1e-3),
                     "chunk_cfgs": wl.peer.dma_chunk_cfgs or slab,
-                    "nvlink_ingest_GBps_per_rank": 16.0 * (units_all - wl.units) / (ms / sub_steps * 1e-3) / 1e9}
+                    "nvlink_ingest_GBps_per_rank": 16.0 * (units_all - wl.units) / (ms / args.steps * 1e-3) / 1e9}
             if wl.peer.multicast:
                 wl.set_mode("mc")
-                ms, _, _ = timed_steps(wl.step, sub_steps, args.warmup, world)
-                reassembly["multicast_stores"] = {"ms_per_step": ms / sub_steps,
-                                                  "value": units_all * sub_steps / (ms * 1e-3),
-                                                  "nvlink_out_GBps_per_rank": 16.0 * wl.units / (ms / sub_steps * 1e-3) / 1e9}
+                ms, _, _ = timed_steps(wl.step, args.steps, args.warmup, world)
+                reassembly["multicast_stores"] = {"ms_per_step": ms / args.steps,
+                                                  "value": units_all * args.steps / (ms * 1e-3),
+                                                  "nvlink_out_GBps_per_rank": 16.0 * wl.units / (ms / args.steps * 1e-3) / 1e9}
             else:
                 reassembly["multicast_stores"] = {"unavailable": wl.peer.backend_note or
                                                   f"no multicast mapping (buffers: {wl.peer.backend})"}
@@ -918,7 +959,7 @@ def main():
             if "ms_per_step" in reassembly.get(k, {}):
                 reassembly[k]["nvlink_ingest_GBps_per_rank"] = \
                     16.0 * (units_all - wl.units) / (reassembly[k]["ms_per_step"] * 1e-3) / 1e9
-        reassembly["nvlink_peak_GBps_per_direction"] = 770.0      # B200_PROFILING.md
+        reassembly["nvlink_peak_GBps_per_direction"] = 450.0      # H100 SXM data sheet: NVLink 4, 900 GB/s both ways
         if args.mode:
             chosen = args.mode
         else:
@@ -944,18 +985,19 @@ def main():
         reassembly["chosen"] = chosen
         wl.set_mode(chosen)
 
-    total_ms, _, issue_us = timed_steps(wl.step, args.steps, args.warmup, world, sampler)
+    total_ms, _, issue_us = timed_steps(wl.step, args.steps, args.warmup, world, sampler, last)
     clocks = sampler.stop()
     value = units_all * args.steps / (total_ms * 1e-3)
     kernel_ms = kernel_time_ms(wl.step)
     roofline = roofline_of(wl, kernel_ms)
     # FK + query through the public API (set_joint_configuration is part of every control-loop iteration)
-    rq_ms, _, _ = timed_steps(wl.step_reconfigure, sub_steps, 3, world)
-    reconfigure = {"ms_per_step": rq_ms / sub_steps, "value": units_all * sub_steps / (rq_ms * 1e-3),
+    rq_ms, _, _ = timed_steps(wl.step_reconfigure, args.steps, 3, world)
+    reconfigure = {"ms_per_step": rq_ms / args.steps, "value": units_all * args.steps / (rq_ms * 1e-3),
+                   "steps": args.steps,
                    "what": "RobotSDF.set_joint_configuration(q[200,7]) + the headline step, device-resident inputs"}
     e2e = None
     if not args.no_e2e:
-        e2e = e2e_arm(wl, units_all, world, max(3, min(args.steps, 10)))
+        e2e = e2e_arm(wl, units_all, world, args.steps)
         wl.restore()
     cpu = None
     if with_cpu:
@@ -973,7 +1015,7 @@ def main():
         others = {}
         for name in OTHER_WORKLOADS:
             try:
-                w, res = run_workload(name, rank, world, min(args.steps, 30), args.warmup, not args.no_e2e,
+                w, res = run_workload(name, rank, world, args.steps, args.warmup, not args.no_e2e,
                                       with_cpu, None, full_affinity)
                 others[name] = res
                 del w

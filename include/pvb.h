@@ -1,9 +1,9 @@
 /*
- * pvb.h -- C ABI of libpvb.so, the B200 (sm_100a) signed-distance query library.
+ * pvb.h -- C ABI of libpvb.so, the H100 (sm_90a) signed-distance query library.
  *
  * The reference (UM-ARM-Lab/pytorch_volumetric) is pure Python and has no FFI
  * of its own; each entry point below replaces the body of one reference
- * operator (file:line under /root/reference) and is what a binding for that
+ * operator (file:line in the reference repository) and is what a binding for that
  * operator would call.  See INTEGRATION.md for the ctypes stub a maintainer
  * would add on the reference side.
  *

@@ -15,9 +15,9 @@ Layout
                              (sdf.py, voxel.py, model_to_sdf.py, chamfer.py)
   shims/                     packages named like the four third-party
                              dependencies that re-export the tp_* modules, so
-                             the UNMODIFIED reference source under
-                             /root/reference can be imported in the build
-                             container (make_golden.py) to pin port.py
+                             the UNMODIFIED reference source of a checkout
+                             (PVB_REFERENCE_SRC) can be imported by
+                             make_golden.py to pin port.py
   make_golden.py             writes tests/golden/*.npz with the real reference
                              code running over the shims
 

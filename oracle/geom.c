@@ -2,7 +2,7 @@
  * oracle/geom.c -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  *
  * CPU restatement of the geometry arithmetic that the reference obtains from
- * Open3D / Embree (third-party, not vendored under /root/reference, version
+ * Open3D / Embree (third-party, not vendored in the reference, version
  * unpinned in pyproject.toml:54-61):
  *
  *   - RaycastingScene.compute_closest_points   (reference call site

@@ -1,28 +1,40 @@
-"""Generate tests/golden/*.npz in the BUILD container (needs /root/reference).
+"""Generate tests/golden/*.npz from a checkout of the reference project (UM-ARM-Lab/pytorch_volumetric), whose
+root directory is given by the PVB_REFERENCE_SRC environment variable.
 
 TEST INFRASTRUCTURE.  Two kinds of fixtures:
 
 1. meshes.npz -- the reference's own test meshes (tests/probe.obj,
    tests/offset_wrench_nogrip.obj, tests/YcbPowerDrill/textured_simple_reoriented.obj,
    tests/pv_sdf_debug/scene_mesh_{overlap,separated}.obj) parsed to (vertices fp64, faces int32) arrays,
-   because /root/reference does not exist on the GPU box.
+   so that the tests need no copy of the reference.
 
 2. ref_*.npz -- input/output vectors produced by the UNMODIFIED reference source
-   (/root/reference/src/pytorch_volumetric) imported over oracle/shims (the restated third-party
+   (src/pytorch_volumetric of the checkout) imported over oracle/shims (the restated third-party
    dependencies).  They pin oracle/port.py (tests/test_oracle_pinning.py) and serve as golden vectors for
    the CUDA path (tests/test_gpu_mesh.py, test_gpu_cached.py, test_gpu_composed.py, test_gpu_chamfer_sample.py).
 
-Run:  python -m oracle.make_golden
+Run:  PVB_REFERENCE_SRC=<checkout> python -m oracle.make_golden [voxel|robot_r008]
 """
+import atexit
 import os
+import shutil
 import sys
+import tempfile
 
 import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("PVB_REFERENCE_SRC", "")
 GOLD = os.path.join(ROOT, "tests", "golden")
+
+
+def scratch_dir():
+    """A fresh temporary directory for the reference's cache files, removed at exit."""
+    d = tempfile.mkdtemp(prefix="pvb_golden_")
+    atexit.register(shutil.rmtree, d, True)
+    return d
+
 
 MESHES = {
     "probe": "tests/probe.obj",
@@ -63,8 +75,7 @@ def ray_noise_for(n, seed):
 def make_reference_vectors():
     pv = import_reference()
     import pytorch_kinematics as pk
-    tmp = "/tmp/pvb_golden_cache"
-    os.makedirs(tmp, exist_ok=True)
+    tmp = scratch_dir()
     g = torch.Generator().manual_seed(1234)
 
     # ---- MeshSDF on probe / wrench / drill: random points around the mesh (sdf.py:122-172) ----
@@ -180,6 +191,7 @@ def make_reference_vectors():
                         table_val=link0.voxels.raw_data.numpy(), table_grad=link0.voxels_grad.numpy(),
                         table_shape=np.array(link0.voxels.shape), ranges=np.array(link0.ranges))
     print("robot:", rv.shape, rbb.shape)
+    make_robot_r008_vectors(pv, pk, tmp)
 
     # ---- chamfer (tests/test_chamfer.py:16-66) ----
     for name in ("probe", "wrench"):
@@ -200,6 +212,28 @@ def make_reference_vectors():
         np.savez_compressed(os.path.join(GOLD, f"ref_chamfer_{name}.npz"), pts_world=pts_world.numpy(),
                             w2o=w2o.numpy(), err0=err0.numpy(), w2o_p=w2o_p.numpy(), err1=err1.numpy())
         print(name, "chamfer: err0 max", float(err0.max()), "err1 mean", float(err1.mean()))
+
+
+def make_robot_r008_vectors(pv, pk, tmp):
+    """The single-link robot of the reference's tests/test_model_to_sdf.py:263-290 with the link table BUILT by the
+    reference (resolution 0.008, padding 0.05, numpy seed 1 for the ray draws): joint values, query points, values,
+    gradients and the surface box -> ref_robot_wrench_r008.npz (tests/test_oracle_pinning.py rebuilds the table with
+    the port and must reproduce every number)."""
+    urdf = open(os.path.join(REF, "tests", "offset_wrench.urdf")).read()
+    chain = pk.build_serial_chain_from_urdf(urdf, "offset_wrench")
+    np.random.seed(1)
+    rs = pv.RobotSDF(chain, path_prefix=os.path.join(REF, "tests"),
+                     link_sdf_cls=pv.cache_link_sdf_factory(resolution=0.008, padding=0.05,
+                                                            cache_path=os.path.join(tmp, "sdf_wrench_r008.pkl"),
+                                                            clean_cache=True))
+    th = torch.tensor([[0.01, -0.02, 0.0, 0.3, -0.2, 0.5], [0.0, 0.0, 0.0, 0.0, 0.0, 0.0]])
+    rs.set_joint_configuration(th)
+    q = (torch.rand(500, 3, generator=torch.Generator().manual_seed(5)) - 0.5) * 0.4
+    v, g = rs(q)
+    bb = rs.surface_bounding_box(padding=0.01)
+    np.savez_compressed(os.path.join(GOLD, "ref_robot_wrench_r008.npz"), th=th.numpy(), q=q.numpy(), val=v.numpy(),
+                        grad=g.numpy(), bbox=bb.numpy())
+    print("robot r008:", v.shape, bb.shape)
 
 
 def make_voxel_vectors():
@@ -258,8 +292,8 @@ def make_voxel_vectors():
     obj = pv.MeshObjectFactory(os.path.join(REF, MESHES["probe"]))
     sdf = pv.MeshSDF(obj)
     np.random.seed(5)
-    cached = pv.CachedSDF("probe", 0.002, obj.bounding_box(padding=0.01), sdf, cache_path="/tmp/pvb_golden_voxel.pkl",
-                          clean_cache=True)
+    cached = pv.CachedSDF("probe", 0.002, obj.bounding_box(padding=0.01), sdf,
+                          cache_path=os.path.join(scratch_dir(), "voxel.pkl"), clean_cache=True)
     inner = cached.get_filtered_points(lambda v: v < -0.001)
     out["fp_interior"] = inner.numpy()
     out["fp_table"] = cached.voxels.raw_data.numpy()
@@ -270,9 +304,16 @@ def make_voxel_vectors():
 
 
 if __name__ == "__main__":
+    if not os.path.isdir(os.path.join(REF, "src", "pytorch_volumetric")):
+        sys.exit("set PVB_REFERENCE_SRC to the root of a UM-ARM-Lab/pytorch_volumetric checkout")
     os.makedirs(GOLD, exist_ok=True)
     if len(sys.argv) > 1 and sys.argv[1] == "voxel":
         make_voxel_vectors()
+    elif len(sys.argv) > 1 and sys.argv[1] == "robot_r008":
+        import_reference()
+        import pytorch_volumetric as pv
+        import pytorch_kinematics as pk
+        make_robot_r008_vectors(pv, pk, scratch_dir())
     else:
         make_meshes()
         make_reference_vectors()

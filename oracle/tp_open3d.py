@@ -3,7 +3,7 @@
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
 Open3D is a third-party dependency of the reference that is NOT vendored under
-/root/reference and is unpinned (pyproject.toml:54-61, "open3d").  The
+the reference and is unpinned (pyproject.toml:54-61, "open3d").  The
 published behaviour of the calls made at the sites below is restated; nothing
 here was checked against a real Open3D build ("parity unpinned" at this
 boundary, see DESIGN.md):

@@ -1,4 +1,4 @@
-"""pytorch_volumetric_b200 -- B200-native (sm_100a) drop-in for pytorch_volumetric's batched SDF query path.
+"""pytorch_volumetric_b200 -- H100-native (sm_90a) drop-in for pytorch_volumetric's batched SDF query path.
 
 The public names of the reference package (`pytorch_volumetric/__init__.py`) that belong to that path are
 re-exported here, so `import pytorch_volumetric_b200 as pv` reads like the original.

@@ -17,7 +17,7 @@ LIB_PATH = os.environ.get("PVB_LIB") or os.path.join(CSRC, "libpvb.so")   # PVB_
 SOURCES = ["pvb_kernels.cu", "bvh_build.cpp"]
 HEADERS = ["pvb_device.cuh", os.path.join("..", "..", "include", "pvb.h")]
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 PVB_KIND_GRID, PVB_KIND_MESH, PVB_KIND_SPHERE = 0, 1, 2
@@ -42,7 +42,7 @@ def lib_missing():
 
 
 def build(force=False, verbose=False):
-    """nvcc-compile the sm_100a library in-tree (cross-compiles without a GPU)."""
+    """nvcc-compile the sm_90a library in-tree (cross-compiles without a GPU)."""
     if not force and not needs_build():
         return LIB_PATH
     nvcc = os.environ.get("PVB_NVCC", "nvcc")
@@ -203,7 +203,7 @@ def check(rc, what=""):
 def compute_device(device=None):
     """The CUDA device queries run on.  Raises when no GPU is present."""
     if not torch.cuda.is_available():
-        raise NativeLibraryError("pytorch_volumetric_b200 needs a CUDA device (B200, sm_100a); "
+        raise NativeLibraryError("pytorch_volumetric_b200 needs a CUDA device (H100, sm_90a); "
                                  "there is no CPU fallback for the SDF query path")
     if device is None:
         return torch.device("cuda", torch.cuda.current_device())

@@ -1,6 +1,6 @@
 """Points-to-mesh chamfer distance and the pose-set metrics built on it.
 
-Mirrors /root/reference/src/pytorch_volumetric/chamfer.py: batch_chamfer_dist (:62-120) runs as one fused
+Mirrors the reference's src/pytorch_volumetric/chamfer.py: batch_chamfer_dist (:62-120) runs as one fused
 kernel (transform -> unsigned nearest distance / table value -> square -> mean, pvb_chamfer);
 pairwise_distance_chamfer (:20-59) and PlausibleDiversity (:130-195) are thin reductions on top of it.
 """

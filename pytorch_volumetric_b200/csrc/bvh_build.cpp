@@ -1,7 +1,7 @@
 // bvh_build.cpp -- host-side BVH4 construction for libpvb.so.
 //
 // Replaces the Embree scene build the reference triggers through
-// RaycastingScene.add_triangles (/root/reference/src/pytorch_volumetric/sdf.py:115-118).
+// RaycastingScene.add_triangles (reference src/pytorch_volumetric/sdf.py:115-118).
 // Binned-SAH binary build -> greedy collapse to 4-wide nodes -> breadth-first
 // layout (so the top of the tree is a contiguous prefix the query kernels stage
 // into shared memory with one bulk copy) -> triangles emitted in leaf order.

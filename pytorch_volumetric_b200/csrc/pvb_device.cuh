@@ -1,4 +1,4 @@
-// pvb_device.cuh -- device-side building blocks shared by the sm_100a kernels.
+// pvb_device.cuh -- device-side building blocks shared by the sm_90a kernels.
 //
 //   grid_eval      CachedSDF.__call__ for one point          (reference sdf.py:535-571)
 //   bvh_closest    closest point on the mesh                 (Embree rtcPointQuery role, sdf.py:134)
@@ -14,7 +14,7 @@ namespace pvb {
 constexpr int kStack = 64;            // traversal stack entries per thread; the builder bounds the depth at 20
 
 // Traversal statistics hook: expands to nothing in the CUDA build; the host build of this header (tests/hostsim)
-// defines it to count node visits and triangle tests per query (SURVEY 8d-iii, reported in profiles/README.md).
+// defines it to count node visits and triangle tests per query (SURVEY 8d-iii, scripts/traversal_stats.py).
 #ifndef PVB_STAT
 #define PVB_STAT(counter)
 #endif
@@ -41,7 +41,7 @@ __device__ __forceinline__ const float4 *node_ptr(const float4 *gnodes, const No
 // ----------------------------------------------------------------------------
 // Closest point on triangle (Ericson, RTCD 5.1.5), fp32.
 // (Round 2 tried deriving d3..d6 from d1, d2 and the Gram terms ab.ab, ab.ac, ac.ac -- 4 subtractions instead of 6
-// subtractions + 12 multiply-adds, about 8 % of the tree-walk kernels' instructions.  Rejected on the CPU tier before it
+// subtractions + 12 multiply-adds in the tree walk's hottest function.  Rejected on the CPU tier before it
 // reached a GPU: on sliver triangles the cancellation costs accuracy, tests/test_hostsim.py's degenerate-soup fuzz read
 // 2.2e-6 relative distance error against the 2e-6 bound the direct dot products meet.)
 __device__ __forceinline__ f3 closest_on_triangle(f3 p, f3 a, f3 b, f3 c) {
@@ -89,13 +89,10 @@ __device__ __forceinline__ float box_d2(float lx, float ly, float lz, float hx, 
 
 // Nearest-first BVH4 descent.  `init_d2` is an initial search radius (squared);
 // candidates farther than that are never reported (face stays -1).
-// (Tried and measured slower, 1e7 queries on the 10k-triangle mesh: leaves as stack entries popped in distance
-// order, 11.3 ms against 9.9 ms for testing leaves inline -- the extra local-memory stack traffic costs more than
-// the better lane occupancy of the triangle code buys; runs of consecutive queries seeded with the previous closest
-// point, 11.4-15.9 ms.)
-// A phase-aligned "while-while" walk (Aila & Laine: advance to a leaf first, then test triangles together) was also
-// measured: mesh10k / C5 / C3 7.6 / 7.7 / 13.9 ms against 7.6 / 7.6 / 13.1 ms for this inline-leaf walk -- no gain,
-// the cost is in the triangle tests themselves; see profiles/README.md.
+// (Rejected alternatives: leaves as stack entries popped in distance order -- the extra local-memory stack traffic
+// costs more than the better lane occupancy of the triangle code buys; runs of consecutive queries seeded with the
+// previous closest point; a phase-aligned "while-while" walk (Aila & Laine: advance to a leaf first, then test
+// triangles together) -- no gain, the cost is in the triangle tests themselves.)
 __device__ __forceinline__ Closest bvh_closest(const float4 *__restrict__ gnodes, const NodeStage &st,
                                                const float4 *__restrict__ tris, f3 p, float init_d2) {
     Closest best;
@@ -467,8 +464,8 @@ __device__ __noinline__ int grid_axis_index_exact(float pv, double min64, double
     return min(max((int)kf, 0), n - 1);
 }
 
-// The evaluator is written branch-free on purpose: the first version of this kernel spent 23 % of its issue slots
-// on BRA/BSSY/BSYNC and saturated the XU pipe (FRND/F2I/MUFU); see profiles/README.md.
+// The evaluator is written branch-free on purpose: the first version of this kernel spent a large share of its issue
+// slots on BRA/BSSY/BSYNC and saturated the XU pipe (FRND/F2I/MUFU).
 //   * rint / float->int by the 1.5*2^23 magic add (FADD on the FMA pipe, no XU op); valid for |q| < 2^22, and
 //     anything larger is out of range anyway
 //   * the fp32 estimate q = (p - min32) * inv_res32 is accepted when |q - rint(q)| <= idx_certain (it then provably
@@ -624,8 +621,8 @@ __device__ __forceinline__ void composed_consider(const pvb_sdf_desc &d, const N
 // Configuration tiles.  The first cfg_count / 32 tiles hold 32 configurations each (lanes = configurations, one point
 // per warp step).  The remainder R = cfg_count % 32 is split by its binary digits into FULL tiles of 16 / 8 / 4 / 2 / 1
 // configurations, in which the 32 lanes are 32 / LC point groups x LC configurations: no lane ever idles because the
-// configuration count is not a multiple of 32 (200 = 6 x 32 + 8 ran a seventh tile at 8 of 32 lanes: 11 % of the time;
-// the 25-configuration slab of an 8-GPU split ran at 25 of 32).
+// configuration count is not a multiple of 32 (200 = 6 x 32 + 8 would run a seventh tile at 8 of 32 lanes; the
+// 25-configuration slab of an 8-GPU split at 25 of 32).
 __device__ __forceinline__ void rs_tile(int cfg_count, int t, int &c0, int &lc_log2) {
     const int n_full = cfg_count >> 5;
     if (t < n_full) { c0 = t << 5; lc_log2 = 5; return; }

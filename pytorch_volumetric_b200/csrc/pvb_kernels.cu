@@ -1,4 +1,4 @@
-// pvb_kernels.cu -- sm_100a kernels and the C ABI of libpvb.so (see include/pvb.h).
+// pvb_kernels.cu -- sm_90a (H100) kernels and the C ABI of libpvb.so (see include/pvb.h).
 //
 // No tensor-core work anywhere on this path (there is no dense contraction).  The kernels are
 //   grid_lookup_tma / vec4 / scalar   HBM-streaming nearest-voxel lookup (CachedSDF)
@@ -6,7 +6,7 @@
 //   sort_hist / sort_scan / sort_scatter  Morton binning of large query batches
 //   mesh_query, chamfer_partial / finish  BVH4 tree walks (MeshSDF, chamfer)
 //   mesh_sample, sphere, transform_points  small helpers
-// Every tuning decision below carries its measurement in a comment; profiles/README.md has the full log.
+// Tuning knobs that are build macros or PVB_* environment variables can be swept without editing the source.
 #include "pvb_device.cuh"
 
 #include <cstdarg>
@@ -58,7 +58,7 @@ static int sm_count() {
     const int dev = current_device();
     if (n[dev] == 0) {
         int v = 0;
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;   // H100 SXM
         n[dev] = v;
     }
     return n[dev];
@@ -166,7 +166,7 @@ __device__ __forceinline__ f3 load_point(const float *__restrict__ pts, long lon
 
 // ===================================================== spatial binning of queries
 // A random query batch makes every lane of a warp walk a different part of the BVH: the first version of the mesh
-// kernel executed 64 000 warp-instructions per 32 queries (~10 % SIMT efficiency, profiles/README.md).  Large
+// kernel kept few lanes of a warp busy.  Large
 // batches are therefore binned into 64^3 Morton-ordered cells over the padded mesh AABB with a counting sort
 // (histogram by atomics, single-block scan, scatter) and the tree walk processes them in that order through an
 // index permutation; results are written to the original slots, so callers see no reordering.
@@ -175,12 +175,11 @@ constexpr int kSortBitsMax = 8;                            // 256^3 cells = 64 M
 
 // Cells per axis for a batch of n queries.  Lanes of a warp are 32 consecutive queries of the binned order: they walk
 // the same part of the tree only if a cell is not much larger than the triangles around it, and a cell holds n / cells
-// queries in arbitrary order.  PVB_SORT_BITS overrides (measurements in profiles/README.md).
+// queries in arbitrary order.  PVB_SORT_BITS overrides.
 static int sort_bits_for(long long n) {
     static const int forced = [] { const char *e = getenv("PVB_SORT_BITS"); return e ? atoi(e) : 0; }();
     if (forced >= 4 && forced <= kSortBitsMax) return forced;
-    // measured (profiles/r02/tune_sort_bits.jsonl, ms per step at 6 / 7 / 8 bits): mesh10k 7.66 / 7.96 / 14.4, C5 6.77 /
-    // 6.74 / 13.1, mesh50k 17.5 / 16.8 / 23.4 -- finer cells do not pay for the larger histogram; 64^3 stays
+    // finer cells than 64^3 cost a larger histogram (zeroing + single-block scan) for little gain in coherence
     (void)n;
     return kSortBits;
 }
@@ -230,7 +229,7 @@ __global__ void sort_hist_kernel(const SortFrame f, const float *__restrict__ pt
 }
 
 // exclusive scan of the cell counters in place, one block of 1024 threads (256 counters per thread, moved as
-// 64 independent 128-bit loads so that the single block is not serialised on L2 latency: 442 us -> tens of us)
+// 64 independent 128-bit loads so that the single block is not serialised on L2 latency)
 __global__ void __launch_bounds__(1024) sort_scan_kernel(uint32_t *__restrict__ hist, int n_cells) {
     __shared__ uint32_t warp_sum[32];
     const int per4 = n_cells / 1024 / 4;              // uint4 per thread (n_cells is a power of two >= 4096)
@@ -274,7 +273,7 @@ __global__ void __launch_bounds__(1024) sort_scan_kernel(uint32_t *__restrict__ 
 // {x, y, z, original index} per lane and write their results as one coalesced 16-byte record {d, gx, gy, gz} into a
 // staging buffer in binned order; unpermute_kernel brings them home with coalesced writes.  (Round 1 walked through an
 // index permutation: 12-byte point loads and 4/12-byte result stores at random addresses, 32-byte sectors half used
-// and read-modify-written -- ncu showed 3.9 GB of DRAM traffic for 0.28 GB of algorithmic bytes.)
+// and read-modify-written -- many times the algorithmic bytes in DRAM traffic.)
 // `cell_inv` holds the cell id of point i on entry and its binned position on exit (same thread reads, then writes).
 __global__ void sort_scatter_kernel(uint32_t *__restrict__ cell_inv, const float *__restrict__ pts, long long n,
                                     uint32_t *__restrict__ offs, float4 *__restrict__ sorted) {
@@ -313,7 +312,7 @@ static size_t sort_workspace_bytes(long long n) {
 // ================================================================ mesh query
 constexpr int kMeshThreads = 256;
 #ifndef PVB_MESH_MINB
-#define PVB_MESH_MINB 4   // 64 registers, 4 CTAs per SM: 8.5 ms against 10.0 ms at 86 registers (1e7 queries, 10k triangles)
+#define PVB_MESH_MINB 4   // 64 registers, 4 CTAs per SM: occupancy over registers for the latency-bound tree walk
 #endif
 
 __global__ void __launch_bounds__(kMeshThreads, PVB_MESH_MINB)
@@ -667,8 +666,8 @@ __global__ void sphere_kernel(float radius, const float *__restrict__ pts, long 
 // evaluate, keep the running min (first index on ties, as torch.argmin), rotate the winning gradient back -- and
 // writes (val, grad) once.  The S*|A|*P*3 intermediates of sdf.py:399-415 never exist.
 //
-// Where the time goes is the LSU: a random 16-byte table gather costs ~2 L1 wavefront-cycles per lane (measured,
-// scripts/ubench_gather.cu), and so does every warp-uniform LDS/LDG.  Hence
+// Where the time goes is the LSU: a random 16-byte table gather costs L1 wavefront-cycles per lane
+// (scripts/ubench_gather.cu measures how many), and so does every warp-uniform LDS/LDG.  Hence
 //   * the descriptors travel as a __grid_constant__ kernel parameter (constant bank, uniform datapath, no LSU);
 //     the first version staged them in shared memory and spent more LSU cycles on descriptor fields than on gathers
 //   * 4 points per thread: one broadcast read of a link transform serves 4 points; points / results move as
@@ -684,7 +683,7 @@ constexpr int kCompSmemXf = 64;
 #define PVB_COMP_MINB 4
 #endif
 #ifndef PVB_COMPMESH_MINB
-#define PVB_COMPMESH_MINB 4   // C3 (16 drills): 16.4 / 14.6 / 13.1 ms at 1 / 3 / 4 CTAs per SM
+#define PVB_COMPMESH_MINB 4   // CTAs per SM of the mesh instantiation (C3, 16 drills): occupancy hides the tree walk
 #endif
 
 // `order` is the sequence in which the sub-SDFs are visited: the bit-reversal permutation of 0..n-1.  Along a
@@ -778,8 +777,8 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
             };
             // every sub-SDF in visiting order, skipped when provably not the argmin (composed_consider,
             // pvb_device.cuh).  (Evaluating the sub-SDF with the smallest AABB lower bound first -- an extra pass
-            // over all of them without table access -- saves lookups but measured 1.8x slower: the kernel is
-            // issue-bound; profiles/README.md.)
+            // over all of them without table access -- saves lookups but adds issue slots to a kernel that is
+            // issue-bound.)
             // ... except when sub-SDFs are MESHES (kMesh, one point per thread): an evaluation is a tree walk of
             // thousands of instructions, so one cheap pass computes every sub-SDF's AABB lower bound and the thread
             // then evaluates them NEAREST BOUND FIRST, stopping as soon as the smallest remaining bound exceeds the
@@ -890,8 +889,8 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
 // the point.  Results are bit-identical to the point-major kernel (same transform / lookup arithmetic; pruning is
 // exact).  A block owns a tile of 32 configurations x 32 points; results are transposed through shared memory so
 // that global stores stay coalesced along the point axis.
-// (Visiting the link with the nearest bounding sphere first was measured on C4 / the README shape: 1.26 / 0.224 ms
-// against 1.05 / 0.182 ms in index order -- the extra pass costs more than the lookups it saves.)
+// (Visiting the link with the nearest bounding sphere first is not done here: the extra pass costs more than the
+// lookups it saves in this configuration-major layout.)
 constexpr int kCmCfg = 32;
 constexpr int kCmWarps = 8;
 constexpr int kCmPts = 4;                         // points per thread
@@ -1007,8 +1006,8 @@ composed_cfgmajor_kernel(const __grid_constant__ DescPack<kCmMaxS> descs, int n_
         if (kMulti && tg.vec && tile * kCmTilePts + kCmTilePts <= n_pts) {
             // Peer destinations are not cached on this side of NVLink, so every store instruction should leave as
             // whole 32-byte sectors: a row is 128 B of values + 384 B of gradients, both contiguous -> lanes 0-7
-            // carry the values, lanes 8-31 the gradients, ONE 16-byte store per lane and destination (the strided
-            // 4-byte stores of the single-destination path measured 363 GB/s per rank on 8 GPUs).
+            // carry the values, lanes 8-31 the gradients, ONE 16-byte store per lane and destination (instead of the
+            // strided 4-byte stores of the single-destination path).
             for (int r = warp; r < ncfg; r += kCmWarps) {
                 const float *row = reinterpret_cast<const float *>(&sm.out[r][0]);     // {val, gx, gy, gz} per point
                 float w[4];
@@ -1051,9 +1050,9 @@ composed_cfgmajor_kernel(const __grid_constant__ DescPack<kCmMaxS> descs, int n_
 // ------------------------------------------------------------------------------------------------------------
 // RobotSDF kernel, second generation (round 2): the configuration-major scheme above, specialised to what a
 // RobotSDF with cached links is -- every sub-SDF a GRID with the bounding-box out-of-range rule -- and rebuilt around
-// what the round-1 profile of composed_cfgmajor_kernel showed (profiles/r02/): 29 warp-instructions per
+// what the first profile of composed_cfgmajor_kernel showed: 29 warp-instructions per
 // (configuration, point) pair, 142 LDC + 183 MOV in the SASS because the descriptors were indexed with a run-time
-// link number, 80 registers (3 CTAs per SM, 36 % warps active), four scalar stores per pair.
+// link number, 80 registers (3 CTAs per SM), four scalar stores per pair.
 //   * the host passes the descriptors ALREADY in visiting order and the link loop is fully unrolled, so every
 //     descriptor field is a constant-bank operand of the instruction that uses it (no LDC, no MOV, no index math);
 //   * the transforms and bounding spheres are staged in visiting order as well: shared-memory addresses are
@@ -1069,11 +1068,11 @@ composed_cfgmajor_kernel(const __grid_constant__ DescPack<kCmMaxS> descs, int n_
 #define PVB_ROBOT_PTS 4       // points per thread (4 or 2)
 #endif
 #ifndef PVB_ROBOT_MINB
-#define PVB_ROBOT_MINB 3      // resident CTAs per SM the <= 8-link instantiation is compiled for: 80 registers, no spills (0.75 ms on C4 against 0.82 ms at 64 registers with spills)
+#define PVB_ROBOT_MINB 3      // resident CTAs per SM the <= 8-link instantiation is compiled for: 80 registers, no spills (64 registers spill)
 #endif
 #ifndef PVB_ROBOT_UNROLL
 #define PVB_ROBOT_UNROLL 0    // 1: fully unrolled link loop (descriptor fields become immediates, but the 8 x kRbPts inlined
-#endif                        // visits overflow the instruction cache: measured 1.61 ms against 0.87 ms, profiles/r02/)
+#endif                        // visits overflow the instruction cache)
 constexpr int kRbCfg = 32;                        // lanes = configurations
 constexpr int kRbWarps = 8;
 constexpr int kRbPts = PVB_ROBOT_PTS;             // points per thread
@@ -1277,8 +1276,8 @@ robot_query_kernel(const __grid_constant__ RobotPack<MAXS> pk, int n_sdf, const 
         if constexpr (kDest == 0) {
             // One destination in local memory: every lane owns kRbPts consecutive points of its configuration's row,
             // 16 B of values + 48 B of gradients, and stores them itself -- no staging, no block barrier in the tile
-            // loop (the barriers of the staged path were 29 % of the warps' time: warps of a block finish their points
-            // at different moments).  The 16-byte pieces of neighbouring warps complete each other's sectors in L2.
+            // loop (the barriers of the staged path cost a large share of the warps' time: warps of a block finish
+            // their points at different moments).  The 16-byte pieces of neighbouring warps complete each other's sectors in L2.
             const size_t o = (size_t)(c0 + lane) * n_pts + pt0;
             if (vec && full_tile) {
                 if (lane_on) {
@@ -1376,14 +1375,14 @@ robot_query_kernel(const __grid_constant__ RobotPack<MAXS> pk, int n_sdf, const 
 
 // ------------------------------------------------------------------------------------------------------------
 // RobotSDF kernel, third generation: point-serial, nearest-sphere-first.
-// What the profiles of robot_query_kernel said (profiles/r02/c4_robot_r_p4m3.ncu.json): 454 M warp-instructions for
-// 2e7 pairs, of which 62 % in link visits that run for 5.3 of the 8 links per (point, 32 configurations) although a lane
-// needs 3.1 -- a fixed visiting order lets the running minimum tighten slowly, and "any lane needs it" makes the whole
-// warp pay; 17 % in the bounding-sphere tests of all 8 links x 4 points; L1 wavefronts at 51 % (16-byte stores to 32
-// different rows per instruction); 80 registers, 33 % warps active, long-scoreboard (gather latency) the top stall.
+// What the profiles of robot_query_kernel said: most instructions go to link visits, which run for 5.3 of the 8 links
+// per (point, 32 configurations) although a lane needs 3.1 -- a fixed visiting order lets the running minimum tighten
+// slowly, and "any lane needs it" makes the whole warp pay; the next share goes to the bounding-sphere tests of all
+// 8 links x 4 points; 16-byte stores to 32 different rows per instruction load the L1; 80 registers limit the
+// resident warps, and gather latency is the top stall.
 //   * one point at a time per warp (lanes = 32 configurations), so the state of a point is 8 registers, not 32;
 //   * the (configuration, link) bounding spheres sit in shared memory, one LDS.128 per link and point (keeping them in
-//     32 registers was measured slower, see below); per point one pass turns them into lower bounds lb_s <= value_s,
+//     32 registers costs occupancy, see below); per point one pass turns them into lower bounds lb_s <= value_s,
 //     kept in 8 registers;
 //   * the link with the smallest bound (lane 0's, shuffled: neighbouring configurations agree) is visited FIRST, so
 //     the running minimum is tight at once and `lb_s > best` (one compare) rejects most other links for most lanes;
@@ -1392,12 +1391,12 @@ robot_query_kernel(const __grid_constant__ RobotPack<MAXS> pk, int n_sdf, const 
 //     values + 96 B of gradients per configuration row), one 16-byte store per lane and destination -- local
 //     buffer, peer buffers or multicast -- with __syncwarp only: no block barrier anywhere in the loop.
 // Pruning stays exact (bounds are conservative), arithmetic of a visit is unchanged: bit-identical to the other kernels.
-// Instruction diet (profiles/r02/c4_serial_diet_lines.txt, tune_c4_diet.jsonl): the nearest sphere from a 5-instruction
+// Instruction diet: the nearest sphere from a 5-instruction
 // min over keys that carry the link index in their low mantissa bits (was compare + select per link), no per-link tests
 // of `point exists` / `si < n_sdf` (slots beyond n_sdf carry a +inf bound), a division-free flush index and per-lane
-// staging pointers: 640 -> 557 warp instructions per (point, 32 configurations), 0.508 -> 0.474 ms on C4.  What bounds
-// it now: L1 data-pipe wavefronts at 78 % (~166 per point: 32 sphere reads, ~54 transform rows, ~66 table gathers of 32
-// distinct sectors, 12 staging) with the issue slots at 70 %.
+// staging pointers: 640 -> 557 warp instructions per (point, 32 configurations).  What is left is L1 data-pipe
+// wavefronts (~166 per point: 32 sphere reads, ~54 transform rows, ~66 table gathers of 32 distinct sectors, 12 staging)
+// and issue slots.
 constexpr int kRsWarps = 8;
 #ifndef PVB_RS_CHUNK
 #define PVB_RS_CHUNK 8
@@ -1408,12 +1407,10 @@ constexpr int kRsValStride = kRsChunk + 1;        // 9: conflict-free STS.32 acr
 constexpr int kRsGradStride = 3 * kRsChunk + 1;   // 25
 
 // (The lane's 8 bounding spheres kept in 32 registers instead of shared memory -- no LDS in the bound pass, but 80
-// registers / 3 CTAs per SM -- measured 0.70 ms against 0.56 ms for the shared-memory form on C4; 48 registers / 5 CTAs
-// with spills 0.70 ms; 80 registers without spills 0.60 ms: profiles/r02/tune_c4_serial_variants.jsonl.)
+// registers / 3 CTAs per SM -- is the slower form; so are 48 registers / 5 CTAs with spills and 80 registers without.)
 // (More than 4 blocks per SM needs <= 48 registers AND <= 45 KB of shared memory per block, i.e. 4-point staging tiles
-// (PVB_RS_CHUNK=4: 35.8 KB).  Measured on C4, kernel only: 4 blocks 0.472 ms (8-point tiles 0.455), 5 blocks / 48
-// registers 0.533, 6 blocks / 40 registers 0.600 -- the spills go through the L1 data pipe that already bounds the
-// kernel.  profiles/r02/tune_c4_occupancy.jsonl)
+// (PVB_RS_CHUNK=4: 35.8 KB); the spills then go through the L1 data pipe that already bounds the kernel.
+// PVB_RS_MINB / PVB_RS_CHUNK are build macros so that the choice can be re-measured.)
 #ifndef PVB_RS_MINB
 #define PVB_RS_MINB 4
 #endif
@@ -1458,9 +1455,9 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
     const int pts_per_step = npt * SUB;                     // points a warp finishes between two flushes
     const int n_chunks = (n_pts + pts_per_step - 1) / pts_per_step;
     // Blocks stride over the tile's steps; small tiles need fewer blocks than the grid is wide (uniform per block).
-    // (A balanced persistent schedule -- every warp exactly ceil(total steps / resident warp slots) steps -- measured
-    // 0.66 ms against 0.50 ms for this oversubscribed grid on C4: the cost of a point varies, and many short-lived
-    // blocks let the hardware scheduler even it out; profiles/r02/tune_c4_serial_balanced_schedule_rejected.jsonl.)
+    // (Not a balanced persistent schedule -- every warp exactly ceil(total steps / resident warp slots) steps: the
+    // cost of a point varies, and many short-lived blocks of an oversubscribed grid let the hardware scheduler even it
+    // out.)
     const int gx_tile = min((int)gridDim.x, (n_chunks + kRsWarps - 1) / kRsWarps);
     if ((int)blockIdx.x >= gx_tile) return;
     // ---- stage the transforms of this configuration tile ----
@@ -1503,9 +1500,9 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
     // Staging tile.  One destination in local memory (kDest 0): every warp owns a tile of LC rows x its own
     // pts_per_step points and flushes it alone (__syncwarp only).  Remote destinations (peer buffers, multicast): the 8
     // warps of the block share ONE tile of LC rows x 8 pts_per_step points and flush it together, so that a row leaves
-    // as 256 contiguous bytes of values + 768 of gradients -- stores into peer memory run at 431 GB/s in 32-byte
-    // segments, 569 in 64-byte ones and 696 GB/s from 128 bytes up (scripts/ubench_peer_store.cu,
-    // profiles/r02/ubench_peer_store.jsonl); the two block barriers per step are the price.
+    // as 256 contiguous bytes of values + 768 of gradients -- stores into peer memory are faster in segments of 128
+    // bytes and up than in 32- or 64-byte ones (scripts/ubench_peer_store.cu); the two block barriers per step are the
+    // price.
     constexpr bool kCoop = kDest != 0;
     constexpr int w_log2 = kCoop ? 3 : 0;                                   // log2(warps sharing a tile)
     float *sv = kCoop ? &sm.sv[0][0][0] : &sm.sv[warp][0][0];
@@ -1570,8 +1567,7 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
                 if (si != pred && !(lb[si] > best)) visit(pk.d[si], si);
             }
             // (Rotating the gradient inside the visit, while the rows are in registers, saves these 3 LDS.128 -- 12 of the
-            // ~166 L1 wavefronts a point costs -- but runs the 9 multiply-adds once per visit instead of once per point:
-            // 0.485 ms against 0.474 ms on C4; with 80 registers / 3 blocks per SM 0.519 ms.  profiles/r02/tune_c4_rot.jsonl)
+            // ~166 L1 wavefronts a point costs -- but runs the 9 multiply-adds once per visit instead of once per point.)
             const int sb = max(bs, 0);
             const f3 go = composed_rotate_back(sm.xf[cl][3 * sb], sm.xf[cl][3 * sb + 1], sm.xf[cl][3 * sb + 2], bg);
             sv_lane[k] = best;
@@ -1792,7 +1788,7 @@ compact_write_kernel(const T *__restrict__ data, long long n, T empty, const uns
 // (row s * A + a) as the 4x4 row-major matrices the composed kernels read.  One thread per configuration walks the
 // serial chain in registers: T <- T @ joint_origin @ motion(q_j) (revolute: Rodrigues rotation about the axis,
 // prismatic: translation along it, fixed: identity), the same fp32 products the eager path took as dozens of small
-// launches (2.4 ms for 200 configurations of a 7-joint arm; this kernel: microseconds).
+// launches (this kernel: one launch for every configuration).
 struct FkPlan {
     pvb_fk_frame frame[PVB_FK_MAX_FRAMES];
     pvb_fk_link link[PVB_FK_MAX_LINKS];
@@ -2004,9 +2000,8 @@ constexpr int kStageNodesMax = 1536;   // 192 KB
 static int stage_nodes_for(int n_nodes) {
     static int max_nodes = -1;
     if (max_nodes < 0) {
-        // Measured (profiles/README.md, 1e7 queries on the 10k-triangle mesh / C5 chamfer): 0 -> 9.1 / 10.2 ms,
-        // 128 -> 9.4 ms, 448 -> 10.0 / 14.6 ms, 1024 -> 16.7 ms, 1536 -> 18.1 / 19.3 ms.  Shared memory taken from
-        // the unified 228 KB array is L1 taken away from the triangles, the deeper nodes and the traversal stacks,
+        // Shared memory taken from the SM's unified 256 KB L1 / shared array (up to 228 KB of it shared on H100) is L1
+        // taken away from the triangles, the deeper nodes and the traversal stacks,
         // and the top of the tree is an L1 hit anyway; the bulk-copy staging path is kept (PVB_STAGE_NODES) but off.
         max_nodes = 0;
         if (const char *e = getenv("PVB_STAGE_NODES")) {
@@ -2133,8 +2128,8 @@ extern "C" int pvb_mesh_query(const pvb_sdf_desc *mesh, const float *pts, int64_
     const SortedQueries sq = sort_queries(mesh, pts, n, nullptr, workspace,
                                           (size_t)(workspace_bytes < 0 ? 0 : workspace_bytes), (cudaStream_t)stream, &rc);
     if (rc != PVB_OK) return rc;
-    // run length (PVB_MESH_RUN).  Measured on the 10k-triangle mesh, 1e7 binned queries: run 1 / 4 / 8 / 16 ->
-    // 10.0 / 11.4 / 12.9 / 15.9 ms: the tighter start radius does not pay for lanes being `run` queries apart.
+    // run length (PVB_MESH_RUN, default 1): the tighter start radius of a run does not pay for lanes being `run`
+    // queries apart.
     static const int run_max = [] { const char *e = getenv("PVB_MESH_RUN"); return e ? atoi(e) : 1; }();
     long long run = n / ((long long)sm_count() * 2048);
     run = run < 1 ? 1 : (run > run_max ? run_max : run);
@@ -2348,8 +2343,7 @@ static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float
     auto steps_of = [&](int lc_log2) { const long long per = (long long)kRsChunk << (5 - lc_log2); return (n_pts + per - 1) / per; };
     long long total_steps = (long long)n_full * steps_of(5);
     for (int b = 4; b >= 0; --b) if (rem & (1 << b)) total_steps += steps_of(b);
-    // (C4 slabs, ms at 8 / 4 points per step: 25 configurations 0.133 / 0.116, 50: 0.177 / 0.162, 100: 0.280 / 0.273, 200:
-    // 0.497 / 0.517 -- profiles/r02/tune_c4_fine_steps.jsonl)
+    // (small configuration slabs favour 4 points per step, the full C4 batch 8; PVB_ROBOT_FINE_STEPS moves the switch)
     static const int fine_below = [] { const char *e = getenv("PVB_ROBOT_FINE_STEPS"); return e ? atoi(e) : 12; }();
     const long long slots = (long long)sm_count() * PVB_RS_MINB * kRsWarps;
     const int chunk_log2 = (kRsChunk == 4 || total_steps < (long long)fine_below * slots) ? 2 : 3;
@@ -2419,7 +2413,7 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
     int rc = PVB_OK;
     static const int cfg_major = [] { const char *e = getenv("PVB_COMP_CFGMAJOR"); return e ? atoi(e) : 1; }();
     // lanes = configurations: only worthwhile when the 32-wide configuration tiles are well filled (25 configurations
-    // per rank on 8 GPUs would idle 22 % of the lanes; measured 0.176 ms against 0.111 ms point-major)
+    // per rank on 8 GPUs would idle 22 % of the lanes, and point-major is faster there)
     const int cm_tiles = (cfg_count + kCmCfg - 1) / kCmCfg;
     // ... except with several destinations: the configuration-major epilogue owns whole rows and stores them as full
     // sectors, which is what the NVLink-bound re-assembly needs; idle lanes cost less than partial-sector packets

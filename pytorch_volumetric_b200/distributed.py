@@ -62,7 +62,7 @@ def bind_to_gpu_numa_node(device_index):
     """Restrict this process to the CPUs of its GPU's NUMA node, so that the pinned host buffers it allocates from
     now on (first touch) and the threads that fill them sit next to the PCIe root of that GPU.  With eight ranks
     streaming results to host memory on a two-socket box, unbound ranks cross the socket interconnect and the
-    end-to-end time per step doubles (SCALE_r01: 3.7 ms at 1 GPU, 8.1 ms at 8).  Returns (node, n_cpus, previous
+    end-to-end time per step suffers.  Returns (node, n_cpus, previous
     affinity) or None when nothing was changed; pass the previous affinity to os.sched_setaffinity to undo."""
     import os
     node = gpu_numa_node(device_index)

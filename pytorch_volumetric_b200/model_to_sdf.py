@@ -1,6 +1,6 @@
 """RobotSDF: one SDF per link mesh, posed by batched forward kinematics, min over links in one fused kernel.
 
-API mirror of /root/reference/src/pytorch_volumetric/model_to_sdf.py (RobotSDF :12-125,
+API mirror of the reference's src/pytorch_volumetric/model_to_sdf.py (RobotSDF :12-125,
 cache_link_sdf_factory :128-133, aabb_to_ordered_end_points :136-171): same constructor arguments, attributes,
 output shapes and state semantics.  `chain` is duck-typed on the pytorch_kinematics Chain surface listed in
 kinematics.py; every query is a single pvb_composed_query launch.

@@ -1,6 +1,6 @@
-"""Signed-distance objects with the reference's Python API, computed by libpvb.so on B200.
+"""Signed-distance objects with the reference's Python API, computed by libpvb.so on H100.
 
-Mirrors /root/reference/src/pytorch_volumetric/sdf.py (same class names, constructor
+Mirrors the reference's src/pytorch_volumetric/sdf.py (same class names, constructor
 arguments, shapes, dtypes and exceptions) for the batched query path:
 
   ObjectFactory / MeshObjectFactory   sdf.py:30-214   mesh load, AABB, closest point + sign
@@ -11,7 +11,7 @@ arguments, shapes, dtypes and exceptions) for the batched query path:
   OutOfBoundsStrategy, CachedSDF      sdf.py:436-614
   sample_mesh_points                  sdf.py:617-670
 
-All arithmetic on the query path runs in hand-written sm_100a kernels behind the
+All arithmetic on the query path runs in hand-written sm_90a kernels behind the
 C ABI of include/pvb.h; there is no CPU fallback.  Host tensors are accepted
 (copied to the GPU, results copied back to the input's device) so that the
 classes drop in for CPU callers of the reference.
@@ -142,8 +142,7 @@ class _HostChunkStream:
     ((), (3,)) for value + gradient; `launch(d_in, m, d_outs)` enqueues the computation of one chunk of m points on
     the current stream.
 
-    (Measured on the pool, CachedSDF, 1e7 points: one copy-in / launch / copy-out 5.1 ms, 2M-point chunks 3.7 ms, 4M
-    4.1 ms, 1M 11 ms -- small chunks are dominated by per-chunk stream/event bookkeeping on this host.)"""
+    (Chunks of a few million points: much smaller ones are dominated by per-chunk stream/event bookkeeping.)"""
 
     def __init__(self, device, chunk, tails):
         self.device, self.chunk, self.tails = device, chunk, tuple(tails)
@@ -788,7 +787,7 @@ class ComposedSDF(ObjectFrameSDF):
 
     def _host_result_pipeline(self, points_in_object_frame):
         """Host points in, pinned host results out, for results so large that the device-to-host copy IS the call
-        (C4: 0.45 ms of lookups, 5.8 ms of PCIe): the configurations are queried in slabs (a first small one, then 64 at
+        (C4: the PCIe copy takes many times the lookups): the configurations are queried in slabs (a first small one, then 64 at
         a time -- whole 32-configuration tiles) into one device buffer, and each slab starts its copy on a side stream
         as soon as its kernel has finished, so only the first slab's lookups are not hidden behind the copy.
         Returns None when the call does not qualify (then __call__ takes the plain path)."""

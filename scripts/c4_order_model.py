@@ -20,7 +20,7 @@ from pytorch_volumetric_b200.sdf import grid_prune_margin  # noqa: E402
 
 def main(n_cfg=24, n_pts=4000):
     tp_open3d.QUERY_METHOD = "bvh"
-    d = os.path.join(tempfile.gettempdir(), "pvb_bench_arm_cpu")
+    d = tempfile.mkdtemp(prefix="pvb_arm_cpu_")
     urdf, end = workloads.write_arm(d)
     chain = opk.build_serial_chain_from_urdf(open(urdf).read(), end)
     robot = port.RobotSDFPort(chain, path_prefix=d, link_sdf_factory=port.cache_link_sdf_factory_port(0.02, 1.0))

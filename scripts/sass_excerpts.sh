@@ -1,14 +1,14 @@
 #!/bin/bash
-# SASS evidence per hot kernel (run in the build container; cuobjdump needs no GPU):
-#   profiles/<round>/sass_<kernel>.txt = resource usage + the instructions that carry the design
+# SASS evidence per hot kernel (cuobjdump needs no GPU), written under the git-ignored tune/ directory:
+#   tune/sass_<round>/<kernel>.txt = resource usage + the instructions that carry the design
 #   (UBLKCP / SYNCS = bulk-copy engine + mbarrier, LDG.E.128 = 16-byte table records, multimem / STG.E.128 row stores).
 set -e
 R=${1:-r02}
 SO=pytorch_volumetric_b200/csrc/libpvb.so
-OUT=profiles/$R
+OUT=tune/sass_$R
 mkdir -p "$OUT"
 dump() {   # name, mangled-name regex, grep pattern
-  local f="$OUT/sass_$1.txt"
+  local f="$OUT/$1.txt"
   { echo "# $1 -- cuobjdump -sass / -res-usage of $SO ($(date -u +%F))"
     cuobjdump -res-usage "$SO" 2>/dev/null | grep -A1 -E "$2" | grep -E "Function|REG" | head -4
     echo "# instruction count: $(cuobjdump -sass "$SO" 2>/dev/null | awk -v pat="$2" '$0 ~ "Function : " {f = ($0 ~ pat)} f' | grep -cE '^\s+/\*[0-9a-f]{4,}\*/')"

@@ -100,7 +100,7 @@ int main(int argc, char** argv) {
     rd.res.linear.desc = cudaCreateChannelDesc<float4>(); rd.res.linear.sizeInBytes = sizeof(float4) * (size_t)nvox;
     cudaTextureDesc td = {}; td.readMode = cudaReadModeElementType;
     cudaTextureObject_t tex; CK(cudaCreateTextureObject(&tex, &rd, &td, nullptr));
-    const int blocks = 148 * 8, thr = 256;
+    const int blocks = 132 * 8, thr = 256;   // 8 blocks per SM of an H100 SXM
     printf("table %d voxels (%.1f MB), %lld gathers, out 160 MB\n", nvox, nvox * 16 / 1e6, n);
     printf("write-only 160MB        : %.1f us\n", 1e3 * timeit([&] { k_write<<<blocks, thr>>>(n, out); }));
     printf("LDG.128 1/thread        : %.1f us\n", 1e3 * timeit([&] { k_ldg<<<blocks, thr>>>(tab, idx, n, out); }));

@@ -1,7 +1,7 @@
 // Peer-store micro-benchmark: how NVLink write throughput depends on the size of the contiguous segment a warp
 // instruction writes.  One process, two GPUs (device 0 stores into device 1's memory through peer access), the access
 // pattern of the RobotSDF row flush: 32 result rows far apart, each written front to back in segments of S bytes, 16 B
-// per lane.   nvcc -O3 -gencode arch=compute_100a,code=sm_100a scripts/ubench_peer_store.cu -o /tmp/ubench_peer_store
+// per lane.   nvcc -O3 -gencode arch=compute_90a,code=sm_90a scripts/ubench_peer_store.cu -o /tmp/ubench_peer_store
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>
@@ -55,7 +55,7 @@ int main() {
             float best = 1e9f;
             for (int it = 0; it < 5; ++it) {
                 cudaEventRecord(a);
-                store_kernel<<<148 * 8, 256>>>(dst, row_f4, rows, seg_f4, segs_per_row, 0);
+                store_kernel<<<132 * 8, 256>>>(dst, row_f4, rows, seg_f4, segs_per_row, 0);
                 cudaEventRecord(b);
                 cudaEventSynchronize(b);
                 float ms; cudaEventElapsedTime(&ms, a, b);

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
     # The libraries normally arrive prebuilt (__graft_entry__.build()); compile them here if a checkout has none.
     # This is test scaffolding: the product itself never builds implicitly and raises when libpvb.so is missing.
     try:
@@ -34,7 +34,7 @@ def pytest_collection_modifyitems(config, items):
 
 @pytest.fixture(scope="session")
 def built_lib():
-    """libpvb.so, compiled if missing (nvcc cross-compiles for sm_100a without a GPU)."""
+    """libpvb.so, compiled if missing (nvcc cross-compiles for sm_90a without a GPU)."""
     from pytorch_volumetric_b200 import _native
     if _native.needs_build():
         _native.build()

@@ -48,18 +48,32 @@ def test_reference_arm_other_ranks_exit_quietly():
     assert out.returncode == 0 and out.stdout.strip() == ""
 
 
-def test_committed_ncu_side_files_cover_every_workload():
-    """roofline.traffic / roofline.ncu are read from committed ncu extracts: every bench workload has an entry, the
-    summaries they cite exist, and the numbers are sane (bytes > 0, percentages in (0, 100])."""
+def test_dump_outputs_full_and_sampled(tmp_path):
+    """--dump-outputs: small results are written whole in their own shape; large ones as the same seeded rows of value
+    and gradient, float32 / float64 only, under 64 MB, identical from run to run."""
+    import numpy as np
+    import torch
     sys.path.insert(0, ROOT)
     import bench
-    names = {bench.HEADLINE, *bench.OTHER_WORKLOADS}
-    traffic = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-    limits = json.load(open(os.path.join(ROOT, "profiles", "ncu_limits.json")))
-    assert names <= set(traffic) and names <= set(limits)
-    for n in names:
-        assert traffic[n] > 0 and bench.ncu_traffic(n) == traffic[n]
-        lim = bench.ncu_limits(n)
-        assert os.path.exists(os.path.join(ROOT, lim["source"])), lim["source"]
-        for k in ("issue_slots_pct", "l1_data_pipe_pct", "dram_pct", "warps_active_pct"):
-            assert 0.0 < lim[k] <= 100.0, (n, k, lim[k])
+    val = torch.arange(6, dtype=torch.float32).reshape(2, 3)
+    bench.dump_outputs((val, torch.stack([val, -val, 2 * val], -1)), str(tmp_path / "small"))
+    assert np.array_equal(np.load(tmp_path / "small" / "value.npy"), val.numpy())
+    assert np.load(tmp_path / "small" / "grad.npy").shape == (2, 3, 3)
+    assert not (tmp_path / "small" / "sample_index.npy").exists()
+
+    rows = bench.DUMP_MAX_ROWS + 12345
+    big_v = torch.randn(rows, generator=torch.Generator().manual_seed(0))
+    big_g = torch.randn(rows, 3, generator=torch.Generator().manual_seed(1)).double()
+    for d in ("a", "b"):
+        bench.dump_outputs((big_v, big_g), str(tmp_path / d))
+    files = {p.name for p in (tmp_path / "a").iterdir()}
+    assert files == {"value.npy", "grad.npy", "sample_index.npy"}
+    assert sum((tmp_path / "a" / f).stat().st_size for f in files) <= bench.DUMP_MAX_BYTES
+    idx = np.load(tmp_path / "a" / "sample_index.npy")
+    v, g = np.load(tmp_path / "a" / "value.npy"), np.load(tmp_path / "a" / "grad.npy")
+    assert idx.dtype == np.float64 and v.dtype == np.float32 and g.dtype == np.float64
+    assert len(np.unique(idx)) == len(idx) == len(v) == len(g) <= bench.DUMP_MAX_ROWS
+    assert np.array_equal(v, big_v.numpy()[idx.astype(np.int64)])
+    assert np.array_equal(g, big_g.numpy()[idx.astype(np.int64)])
+    for f in files:
+        assert np.array_equal(np.load(tmp_path / "a" / f), np.load(tmp_path / "b" / f))

@@ -1,6 +1,6 @@
 """Synthetic workloads shared by bench.py and tests/ (BASELINE.json configs made concrete, SURVEY.md section 8d).
 
-Nothing here reads /root/reference: the reference's test meshes come from tests/golden/meshes.npz (written by
+Nothing here reads the reference project: the reference's test meshes come from tests/golden/meshes.npz (written by
 oracle/make_golden.py in the build container), everything else is procedural and seeded.
 """
 import math
