@@ -50,7 +50,11 @@ enum {
                                       composed kernels may skip lookups that provably cannot win the min */
     PVB_GRID_TRILINEAR  = 1u << 4, /* EXTENSION (not reference behaviour): value = trilinear interpolation of the
                                       8 surrounding voxel values, gradient = analytic gradient of that interpolant
-                                      (cell-wise finite differences).  pvb_grid_lookup only. */
+                                      (cell-wise finite differences).  Honoured by pvb_grid_lookup,
+                                      pvb_composed_query, pvb_composed_query_multi and (where the point-serial
+                                      robot kernel runs: <= 8 GRID sub-SDFs, >= PVB_ROBOT_MIN_CFG configurations)
+                                      pvb_composed_query_multicast; needs the bounding-box rule (not
+                                      PVB_GRID_OOB_GT).  pvb_chamfer rejects it (PVB_ERR_INVALID). */
     PVB_MESH_CLOSED     = 1u << 3  /* every directed edge is matched by its reverse (closed, consistently oriented
                                       surface): crossing parity is direction independent, so the sign test may use
                                       the exact axis-aligned walk instead of the reference's diagonal ray */

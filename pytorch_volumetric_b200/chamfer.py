@@ -43,8 +43,9 @@ def batch_chamfer_dist(world_to_object: torch.tensor, model_points_world_frame_e
     if obj_sdf is not None:
         dev = nat.compute_device(world_to_object.device)
         desc = obj_sdf.native_desc(dev)
-        if desc is None:
-            # arbitrary ObjectFrameSDF: evaluate through its __call__ (chamfer.py:84-85)
+        if desc is None or (desc.kind == nat.PVB_KIND_GRID and desc.flags & nat.PVB_GRID_TRILINEAR):
+            # arbitrary ObjectFrameSDF, or a trilinear CachedSDF (the chamfer kernel has the nearest-voxel rule
+            # only): evaluate through its __call__ (chamfer.py:84-85)
             m = world_to_object
             pts = model_points_world_frame_eval
             pts_obj = pts @ m[:, :3, :3].transpose(-1, -2) + m[:, :3, 3].unsqueeze(1)

@@ -536,6 +536,67 @@ __device__ __forceinline__ SdfOut grid_eval(const pvb_sdf_desc &g, const NodeSta
     return o;
 }
 
+// ----------------------------------------------------------------------------
+// EXTENSION, opt-in (CachedSDF(interpolation="trilinear"), PVB_GRID_TRILINEAR): the reference looks up the NEAREST
+// voxel and a stored gradient table (sdf.py:537-550).  This interpolates the value table trilinearly and returns the
+// analytic gradient of the interpolant (per-cell finite differences of the corner values) -- smoother for
+// optimisation, not comparable to the reference within 1e-5 (the difference is O(resolution)); it is validated
+// against its own CPU restatement (oracle/port.py).  One arithmetic for every kernel that honours the flag
+// (grid_trilinear_kernel, the composed kernels, robot_serial_kernel), so their results agree bit for bit.
+__device__ __forceinline__ bool grid_in_range(const pvb_sdf_desc &g, f3 p) {
+    return (p.x >= g.valid_lo[0]) & (p.x <= g.valid_hi[0]) & (p.y >= g.valid_lo[1]) & (p.y <= g.valid_hi[1]) &
+           (p.z >= g.valid_lo[2]) & (p.z <= g.valid_hi[2]);
+}
+
+// In range only (grid_in_range(g, p)): the interpolant and its gradient.
+__device__ __forceinline__ SdfOut grid_trilinear_interp(const pvb_sdf_desc &g, f3 p) {
+    const float4 *tab = reinterpret_cast<const float4 *>(g.table);
+    const int n0 = g.dims[0], n1 = g.dims[1], n2 = g.dims[2];
+    const float u[3] = {(p.x - g.min32[0]) * g.inv_res32[0], (p.y - g.min32[1]) * g.inv_res32[1],
+                        (p.z - g.min32[2]) * g.inv_res32[2]};
+    const int nn[3] = {n0, n1, n2};
+    int c0[3];
+    float f[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        c0[a] = min(max((int)floorf(u[a]), 0), max(nn[a] - 2, 0));
+        f[a] = nn[a] > 1 ? fminf(fmaxf(u[a] - (float)c0[a], 0.f), 1.f) : 0.f;
+    }
+    const int s0 = n1 * n2, s1 = n2;
+    const int base = c0[0] * s0 + c0[1] * s1 + c0[2];
+    const int dx = n0 > 1 ? s0 : 0, dy = n1 > 1 ? s1 : 0, dz = n2 > 1 ? 1 : 0;
+    const float v000 = __ldg(tab + base).x, v001 = __ldg(tab + base + dz).x;
+    const float v010 = __ldg(tab + base + dy).x, v011 = __ldg(tab + base + dy + dz).x;
+    const float v100 = __ldg(tab + base + dx).x, v101 = __ldg(tab + base + dx + dz).x;
+    const float v110 = __ldg(tab + base + dx + dy).x, v111 = __ldg(tab + base + dx + dy + dz).x;
+    const float fx = f[0], fy = f[1], fz = f[2];
+    const float c00 = v000 + fz * (v001 - v000), c01 = v010 + fz * (v011 - v010);
+    const float c10 = v100 + fz * (v101 - v100), c11 = v110 + fz * (v111 - v110);
+    const float c0_ = c00 + fy * (c01 - c00), c1_ = c10 + fy * (c11 - c10);
+    SdfOut o;
+    o.val = c0_ + fx * (c1_ - c0_);
+    // d/dx: difference of the two y-z interpolated faces over the cell size, and likewise for y, z
+    const float gx = (c1_ - c0_) * g.inv_res32[0];
+    const float e0 = c01 - c00, e1 = c11 - c10;
+    const float gy = (e0 + fx * (e1 - e0)) * g.inv_res32[1];
+    const float z00 = v001 - v000, z01 = v011 - v010, z10 = v101 - v100, z11 = v111 - v110;
+    const float z0 = z00 + fy * (z01 - z00), z1 = z10 + fy * (z11 - z10);
+    const float gz = (z0 + fx * (z1 - z0)) * g.inv_res32[2];
+    o.grad = mk3(n0 > 1 ? gx : 0.f, n1 > 1 ? gy : 0.f, n2 > 1 ? gz : 0.f);
+    return o;
+}
+
+// Any point: the interpolant in range, the reference's point-to-AABB rule (sdf.py:555-571) out of range.
+__device__ __forceinline__ SdfOut grid_trilinear_eval(const pvb_sdf_desc &g, f3 p) {
+    if (grid_in_range(g, p)) return grid_trilinear_interp(g, p);
+    float dist, ex, ey, ez, r;
+    aabb_rule(g, p, dist, ex, ey, ez, r);
+    SdfOut o;
+    o.val = dist;
+    o.grad = mk3(ex * r, ey * r, ez * r);
+    return o;
+}
+
 __device__ __forceinline__ SdfOut sphere_eval(float radius, f3 p) {   // sdf.py:291-295
     const float r = sqrtf(p.x * p.x + p.y * p.y + p.z * p.z);
     const float den = r + 1e-12f;
@@ -577,8 +638,9 @@ __device__ __forceinline__ f3 composed_rotate_back(const float4 &r0, const float
 // (best, bg, bs) of one point; bs < 0 = nothing evaluated yet.  Skipped without touching its table / tree when
 // provably not the argmin: value >= dist(q, box) - prune_margin (measured on the table for grids, fp32 slack for
 // closed meshes).  torch.argmin semantics (sdf.py:421): smallest value, first index on ties -- whatever the
-// visiting order.
-template <bool kMesh>
+// visiting order.  kTri: GRID descriptors with PVB_GRID_TRILINEAR are evaluated through grid_trilinear_eval (a
+// template flag, so that the nearest-voxel instantiations carry no code for the opt-in mode).
+template <bool kMesh, bool kTri = false>
 __device__ __forceinline__ void composed_consider(const pvb_sdf_desc &d, const NodeStage &st, int s, f3 q,
                                                   uint32_t mesh_mode, uint64_t idx, float &best, f3 &bg, int &bs) {
     SdfOut o;
@@ -587,7 +649,10 @@ __device__ __forceinline__ void composed_consider(const pvb_sdf_desc &d, const N
             const float thr = best + d.prune_margin;
             if (thr < 0.f || composed_aabb_lb2(d, q) > thr * thr) return;
         }
-        o = grid_eval<kMesh, true>(d, st, q, mesh_mode, idx, nullptr);
+        // (the bound holds for the interpolant too: it is a convex combination of 8 corner values, and the weighted
+        // mean distance of q to those corners is at most half a cell diagonal -- tests/test_trilinear_composed_cpu.py)
+        if (kTri && (d.flags & PVB_GRID_TRILINEAR)) o = grid_trilinear_eval(d, q);
+        else o = grid_eval<kMesh, true>(d, st, q, mesh_mode, idx, nullptr);
     } else if (kMesh && d.kind == PVB_KIND_MESH) {
         // closed mesh, query outside its AABB: the value is +distance >= dist(q, AABB), so (a) skip it when that
         // bound already exceeds the running min, (b) otherwise search only within the running min and (c) skip

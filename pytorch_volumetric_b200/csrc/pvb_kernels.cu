@@ -68,7 +68,7 @@ static int sm_count() {
 // id; returns false when the runtime refuses.
 enum { kSlotMesh = 0, kSlotGridTma, kSlotCfgMajor, kSlotCfgMajorMulti, kSlotChamfer, kSlotRobot, kSlotRobotMulti,
        kSlotRobotMc, kSlotRobotWide, kSlotRobotWideMulti, kSlotRobotWideMc, kSlotSerial, kSlotSerialMulti, kSlotSerialMc,
-       kSlotCount };
+       kSlotSerialTri, kSlotSerialTriMulti, kSlotSerialTriMc, kSlotCfgMajorTri, kSlotCfgMajorTriMulti, kSlotCount };
 template <typename K>
 static bool ensure_smem(K kernel, int slot, int bytes) {
     static unsigned char done[kSlotCount][kMaxDevices] = {{0}};
@@ -573,59 +573,15 @@ grid_lookup_tma_kernel(const pvb_sdf_desc g, const float *__restrict__ pts, long
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// EXTENSION, opt-in (CachedSDF(interpolation="trilinear")): the reference looks up the NEAREST voxel and a stored
-// gradient table (sdf.py:537-550), which is what every other kernel in this file reproduces.  This one
-// interpolates the value table trilinearly and returns the analytic gradient of the interpolant (per-cell finite
-// differences of the corner values) -- smoother for optimisation, not comparable to the reference within 1e-5
-// (the difference is O(resolution)); it is validated against its own CPU restatement (oracle/port.py).
+// EXTENSION, opt-in (CachedSDF(interpolation="trilinear")): the trilinear interpolant of the value table and its
+// analytic gradient, grid_trilinear_eval (pvb_device.cuh) per point.  Every other kernel in this section reproduces
+// the reference's nearest-voxel rule.
 __global__ void __launch_bounds__(256)
 grid_trilinear_kernel(const pvb_sdf_desc g, const float *__restrict__ pts, long long n, float *__restrict__ out_val,
                       float *__restrict__ out_grad) {
-    const float4 *tab = reinterpret_cast<const float4 *>(g.table);
     const long long stride = (long long)gridDim.x * blockDim.x;
-    const int n0 = g.dims[0], n1 = g.dims[1], n2 = g.dims[2];
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        const f3 p = load_point(pts, i);
-        const bool inb = (p.x >= g.valid_lo[0]) & (p.x <= g.valid_hi[0]) & (p.y >= g.valid_lo[1]) &
-                         (p.y <= g.valid_hi[1]) & (p.z >= g.valid_lo[2]) & (p.z <= g.valid_hi[2]);
-        SdfOut o;
-        if (inb) {
-            const float u[3] = {(p.x - g.min32[0]) * g.inv_res32[0], (p.y - g.min32[1]) * g.inv_res32[1],
-                                (p.z - g.min32[2]) * g.inv_res32[2]};
-            const int nn[3] = {n0, n1, n2};
-            int c0[3];
-            float f[3];
-#pragma unroll
-            for (int a = 0; a < 3; ++a) {
-                c0[a] = min(max((int)floorf(u[a]), 0), max(nn[a] - 2, 0));
-                f[a] = nn[a] > 1 ? fminf(fmaxf(u[a] - (float)c0[a], 0.f), 1.f) : 0.f;
-            }
-            const int s0 = n1 * n2, s1 = n2;
-            const int base = c0[0] * s0 + c0[1] * s1 + c0[2];
-            const int dx = n0 > 1 ? s0 : 0, dy = n1 > 1 ? s1 : 0, dz = n2 > 1 ? 1 : 0;
-            const float v000 = __ldg(tab + base).x, v001 = __ldg(tab + base + dz).x;
-            const float v010 = __ldg(tab + base + dy).x, v011 = __ldg(tab + base + dy + dz).x;
-            const float v100 = __ldg(tab + base + dx).x, v101 = __ldg(tab + base + dx + dz).x;
-            const float v110 = __ldg(tab + base + dx + dy).x, v111 = __ldg(tab + base + dx + dy + dz).x;
-            const float fx = f[0], fy = f[1], fz = f[2];
-            const float c00 = v000 + fz * (v001 - v000), c01 = v010 + fz * (v011 - v010);
-            const float c10 = v100 + fz * (v101 - v100), c11 = v110 + fz * (v111 - v110);
-            const float c0_ = c00 + fy * (c01 - c00), c1_ = c10 + fy * (c11 - c10);
-            o.val = c0_ + fx * (c1_ - c0_);
-            // d/dx: difference of the two y-z interpolated faces over the cell size, and likewise for y, z
-            const float gx = (c1_ - c0_) * g.inv_res32[0];
-            const float e0 = c01 - c00, e1 = c11 - c10;
-            const float gy = (e0 + fx * (e1 - e0)) * g.inv_res32[1];
-            const float z00 = v001 - v000, z01 = v011 - v010, z10 = v101 - v100, z11 = v111 - v110;
-            const float z0 = z00 + fy * (z01 - z00), z1 = z10 + fy * (z11 - z10);
-            const float gz = (z0 + fx * (z1 - z0)) * g.inv_res32[2];
-            o.grad = mk3(n0 > 1 ? gx : 0.f, n1 > 1 ? gy : 0.f, n2 > 1 ? gz : 0.f);
-        } else {
-            float dist, ex, ey, ez, r;        // out of range: the reference's AABB rule, unchanged
-            aabb_rule(g, p, dist, ex, ey, ez, r);
-            o.val = dist;
-            o.grad = mk3(ex * r, ey * r, ez * r);
-        }
+        const SdfOut o = grid_trilinear_eval(g, load_point(pts, i));
         out_val[i] = o.val;
         out_grad[3 * i] = o.grad.x; out_grad[3 * i + 1] = o.grad.y; out_grad[3 * i + 2] = o.grad.z;
     }
@@ -723,7 +679,7 @@ struct OutTargets {
     int mc;         // val[0] / grad[0] are MULTICAST addresses (NVLS): one multimem.st reaches every bound GPU
 };
 
-template <bool kMesh, int PTS, int MAXS, bool kMulti>
+template <bool kMesh, int PTS, int MAXS, bool kMulti, bool kTri>
 __global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : (PTS > 1 ? PVB_COMP_MINB : 1)))
 composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
                       int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long first_pt,
@@ -821,7 +777,7 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
                         float4 r0, r1, r2;
                         load_xf(s, r0, r1, r2);
                         const uint64_t idx = ((uint64_t)cfg * (uint64_t)n_pts + (uint64_t)i0) * (uint64_t)n_sdf + (uint64_t)s;
-                        composed_consider<kMesh>(d, st, s, composed_xform(r0, r1, r2, p[0]), mesh_mode, idx, best[0], bg[0], bs[0]);
+                        composed_consider<kMesh, kTri>(d, st, s, composed_xform(r0, r1, r2, p[0]), mesh_mode, idx, best[0], bg[0], bs[0]);
                     }
                 }
             }
@@ -833,8 +789,8 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
 #pragma unroll
                 for (int k = 0; k < PTS; ++k) {
                     const uint64_t idx = ((uint64_t)cfg * (uint64_t)n_pts + (uint64_t)(i0 + k)) * (uint64_t)n_sdf + (uint64_t)s;   // absolute cfg: sharding-independent jitter
-                    composed_consider<kMesh>(d, st, s, composed_xform(r0, r1, r2, p[k]), mesh_mode, idx, best[k], bg[k],
-                                             bs[k]);
+                    composed_consider<kMesh, kTri>(d, st, s, composed_xform(r0, r1, r2, p[k]), mesh_mode, idx, best[k], bg[k],
+                                                   bs[k]);
                 }
             }
             f3 go[PTS];
@@ -903,7 +859,7 @@ struct __align__(16) CmSmem {
     int which[kCmCfg][kCmTilePts + 1];
 };
 
-template <bool kMulti>
+template <bool kMulti, bool kTri>
 __global__ void __launch_bounds__(kCmCfg * kCmWarps, 3)
 composed_cfgmajor_kernel(const __grid_constant__ DescPack<kCmMaxS> descs, int n_sdf, const float *__restrict__ xforms,
                          int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_pts,
@@ -972,7 +928,7 @@ composed_cfgmajor_kernel(const __grid_constant__ DescPack<kCmMaxS> descs, int n_
 #pragma unroll
             for (int k = 0; k < kCmPts; ++k) {
                 if (!need[k]) continue;
-                composed_consider<false>(d, st, s, composed_xform(r0, r1, r2, p[k]), 0u, 0ull, best[k], bg[k], bs[k]);
+                composed_consider<false, kTri>(d, st, s, composed_xform(r0, r1, r2, p[k]), 0u, 0ull, best[k], bg[k], bs[k]);
             }
         };
         for (int si = 0; si < n_sdf; ++si) {
@@ -1131,6 +1087,16 @@ __device__ __forceinline__ float4 robot_lookup(const pvb_sdf_desc &g, f3 p) {
                      (p.y <= g.valid_hi[1]) & (p.z >= g.valid_lo[2]) & (p.z <= g.valid_hi[2]);
     if (inb & certain)      // the index is exact and inside the table: no clamp needed
         return __ldg(reinterpret_cast<const float4 *>(g.table) + ((kx * g.dims[1] + ky) * g.dims[2] + kz));
+    return robot_lookup_slow(&g, p.x, p.y, p.z);
+}
+
+// PVB_GRID_TRILINEAR link: the interpolant of grid_trilinear_eval (pvb_device.cuh) in range; out of range the
+// point-to-AABB rule, which is the same for both modes, out of line as above.
+__device__ __forceinline__ float4 robot_lookup_trilinear(const pvb_sdf_desc &g, f3 p) {
+    if (grid_in_range(g, p)) {
+        const SdfOut o = grid_trilinear_interp(g, p);
+        return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
+    }
     return robot_lookup_slow(&g, p.x, p.y, p.z);
 }
 
@@ -1434,7 +1400,10 @@ __device__ __forceinline__ float rsqrt_approx(float x) {      // one MUFU.RSQ, n
 }
 
 // (configuration tiles and the flush index arithmetic: rs_tile / rs_flush_piece in pvb_device.cuh, checked on the CPU tier)
-template <int kDest>
+// kTri: some links carry PVB_GRID_TRILINEAR; each visit then picks its lookup by the link's flag (uniform across the
+// lanes of a point group), so nearest and trilinear links mix.  The bounds are unchanged: prune_margin holds for the
+// interpolant as well.  kTri = false is the nearest-voxel kernel as it always was.
+template <int kDest, bool kTri>
 __global__ void __launch_bounds__(kRbCfg * kRsWarps, PVB_RS_MINB)
 robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, const float *__restrict__ xforms,
                     int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, int n_pts, int vec,
@@ -1553,7 +1522,8 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
                     const float thr = best + d.prune_margin;
                     if (thr < 0.f || composed_aabb_lb2(d, q) > thr * thr) return;
                 }
-                const float4 o = robot_lookup(d, q);
+                const float4 o = (kTri && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
+                                                                           : robot_lookup(d, q);
                 if (bs < 0 || o.x < best || (o.x == best && si < bs)) {
                     best = o.x; bg = mk3(o.y, o.z, o.w); bs = si;
                 }
@@ -2240,7 +2210,7 @@ extern "C" int pvb_sphere_query(float radius, const float *pts, int64_t n, float
     return PVB_OK;
 }
 
-template <bool kMesh, int PTS, int MAXS>
+template <bool kMesh, int PTS, int MAXS, bool kTri>
 static int launch_composed(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                            int cfg_count, const float *pts, long long first_pt, long long n_pts, uint32_t mesh_mode,
                            float *out_val, float *out_grad, int *out_which, const OutTargets *tg, cudaStream_t stream) {
@@ -2260,11 +2230,11 @@ static int launch_composed(const pvb_sdf_desc *descs, int n_sdf, const float *xf
     for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
     timing_mark(0, stream);
     if (tg)
-        composed_query_kernel<kMesh, PTS, MAXS, true><<<grid, kCompThreads, 0, stream>>>(
+        composed_query_kernel<kMesh, PTS, MAXS, true, kTri><<<grid, kCompThreads, 0, stream>>>(
             pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, first_pt, n_pts, mesh_mode, nullptr, nullptr,
             out_which, *tg, nearest_first, margin_max);
     else
-        composed_query_kernel<kMesh, PTS, MAXS, false><<<grid, kCompThreads, 0, stream>>>(
+        composed_query_kernel<kMesh, PTS, MAXS, false, kTri><<<grid, kCompThreads, 0, stream>>>(
             pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, first_pt, n_pts, mesh_mode, out_val, out_grad,
             out_which, OutTargets{}, nearest_first, margin_max);
     timing_mark(1, stream);
@@ -2319,20 +2289,20 @@ static int launch_robot(const pvb_sdf_desc *descs, int n_sdf, const float *xform
     return PVB_OK;
 }
 
-// Launch robot_serial_kernel (<= 8 GRID sub-SDFs with the bounding-box rule).
+// Launch robot_serial_kernel (<= 8 GRID sub-SDFs with the bounding-box rule; `tri`: some of them PVB_GRID_TRILINEAR).
 static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                                int cfg_count, const float *pts, long long n_pts, int vec, float *out_val,
-                               float *out_grad, int *out_which, const OutTargets *tg, cudaStream_t stream) {
+                               float *out_grad, int *out_which, const OutTargets *tg, bool tri, cudaStream_t stream) {
     RobotPack<kRsMaxS> pack;
     memset(&pack, 0, sizeof(pack));
     for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
     const int kind = !tg ? 0 : (tg->mc ? 2 : 1);
-    auto k0 = robot_serial_kernel<0>;
-    auto k1 = robot_serial_kernel<1>;
-    auto k2 = robot_serial_kernel<2>;
+    auto k0 = tri ? robot_serial_kernel<0, true> : robot_serial_kernel<0, false>;
+    auto k1 = tri ? robot_serial_kernel<1, true> : robot_serial_kernel<1, false>;
+    auto k2 = tri ? robot_serial_kernel<2, true> : robot_serial_kernel<2, false>;
     const int smem = (int)sizeof(RsSmem);
-    if (!ensure_smem(k0, kSlotSerial, smem) || !ensure_smem(k1, kSlotSerial + 1, smem) ||
-        !ensure_smem(k2, kSlotSerial + 2, smem)) {
+    const int slot0 = tri ? kSlotSerialTri : kSlotSerial;
+    if (!ensure_smem(k0, slot0, smem) || !ensure_smem(k1, slot0 + 1, smem) || !ensure_smem(k2, slot0 + 2, smem)) {
         pvb_set_error("pvb_composed_query: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
         return PVB_ERR_CUDA;
     }
@@ -2386,6 +2356,15 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
         pvb_set_error("pvb_composed_query: at most 128 sub-SDFs per call (got %d)", n_sdf);
         return PVB_ERR_INVALID;
     }
+    bool any_tri = false;
+    for (int i = 0; i < n_sdf; ++i) {
+        if (descs[i].kind != PVB_KIND_GRID || !(descs[i].flags & PVB_GRID_TRILINEAR)) continue;
+        if (descs[i].flags & PVB_GRID_OOB_GT) {
+            pvb_set_error("pvb_composed_query: sub-SDF %d: PVB_GRID_TRILINEAR supports the bounding-box rule only", i);
+            return PVB_ERR_INVALID;
+        }
+        any_tri = true;
+    }
     if (n_pts == 0 || cfg_count == 0) return PVB_OK;
     cudaStream_t s = (cudaStream_t)stream;
     auto aligned16 = [](const void *p) { return p == nullptr || ((uintptr_t)p % 16) == 0; };
@@ -2398,20 +2377,33 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
         tgv.vec = out_aligned && (n_pts % 4 == 0);
         tg = &tgv;
     }
+    static const int cfg_major = [] { const char *e = getenv("PVB_COMP_CFGMAJOR"); return e ? atoi(e) : 1; }();
+    static const int robot_kernel = [] { const char *e = getenv("PVB_ROBOT_KERNEL"); return e ? atoi(e) : 2; }();
+    // every sub-SDF a GRID with the bounding-box rule (nearest or trilinear): the robot kernels' precondition
+    bool all_grid = !needs_mesh && n_sdf <= 16 && n_pts < (1ll << 31);
+    for (int i = 0; i < n_sdf && all_grid; ++i)
+        all_grid = descs[i].kind == PVB_KIND_GRID && !(descs[i].flags & PVB_GRID_OOB_GT);
+    // the point-serial kernel has no fill problem (remainder configurations run in lane-split tiles): any batch of
+    // PVB_ROBOT_MIN_CFG or more configurations takes it
+    static const int serial_min_cfg = [] { const char *e = getenv("PVB_ROBOT_MIN_CFG"); return e ? atoi(e) : 8; }();
+    const bool serial_ok = robot_kernel >= 2 && n_sdf <= kRsMaxS && cfg_count >= serial_min_cfg &&
+                           cfg_count <= 65535 * kRbCfg;          // one grid row per 32-configuration tile
+    // sets with trilinear links take the serial kernel where nearest sets would; robot_query_kernel (9-16 links) is
+    // nearest-voxel only, so otherwise they fall through to the configuration-major or point-major kernel
+    const bool serial_taken = robot_kernel && cfg_major && all_grid && serial_ok;
     if (tg && tg->mc) {
-        // multicast destinations exist only in robot_query_kernel: refuse anything that would fall through
-        bool grids = !needs_mesh && n_sdf <= 16;
-        for (int i = 0; i < n_sdf && grids; ++i)
-            grids = descs[i].kind == PVB_KIND_GRID && !(descs[i].flags & (PVB_GRID_OOB_GT | PVB_GRID_TRILINEAR));
-        if (!grids || n_pts >= (1ll << 31)) {
-            pvb_set_error("pvb_composed_query_multicast: needs <= 16 GRID sub-SDFs with the bounding-box rule");
+        // multicast destinations exist only in the robot kernels: refuse anything that would fall through
+        if (!all_grid || (any_tri && !serial_taken)) {
+            pvb_set_error(any_tri ? "pvb_composed_query_multicast: trilinear sub-SDFs need <= %d GRID sub-SDFs with the "
+                                    "bounding-box rule and >= PVB_ROBOT_MIN_CFG configurations"
+                                  : "pvb_composed_query_multicast: needs <= 16 GRID sub-SDFs with the bounding-box rule",
+                          kRsMaxS);
             return PVB_ERR_INVALID;
         }
     }
     const bool vec = !needs_mesh && aligned16(pts) && out_aligned && aligned16(out_which) && (n_pts % 4 == 0);
     const long long n_vec = vec ? n_pts : 0;
     int rc = PVB_OK;
-    static const int cfg_major = [] { const char *e = getenv("PVB_COMP_CFGMAJOR"); return e ? atoi(e) : 1; }();
     // lanes = configurations: only worthwhile when the 32-wide configuration tiles are well filled (25 configurations
     // per rank on 8 GPUs would idle 22 % of the lanes, and point-major is faster there)
     const int cm_tiles = (cfg_count + kCmCfg - 1) / kCmCfg;
@@ -2419,34 +2411,27 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
     // sectors, which is what the NVLink-bound re-assembly needs; idle lanes cost less than partial-sector packets
     const bool cm_filled = (cfg_count >= 16 && (double)cfg_count >= 0.85 * (double)(cm_tiles * kCmCfg)) ||
                            (tg && tg->vec && cfg_count >= 8);
-    static const int robot_kernel = [] { const char *e = getenv("PVB_ROBOT_KERNEL"); return e ? atoi(e) : 2; }();
     static const double robot_fill = [] { const char *e = getenv("PVB_ROBOT_MIN_FILL"); return e ? atof(e) : 0.85; }();
-    bool all_grid = !needs_mesh && n_sdf <= 16 && n_pts < (1ll << 31);
-    for (int i = 0; i < n_sdf && all_grid; ++i)
-        all_grid = descs[i].kind == PVB_KIND_GRID && !(descs[i].flags & (PVB_GRID_OOB_GT | PVB_GRID_TRILINEAR));
     const bool rb_filled = (cfg_count >= 16 && (double)cfg_count >= robot_fill * (double)(cm_tiles * kCmCfg)) ||
                            (tg && tg->vec && cfg_count >= 8) || (tg && tg->mc);
-    // the point-serial kernel has no fill problem (remainder configurations run in lane-split tiles): any batch of
-    // PVB_ROBOT_MIN_CFG or more configurations takes it
-    static const int serial_min_cfg = [] { const char *e = getenv("PVB_ROBOT_MIN_CFG"); return e ? atoi(e) : 8; }();
-    const bool serial_ok = robot_kernel >= 2 && n_sdf <= kRsMaxS && cfg_count >= serial_min_cfg &&
-                           cfg_count <= 65535 * kRbCfg;          // one grid row per 32-configuration tile
-    if (robot_kernel && cfg_major && all_grid && (rb_filled || serial_ok)) {
+    // PVB_ROBOT_KERNEL: 2 (default) = point-serial nearest-sphere-first kernel for <= 8 links, 1 = the
+    // 4-points-per-thread kernel, 0 = round 1's configuration-major kernel
+    if (serial_taken)
+        return launch_robot_serial(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,
+                                   (tg ? tg->vec : (out_aligned && (n_pts % 4 == 0))), out_val, out_grad, out_which,
+                                   tg, any_tri, s);
+    if (robot_kernel && cfg_major && all_grid && !any_tri && rb_filled) {
         const int vec_rows = (tg ? tg->vec : (out_aligned && (n_pts % 4 == 0))) && aligned16(pts);
-        // PVB_ROBOT_KERNEL: 2 (default) = point-serial nearest-sphere-first kernel for <= 8 links, 1 = the
-        // 4-points-per-thread kernel, 0 = round 1's configuration-major kernel
-        if (serial_ok)
-            return launch_robot_serial(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,
-                                       (tg ? tg->vec : (out_aligned && (n_pts % 4 == 0))), out_val, out_grad, out_which,
-                                       tg, s);
         return n_sdf <= 8 ? launch_robot<8, true>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, vec_rows,
                                                   out_val, out_grad, out_which, tg, s)
                           : launch_robot<16, false>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,
                                                     vec_rows, out_val, out_grad, out_which, tg, s);
     }
     if (cfg_major && !needs_mesh && n_sdf <= kCmMaxS && cm_filled) {
-        if (!ensure_smem(composed_cfgmajor_kernel<false>, kSlotCfgMajor, (int)sizeof(CmSmem)) ||
-            !ensure_smem(composed_cfgmajor_kernel<true>, kSlotCfgMajorMulti, (int)sizeof(CmSmem))) {
+        auto kl = any_tri ? composed_cfgmajor_kernel<false, true> : composed_cfgmajor_kernel<false, false>;
+        auto km = any_tri ? composed_cfgmajor_kernel<true, true> : composed_cfgmajor_kernel<true, false>;
+        const int slot = any_tri ? kSlotCfgMajorTri : kSlotCfgMajor;
+        if (!ensure_smem(kl, slot, (int)sizeof(CmSmem)) || !ensure_smem(km, slot + 1, (int)sizeof(CmSmem))) {
             pvb_set_error("pvb_composed_query: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
             return PVB_ERR_CUDA;
         }
@@ -2461,28 +2446,29 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
         dim3 grid((unsigned)gx, (unsigned)gy);
         timing_mark(0, s);
         if (tg)
-            composed_cfgmajor_kernel<true><<<grid, kCmCfg * kCmWarps, sizeof(CmSmem), s>>>(
-                pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, nullptr, nullptr, out_which, *tg);
+            km<<<grid, kCmCfg * kCmWarps, sizeof(CmSmem), s>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,
+                                                               n_pts, nullptr, nullptr, out_which, *tg);
         else
-            composed_cfgmajor_kernel<false><<<grid, kCmCfg * kCmWarps, sizeof(CmSmem), s>>>(
-                pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_val, out_grad, out_which,
-                OutTargets{});
+            kl<<<grid, kCmCfg * kCmWarps, sizeof(CmSmem), s>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,
+                                                               n_pts, out_val, out_grad, out_which, OutTargets{});
         timing_mark(1, s);
         PVB_CHECK_LAUNCH("pvb_composed_query(cfg-major)");
         return PVB_OK;
     }
-#define PVB_COMP(MESH, PTS, FIRST, N)                                                                              \
-    (n_sdf <= 16 ? launch_composed<MESH, PTS, 16>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, FIRST, N,  \
-                                                  mesh_mode, out_val, out_grad, out_which, tg, s)                  \
-                 : launch_composed<MESH, PTS, 128>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, FIRST, N, \
-                                                   mesh_mode, out_val, out_grad, out_which, tg, s))
+#define PVB_COMP(MESH, PTS, FIRST, N, TRI)                                                                         \
+    (n_sdf <= 16 ? launch_composed<MESH, PTS, 16, TRI>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, FIRST,  \
+                                                       N, mesh_mode, out_val, out_grad, out_which, tg, s)          \
+                 : launch_composed<MESH, PTS, 128, TRI>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, FIRST, \
+                                                        N, mesh_mode, out_val, out_grad, out_which, tg, s))
+#define PVB_COMP_ANY(MESH, PTS, FIRST, N) (any_tri ? PVB_COMP(MESH, PTS, FIRST, N, true) : PVB_COMP(MESH, PTS, FIRST, N, false))
     if (n_vec > 0) {
-        rc = PVB_COMP(false, PVB_COMP_PTS, 0, n_pts);
+        rc = PVB_COMP_ANY(false, PVB_COMP_PTS, 0, n_pts);
     } else if (needs_mesh) {
-        rc = PVB_COMP(true, 1, 0, n_pts);
+        rc = PVB_COMP_ANY(true, 1, 0, n_pts);
     } else {
-        rc = PVB_COMP(false, 1, 0, n_pts);
+        rc = PVB_COMP_ANY(false, 1, 0, n_pts);
     }
+#undef PVB_COMP_ANY
 #undef PVB_COMP
     return rc;
 }
@@ -2751,6 +2737,11 @@ extern "C" int pvb_chamfer(const pvb_sdf_desc *obj, const float *world_to_object
     }
     if (obj->kind == PVB_KIND_MESH)
         if (int rc = check_mesh(obj, "pvb_chamfer")) return rc;
+    if (obj->kind == PVB_KIND_GRID && (obj->flags & PVB_GRID_TRILINEAR)) {
+        // the chamfer kernel evaluates grids with the nearest-voxel rule only; refuse rather than answer differently
+        pvb_set_error("pvb_chamfer: PVB_GRID_TRILINEAR descriptors are not supported");
+        return PVB_ERR_INVALID;
+    }
     if (n_tf == 0) return PVB_OK;
     if (n_tf > 65535) {
         pvb_set_error("pvb_chamfer: at most 65535 transforms per call (got %d)", n_tf);

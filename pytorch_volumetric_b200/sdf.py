@@ -883,6 +883,9 @@ def grid_prune_margin(values, lo, hi, bb):
     of the nearest voxel c, |q - c| <= half a cell diagonal, dist(., bb) is 1-Lipschitz, and t = max over the table
     of (dist(c, bb) - value(c))+ is measured on the table itself, so the bound holds for any table contents:
     value(c) >= dist(c, bb) - t >= dist(q, bb) - half_diag - t.  (1e-5 absorbs the kernels' fp32 arithmetic.)
+    The same margin bounds the trilinear interpolant sum_i w_i value(c_i) over the 8 corners c_i of q's cell:
+    value(c_i) >= dist(q, bb) - |q - c_i| - t, and sum_i w_i |q - c_i| <= sqrt(sum_i w_i |q - c_i|^2) (Jensen)
+    = sqrt(sum_a r_a^2 f_a (1 - f_a)) <= half_diag, with r_a the cell size and f_a the fraction along axis a.
     values: (nx, ny, nz) table; lo / hi: per-axis range; bb: (3, 2) box the out-of-range rule measures against."""
     shape = tuple(values.shape)
     dev = values.device
@@ -943,7 +946,10 @@ class CachedSDF(ObjectFrameSDF):
         :param cache_path: torch.save file holding {name: (val[nx,ny,nz], grad[Nvox,3])}, same format as the reference
         :param interpolation: "nearest" (the reference's behaviour: nearest voxel value and stored gradient) or
         "trilinear" -- an EXTENSION that interpolates the value table trilinearly and returns the gradient of the
-        interpolant (cell-wise finite differences); smoother, but O(resolution) away from the reference's output
+        interpolant (cell-wise finite differences); smoother, but O(resolution) away from the reference's output.
+        Trilinear needs OutOfBoundsStrategy.BOUNDING_BOX.  It runs on the fused ComposedSDF / RobotSDF kernels like
+        "nearest" does (point-serial robot kernel for <= 8 links, configuration-major and point-major kernels
+        otherwise); batch_chamfer_dist evaluates a trilinear obj_sdf through its __call__
         """
         if interpolation not in ("nearest", "trilinear"):
             raise ValueError(f"interpolation must be 'nearest' or 'trilinear', got {interpolation!r}")
@@ -1040,6 +1046,7 @@ class CachedSDF(ObjectFrameSDF):
         self._gt_in_kernel = gt_native is not None
         # Pruning bound for the composed kernels: table value at the nearest voxel of q is never below
         # aabb_distance(q) - prune_margin.  t is measured on the table itself, so the bound holds for any table.
+        # It holds for the trilinear interpolant as well (grid_prune_margin).
         if self.out_of_bounds_strategy == OutOfBoundsStrategy.BOUNDING_BOX:
             margin = grid_prune_margin(self.voxels.raw_data.reshape(shape), lo, hi, bb)
             if math.isfinite(margin):
@@ -1048,14 +1055,17 @@ class CachedSDF(ObjectFrameSDF):
         if self.interpolation == "trilinear":
             if self.out_of_bounds_strategy != OutOfBoundsStrategy.BOUNDING_BOX:
                 raise ValueError("interpolation='trilinear' supports OutOfBoundsStrategy.BOUNDING_BOX only")
-            flags = (flags | nat.PVB_GRID_TRILINEAR) & ~nat.PVB_GRID_PRUNE_OK
+            flags |= nat.PVB_GRID_TRILINEAR
         d.flags = flags
         return d
 
     def native_desc(self, device):
+        """Descriptor for the fused kernels on `device` (None: not queryable there natively).  With
+        interpolation="trilinear" it carries PVB_GRID_TRILINEAR, which pvb_grid_lookup and the composed kernels
+        honour and pvb_chamfer rejects."""
         device = nat.compute_device(device)
-        if device != self._cdev or self.interpolation != "nearest":
-            return None          # the fused composition kernels implement the reference's nearest-voxel rule only
+        if device != self._cdev:
+            return None
         if self.out_of_bounds_strategy == OutOfBoundsStrategy.LOOKUP_GT_SDF and not self._gt_in_kernel:
             return None
         return self._desc
