@@ -190,6 +190,19 @@ int pvb_composed_query(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_m
                        const float *pts, int64_t n_pts, uint32_t mesh_mode,
                        float *out_val, float *out_grad, int32_t *out_which, void *stream);
 
+/* ---- EXTENSION: paired query, every configuration at its own points ----
+ * The reference has no such operator; its equivalent is the diagonal of ComposedSDF.__call__ (sdf.py:392-433) over
+ * points [|A|, n_pts, 3], which costs |A| times the work and memory.  Configuration cfg_begin + c is evaluated at
+ * pts[c][0 .. n_pts) only: pts DEVICE [cfg_count][n_pts][3], out_val [cfg_count * n_pts], out_grad
+ * [cfg_count * n_pts * 3], out_which optional; everything else as pvb_composed_query.  Results are bit-identical to
+ * pvb_composed_query(pts + 3 * c * n_pts, n_pts, cfg_begin + c, cfg_count = 1) for every c, including the mesh ray
+ * jitter (seeded by the absolute configuration index), and so, for GRID and SPHERE sets, to the diagonal of the cross
+ * product.  PVB_ERR_INVALID also when cfg_count * n_pts overflows int64_t. */
+int pvb_composed_query_paired(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh, const float *xforms,
+                              int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                              const float *pts, int64_t n_pts, uint32_t mesh_mode,
+                              float *out_val, float *out_grad, int32_t *out_which, void *stream);
+
 /* ---- the same query with the result slab stored to several destinations from the kernel epilogue ----
  * Multi-GPU re-assembly of a configuration-sharded RobotSDF result (model_to_sdf.py:117-125 returns the full
  * (|A|, N) tensors): every rank evaluates its slab [cfg_begin, cfg_begin + cfg_count) and writes it straight into
@@ -304,6 +317,10 @@ int pvb_compact_nonempty(const void *data, int64_t n, int32_t elem_bytes, double
 /* ---- rigid transform helpers used by the generic (unfused) composition path ---- */
 int pvb_transform_points(const float *xforms, int32_t n_tf, const float *pts, int64_t n_pts,
                          float *out, void *stream);
+/* paired: out[b][i] = xforms[b] applied to pts[b][i] (pts / out DEVICE [n_tf][n_pts][3]), same arithmetic as the
+ * composed kernels' transform -- the generic path of the paired query (pvb_composed_query_paired) */
+int pvb_transform_points_paired(const float *xforms, int32_t n_tf, const float *pts, int64_t n_pts,
+                                float *out, void *stream);
 
 #ifdef __cplusplus
 }

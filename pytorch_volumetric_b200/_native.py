@@ -129,6 +129,10 @@ _SIGNATURES = {
                                           ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                           ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint32, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "pvb_composed_query_paired": (ctypes.c_int, [ctypes.POINTER(SdfDesc), ctypes.c_int32, ctypes.c_int32,
+                                                 ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                                 ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint32, ctypes.c_void_p,
+                                                 ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "pvb_composed_query_multi": (ctypes.c_int, [ctypes.POINTER(SdfDesc), ctypes.c_int32, ctypes.c_int32,
                                                 ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                                 ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint32, ctypes.c_void_p,
@@ -166,6 +170,8 @@ _SIGNATURES = {
                                        ctypes.c_void_p]),
     "pvb_transform_points": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,
                                             ctypes.c_void_p, ctypes.c_void_p]),
+    "pvb_transform_points_paired": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,
+                                                   ctypes.c_void_p, ctypes.c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

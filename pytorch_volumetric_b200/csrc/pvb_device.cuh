@@ -4,6 +4,7 @@
 //   bvh_closest    closest point on the mesh                 (Embree rtcPointQuery role, sdf.py:134)
 //   bvh_parity     ray/triangle crossing parity              (count_intersections role, sdf.py:152-154)
 //   mesh_eval      ObjectFactory._do_object_frame_closest_point epilogue (sdf.py:139-164)
+//   composed_point ComposedSDF.__call__ for one (configuration, point) pair (sdf.py:392-433)
 #pragma once
 #include "../../include/pvb.h"
 #include <cuda_runtime.h>
@@ -677,6 +678,96 @@ __device__ __forceinline__ void composed_consider(const pvb_sdf_desc &d, const N
     if (bs < 0 || o.val < best || (o.val == best && s < bs)) {
         best = o.val; bg = o.grad; bs = s;
     }
+}
+
+// One (configuration, point) pair of the composition: every sub-SDF through composed_consider, then the winning
+// gradient rotated back to the object frame.  The per-pair work of composed_paired_kernel: the same sequence as the
+// one-point path of composed_query_kernel (visiting order, nearest-bound-first for meshes, jitter index, rotation
+// back), so that a paired query equals the per-configuration query on the same points bit for bit.
+// (composed_query_kernel keeps its own copy of the loop: routed through this function, its mesh instantiations
+// compiled to different SASS with more spills.)
+//   descs / order: the sub-SDFs and the fixed visiting order (DescPack::order, bit-reversed)
+//   load_xf(s, r0, r1, r2): rows 0..2 of sub-SDF s's object->sub-frame matrix for this configuration
+//   pair: cfg * n_pts + i with the ABSOLUTE configuration index; the mesh ray jitter of sub-SDF s is seeded by
+//   pair * n_sdf + s, so results do not depend on how the configurations are split over launches or GPUs
+//   nearest_first / margin_max: see below (kMesh only)
+struct ComposedOut { float val; f3 grad; int which; };
+
+template <bool kMesh, bool kTri, class LoadXf>
+__device__ __forceinline__ ComposedOut composed_point(const pvb_sdf_desc *descs, const unsigned char *order, int n_sdf,
+                                                      const LoadXf &load_xf, const NodeStage &st, f3 p,
+                                                      uint32_t mesh_mode, uint64_t pair, int nearest_first,
+                                                      float margin_max) {
+    float best = PVB_INF;
+    f3 bg = mk3(0.f, 0.f, 0.f);
+    int bs = -1;
+    // Every sub-SDF in visiting order, skipped when provably not the argmin (composed_consider).  (Evaluating the
+    // sub-SDF with the smallest AABB lower bound first -- an extra pass over all of them without table access -- saves
+    // lookups but adds issue slots to a kernel that is issue-bound.)
+    // ... except when sub-SDFs are MESHES (kMesh): an evaluation is a tree walk of thousands of instructions, so one
+    // cheap pass computes every sub-SDF's AABB lower bound and the thread then evaluates them NEAREST BOUND FIRST,
+    // stopping as soon as the smallest remaining bound exceeds the running minimum.  A fixed order evaluates every
+    // sub-SDF that is a running record when its turn comes (~H_16 = 3.4 of 16 at C3, plus those inside the slack);
+    // nearest-first evaluates the winner and its near ties.  Exact for the same reason as the fixed order: bounds are
+    // conservative and the argmin keeps torch's first-index rule explicitly.
+    bool ordered = false;
+    if constexpr (kMesh) {
+        if (n_sdf <= 32 && nearest_first) {
+            ordered = true;
+            float key[32];                           // squared lower bound; -1 = no valid bound (evaluate)
+            unsigned todo = n_sdf >= 32 ? 0xffffffffu : ((1u << n_sdf) - 1u);
+            for (int s = 0; s < n_sdf; ++s) {
+                const pvb_sdf_desc &d = descs[s];
+                float4 r0, r1, r2;
+                load_xf(s, r0, r1, r2);
+                const bool bounded = d.kind == PVB_KIND_GRID ? (d.flags & PVB_GRID_PRUNE_OK) != 0
+                                     : (d.kind == PVB_KIND_MESH && (d.flags & PVB_MESH_CLOSED) && (mesh_mode & PVB_MESH_SIGNED));
+                key[s] = bounded ? composed_aabb_lb2(d, composed_xform(r0, r1, r2, p)) : -1.f;
+            }
+            while (todo) {
+                int s = -1;
+                float kmin = PVB_INF;
+                for (int t = 0; t < n_sdf; ++t)
+                    if ((todo >> t) & 1u) { if (key[t] < kmin) { kmin = key[t]; s = t; } }
+                if (s < 0) break;
+                todo &= ~(1u << s);
+                const pvb_sdf_desc &d = descs[s];
+                if (bs >= 0 && kmin >= 0.f) {
+                    // every remaining bound is at least kmin: when even the most generous margin cannot bring it under
+                    // the running minimum, nothing left can win (margins are per sub-SDF: test this one exactly, and
+                    // stop the loop only on the margin-free comparison)
+                    const float thr = best + d.prune_margin;
+                    if (thr < 0.f || kmin > thr * thr) {
+                        if (best + margin_max < 0.f || kmin > (best + margin_max) * (best + margin_max)) break;
+                        continue;
+                    }
+                }
+                float4 r0, r1, r2;
+                load_xf(s, r0, r1, r2);
+                composed_consider<kMesh, kTri>(d, st, s, composed_xform(r0, r1, r2, p), mesh_mode,
+                                               pair * (uint64_t)n_sdf + (uint64_t)s, best, bg, bs);
+            }
+        }
+    }
+    for (int si = 0; si < (ordered ? 0 : n_sdf); ++si) {
+        const int s = order[si];
+        float4 r0, r1, r2;
+        load_xf(s, r0, r1, r2);
+        composed_consider<kMesh, kTri>(descs[s], st, s, composed_xform(r0, r1, r2, p), mesh_mode,
+                                       pair * (uint64_t)n_sdf + (uint64_t)s, best, bg, bs);
+    }
+    float4 r0, r1, r2;
+    load_xf(max(bs, 0), r0, r1, r2);
+    ComposedOut o;
+    o.val = best; o.grad = composed_rotate_back(r0, r1, r2, bg); o.which = bs;
+    return o;
+}
+
+// Paired queries (composed_paired_kernel): flat pair index t in [0, cfg_count * n_pts) -> (configuration c relative
+// to cfg_begin, point i).  64-bit throughout: cfg_count * n_pts may exceed 2^31 where n_pts alone does not.
+__device__ __forceinline__ void paired_index(long long t, long long n_pts, long long &c, long long &i) {
+    c = t / n_pts;
+    i = t - c * n_pts;
 }
 
 // ----------------------------------------------------------------------------

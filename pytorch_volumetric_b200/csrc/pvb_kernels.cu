@@ -834,6 +834,39 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// Paired query: configuration c is evaluated at its OWN points pts[c][0 .. n_pts) instead of the point set all
+// configurations share (trajectory steps against per-step obstacles, MPC rollouts, batched environments):
+// cfg_count * n_pts pairs instead of the cfg_count x (cfg_count * n_pts) cross product.  One thread per pair
+// t = c * n_pts + i, running composed_point with the jitter index of the absolute configuration, so the result equals
+// pvb_composed_query(pts[c], cfg_begin + c, 1) bit for bit.  The transform rows are read per thread with __ldg rather
+// than staged per block like composed_query_kernel does: with few points per configuration one block spans many
+// configurations, and the lanes of one configuration read the same rows (L1 broadcasts).
+template <bool kMesh, bool kTri, int MAXS>
+__global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
+composed_paired_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
+                       int n_cfg, int cfg_begin, const float *__restrict__ pts, long long n_pts, long long n_pairs,
+                       uint32_t mesh_mode, float *__restrict__ out_val, float *__restrict__ out_grad,
+                       int *__restrict__ out_which, int nearest_first, float margin_max) {
+    NodeStage st; st.smem = nullptr; st.n = 0;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n_pairs; t += stride) {
+        long long c, i;
+        paired_index(t, n_pts, c, i);
+        const int cfg = cfg_begin + (int)c;
+        auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) {
+            const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
+            r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
+        };
+        const ComposedOut o = composed_point<kMesh, kTri>(descs.d, descs.order, n_sdf, load_xf, st, load_point(pts, t),
+                                                          mesh_mode, (uint64_t)cfg * (uint64_t)n_pts + (uint64_t)i,
+                                                          nearest_first, margin_max);
+        out_val[t] = o.val;
+        out_grad[3 * t] = o.grad.x; out_grad[3 * t + 1] = o.grad.y; out_grad[3 * t + 2] = o.grad.z;
+        if (out_which) out_which[t] = o.which;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // Configuration-major variant for RobotSDF-style batches (many joint configurations, shared points).
 //
 // Lanes of a warp are 32 CONFIGURATIONS of the same point instead of 32 points of the same configuration:
@@ -1959,6 +1992,20 @@ __global__ void transform_points_kernel(const float *__restrict__ xforms, int n_
     }
 }
 
+// out[t] = M_{t / n_pts} applied to pts[t]: every transform to its own n_pts points (the unfused paired composition),
+// with the arithmetic of composed_xform so that the sub-frame points equal what the fused kernels compute
+__global__ void transform_points_paired_kernel(const float *__restrict__ xforms, const float *__restrict__ pts,
+                                               long long n_pts, long long n, float *__restrict__ out) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
+        long long b, i;
+        paired_index(t, n_pts, b, i);
+        const float4 *row = reinterpret_cast<const float4 *>(xforms + b * 16);
+        const f3 q = composed_xform(__ldg(row), __ldg(row + 1), __ldg(row + 2), load_point(pts, t));
+        out[3 * t] = q.x; out[3 * t + 1] = q.y; out[3 * t + 2] = q.z;
+    }
+}
+
 static int grid_for(long long work_items, int threads, int blocks_per_sm) {
     const long long want = (work_items + threads - 1) / threads;
     const long long cap = (long long)sm_count() * blocks_per_sm;
@@ -2341,30 +2388,42 @@ static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float
     return PVB_OK;
 }
 
+// Argument checks shared by the composed entry points (`fn` names the entry point in the error message); any_tri:
+// some sub-SDF is PVB_GRID_TRILINEAR.
+static int composed_check_args(const char *fn, const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,
+                               int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count, const float *pts, int64_t n_pts,
+                               const float *out_val, const float *out_grad, bool &any_tri) {
+    if (!descs || !xforms || n_sdf < 1 || n_cfg < 1 || cfg_begin < 0 || cfg_count < 0 ||
+        cfg_begin + cfg_count > n_cfg || n_pts < 0 || (n_pts > 0 && cfg_count > 0 && (!pts || !out_val || !out_grad))) {
+        pvb_set_error("%s: invalid argument (n_sdf=%d n_cfg=%d cfg=[%d,+%d) n_pts=%lld)", fn, n_sdf, n_cfg,
+                      cfg_begin, cfg_count, (long long)n_pts);
+        return PVB_ERR_INVALID;
+    }
+    if (n_sdf > 128) {
+        pvb_set_error("%s: at most 128 sub-SDFs per call (got %d)", fn, n_sdf);
+        return PVB_ERR_INVALID;
+    }
+    any_tri = false;
+    for (int i = 0; i < n_sdf; ++i) {
+        if (descs[i].kind != PVB_KIND_GRID || !(descs[i].flags & PVB_GRID_TRILINEAR)) continue;
+        if (descs[i].flags & PVB_GRID_OOB_GT) {
+            pvb_set_error("%s: sub-SDF %d: PVB_GRID_TRILINEAR supports the bounding-box rule only", fn, i);
+            return PVB_ERR_INVALID;
+        }
+        any_tri = true;
+    }
+    return PVB_OK;
+}
+
 // tg == nullptr: one destination (out_val / out_grad); otherwise the kMulti instantiations store to every target
 static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh, const float *xforms,
                              int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count, const float *pts, int64_t n_pts,
                              uint32_t mesh_mode, float *out_val, float *out_grad, int32_t *out_which,
                              const OutTargets *tg, void *stream) {
-    if (!descs || !xforms || n_sdf < 1 || n_cfg < 1 || cfg_begin < 0 || cfg_count < 0 ||
-        cfg_begin + cfg_count > n_cfg || n_pts < 0 || (n_pts > 0 && cfg_count > 0 && (!pts || !out_val || !out_grad))) {
-        pvb_set_error("pvb_composed_query: invalid argument (n_sdf=%d n_cfg=%d cfg=[%d,+%d) n_pts=%lld)", n_sdf, n_cfg,
-                      cfg_begin, cfg_count, (long long)n_pts);
-        return PVB_ERR_INVALID;
-    }
-    if (n_sdf > 128) {
-        pvb_set_error("pvb_composed_query: at most 128 sub-SDFs per call (got %d)", n_sdf);
-        return PVB_ERR_INVALID;
-    }
-    bool any_tri = false;
-    for (int i = 0; i < n_sdf; ++i) {
-        if (descs[i].kind != PVB_KIND_GRID || !(descs[i].flags & PVB_GRID_TRILINEAR)) continue;
-        if (descs[i].flags & PVB_GRID_OOB_GT) {
-            pvb_set_error("pvb_composed_query: sub-SDF %d: PVB_GRID_TRILINEAR supports the bounding-box rule only", i);
-            return PVB_ERR_INVALID;
-        }
-        any_tri = true;
-    }
+    bool any_tri;
+    const int bad = composed_check_args("pvb_composed_query", descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,
+                                        n_pts, out_val, out_grad, any_tri);
+    if (bad) return bad;
     if (n_pts == 0 || cfg_count == 0) return PVB_OK;
     cudaStream_t s = (cudaStream_t)stream;
     auto aligned16 = [](const void *p) { return p == nullptr || ((uintptr_t)p % 16) == 0; };
@@ -2479,6 +2538,53 @@ extern "C" int pvb_composed_query(const pvb_sdf_desc *descs, int32_t n_sdf, int3
                                   int32_t *out_which, void *stream) {
     return composed_dispatch(descs, n_sdf, needs_mesh, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, mesh_mode,
                              out_val, out_grad, out_which, nullptr, stream);
+}
+
+template <bool kMesh, bool kTri, int MAXS>
+static int launch_paired(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
+                         const float *pts, long long n_pts, long long n_pairs, uint32_t mesh_mode, float *out_val,
+                         float *out_grad, int *out_which, cudaStream_t stream) {
+    DescPack<MAXS> pack;
+    memcpy(pack.d, descs, sizeof(pvb_sdf_desc) * (size_t)n_sdf);
+    fill_order(pack, n_sdf);
+    // the same switch as launch_composed: nearest-bound-first evaluation of mesh sub-SDFs
+    static const int nearest_first = [] { const char *e = getenv("PVB_COMP_NEAREST_FIRST"); return e ? atoi(e) : 1; }();
+    float margin_max = 0.f;
+    for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
+    timing_mark(0, stream);
+    composed_paired_kernel<kMesh, kTri, MAXS><<<grid_for(n_pairs, kCompThreads, 8), kCompThreads, 0, stream>>>(
+        pack, n_sdf, xforms, n_cfg, cfg_begin, pts, n_pts, n_pairs, mesh_mode, out_val, out_grad, out_which,
+        nearest_first, margin_max);
+    timing_mark(1, stream);
+    PVB_CHECK_LAUNCH("pvb_composed_query_paired");
+    return PVB_OK;
+}
+
+extern "C" int pvb_composed_query_paired(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,
+                                         const float *xforms, int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                                         const float *pts, int64_t n_pts, uint32_t mesh_mode, float *out_val,
+                                         float *out_grad, int32_t *out_which, void *stream) {
+    bool any_tri;
+    const int bad = composed_check_args("pvb_composed_query_paired", descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count,
+                                        pts, n_pts, out_val, out_grad, any_tri);
+    if (bad) return bad;
+    if (n_pts == 0 || cfg_count == 0) return PVB_OK;
+    if (n_pts > INT64_MAX / cfg_count) {
+        pvb_set_error("pvb_composed_query_paired: cfg_count * n_pts overflows int64 (cfg_count=%d n_pts=%lld)",
+                      cfg_count, (long long)n_pts);
+        return PVB_ERR_INVALID;
+    }
+    const long long n_pairs = (long long)cfg_count * n_pts;
+    cudaStream_t s = (cudaStream_t)stream;
+#define PVB_PAIRED(MESH, TRI)                                                                                      \
+    (n_sdf <= 16 ? launch_paired<MESH, TRI, 16>(descs, n_sdf, xforms, n_cfg, cfg_begin, pts, n_pts, n_pairs,       \
+                                                 mesh_mode, out_val, out_grad, out_which, s)                         \
+                 : launch_paired<MESH, TRI, 128>(descs, n_sdf, xforms, n_cfg, cfg_begin, pts, n_pts, n_pairs,      \
+                                                  mesh_mode, out_val, out_grad, out_which, s))
+    const int rc = needs_mesh ? (any_tri ? PVB_PAIRED(true, true) : PVB_PAIRED(true, false))
+                              : (any_tri ? PVB_PAIRED(false, true) : PVB_PAIRED(false, false));
+#undef PVB_PAIRED
+    return rc;
 }
 
 extern "C" int pvb_composed_query_multi(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,
@@ -2781,6 +2887,20 @@ extern "C" int pvb_mesh_sample(const double *verts64, const int32_t *faces, int6
     mesh_sample_kernel<<<grid_for(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(
         verts64, faces, n_faces, (const long long *)cum_counts, n, seed, out_pts, out_face);
     PVB_CHECK_LAUNCH("pvb_mesh_sample");
+    return PVB_OK;
+}
+
+extern "C" int pvb_transform_points_paired(const float *xforms, int32_t n_tf, const float *pts, int64_t n_pts,
+                                           float *out, void *stream) {
+    if (!xforms || n_tf < 0 || n_pts < 0 || (n_tf > 0 && n_pts > 0 && (!pts || !out)) ||
+        (n_tf > 0 && n_pts > INT64_MAX / 3 / n_tf)) {
+        pvb_set_error("pvb_transform_points_paired: invalid argument");
+        return PVB_ERR_INVALID;
+    }
+    if (n_tf == 0 || n_pts == 0) return PVB_OK;
+    const long long n = (long long)n_tf * n_pts;
+    transform_points_paired_kernel<<<grid_for(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(xforms, pts, n_pts, n, out);
+    PVB_CHECK_LAUNCH("pvb_transform_points_paired");
     return PVB_OK;
 }
 

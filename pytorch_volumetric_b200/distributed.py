@@ -347,18 +347,34 @@ class PeerResult:
                 self.nat.check(self.nat.lib().pvb_ipc_free(self._local), "pvb_ipc_free")
 
 
-def sharded_robot_query(robot_sdf, points, gather=True, group=None, result=None):
+def sharded_robot_query(robot_sdf, points, gather=True, group=None, result=None, paired=False):
     """RobotSDF over this rank's contiguous slab of the (flattened) configuration batch.
 
     The output slab (cfg_count, P) is a contiguous block of the (|A|, P) result, so re-assembly is a plain
     concatenation on dim 0.  Returns ([A,] *B, N) / (..., 3) when gather=True, else the local slab and its range.
     gather="peer" with a PeerResult: the kernel stores the slab into every rank's buffer directly (no all-gather);
     the returned tensors are views of one of `result`'s two slots and stay valid until the second-next query into
-    it (see PeerResult for the cross-rank ordering this relies on)."""
+    it (see PeerResult for the cross-rank ordering this relies on).
+    paired=True: RobotSDF.paired sharded the same way -- points [*A, *B, N, 3], and this rank evaluates its
+    configurations on their own points[begin:end] only; gather must be True or False."""
     rank, world = _world(group)
     comp = robot_sdf.sdf
     n_cfg = 1 if comp.tsf_batch is None else math.prod(list(comp.tsf_batch))
     begin, end = shard_range(n_cfg, rank, world)
+    batch = tuple(comp.tsf_batch) if comp.tsf_batch is not None else ()
+    if paired:
+        if isinstance(gather, str):
+            raise ValueError("paired queries re-assemble with gather=True or gather=False only")
+        pts_shape = tuple(points.shape)
+        if len(pts_shape) < len(batch) + 1 or pts_shape[:len(batch)] != tuple(int(a) for a in batch) \
+                or pts_shape[-1] != 3:
+            raise ValueError(f"paired query: points {pts_shape} must be [*A, ..., 3] with the configuration batch "
+                             f"A = {batch} leading")
+        per_cfg = points.reshape(n_cfg, -1, 3)
+        P = per_cfg.shape[1]
+        val, grad = comp.query_paired(per_cfg[begin:end], cfg_begin=begin, cfg_count=end - begin)
+        lead = pts_shape[len(batch):-1]
+        return _slab_result(val, grad, begin, end, n_cfg, P, batch, lead, gather, group)
     P = points.reshape(-1, 3).shape[0]
     if isinstance(gather, str):
         if gather not in ("peer", "multicast", "dma") or result is None:
@@ -377,9 +393,15 @@ def sharded_robot_query(robot_sdf, points, gather=True, group=None, result=None)
             comp.query_into(points, targets, cfg_begin=begin, cfg_count=end - begin)
         result.publish()
         lead = tuple(points.shape[:-1])
-        batch = tuple(comp.tsf_batch) if comp.tsf_batch is not None else ()
         return result.val.view(*batch, *lead), result.grad.view(*batch, *lead, 3)
     val, grad = comp.query(points, cfg_begin=begin, cfg_count=end - begin)
+    return _slab_result(val, grad, begin, end, n_cfg, P, batch, tuple(points.shape[:-1]), gather, group)
+
+
+def _slab_result(val, grad, begin, end, n_cfg, P, batch, lead, gather, group):
+    """This rank's (cfg_count, P) slab, or with gather=True the full result re-assembled by all_gather_slabs and
+    shaped (*batch, *lead) / (..., 3)."""
+    _, world = _world(group)
     val = val.reshape(end - begin, P)
     grad = grad.reshape(end - begin, P, 3)
     if not gather:
@@ -387,8 +409,6 @@ def sharded_robot_query(robot_sdf, points, gather=True, group=None, result=None)
     counts = [shard_range(n_cfg, r, world)[1] - shard_range(n_cfg, r, world)[0] for r in range(world)]
     val = all_gather_slabs(val, counts, group)
     grad = all_gather_slabs(grad, counts, group)
-    lead = tuple(points.shape[:-1])
-    batch = tuple(comp.tsf_batch) if comp.tsf_batch is not None else ()
     return val.reshape(*batch, *lead), grad.reshape(*batch, *lead, 3)
 
 

@@ -140,6 +140,12 @@ class RobotSDF(sdf.ObjectFrameSDF):
         """points [*B, N, 3] in the robot frame -> (values [*A, *B, N], gradients [*A, *B, N, 3])."""
         return self.sdf(points_in_object_frame)
 
+    def paired(self, points_in_object_frame):
+        """Every installed joint configuration at its own points: points [*A, *B, N, 3] in the robot frame ->
+        (values [*A, *B, N], gradients [*A, *B, N, 3]), entry [a, ...] = configuration a at points[a, ...]
+        (ComposedSDF.paired)."""
+        return self.sdf.paired(points_in_object_frame)
+
     def surface_bounding_box(self, **kwargs):
         return self.sdf.surface_bounding_box(**kwargs)
 

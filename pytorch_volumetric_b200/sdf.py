@@ -682,6 +682,60 @@ class ComposedSDF(ObjectFrameSDF):
                                                    nat.stream_ptr(device)), "pvb_composed_query")
         return (val, grad, which) if return_which else (val, grad)
 
+    def query_paired(self, points_in_object_frame, cfg_begin=0, cfg_count=None, return_which=False):
+        """Paired form of `query`: configuration cfg_begin + c is evaluated at its own points only.  The points
+        reshape to [cfg_count, P, 3]; entry c * P + i of the result is configuration cfg_begin + c at points[c, i].
+        Bit-identical to query(points[c], cfg_begin=cfg_begin + c, cfg_count=1) for every c, mesh ray jitter
+        included.  Returns flat (cfg_count * P,) / (cfg_count * P, 3) fp32 tensors on the GPU."""
+        S = len(self.sdfs)
+        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
+        if cfg_count is None:
+            cfg_count = n_cfg - cfg_begin
+        shape = tuple(points_in_object_frame.shape)
+        n = math.prod(shape[:-1])
+        if shape[-1:] != (3,) or (n % cfg_count if cfg_count else n):
+            raise ValueError(f"paired query: points {shape} do not split into {cfg_count} blocks of [P, 3]")
+        P = n // cfg_count if cfg_count else 0
+        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
+        with torch.cuda.device(device):
+            p = nat.as_f32_points(points_in_object_frame, device)
+            descs_arr, needs_mesh = self._native_descs(device)
+            if descs_arr is None:
+                return self._generic_query(p, cfg_begin, cfg_count, n_cfg, return_which, paired=True)
+            xf = self._xforms_on(device)
+            val = torch.empty(cfg_count * P, dtype=torch.float32, device=device)
+            grad = torch.empty(cfg_count * P, 3, dtype=torch.float32, device=device)
+            which = torch.empty(cfg_count * P, dtype=torch.int32, device=device) if return_which else None
+            nat.check(nat.lib().pvb_composed_query_paired(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg,
+                                                          cfg_begin, cfg_count, nat.ptr(p), P, nat.PVB_MESH_DEFAULT,
+                                                          nat.ptr(val), nat.ptr(grad), nat.ptr(which),
+                                                          nat.stream_ptr(device)), "pvb_composed_query_paired")
+        return (val, grad, which) if return_which else (val, grad)
+
+    def paired(self, points_in_object_frame):
+        """Every installed configuration at its own points: points [*A, *B, N, 3], with A the configuration batch
+        (`tsf_batch`), give (values [*A, *B, N], gradients [*A, *B, N, 3]) in the points' dtype and on their device;
+        entry [a, ...] is configuration a evaluated at points[a, ...].
+
+        For GRID and SPHERE sub-SDFs this equals the diagonal of __call__ over the same points, without computing
+        the |A|-fold cross product.  For mesh sub-SDFs it equals the per-configuration slab query
+        query(points[a], cfg_begin=a, cfg_count=1), ray jitter included.  Without a configuration batch it is
+        __call__.  Not a reference operator (an extension); raises ValueError before any device work when the
+        leading dimensions of the points are not A."""
+        if self.tsf_batch is None:
+            return self(points_in_object_frame)
+        batch = tuple(int(a) for a in self.tsf_batch)
+        pts_shape = tuple(points_in_object_frame.shape)
+        if len(pts_shape) < len(batch) + 1 or pts_shape[:len(batch)] != batch or pts_shape[-1] != 3:
+            raise ValueError(f"paired query: points {pts_shape} must be [*A, ..., 3] with the configuration batch "
+                             f"A = {batch} leading")
+        vv, gg = self.query_paired(points_in_object_frame)
+        dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
+        out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
+        vv = nat.deliver(vv, out_device, dtype)
+        gg = nat.deliver(gg, out_device, dtype)
+        return vv.reshape(pts_shape[:-1]), gg.reshape(*pts_shape[:-1], 3)
+
     def query_into(self, points_in_object_frame, targets, cfg_begin=0, cfg_count=None):
         """`query` whose result slab is stored by the kernel epilogue into several full-size result buffers at once
         (pvb_composed_query_multi): `targets` is a list of (val, grad) pairs, each a float32 tensor or a raw device
@@ -758,21 +812,23 @@ class ComposedSDF(ObjectFrameSDF):
                                                              int(mc_grad) + 12 * cfg_begin * P,
                                                              nat.stream_ptr(device)), "pvb_composed_query_multicast")
 
-    def _generic_query(self, p, cfg_begin, cfg_count, n_cfg, return_which):
+    def _generic_query(self, p, cfg_begin, cfg_count, n_cfg, return_which, paired=False):
         """Sub-SDFs without a native descriptor (user subclasses, nested compositions): per-SDF evaluation through
-        their own __call__, with the transform and the running min still on the GPU."""
+        their own __call__, with the transform and the running min still on the GPU.  paired: p holds cfg_count
+        blocks of P points, block c for configuration cfg_begin + c only (query_paired)."""
         S = len(self.sdfs)
         device = p.device
-        P = p.shape[0]
+        P = (p.shape[0] // cfg_count if cfg_count else 0) if paired else p.shape[0]
         M = self._xforms_on(device).reshape(S, n_cfg, 4, 4)[:, cfg_begin:cfg_begin + cfg_count]
         best = torch.full((cfg_count * P,), float("inf"), dtype=torch.float32, device=device)
         bgrad = torch.zeros(cfg_count * P, 3, dtype=torch.float32, device=device)
         bwhich = torch.full((cfg_count * P,), -1, dtype=torch.int32, device=device)
+        transform = nat.lib().pvb_transform_points_paired if paired else nat.lib().pvb_transform_points
         for i, sdf in enumerate(self.sdfs):
             xf = M[i].contiguous()
             local = torch.empty(cfg_count, P, 3, dtype=torch.float32, device=device)
-            nat.check(nat.lib().pvb_transform_points(nat.ptr(xf), cfg_count, nat.ptr(p), P, nat.ptr(local),
-                                                     nat.stream_ptr(device)), "pvb_transform_points")
+            nat.check(transform(nat.ptr(xf), cfg_count, nat.ptr(p), P, nat.ptr(local), nat.stream_ptr(device)),
+                      "pvb_transform_points")
             v, g = sdf(local)
             v = v.to(device=device, dtype=torch.float32).reshape(cfg_count, P)
             g = g.to(device=device, dtype=torch.float32).reshape(cfg_count, P, 3) @ xf[:, :3, :3]
