@@ -845,4 +845,60 @@ __device__ __forceinline__ int rs_nearest(const float (&key)[8], int n_sdf) {
     return si < n_sdf - 1 ? si : n_sdf - 1;
 }
 
+// The bounding-sphere bound of robot_serial_kernel: value_s(p) >= |p - c_s| - r_s - prune_margin_s, c_s the centre of
+// link s's AABB carried to the object frame, r_s its half-diagonal.  Split by what it varies with: the radius term is
+// per link (host, constant bank), the centre per (configuration, link) (shared memory), the bound per point.
+// sph_rad: r (+1e-4 relative, +1e-6: the fp32 roundings of the radius and the centre) + prune_margin; +inf without
+// PVB_GRID_PRUNE_OK, so that the bound is -inf and never rejects.  visit_margin: the margin of the exact AABB test at
+// the head of a visit, +inf without PVB_GRID_PRUNE_OK (best + inf never rejects either).
+__host__ __device__ inline void rs_link_consts(const pvb_sdf_desc &d, float &sph_rad, float &visit_margin) {
+    const float hx = 0.5f * (d.bb_max[0] - d.bb_min[0]), hy = 0.5f * (d.bb_max[1] - d.bb_min[1]),
+                hz = 0.5f * (d.bb_max[2] - d.bb_min[2]);
+    const float rad = sqrtf(hx * hx + hy * hy + hz * hz) * 1.0001f + 1e-6f;
+    const bool ok = (d.flags & PVB_GRID_PRUNE_OK) != 0;
+    sph_rad = ok ? rad + d.prune_margin : PVB_INF;
+    visit_margin = ok ? d.prune_margin : PVB_INF;
+}
+
+// c_obj = R^T (c_link - t) from the rows r0..r2 of the object->link transform.  The bound needs an isometry: when
+// |R R^T - I| exceeds 1e-5 the centre is NaN, which makes the bound NaN -- `lb > best` never rejects it and the
+// nearest-link key (rs_bound_key / rs_nearest) ignores it.
+__device__ __forceinline__ f3 rs_sphere_centre(const pvb_sdf_desc &d, float4 r0, float4 r1, float4 r2) {
+    const f3 cen = mk3(0.5f * (d.bb_min[0] + d.bb_max[0]), 0.5f * (d.bb_min[1] + d.bb_max[1]),
+                       0.5f * (d.bb_min[2] + d.bb_max[2]));
+    const f3 u = mk3(cen.x - r0.w, cen.y - r1.w, cen.z - r2.w);
+    const f3 co = mk3(r0.x * u.x + r1.x * u.y + r2.x * u.z, r0.y * u.x + r1.y * u.y + r2.y * u.z,
+                      r0.z * u.x + r1.z * u.y + r2.z * u.z);
+    const float e00 = r0.x * r0.x + r0.y * r0.y + r0.z * r0.z - 1.f, e11 = r1.x * r1.x + r1.y * r1.y + r1.z * r1.z - 1.f,
+                e22 = r2.x * r2.x + r2.y * r2.y + r2.z * r2.z - 1.f;
+    const float e01 = r0.x * r1.x + r0.y * r1.y + r0.z * r1.z, e02 = r0.x * r2.x + r0.y * r2.y + r0.z * r2.z,
+                e12 = r1.x * r2.x + r1.y * r2.y + r1.z * r2.z;
+    const float dev = fmaxf(fmaxf(fmaxf(fabsf(e00), fabsf(e11)), fmaxf(fabsf(e22), fabsf(e01))),
+                            fmaxf(fabsf(e02), fabsf(e12)));
+    return dev < 1e-5f ? co : mk3(__int_as_float(0x7fffffff), 0.f, 0.f);
+}
+
+__device__ __forceinline__ float rsqrt_approx(float x) {      // one MUFU.RSQ, no denormal fix-up (callers keep x >= 1e-20)
+#ifdef __CUDA_ARCH__
+    float r;
+    asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+    return r;
+#else
+    return 1.0f / sqrtf(x);
+#endif
+}
+
+// sqrt(0.9998) * 0.999999: 0.9998 on the squared distance absorbs the 1e-5 non-rigidity tolerated above, 0.999999 the
+// approximate reciprocal square root (2 ulp) and the roundings of the three fused multiply-adds
+constexpr float kRsBoundScale = 0.99989899f;
+
+// lb <= value_s(p) for the centre c and the link's sph_rad.  + 1e-20 keeps the argument of the reciprocal square root
+// a normal number (and raises the bound by < 1e-10, inside the 1e-6 slack of the radius).  Slots beyond n_sdf: c = 0
+// and sph_rad = -inf give +inf.
+__device__ __forceinline__ float rs_sphere_lb(f3 p, float cx, float cy, float cz, float sph_rad) {
+    const float dx = p.x - cx, dy = p.y - cy, dz = p.z - cz;
+    const float d2 = fmaf(dz, dz, fmaf(dy, dy, fmaf(dx, dx, 1e-20f)));
+    return fmaf(d2 * rsqrt_approx(d2), kRsBoundScale, -sph_rad);
+}
+
 }  // namespace pvb

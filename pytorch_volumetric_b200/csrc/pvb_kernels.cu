@@ -1074,6 +1074,9 @@ template <int MAXS>
 struct RobotPack {
     pvb_sdf_desc d[MAXS];       // visiting order
     int orig[MAXS];             // visiting position -> original sub-SDF index (transforms, tie rule, out_which)
+    // robot_serial_kernel only (rs_link_consts in pvb_device.cuh): the link-only terms of its bounds, constant bank
+    float sph_rad[MAXS];        // bounding-sphere radius + prune_margin; +inf: never rejected; -inf: slot beyond n_sdf
+    float visit_margin[MAXS];   // prune_margin, +inf without PVB_GRID_PRUNE_OK: the AABB test then never rejects
 };
 
 template <int MAXS>
@@ -1394,8 +1397,16 @@ robot_query_kernel(const __grid_constant__ RobotPack<MAXS> pk, int n_sdf, const 
 // min over keys that carry the link index in their low mantissa bits (was compare + select per link), no per-link tests
 // of `point exists` / `si < n_sdf` (slots beyond n_sdf carry a +inf bound), a division-free flush index and per-lane
 // staging pointers: 640 -> 557 warp instructions per (point, 32 configurations).  What is left is L1 data-pipe
-// wavefronts (~166 per point: 32 sphere reads, ~54 transform rows, ~66 table gathers of 32 distinct sectors, 12 staging)
-// and issue slots.
+// wavefronts (~158 per point: 24 sphere-centre reads, ~54 transform rows, ~66 table gathers of 32 distinct sectors,
+// 12 staging) and issue slots.
+// The link-only terms of the bounds (sphere radius + margin, the visit's margin) sit in the constant bank
+// (RobotPack::sph_rad / visit_margin), so the per-lane shared data is the 8 centres alone: 6 LDS.128 per point instead
+// of 8, and the visits test no descriptor flags.  Tighter per-lane bounds were modelled on the host
+// (scripts/c4_bound_model.py, 64 configurations x 2e4 C4 points, per warp step): the sphere costs 3.39 warp visits,
+// 2.13 lookups per lane and 0.48 visits in which no lane passes the exact AABB test; max(sphere, slab of the thinnest
+// AABB axis) 3.30 / 2.14 / 0.39; even the exact AABB test itself as the pre-bound 2.90 / 2.11 / 0.  The slab saves
+// 0.09 visits (about 1 wavefront and 3 instructions) per point for 8 more dot products and 8 more floats per lane, so
+// the bound stays a sphere.
 constexpr int kRsWarps = 8;
 #ifndef PVB_RS_CHUNK
 #define PVB_RS_CHUNK 8
@@ -1416,21 +1427,13 @@ constexpr int kRsGradStride = 3 * kRsChunk + 1;   // 25
 
 struct __align__(16) RsSmem {
     float4 xf[kRbCfg][3 * kRsMaxS + 1];
-    float4 sph[kRbCfg][kRsMaxS + 1];
+    // object-frame centres of the lane's bounding spheres, {x, y, z} of the 8 links back to back: 6 LDS.128 (24
+    // wavefronts) per point instead of one 16-byte record per link (32); + 1 float4: odd row stride, conflict-free
+    float4 sph[kRbCfg][3 * kRsMaxS / 4 + 1];
     // per-warp staging, LC rows x (8 * 32/LC values + 1) resp. (24 * 32/LC gradient floats + 1): at most 32 x 9 / 32 x 25
     float sv[kRsWarps][kRbCfg][kRsValStride];
     float sg[kRsWarps][kRbCfg][kRsGradStride];
 };
-
-// sqrt(0.9998) * 0.999999: 0.9998 on the squared distance absorbs the 1e-5 non-rigidity tolerated below, 0.999999 the
-// approximate reciprocal square root (2 ulp) and the roundings of the three fused multiply-adds
-constexpr float kRsBoundScale = 0.99989899f;
-
-__device__ __forceinline__ float rsqrt_approx(float x) {      // one MUFU.RSQ, no denormal fix-up (callers keep x >= 1e-20)
-    float r;
-    asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-    return r;
-}
 
 // (configuration tiles and the flush index arithmetic: rs_tile / rs_flush_piece in pvb_device.cuh, checked on the CPU tier)
 // kTri: some links carry PVB_GRID_TRILINEAR; each visit then picks its lookup by the link's flag (uniform across the
@@ -1469,34 +1472,16 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
         sm.xf[ci][3 * si] = __ldg(row); sm.xf[ci][3 * si + 1] = __ldg(row + 1); sm.xf[ci][3 * si + 2] = __ldg(row + 2);
     }
     __syncthreads();
-    // ---- bounding spheres (object frame) of every (configuration, link) of the tile ----
+    // ---- bounding-sphere centres (object frame) of every (configuration, link) of the tile (rs_sphere_centre); the
+    // radii are per link, in pk.sph_rad.  Slots beyond n_sdf: centre 0 and radius -inf, so that their bound is +inf --
+    // never the nearest, never visited ----
     for (int item = threadIdx.x; item < LC * kRsMaxS; item += blockDim.x) {
         const int ci = item & (LC - 1), si = item >> lc_log2;
-        // slots beyond n_sdf: radius -inf, so that their bound is +inf -- never the nearest, never visited
-        float4 sp = make_float4(0.f, 0.f, 0.f, -PVB_INF);
-        if (si < n_sdf) {
-            const pvb_sdf_desc &d = pk.d[si];
-            const float4 r0 = sm.xf[ci][3 * si], r1 = sm.xf[ci][3 * si + 1], r2 = sm.xf[ci][3 * si + 2];
-            // sphere around the link AABB, centre carried to the object frame: c_obj = R^T (c_link - t)
-            const f3 cen = mk3(0.5f * (d.bb_min[0] + d.bb_max[0]), 0.5f * (d.bb_min[1] + d.bb_max[1]),
-                               0.5f * (d.bb_min[2] + d.bb_max[2]));
-            const f3 hl = mk3(0.5f * (d.bb_max[0] - d.bb_min[0]), 0.5f * (d.bb_max[1] - d.bb_min[1]),
-                              0.5f * (d.bb_max[2] - d.bb_min[2]));
-            const f3 u = mk3(cen.x - r0.w, cen.y - r1.w, cen.z - r2.w);
-            const f3 co = mk3(r0.x * u.x + r1.x * u.y + r2.x * u.z, r0.y * u.x + r1.y * u.y + r2.y * u.z,
-                              r0.z * u.x + r1.z * u.y + r2.z * u.z);
-            const float rad = sqrtf(hl.x * hl.x + hl.y * hl.y + hl.z * hl.z) * 1.0001f + 1e-6f;
-            // the bound needs an isometry: |R R^T - I| must vanish, otherwise this (cfg, link) is never rejected by it
-            const float e00 = r0.x * r0.x + r0.y * r0.y + r0.z * r0.z - 1.f, e11 = r1.x * r1.x + r1.y * r1.y + r1.z * r1.z - 1.f,
-                        e22 = r2.x * r2.x + r2.y * r2.y + r2.z * r2.z - 1.f;
-            const float e01 = r0.x * r1.x + r0.y * r1.y + r0.z * r1.z, e02 = r0.x * r2.x + r0.y * r2.y + r0.z * r2.z,
-                        e12 = r1.x * r2.x + r1.y * r2.y + r1.z * r2.z;
-            const float dev = fmaxf(fmaxf(fmaxf(fabsf(e00), fabsf(e11)), fmaxf(fabsf(e22), fabsf(e01))),
-                                    fmaxf(fabsf(e02), fabsf(e12)));
-            const bool ok = (d.flags & PVB_GRID_PRUNE_OK) && dev < 1e-5f;
-            sp = make_float4(co.x, co.y, co.z, ok ? rad + d.prune_margin : PVB_INF);
-        }
-        sm.sph[ci][si] = sp;
+        const f3 co = si < n_sdf ? rs_sphere_centre(pk.d[si], sm.xf[ci][3 * si], sm.xf[ci][3 * si + 1],
+                                                    sm.xf[ci][3 * si + 2])
+                                 : mk3(0.f, 0.f, 0.f);
+        float *c = reinterpret_cast<float *>(&sm.sph[ci][0]) + 3 * si;
+        c[0] = co.x; c[1] = co.y; c[2] = co.z;
     }
     __syncthreads();
     // Staging tile.  One destination in local memory (kDest 0): every warp owns a tile of LC rows x its own
@@ -1528,17 +1513,18 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
             const bool on = pt < n_pts;
             if (!full && !__any_sync(0xffffffffu, on)) break;
             const f3 p = on ? load_point(pts, pt) : mk3(0.f, 0.f, 0.f);     // the same for the LC lanes of a point group
-            // ---- lower bounds of every link's value from its bounding sphere: value_s >= |p - c_s| - radius_s.
-            // 0.9998 absorbs the 1e-5 non-rigidity tolerated above, 0.999999 the approximate reciprocal square root
-            // (2 ulp); + 1e-20 keeps its argument a normal number (and raises the bound by < 1e-10, inside the 1e-5
-            // slack of the radius).  radius = inf (bound not valid) gives -inf: never rejected.
+            // ---- lower bounds of every link's value from its bounding sphere (rs_sphere_lb): value_s >= lb_s.
+            // radius = inf (bound not valid) gives -inf, a NaN centre (not an isometry) NaN: never rejected.
+            float cen[3 * kRsMaxS];
+#pragma unroll
+            for (int j = 0; j < 3 * kRsMaxS / 4; ++j) {
+                const float4 c4 = sm.sph[cl][j];
+                cen[4 * j] = c4.x; cen[4 * j + 1] = c4.y; cen[4 * j + 2] = c4.z; cen[4 * j + 3] = c4.w;
+            }
             float lb[kRsMaxS], key[kRsMaxS];
 #pragma unroll
             for (int si = 0; si < kRsMaxS; ++si) {
-                const float4 sp = sm.sph[cl][si];
-                const float dx = p.x - sp.x, dy = p.y - sp.y, dz = p.z - sp.z;
-                const float d2 = fmaf(dz, dz, fmaf(dy, dy, fmaf(dx, dx, 1e-20f)));
-                lb[si] = fmaf(d2 * rsqrt_approx(d2), kRsBoundScale, -sp.w);
+                lb[si] = rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], pk.sph_rad[si]);
                 key[si] = rs_bound_key(lb[si], low3_off, si);       // link index in the 3 low mantissa bits
             }
             // one visiting order per point group: its first lane's nearest sphere (neighbouring configurations agree;
@@ -1547,27 +1533,29 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
             float best = PVB_INF;
             f3 bg = mk3(0.f, 0.f, 0.f);
             int bs = -1;
-            // one link: transform, AABB bound against the running minimum, nearest-voxel lookup, running argmin
-            auto visit = [&](const pvb_sdf_desc &d, const int si) {
+            // one link: transform, AABB bound against the running minimum, nearest-voxel lookup, running argmin.  The
+            // first visit (nothing evaluated yet) always looks up and takes the result; every later one has bs >= 0.
+            // visit_margin is +inf for a link without PVB_GRID_PRUNE_OK, so the AABB test never rejects it.
+            auto visit = [&](const pvb_sdf_desc &d, const int si, const bool first) {
                 const float4 r0 = sm.xf[cl][3 * si], r1 = sm.xf[cl][3 * si + 1], r2 = sm.xf[cl][3 * si + 2];
                 const f3 q = composed_xform(r0, r1, r2, p);
-                if ((d.flags & PVB_GRID_PRUNE_OK) && bs >= 0) {
-                    const float thr = best + d.prune_margin;
+                if (!first) {
+                    const float thr = best + pk.visit_margin[si];
                     if (thr < 0.f || composed_aabb_lb2(d, q) > thr * thr) return;
                 }
                 const float4 o = (kTri && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
                                                                            : robot_lookup(d, q);
-                if (bs < 0 || o.x < best || (o.x == best && si < bs)) {
+                if (first || o.x < best || (o.x == best && si < bs)) {
                     best = o.x; bg = mk3(o.y, o.z, o.w); bs = si;
                 }
             };
             // (lanes past the last point work on p = 0 and are not stored: no `on` in the conditions below)
-            visit(pk.d[pred], pred);
+            visit(pk.d[pred], pred, true);
 #pragma unroll
             for (int si = 0; si < kRsMaxS; ++si) {
                 // reject when the sphere bound already exceeds the running minimum (exact: lb <= value); best is finite
                 // after the first visit, so the +inf bound of a slot beyond n_sdf never passes
-                if (si != pred && !(lb[si] > best)) visit(pk.d[si], si);
+                if (si != pred && !(lb[si] > best)) visit(pk.d[si], si, false);
             }
             // (Rotating the gradient inside the visit, while the rows are in registers, saves these 3 LDS.128 -- 12 of the
             // ~166 L1 wavefronts a point costs -- but runs the 9 multiply-adds once per visit instead of once per point.)
@@ -2343,6 +2331,10 @@ static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float
     RobotPack<kRsMaxS> pack;
     memset(&pack, 0, sizeof(pack));
     for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
+    for (int si = 0; si < kRsMaxS; ++si) {
+        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
+        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
+    }
     const int kind = !tg ? 0 : (tg->mc ? 2 : 1);
     auto k0 = tri ? robot_serial_kernel<0, true> : robot_serial_kernel<0, false>;
     auto k1 = tri ? robot_serial_kernel<1, true> : robot_serial_kernel<1, false>;
