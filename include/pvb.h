@@ -37,8 +37,11 @@ typedef enum pvb_status {
     PVB_ERR_CAPACITY = -3   /* caller-provided buffer too small */
 } pvb_status;
 
-/* sub-SDF kinds understood by the fused kernels */
-enum { PVB_KIND_GRID = 0, PVB_KIND_MESH = 1, PVB_KIND_SPHERE = 2 };
+/* sub-SDF kinds understood by the fused kernels.  BOX and CYLINDER are an EXTENSION (not reference behaviour): the
+ * analytic URDF primitives, exact Euclidean SDFs centred at the origin (pvb_device.cuh box_eval / cylinder_eval).
+ * Honoured by pvb_composed_query, _paired, _multi, _multicast (where the point-serial robot kernel runs, see
+ * PVB_GRID_TRILINEAR) and pvb_chamfer.  Every entry point taking descriptors refuses a kind outside 0..4. */
+enum { PVB_KIND_GRID = 0, PVB_KIND_MESH = 1, PVB_KIND_SPHERE = 2, PVB_KIND_BOX = 3, PVB_KIND_CYLINDER = 4 };
 
 /* pvb_sdf_desc.flags */
 enum {
@@ -47,12 +50,15 @@ enum {
     PVB_GRID_OOB_GT     = 1u << 1, /* OutOfBoundsStrategy.LOOKUP_GT_SDF: out-of-range points take the
                                       mesh query (mesh fields must be filled); default BOUNDING_BOX */
     PVB_GRID_PRUNE_OK   = 1u << 2, /* table verified to satisfy val >= dist(voxel centre, bb) - prune_margin:
-                                      composed kernels may skip lookups that provably cannot win the min */
+                                      composed kernels may skip lookups that provably cannot win the min.  On
+                                      SPHERE / BOX / CYLINDER: the same bound holds for the primitive and its
+                                      bb_min / bb_max (prune_margin = inradius + fp32 slack) */
     PVB_GRID_TRILINEAR  = 1u << 4, /* EXTENSION (not reference behaviour): value = trilinear interpolation of the
                                       8 surrounding voxel values, gradient = analytic gradient of that interpolant
                                       (cell-wise finite differences).  Honoured by pvb_grid_lookup,
                                       pvb_composed_query, pvb_composed_query_multi and (where the point-serial
-                                      robot kernel runs: <= 8 GRID sub-SDFs, >= PVB_ROBOT_MIN_CFG configurations)
+                                      robot kernel runs: <= 8 GRID or primitive sub-SDFs, >= PVB_ROBOT_MIN_CFG
+                                      configurations)
                                       pvb_composed_query_multicast; needs the bounding-box rule (not
                                       PVB_GRID_OOB_GT).  pvb_chamfer rejects it (PVB_ERR_INVALID). */
     PVB_MESH_CLOSED     = 1u << 3  /* every directed edge is matched by its reverse (closed, consistently oriented
@@ -82,7 +88,11 @@ enum {
  * MESH part  = ObjectFactory state (sdf.py:115-120): BVH4 nodes + leaf-ordered
  *              triangles from pvb_bvh_build, fp32 face normals in ORIGINAL
  *              face order, ray "destination" bbox(padding=1.0).max (sdf.py:147).
- * SPHERE     = SphereSDF radius (sdf.py:285-299).
+ * SPHERE     = SphereSDF radius (sdf.py:285-299); bb_min / bb_max = -/+radius.
+ * BOX        = EXTENSION: half extents h in bb_max, bb_min = -h.
+ * CYLINDER   = EXTENSION: axis along z, radius in `radius`, bb_min / bb_max = (-r, -r, -h) / (r, r, h) with h the
+ *              half length.
+ * Primitives set PVB_GRID_PRUNE_OK with prune_margin = inradius (sphere r, box min h, cylinder min(r, h)) + slack.
  */
 typedef struct pvb_sdf_desc {
     int32_t kind;
@@ -97,7 +107,7 @@ typedef struct pvb_sdf_desc {
     float res32[3];
     float valid_lo[3];          /* inclusive fp32 bounds equivalent to all(min <= p <= max) */
     float valid_hi[3];
-    float bb_min[3];            /* surface AABB, fp32 */
+    float bb_min[3];            /* surface AABB, fp32 (primitives: their box, see above) */
     float bb_max[3];
     float prune_margin;         /* see PVB_GRID_PRUNE_OK */
     /* ---- mesh ---- */
@@ -108,7 +118,7 @@ typedef struct pvb_sdf_desc {
     int32_t n_tris;
     float ray_far[3];
     uint32_t ray_seed;          /* seed of the deterministic stand-in for sdf.py:149's jitter */
-    /* ---- sphere ---- */
+    /* ---- sphere, cylinder ---- */
     float radius;
     /* ---- grid: fast index path ----
      * k = rintf((p - min32) * inv_res32) is taken as the voxel index when |q - k| <= idx_certain (the fp32
@@ -226,7 +236,8 @@ int pvb_composed_query_multi(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
  * mc_val / mc_grad are multicast addresses (cuMulticast* / torch symmetric memory) of the full-size result buffers,
  * already advanced to the slab: the kernel epilogue issues one multimem.st per 16-byte chunk and the NVSwitch
  * replicates it into every bound GPU's buffer (the sender emits each byte once instead of once per peer).  Needs
- * <= 16 GRID sub-SDFs with the bounding-box out-of-range rule (a RobotSDF of cached links). */
+ * <= 16 GRID sub-SDFs with the bounding-box out-of-range rule (a RobotSDF of cached links); sets with trilinear or
+ * primitive sub-SDFs only where the point-serial robot kernel runs (<= 8 sub-SDFs, >= PVB_ROBOT_MIN_CFG configurations). */
 int pvb_composed_query_multicast(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh, const float *xforms,
                                  int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
                                  const float *pts, int64_t n_pts, uint32_t mesh_mode,

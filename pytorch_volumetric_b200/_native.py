@@ -20,7 +20,7 @@ HEADERS = ["pvb_device.cuh", os.path.join("..", "..", "include", "pvb.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
-PVB_KIND_GRID, PVB_KIND_MESH, PVB_KIND_SPHERE = 0, 1, 2
+PVB_KIND_GRID, PVB_KIND_MESH, PVB_KIND_SPHERE, PVB_KIND_BOX, PVB_KIND_CYLINDER = 0, 1, 2, 3, 4
 PVB_GRID_INDEX_FP32, PVB_GRID_OOB_GT, PVB_GRID_PRUNE_OK, PVB_MESH_CLOSED, PVB_GRID_TRILINEAR = 1, 2, 4, 8, 16
 PVB_MESH_SIGNED, PVB_MESH_SURFACE_NORMAL, PVB_MESH_DEFAULT, PVB_MESH_WINDING = 1, 2, 3, 4
 

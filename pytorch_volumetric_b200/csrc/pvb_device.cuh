@@ -607,6 +607,73 @@ __device__ __forceinline__ SdfOut sphere_eval(float radius, f3 p) {   // sdf.py:
     return o;
 }
 
+// ----------------------------------------------------------------------------
+// EXTENSION (not reference behaviour; the reference skips non-mesh URDF visuals): analytic URDF primitives, centred at
+// the origin, exact Euclidean SDF.  Every operation is an explicit fmaf / _rn intrinsic or cannot be contracted, so
+// the host build (-ffp-contract=off) gives the same bits as the device.
+//
+// BOX (PVB_KIND_BOX): half extents h = bb_max (bb_min = -h), e = |q| - h per axis.
+//   outside (|max(e, 0)| > 0): value |max(e, 0)|, gradient the unit vector from the closest box point to q,
+//     (sign(q_k) max(e_k, 0)) / value;
+//   inside or on the surface: value max_k e_k, gradient s e_k for that axis -- the FIRST axis on ties -- with
+//     s = q_k >= 0 ? +1 : -1 (-0 counts as +).
+__device__ __forceinline__ SdfOut box_eval(const pvb_sdf_desc &d, f3 q) {
+    const float ex = __fsub_rn(fabsf(q.x), d.bb_max[0]), ey = __fsub_rn(fabsf(q.y), d.bb_max[1]),
+                ez = __fsub_rn(fabsf(q.z), d.bb_max[2]);
+    const float wx = fmaxf(ex, 0.f), wy = fmaxf(ey, 0.f), wz = fmaxf(ez, 0.f);
+    const float w2 = fmaf(wx, wx, fmaf(wy, wy, __fmul_rn(wz, wz)));
+    SdfOut o;
+    if (w2 > 0.f) {
+        const float dist = sqrtf(w2);
+        o.val = dist;
+        o.grad = mk3(copysignf(__fdiv_rn(wx, dist), q.x), copysignf(__fdiv_rn(wy, dist), q.y),
+                     copysignf(__fdiv_rn(wz, dist), q.z));
+        return o;
+    }
+    // (also when max(e, 0) is nonzero but its square underflows: value max_k e_k, a few 1e-20 at most)
+    int k = 0;
+    float m = ex;
+    if (ey > m) { m = ey; k = 1; }
+    if (ez > m) { m = ez; k = 2; }
+    o.val = m;
+    o.grad = mk3(k == 0 ? (q.x >= 0.f ? 1.f : -1.f) : 0.f, k == 1 ? (q.y >= 0.f ? 1.f : -1.f) : 0.f,
+                 k == 2 ? (q.z >= 0.f ? 1.f : -1.f) : 0.f);
+    return o;
+}
+
+// CYLINDER (PVB_KIND_CYLINDER): axis along local z, radius r = radius, half length h = bb_max[2].  rho = |(x, y)|,
+// radial unit u = (x, y) / rho, or (1, 0) when rho = 0; d = (rho - r, |z| - h); sz = z >= 0 ? +1 : -1.
+//   outside (|max(d, 0)| > 0): w = max(d, 0), value |w|, gradient (w_0 u, w_1 sz) / |w|;
+//   inside or on the surface: value max(d), gradient (u, 0) when d_0 >= d_1 (radial wins ties), else (0, 0, sz).
+__device__ __forceinline__ SdfOut cylinder_eval(const pvb_sdf_desc &d, f3 q) {
+    const float rho = sqrtf(fmaf(q.x, q.x, __fmul_rn(q.y, q.y)));
+    const float ux = rho > 0.f ? __fdiv_rn(q.x, rho) : 1.f, uy = rho > 0.f ? __fdiv_rn(q.y, rho) : 0.f;
+    const float sz = q.z >= 0.f ? 1.f : -1.f;
+    const float dr = __fsub_rn(rho, d.radius), dz = __fsub_rn(fabsf(q.z), d.bb_max[2]);
+    const float wr = fmaxf(dr, 0.f), wz = fmaxf(dz, 0.f);
+    const float w2 = fmaf(wr, wr, __fmul_rn(wz, wz));
+    SdfOut o;
+    if (w2 > 0.f) {
+        const float dist = sqrtf(w2);
+        const float a = __fdiv_rn(wr, dist);
+        o.val = dist;
+        o.grad = mk3(__fmul_rn(a, ux), __fmul_rn(a, uy), __fmul_rn(__fdiv_rn(wz, dist), sz));
+        return o;
+    }
+    const bool radial = dr >= dz;
+    o.val = radial ? dr : dz;
+    o.grad = radial ? mk3(ux, uy, 0.f) : mk3(0.f, 0.f, sz);
+    return o;
+}
+
+// SPHERE / BOX / CYLINDER descriptor at q (in its own frame).  Any other kind is evaluated as a sphere: the entry
+// points refuse kinds outside PVB_KIND_GRID .. PVB_KIND_CYLINDER, and GRID / MESH never reach this function.
+__device__ __forceinline__ SdfOut primitive_eval(const pvb_sdf_desc &d, f3 q) {
+    if (d.kind == PVB_KIND_BOX) return box_eval(d, q);
+    if (d.kind == PVB_KIND_CYLINDER) return cylinder_eval(d, q);
+    return sphere_eval(d.radius, q);
+}
+
 
 // ----------------------------------------------------------------------------
 // Composition primitives shared by the point-major and the configuration-major kernels (ComposedSDF.__call__,
@@ -639,20 +706,23 @@ __device__ __forceinline__ f3 composed_rotate_back(const float4 &r0, const float
 // (best, bg, bs) of one point; bs < 0 = nothing evaluated yet.  Skipped without touching its table / tree when
 // provably not the argmin: value >= dist(q, box) - prune_margin (measured on the table for grids, fp32 slack for
 // closed meshes).  torch.argmin semantics (sdf.py:421): smallest value, first index on ties -- whatever the
-// visiting order.  kTri: GRID descriptors with PVB_GRID_TRILINEAR are evaluated through grid_trilinear_eval (a
-// template flag, so that the nearest-voxel instantiations carry no code for the opt-in mode).
-template <bool kMesh, bool kTri = false>
+// visiting order.  kExt: the extension kinds are present -- GRID descriptors with PVB_GRID_TRILINEAR are evaluated
+// through grid_trilinear_eval, SPHERE / BOX / CYLINDER through primitive_eval and pruned by the grid rule (their
+// PVB_GRID_PRUNE_OK means the same bound holds).  A template flag, so that the nearest-voxel instantiations carry no
+// code for the opt-in modes.
+template <bool kMesh, bool kExt = false>
 __device__ __forceinline__ void composed_consider(const pvb_sdf_desc &d, const NodeStage &st, int s, f3 q,
                                                   uint32_t mesh_mode, uint64_t idx, float &best, f3 &bg, int &bs) {
     SdfOut o;
-    if (d.kind == PVB_KIND_GRID) {
+    if (d.kind == PVB_KIND_GRID || (kExt && d.kind != PVB_KIND_MESH)) {
         if ((d.flags & PVB_GRID_PRUNE_OK) && bs >= 0) {
             const float thr = best + d.prune_margin;
             if (thr < 0.f || composed_aabb_lb2(d, q) > thr * thr) return;
         }
         // (the bound holds for the interpolant too: it is a convex combination of 8 corner values, and the weighted
         // mean distance of q to those corners is at most half a cell diagonal -- tests/test_trilinear_composed_cpu.py)
-        if (kTri && (d.flags & PVB_GRID_TRILINEAR)) o = grid_trilinear_eval(d, q);
+        if (kExt && d.kind != PVB_KIND_GRID) o = primitive_eval(d, q);
+        else if (kExt && (d.flags & PVB_GRID_TRILINEAR)) o = grid_trilinear_eval(d, q);
         else o = grid_eval<kMesh, true>(d, st, q, mesh_mode, idx, nullptr);
     } else if (kMesh && d.kind == PVB_KIND_MESH) {
         // closed mesh, query outside its AABB: the value is +distance >= dist(q, AABB), so (a) skip it when that
@@ -693,7 +763,7 @@ __device__ __forceinline__ void composed_consider(const pvb_sdf_desc &d, const N
 //   nearest_first / margin_max: see below (kMesh only)
 struct ComposedOut { float val; f3 grad; int which; };
 
-template <bool kMesh, bool kTri, class LoadXf>
+template <bool kMesh, bool kExt, class LoadXf>
 __device__ __forceinline__ ComposedOut composed_point(const pvb_sdf_desc *descs, const unsigned char *order, int n_sdf,
                                                       const LoadXf &load_xf, const NodeStage &st, f3 p,
                                                       uint32_t mesh_mode, uint64_t pair, int nearest_first,
@@ -720,8 +790,9 @@ __device__ __forceinline__ ComposedOut composed_point(const pvb_sdf_desc *descs,
                 const pvb_sdf_desc &d = descs[s];
                 float4 r0, r1, r2;
                 load_xf(s, r0, r1, r2);
-                const bool bounded = d.kind == PVB_KIND_GRID ? (d.flags & PVB_GRID_PRUNE_OK) != 0
-                                     : (d.kind == PVB_KIND_MESH && (d.flags & PVB_MESH_CLOSED) && (mesh_mode & PVB_MESH_SIGNED));
+                const bool bounded = (d.kind == PVB_KIND_GRID || (kExt && d.kind != PVB_KIND_MESH))
+                                         ? (d.flags & PVB_GRID_PRUNE_OK) != 0
+                                         : (d.kind == PVB_KIND_MESH && (d.flags & PVB_MESH_CLOSED) && (mesh_mode & PVB_MESH_SIGNED));
                 key[s] = bounded ? composed_aabb_lb2(d, composed_xform(r0, r1, r2, p)) : -1.f;
             }
             while (todo) {
@@ -744,7 +815,7 @@ __device__ __forceinline__ ComposedOut composed_point(const pvb_sdf_desc *descs,
                 }
                 float4 r0, r1, r2;
                 load_xf(s, r0, r1, r2);
-                composed_consider<kMesh, kTri>(d, st, s, composed_xform(r0, r1, r2, p), mesh_mode,
+                composed_consider<kMesh, kExt>(d, st, s, composed_xform(r0, r1, r2, p), mesh_mode,
                                                pair * (uint64_t)n_sdf + (uint64_t)s, best, bg, bs);
             }
         }
@@ -753,7 +824,7 @@ __device__ __forceinline__ ComposedOut composed_point(const pvb_sdf_desc *descs,
         const int s = order[si];
         float4 r0, r1, r2;
         load_xf(s, r0, r1, r2);
-        composed_consider<kMesh, kTri>(descs[s], st, s, composed_xform(r0, r1, r2, p), mesh_mode,
+        composed_consider<kMesh, kExt>(descs[s], st, s, composed_xform(r0, r1, r2, p), mesh_mode,
                                        pair * (uint64_t)n_sdf + (uint64_t)s, best, bg, bs);
     }
     float4 r0, r1, r2;

@@ -68,7 +68,7 @@ static int sm_count() {
 // id; returns false when the runtime refuses.
 enum { kSlotMesh = 0, kSlotGridTma, kSlotCfgMajor, kSlotCfgMajorMulti, kSlotChamfer, kSlotRobot, kSlotRobotMulti,
        kSlotRobotMc, kSlotRobotWide, kSlotRobotWideMulti, kSlotRobotWideMc, kSlotSerial, kSlotSerialMulti, kSlotSerialMc,
-       kSlotSerialTri, kSlotSerialTriMulti, kSlotSerialTriMc, kSlotCfgMajorTri, kSlotCfgMajorTriMulti, kSlotCount };
+       kSlotSerialExt, kSlotSerialExtMulti, kSlotSerialExtMc, kSlotCfgMajorExt, kSlotCfgMajorExtMulti, kSlotCount };
 template <typename K>
 static bool ensure_smem(K kernel, int slot, int bytes) {
     static unsigned char done[kSlotCount][kMaxDevices] = {{0}};
@@ -679,7 +679,7 @@ struct OutTargets {
     int mc;         // val[0] / grad[0] are MULTICAST addresses (NVLS): one multimem.st reaches every bound GPU
 };
 
-template <bool kMesh, int PTS, int MAXS, bool kMulti, bool kTri>
+template <bool kMesh, int PTS, int MAXS, bool kMulti, bool kExt>
 __global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : (PTS > 1 ? PVB_COMP_MINB : 1)))
 composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
                       int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long first_pt,
@@ -752,8 +752,9 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
                         const pvb_sdf_desc &d = descs.d[s];
                         float4 r0, r1, r2;
                         load_xf(s, r0, r1, r2);
-                        const bool bounded = d.kind == PVB_KIND_GRID ? (d.flags & PVB_GRID_PRUNE_OK) != 0
-                                             : (d.kind == PVB_KIND_MESH && (d.flags & PVB_MESH_CLOSED) && (mesh_mode & PVB_MESH_SIGNED));
+                        const bool bounded = (d.kind == PVB_KIND_GRID || (kExt && d.kind != PVB_KIND_MESH))
+                                                 ? (d.flags & PVB_GRID_PRUNE_OK) != 0
+                                                 : (d.kind == PVB_KIND_MESH && (d.flags & PVB_MESH_CLOSED) && (mesh_mode & PVB_MESH_SIGNED));
                         key[s] = bounded ? composed_aabb_lb2(d, composed_xform(r0, r1, r2, p[0])) : -1.f;
                     }
                     while (todo) {
@@ -777,7 +778,7 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
                         float4 r0, r1, r2;
                         load_xf(s, r0, r1, r2);
                         const uint64_t idx = ((uint64_t)cfg * (uint64_t)n_pts + (uint64_t)i0) * (uint64_t)n_sdf + (uint64_t)s;
-                        composed_consider<kMesh, kTri>(d, st, s, composed_xform(r0, r1, r2, p[0]), mesh_mode, idx, best[0], bg[0], bs[0]);
+                        composed_consider<kMesh, kExt>(d, st, s, composed_xform(r0, r1, r2, p[0]), mesh_mode, idx, best[0], bg[0], bs[0]);
                     }
                 }
             }
@@ -789,7 +790,7 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
 #pragma unroll
                 for (int k = 0; k < PTS; ++k) {
                     const uint64_t idx = ((uint64_t)cfg * (uint64_t)n_pts + (uint64_t)(i0 + k)) * (uint64_t)n_sdf + (uint64_t)s;   // absolute cfg: sharding-independent jitter
-                    composed_consider<kMesh, kTri>(d, st, s, composed_xform(r0, r1, r2, p[k]), mesh_mode, idx, best[k], bg[k],
+                    composed_consider<kMesh, kExt>(d, st, s, composed_xform(r0, r1, r2, p[k]), mesh_mode, idx, best[k], bg[k],
                                                    bs[k]);
                 }
             }
@@ -841,7 +842,7 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
 // pvb_composed_query(pts[c], cfg_begin + c, 1) bit for bit.  The transform rows are read per thread with __ldg rather
 // than staged per block like composed_query_kernel does: with few points per configuration one block spans many
 // configurations, and the lanes of one configuration read the same rows (L1 broadcasts).
-template <bool kMesh, bool kTri, int MAXS>
+template <bool kMesh, bool kExt, int MAXS>
 __global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
 composed_paired_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
                        int n_cfg, int cfg_begin, const float *__restrict__ pts, long long n_pts, long long n_pairs,
@@ -857,7 +858,7 @@ composed_paired_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, 
             const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
             r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
         };
-        const ComposedOut o = composed_point<kMesh, kTri>(descs.d, descs.order, n_sdf, load_xf, st, load_point(pts, t),
+        const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st, load_point(pts, t),
                                                           mesh_mode, (uint64_t)cfg * (uint64_t)n_pts + (uint64_t)i,
                                                           nearest_first, margin_max);
         out_val[t] = o.val;
@@ -892,7 +893,7 @@ struct __align__(16) CmSmem {
     int which[kCmCfg][kCmTilePts + 1];
 };
 
-template <bool kMulti, bool kTri>
+template <bool kMulti, bool kExt>
 __global__ void __launch_bounds__(kCmCfg * kCmWarps, 3)
 composed_cfgmajor_kernel(const __grid_constant__ DescPack<kCmMaxS> descs, int n_sdf, const float *__restrict__ xforms,
                          int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_pts,
@@ -931,7 +932,8 @@ composed_cfgmajor_kernel(const __grid_constant__ DescPack<kCmMaxS> descs, int n_
                     e12 = r1.x * r2.x + r1.y * r2.y + r1.z * r2.z;
         const float dev = fmaxf(fmaxf(fmaxf(fabsf(e00), fabsf(e11)), fmaxf(fabsf(e22), fabsf(e01))),
                                 fmaxf(fabsf(e02), fabsf(e12)));
-        const bool ok = d.kind == PVB_KIND_GRID && (d.flags & PVB_GRID_PRUNE_OK) && dev < 1e-5f;
+        const bool ok = (d.kind == PVB_KIND_GRID || (kExt && d.kind != PVB_KIND_MESH)) && (d.flags & PVB_GRID_PRUNE_OK) &&
+                        dev < 1e-5f;
         if (!ok) rad = PVB_INF;
         else rad += d.prune_margin;
         sm.sph[ci][s] = make_float4(co.x, co.y, co.z, rad);
@@ -961,7 +963,7 @@ composed_cfgmajor_kernel(const __grid_constant__ DescPack<kCmMaxS> descs, int n_
 #pragma unroll
             for (int k = 0; k < kCmPts; ++k) {
                 if (!need[k]) continue;
-                composed_consider<false, kTri>(d, st, s, composed_xform(r0, r1, r2, p[k]), 0u, 0ull, best[k], bg[k], bs[k]);
+                composed_consider<false, kExt>(d, st, s, composed_xform(r0, r1, r2, p[k]), 0u, 0ull, best[k], bg[k], bs[k]);
             }
         };
         for (int si = 0; si < n_sdf; ++si) {
@@ -1134,6 +1136,14 @@ __device__ __forceinline__ float4 robot_lookup_trilinear(const pvb_sdf_desc &g, 
         return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
     }
     return robot_lookup_slow(&g, p.x, p.y, p.z);
+}
+
+// SPHERE / BOX / CYLINDER link: primitive_eval (pvb_device.cuh), the arithmetic of every other kernel.  Out of line,
+// like robot_lookup_slow: 9 inlined copies (the first visit + 8 unrolled links) would nearly double the code of the
+// kernel's extension instantiations, which trilinear robots run too.
+__device__ __noinline__ float4 robot_primitive(const pvb_sdf_desc *dp, float qx, float qy, float qz) {
+    const SdfOut o = primitive_eval(*dp, mk3(qx, qy, qz));
+    return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
 }
 
 // kDest: 0 = out_val / out_grad, 1 = every (val, grad) pair of tg, 2 = tg.val[0] / tg.grad[0] are multicast addresses
@@ -1436,10 +1446,12 @@ struct __align__(16) RsSmem {
 };
 
 // (configuration tiles and the flush index arithmetic: rs_tile / rs_flush_piece in pvb_device.cuh, checked on the CPU tier)
-// kTri: some links carry PVB_GRID_TRILINEAR; each visit then picks its lookup by the link's flag (uniform across the
-// lanes of a point group), so nearest and trilinear links mix.  The bounds are unchanged: prune_margin holds for the
-// interpolant as well.  kTri = false is the nearest-voxel kernel as it always was.
-template <int kDest, bool kTri>
+// kExt: some links carry PVB_GRID_TRILINEAR or are analytic primitives (SPHERE / BOX / CYLINDER); each visit then picks
+// its evaluation by the link's kind and flag (uniform across the lanes of a point group), so nearest, trilinear and
+// primitive links mix.  The bounds are unchanged: they read only bb_min / bb_max, prune_margin and PVB_GRID_PRUNE_OK,
+// and prune_margin holds for the interpolant and the primitives as well.  kExt = false is the nearest-voxel kernel as
+// it always was.
+template <int kDest, bool kExt>
 __global__ void __launch_bounds__(kRbCfg * kRsWarps, PVB_RS_MINB)
 robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, const float *__restrict__ xforms,
                     int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, int n_pts, int vec,
@@ -1543,8 +1555,9 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
                     const float thr = best + pk.visit_margin[si];
                     if (thr < 0.f || composed_aabb_lb2(d, q) > thr * thr) return;
                 }
-                const float4 o = (kTri && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
-                                                                           : robot_lookup(d, q);
+                const float4 o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
+                                 : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
+                                                                            : robot_lookup(d, q);
                 if (first || o.x < best || (o.x == best && si < bs)) {
                     best = o.x; bg = mk3(o.y, o.z, o.w); bs = si;
                 }
@@ -1897,7 +1910,7 @@ chamfer_partial_kernel(const pvb_sdf_desc obj, const float *__restrict__ w2o, co
         } else if (obj.kind == PVB_KIND_GRID) {
             d = grid_eval<true>(obj, st, q, PVB_MESH_DEFAULT, (uint64_t)i, nullptr).val;
         } else {
-            d = sphere_eval(obj.radius, q).val;
+            d = primitive_eval(obj, q).val;
         }
         const float sd = scale * d;
         acc = fmaf(sd, sd, acc);
@@ -2245,7 +2258,7 @@ extern "C" int pvb_sphere_query(float radius, const float *pts, int64_t n, float
     return PVB_OK;
 }
 
-template <bool kMesh, int PTS, int MAXS, bool kTri>
+template <bool kMesh, int PTS, int MAXS, bool kExt>
 static int launch_composed(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                            int cfg_count, const float *pts, long long first_pt, long long n_pts, uint32_t mesh_mode,
                            float *out_val, float *out_grad, int *out_which, const OutTargets *tg, cudaStream_t stream) {
@@ -2265,11 +2278,11 @@ static int launch_composed(const pvb_sdf_desc *descs, int n_sdf, const float *xf
     for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
     timing_mark(0, stream);
     if (tg)
-        composed_query_kernel<kMesh, PTS, MAXS, true, kTri><<<grid, kCompThreads, 0, stream>>>(
+        composed_query_kernel<kMesh, PTS, MAXS, true, kExt><<<grid, kCompThreads, 0, stream>>>(
             pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, first_pt, n_pts, mesh_mode, nullptr, nullptr,
             out_which, *tg, nearest_first, margin_max);
     else
-        composed_query_kernel<kMesh, PTS, MAXS, false, kTri><<<grid, kCompThreads, 0, stream>>>(
+        composed_query_kernel<kMesh, PTS, MAXS, false, kExt><<<grid, kCompThreads, 0, stream>>>(
             pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, first_pt, n_pts, mesh_mode, out_val, out_grad,
             out_which, OutTargets{}, nearest_first, margin_max);
     timing_mark(1, stream);
@@ -2324,10 +2337,11 @@ static int launch_robot(const pvb_sdf_desc *descs, int n_sdf, const float *xform
     return PVB_OK;
 }
 
-// Launch robot_serial_kernel (<= 8 GRID sub-SDFs with the bounding-box rule; `tri`: some of them PVB_GRID_TRILINEAR).
+// Launch robot_serial_kernel (<= 8 GRID sub-SDFs with the bounding-box rule or primitives; `ext`: some of them
+// PVB_GRID_TRILINEAR or primitives).
 static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                                int cfg_count, const float *pts, long long n_pts, int vec, float *out_val,
-                               float *out_grad, int *out_which, const OutTargets *tg, bool tri, cudaStream_t stream) {
+                               float *out_grad, int *out_which, const OutTargets *tg, bool ext, cudaStream_t stream) {
     RobotPack<kRsMaxS> pack;
     memset(&pack, 0, sizeof(pack));
     for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
@@ -2336,11 +2350,11 @@ static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float
         else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
     }
     const int kind = !tg ? 0 : (tg->mc ? 2 : 1);
-    auto k0 = tri ? robot_serial_kernel<0, true> : robot_serial_kernel<0, false>;
-    auto k1 = tri ? robot_serial_kernel<1, true> : robot_serial_kernel<1, false>;
-    auto k2 = tri ? robot_serial_kernel<2, true> : robot_serial_kernel<2, false>;
+    auto k0 = ext ? robot_serial_kernel<0, true> : robot_serial_kernel<0, false>;
+    auto k1 = ext ? robot_serial_kernel<1, true> : robot_serial_kernel<1, false>;
+    auto k2 = ext ? robot_serial_kernel<2, true> : robot_serial_kernel<2, false>;
     const int smem = (int)sizeof(RsSmem);
-    const int slot0 = tri ? kSlotSerialTri : kSlotSerial;
+    const int slot0 = ext ? kSlotSerialExt : kSlotSerial;
     if (!ensure_smem(k0, slot0, smem) || !ensure_smem(k1, slot0 + 1, smem) || !ensure_smem(k2, slot0 + 2, smem)) {
         pvb_set_error("pvb_composed_query: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
         return PVB_ERR_CUDA;
@@ -2380,11 +2394,11 @@ static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float
     return PVB_OK;
 }
 
-// Argument checks shared by the composed entry points (`fn` names the entry point in the error message); any_tri:
-// some sub-SDF is PVB_GRID_TRILINEAR.
+// Argument checks shared by the composed entry points (`fn` names the entry point in the error message); any_ext:
+// some sub-SDF is PVB_GRID_TRILINEAR or a primitive (SPHERE / BOX / CYLINDER), so the kExt instantiations run.
 static int composed_check_args(const char *fn, const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,
                                int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count, const float *pts, int64_t n_pts,
-                               const float *out_val, const float *out_grad, bool &any_tri) {
+                               const float *out_val, const float *out_grad, bool &any_ext) {
     if (!descs || !xforms || n_sdf < 1 || n_cfg < 1 || cfg_begin < 0 || cfg_count < 0 ||
         cfg_begin + cfg_count > n_cfg || n_pts < 0 || (n_pts > 0 && cfg_count > 0 && (!pts || !out_val || !out_grad))) {
         pvb_set_error("%s: invalid argument (n_sdf=%d n_cfg=%d cfg=[%d,+%d) n_pts=%lld)", fn, n_sdf, n_cfg,
@@ -2395,14 +2409,19 @@ static int composed_check_args(const char *fn, const pvb_sdf_desc *descs, int32_
         pvb_set_error("%s: at most 128 sub-SDFs per call (got %d)", fn, n_sdf);
         return PVB_ERR_INVALID;
     }
-    any_tri = false;
+    any_ext = false;
     for (int i = 0; i < n_sdf; ++i) {
+        if (descs[i].kind < PVB_KIND_GRID || descs[i].kind > PVB_KIND_CYLINDER) {
+            pvb_set_error("%s: sub-SDF %d: unknown kind %d", fn, i, descs[i].kind);
+            return PVB_ERR_INVALID;
+        }
+        if (descs[i].kind != PVB_KIND_MESH && descs[i].kind != PVB_KIND_GRID) any_ext = true;
         if (descs[i].kind != PVB_KIND_GRID || !(descs[i].flags & PVB_GRID_TRILINEAR)) continue;
         if (descs[i].flags & PVB_GRID_OOB_GT) {
             pvb_set_error("%s: sub-SDF %d: PVB_GRID_TRILINEAR supports the bounding-box rule only", fn, i);
             return PVB_ERR_INVALID;
         }
-        any_tri = true;
+        any_ext = true;
     }
     return PVB_OK;
 }
@@ -2412,9 +2431,9 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
                              int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count, const float *pts, int64_t n_pts,
                              uint32_t mesh_mode, float *out_val, float *out_grad, int32_t *out_which,
                              const OutTargets *tg, void *stream) {
-    bool any_tri;
+    bool any_ext;
     const int bad = composed_check_args("pvb_composed_query", descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,
-                                        n_pts, out_val, out_grad, any_tri);
+                                        n_pts, out_val, out_grad, any_ext);
     if (bad) return bad;
     if (n_pts == 0 || cfg_count == 0) return PVB_OK;
     cudaStream_t s = (cudaStream_t)stream;
@@ -2430,23 +2449,24 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
     }
     static const int cfg_major = [] { const char *e = getenv("PVB_COMP_CFGMAJOR"); return e ? atoi(e) : 1; }();
     static const int robot_kernel = [] { const char *e = getenv("PVB_ROBOT_KERNEL"); return e ? atoi(e) : 2; }();
-    // every sub-SDF a GRID with the bounding-box rule (nearest or trilinear): the robot kernels' precondition
+    // every sub-SDF a GRID with the bounding-box rule (nearest or trilinear) or a primitive: the robot kernels'
+    // precondition (primitives and trilinear grids then need the serial kernel, see serial_taken)
     bool all_grid = !needs_mesh && n_sdf <= 16 && n_pts < (1ll << 31);
     for (int i = 0; i < n_sdf && all_grid; ++i)
-        all_grid = descs[i].kind == PVB_KIND_GRID && !(descs[i].flags & PVB_GRID_OOB_GT);
+        all_grid = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
     // the point-serial kernel has no fill problem (remainder configurations run in lane-split tiles): any batch of
     // PVB_ROBOT_MIN_CFG or more configurations takes it
     static const int serial_min_cfg = [] { const char *e = getenv("PVB_ROBOT_MIN_CFG"); return e ? atoi(e) : 8; }();
     const bool serial_ok = robot_kernel >= 2 && n_sdf <= kRsMaxS && cfg_count >= serial_min_cfg &&
                            cfg_count <= 65535 * kRbCfg;          // one grid row per 32-configuration tile
-    // sets with trilinear links take the serial kernel where nearest sets would; robot_query_kernel (9-16 links) is
-    // nearest-voxel only, so otherwise they fall through to the configuration-major or point-major kernel
+    // sets with trilinear or primitive links take the serial kernel where nearest sets would; robot_query_kernel (9-16
+    // links) is nearest-voxel only, so otherwise they fall through to the configuration-major or point-major kernel
     const bool serial_taken = robot_kernel && cfg_major && all_grid && serial_ok;
     if (tg && tg->mc) {
         // multicast destinations exist only in the robot kernels: refuse anything that would fall through
-        if (!all_grid || (any_tri && !serial_taken)) {
-            pvb_set_error(any_tri ? "pvb_composed_query_multicast: trilinear sub-SDFs need <= %d GRID sub-SDFs with the "
-                                    "bounding-box rule and >= PVB_ROBOT_MIN_CFG configurations"
+        if (!all_grid || (any_ext && !serial_taken)) {
+            pvb_set_error(any_ext ? "pvb_composed_query_multicast: trilinear and primitive sub-SDFs need <= %d GRID "
+                                    "(bounding-box rule) or primitive sub-SDFs and >= PVB_ROBOT_MIN_CFG configurations"
                                   : "pvb_composed_query_multicast: needs <= 16 GRID sub-SDFs with the bounding-box rule",
                           kRsMaxS);
             return PVB_ERR_INVALID;
@@ -2470,8 +2490,8 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
     if (serial_taken)
         return launch_robot_serial(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,
                                    (tg ? tg->vec : (out_aligned && (n_pts % 4 == 0))), out_val, out_grad, out_which,
-                                   tg, any_tri, s);
-    if (robot_kernel && cfg_major && all_grid && !any_tri && rb_filled) {
+                                   tg, any_ext, s);
+    if (robot_kernel && cfg_major && all_grid && !any_ext && rb_filled) {
         const int vec_rows = (tg ? tg->vec : (out_aligned && (n_pts % 4 == 0))) && aligned16(pts);
         return n_sdf <= 8 ? launch_robot<8, true>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, vec_rows,
                                                   out_val, out_grad, out_which, tg, s)
@@ -2479,9 +2499,9 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
                                                     vec_rows, out_val, out_grad, out_which, tg, s);
     }
     if (cfg_major && !needs_mesh && n_sdf <= kCmMaxS && cm_filled) {
-        auto kl = any_tri ? composed_cfgmajor_kernel<false, true> : composed_cfgmajor_kernel<false, false>;
-        auto km = any_tri ? composed_cfgmajor_kernel<true, true> : composed_cfgmajor_kernel<true, false>;
-        const int slot = any_tri ? kSlotCfgMajorTri : kSlotCfgMajor;
+        auto kl = any_ext ? composed_cfgmajor_kernel<false, true> : composed_cfgmajor_kernel<false, false>;
+        auto km = any_ext ? composed_cfgmajor_kernel<true, true> : composed_cfgmajor_kernel<true, false>;
+        const int slot = any_ext ? kSlotCfgMajorExt : kSlotCfgMajor;
         if (!ensure_smem(kl, slot, (int)sizeof(CmSmem)) || !ensure_smem(km, slot + 1, (int)sizeof(CmSmem))) {
             pvb_set_error("pvb_composed_query: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
             return PVB_ERR_CUDA;
@@ -2511,7 +2531,7 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
                                                        N, mesh_mode, out_val, out_grad, out_which, tg, s)          \
                  : launch_composed<MESH, PTS, 128, TRI>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, FIRST, \
                                                         N, mesh_mode, out_val, out_grad, out_which, tg, s))
-#define PVB_COMP_ANY(MESH, PTS, FIRST, N) (any_tri ? PVB_COMP(MESH, PTS, FIRST, N, true) : PVB_COMP(MESH, PTS, FIRST, N, false))
+#define PVB_COMP_ANY(MESH, PTS, FIRST, N) (any_ext ? PVB_COMP(MESH, PTS, FIRST, N, true) : PVB_COMP(MESH, PTS, FIRST, N, false))
     if (n_vec > 0) {
         rc = PVB_COMP_ANY(false, PVB_COMP_PTS, 0, n_pts);
     } else if (needs_mesh) {
@@ -2532,7 +2552,7 @@ extern "C" int pvb_composed_query(const pvb_sdf_desc *descs, int32_t n_sdf, int3
                              out_val, out_grad, out_which, nullptr, stream);
 }
 
-template <bool kMesh, bool kTri, int MAXS>
+template <bool kMesh, bool kExt, int MAXS>
 static int launch_paired(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                          const float *pts, long long n_pts, long long n_pairs, uint32_t mesh_mode, float *out_val,
                          float *out_grad, int *out_which, cudaStream_t stream) {
@@ -2544,7 +2564,7 @@ static int launch_paired(const pvb_sdf_desc *descs, int n_sdf, const float *xfor
     float margin_max = 0.f;
     for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
     timing_mark(0, stream);
-    composed_paired_kernel<kMesh, kTri, MAXS><<<grid_for(n_pairs, kCompThreads, 8), kCompThreads, 0, stream>>>(
+    composed_paired_kernel<kMesh, kExt, MAXS><<<grid_for(n_pairs, kCompThreads, 8), kCompThreads, 0, stream>>>(
         pack, n_sdf, xforms, n_cfg, cfg_begin, pts, n_pts, n_pairs, mesh_mode, out_val, out_grad, out_which,
         nearest_first, margin_max);
     timing_mark(1, stream);
@@ -2556,9 +2576,9 @@ extern "C" int pvb_composed_query_paired(const pvb_sdf_desc *descs, int32_t n_sd
                                          const float *xforms, int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
                                          const float *pts, int64_t n_pts, uint32_t mesh_mode, float *out_val,
                                          float *out_grad, int32_t *out_which, void *stream) {
-    bool any_tri;
+    bool any_ext;
     const int bad = composed_check_args("pvb_composed_query_paired", descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count,
-                                        pts, n_pts, out_val, out_grad, any_tri);
+                                        pts, n_pts, out_val, out_grad, any_ext);
     if (bad) return bad;
     if (n_pts == 0 || cfg_count == 0) return PVB_OK;
     if (n_pts > INT64_MAX / cfg_count) {
@@ -2573,8 +2593,8 @@ extern "C" int pvb_composed_query_paired(const pvb_sdf_desc *descs, int32_t n_sd
                                                  mesh_mode, out_val, out_grad, out_which, s)                         \
                  : launch_paired<MESH, TRI, 128>(descs, n_sdf, xforms, n_cfg, cfg_begin, pts, n_pts, n_pairs,      \
                                                   mesh_mode, out_val, out_grad, out_which, s))
-    const int rc = needs_mesh ? (any_tri ? PVB_PAIRED(true, true) : PVB_PAIRED(true, false))
-                              : (any_tri ? PVB_PAIRED(false, true) : PVB_PAIRED(false, false));
+    const int rc = needs_mesh ? (any_ext ? PVB_PAIRED(true, true) : PVB_PAIRED(true, false))
+                              : (any_ext ? PVB_PAIRED(false, true) : PVB_PAIRED(false, false));
 #undef PVB_PAIRED
     return rc;
 }
@@ -2831,6 +2851,10 @@ extern "C" int pvb_chamfer(const pvb_sdf_desc *obj, const float *world_to_object
                            int64_t sort_workspace_bytes, void *stream) {
     if (!obj || !world_to_object || n_tf < 0 || n_pts < 1 || !pts || !workspace || !out) {
         pvb_set_error("pvb_chamfer: invalid argument");
+        return PVB_ERR_INVALID;
+    }
+    if (obj->kind < PVB_KIND_GRID || obj->kind > PVB_KIND_CYLINDER) {
+        pvb_set_error("pvb_chamfer: unknown kind %d", obj->kind);
         return PVB_ERR_INVALID;
     }
     if (obj->kind == PVB_KIND_MESH)

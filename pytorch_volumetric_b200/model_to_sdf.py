@@ -17,16 +17,32 @@ from .transforms import Transform3d, invert_rigid, matrix_of
 logger = logging.getLogger(__file__)
 
 
-def _mesh_visuals(chain, frame_names):
-    """(link name, visual) for every mesh visual along the chain, in frame order; other geometry types are
-    reported and skipped, like the reference does (model_to_sdf.py:41-56)."""
+_PRIMITIVES = ("box", "cylinder", "sphere")
+
+
+def _mesh_visuals(chain, frame_names, primitives=False):
+    """(link name, visual) for every mesh visual along the chain -- and with `primitives` every box, cylinder and
+    sphere visual -- in frame order; other geometry types are reported and skipped, like the reference does
+    (model_to_sdf.py:41-56)."""
     for fname in frame_names:
         link = chain.find_frame(fname).link
         for vis in link.visuals:
-            if vis.geom_type == "mesh":
+            if vis.geom_type == "mesh" or (primitives and vis.geom_type in _PRIMITIVES):
                 yield link.name, vis
             else:
                 logger.warning("Cannot handle non-mesh link visual type %s for %s", vis, link.name)
+
+
+def _primitive_sdf(vis):
+    """BoxSDF / CylinderSDF / SphereSDF of a URDF primitive visual (pytorch_kinematics' geom_param conventions: box
+    size [x, y, z], cylinder (radius, length), sphere radius)."""
+    if vis.geom_type == "box":
+        return sdf.BoxSDF(vis.geom_param)
+    if vis.geom_type == "cylinder":
+        radius, length = vis.geom_param
+        return sdf.CylinderSDF(radius, length)
+    radius = sdf._check_extent("sphere radius", vis.geom_param)
+    return sdf.SphereSDF(radius)
 
 
 class RobotSDF(sdf.ObjectFrameSDF):
@@ -37,12 +53,16 @@ class RobotSDF(sdf.ObjectFrameSDF):
     """
 
     def __init__(self, chain, default_joint_config=None, path_prefix='',
-                 link_sdf_cls: typing.Callable[[sdf.ObjectFactory], sdf.ObjectFrameSDF] = sdf.MeshSDF):
+                 link_sdf_cls: typing.Callable[[sdf.ObjectFactory], sdf.ObjectFrameSDF] = sdf.MeshSDF,
+                 primitive_visuals=False):
         """
-        :param chain: kinematic description; only mesh visuals become SDFs
+        :param chain: kinematic description; only mesh visuals become SDFs (and primitives, see primitive_visuals)
         :param default_joint_config: joint values installed at construction (zeros when None)
         :param path_prefix: directory the relative mesh paths of the description are resolved against
-        :param link_sdf_cls: callable turning a link's ObjectFactory into its ObjectFrameSDF
+        :param link_sdf_cls: callable turning a link's ObjectFactory into its ObjectFrameSDF (mesh visuals only)
+        :param primitive_visuals: EXTENSION (the reference skips them with a warning, which stays the default): box,
+        cylinder and sphere visuals become BoxSDF / CylinderSDF / SphereSDF links, in frame / visual order with the
+        mesh links and placed by their <origin> like them; the fused kernels evaluate them analytically
         """
         self.chain = chain
         self.dtype, self.device = chain.dtype, chain.device
@@ -52,12 +72,15 @@ class RobotSDF(sdf.ObjectFrameSDF):
         self.joint_names = chain.get_joint_parameter_names()
         self.frame_names = chain.get_frame_names(exclude_fixed=False)
 
-        visuals = list(_mesh_visuals(chain, self.frame_names))
+        visuals = list(_mesh_visuals(chain, self.frame_names, primitive_visuals))
         self.sdf_to_link_name = [name for name, _ in visuals]
         link_sdfs = []
         for name, vis in visuals:
-            mesh_file, mesh_scale = vis.geom_param[0], vis.geom_param[1]
             logger.info("%s offset %s", name, vis.offset)
+            if vis.geom_type != "mesh":
+                link_sdfs.append(_primitive_sdf(vis))
+                continue
+            mesh_file, mesh_scale = vis.geom_param[0], vis.geom_param[1]
             link_sdfs.append(link_sdf_cls(sdf.MeshObjectFactory(mesh_file, scale=mesh_scale, path_prefix=path_prefix)))
         # visual origin of every mesh inside its link frame, stacked link-major
         self.offset_transforms = Transform3d(

@@ -524,9 +524,96 @@ class SphereSDF(ObjectFrameSDF):
         d = nat.SdfDesc()
         d.kind = nat.PVB_KIND_SPHERE
         d.radius = float(self.radius)
-        for k in range(3):
-            d.bb_min[k] = -float(self.radius)
-            d.bb_max[k] = float(self.radius)
+        r = float(np.float32(self.radius))
+        _set_primitive_bound(d, [r] * 3, r)
+        return d
+
+
+def _set_primitive_bound(d, half, inradius):
+    """Box -half..half and the pruning bound of an analytic primitive descriptor (SPHERE / BOX / CYLINDER).
+
+    The fused kernels skip a sub-SDF when dist(q, bb) - prune_margin exceeds the running minimum, so the value must
+    never be below that.  The shape is convex and lies inside its box, so its exact value is >= dist(q, bb) outside
+    the shape and >= -inradius inside.  In fp32: inside the box every per-axis term (|q_k| - h_k, rho - r, |q| - r)
+    is >= -h_k, -r resp. by monotone rounding, so the value is never below -inradius; outside, the value is the fp32
+    rounding of a distance >= dist(q, bb), a few ulp of |q| low at most, and the kernels' own fp32 dist(q, bb) a few
+    ulp high.  The slack 1e-5 * max(1, |bb|) (the one MeshSDF uses for the same bound) covers those roundings for
+    |q| up to ~30 max(1, |bb|) in the primitive's frame (tests/test_primitive_cpu.py checks it densely)."""
+    h = [float(np.float32(v)) for v in half]
+    for k in range(3):
+        d.bb_min[k] = -h[k]
+        d.bb_max[k] = h[k]
+    d.prune_margin = float(inradius) + 1e-5 * max(1.0, max(h))
+    d.flags = nat.PVB_GRID_PRUNE_OK
+
+
+def _check_extent(name, v):
+    v = float(v)
+    if not math.isfinite(v) or v < 0:
+        raise ValueError(f"{name} must be finite and >= 0, got {v}")
+    return v
+
+
+class _PrimitiveSDF(ObjectFrameSDF):
+    """Analytic primitive evaluated by the fused composition kernels: __call__ is a one-sub-SDF ComposedSDF under
+    the identity transform (exact up to the sign of zero), so it shares their arithmetic bit for bit."""
+    _half = None      # per-axis half extents of the primitive's box
+
+    def __call__(self, points_in_object_frame):
+        comp = self.__dict__.get("_self_composed")
+        if comp is None:
+            comp = self._self_composed = ComposedSDF([self], Transform3d(matrix=torch.eye(4).unsqueeze(0)))
+        lead = tuple(points_in_object_frame.shape[:-1])
+        vv, gg = comp(points_in_object_frame)
+        return vv.reshape(lead), gg.reshape(*lead, 3)
+
+    def surface_bounding_box(self, padding=0., padding_ratio=0.):
+        return torch.tensor([[-(h + padding + padding_ratio * h), h + padding + padding_ratio * h]
+                             for h in self._half])
+
+
+class BoxSDF(_PrimitiveSDF):
+    """EXTENSION (the reference has no primitive SDFs): exact SDF of the box with full edge lengths `size`, centred
+    at the origin (URDF <box size=...>).
+
+    Outside: the distance to the box, gradient the unit vector from the closest box point.  Inside or on the
+    surface: max_k(|q_k| - h_k) with h = size / 2, gradient +-e_k for that axis -- the first axis on ties, + where
+    q_k >= 0 (-0 included)."""
+
+    def __init__(self, size):
+        size = [_check_extent("BoxSDF size", s) for s in np.asarray(size, dtype=np.float64).reshape(-1)]
+        if len(size) != 3:
+            raise ValueError(f"BoxSDF size needs 3 edge lengths, got {len(size)}")
+        self.size = size
+        self._half = [0.5 * s for s in size]
+
+    def native_desc(self, device):
+        d = nat.SdfDesc()
+        d.kind = nat.PVB_KIND_BOX
+        _set_primitive_bound(d, self._half, min(float(np.float32(h)) for h in self._half))
+        return d
+
+
+class CylinderSDF(_PrimitiveSDF):
+    """EXTENSION (the reference has no primitive SDFs): exact SDF of the cylinder of `radius` r and total `length`
+    along the local z axis, centred at the origin (URDF <cylinder radius=... length=...>).
+
+    With rho = |(x, y)|, u = (x, y) / rho ((1, 0) on the axis) and d = (rho - r, |z| - length / 2): outside,
+    w = max(d, 0), value |w| and gradient (w_0 u, w_1 sign z) / |w|; inside or on the surface, value max(d) and
+    gradient (u, 0) when d_0 >= d_1 (radial wins ties), else (0, 0, sign z), with sign z = +1 for z >= 0 (-0
+    included)."""
+
+    def __init__(self, radius, length):
+        self.radius = _check_extent("CylinderSDF radius", radius)
+        self.length = _check_extent("CylinderSDF length", length)
+        self._half = [self.radius, self.radius, 0.5 * self.length]
+
+    def native_desc(self, device):
+        d = nat.SdfDesc()
+        d.kind = nat.PVB_KIND_CYLINDER
+        d.radius = self.radius
+        r, h = float(np.float32(self.radius)), float(np.float32(0.5 * self.length))
+        _set_primitive_bound(d, self._half, min(r, h))
         return d
 
 

@@ -124,6 +124,50 @@ def write_arm(dirname, mesh_scale=3.0):
     return path, "link_7"
 
 
+# The same chain with every link an analytic URDF primitive (RobotSDF(..., primitive_visuals=True)): a box base, then
+# cylinders and boxes of about 0.2 m and a sphere at the end, each placed by an <origin> with a non-trivial rpy.
+PRIMITIVE_ARM_LINKS = [
+    # (geometry element, origin xyz, origin rpy)
+    ('<box size="0.24 0.2 0.15"/>', "0 0 0.075", "0 0 0.3"),
+    ('<cylinder radius="0.065" length="0.2"/>', "0 0 0.1", "0.2 0 0"),
+    ('<box size="0.1 0.12 0.21"/>', "0 0 0.1", "0 0.15 0.6"),
+    ('<cylinder radius="0.06" length="0.22"/>', "0 0 0.11", "0.1 -0.1 0.9"),
+    ('<box size="0.09 0.11 0.19"/>', "0 0 0.09", "-0.2 0 1.2"),
+    ('<cylinder radius="0.055" length="0.21"/>', "0 0 0.1", "0 0.25 1.5"),
+    ('<box size="0.08 0.09 0.1"/>', "0 0 0.04", "0.3 0.2 0.1"),
+    ('<sphere radius="0.05"/>', "0 0 0.05", "0 0 0"),
+]
+# links of the mixed arm that are the probe mesh (as in write_arm) instead of their primitive
+MIXED_ARM_MESH_LINKS = (1, 4, 6)
+
+
+def write_primitive_arm(dirname, mesh_links=(), mesh_scale=3.0):
+    """Writes arm.urdf (+ link.obj when `mesh_links` is not empty) into `dirname`: the chain of write_arm with link i
+    the primitive PRIMITIVE_ARM_LINKS[i], or the probe mesh of write_arm for i in `mesh_links`
+    (MIXED_ARM_MESH_LINKS: the mixed arm).  Returns the URDF path and end link name."""
+    from pytorch_volumetric_b200.meshio import write_obj
+    os.makedirs(dirname, exist_ok=True)
+    if mesh_links:
+        v, f = fixture_mesh("probe")
+        write_obj(os.path.join(dirname, "link.obj"), v, f)
+    parts = ['<robot name="arm7_primitive">']
+    for i, (geom, xyz, rpy) in enumerate(PRIMITIVE_ARM_LINKS):
+        if i in mesh_links:
+            xyz, rpy = "0 0 0.02", f"0 0 {0.3 * i:.3f}"
+            geom = f'<mesh filename="link.obj" scale="{mesh_scale} {mesh_scale} {mesh_scale}"/>'
+        parts.append(f'<link name="link_{i}"><visual><origin xyz="{xyz}" rpy="{rpy}"/><geometry>{geom}</geometry>'
+                     f'</visual></link>')
+    for i, (xyz, axis) in enumerate(ARM_JOINTS):
+        parts.append(f'<joint name="joint_{i + 1}" type="revolute"><parent link="link_{i}"/>'
+                     f'<child link="link_{i + 1}"/><origin xyz="{xyz[0]} {xyz[1]} {xyz[2]}" rpy="0 0 0"/>'
+                     f'<axis xyz="{axis[0]} {axis[1]} {axis[2]}"/></joint>')
+    parts.append("</robot>")
+    path = os.path.join(dirname, "arm.urdf")
+    with open(path, "w") as fh:
+        fh.write("\n".join(parts))
+    return path, "link_7"
+
+
 def arm_configurations(n, seed=3, dtype=torch.float32):
     """nominal pose + 0.1 * randn perturbations stacked under it (README.md:166-170 of the reference)."""
     g = torch.Generator().manual_seed(seed)
