@@ -213,6 +213,20 @@ int pvb_composed_query_paired(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t 
                               const float *pts, int64_t n_pts, uint32_t mesh_mode,
                               float *out_val, float *out_grad, int32_t *out_which, void *stream);
 
+/* ---- EXTENSION: swept query, the minimum over the configurations at every point ----
+ * The reference has no such operator; its equivalent is the minimum over dim 0 of ComposedSDF.__call__'s result
+ * (sdf.py:392-433), which materialises 16 * cfg_count * n_pts bytes.  For point i, the result is the
+ * per-configuration result (pvb_composed_query: value, gradient, which) of the configuration c* that minimises
+ * (value, c, which) lexicographically over [cfg_begin, cfg_begin + cfg_count): the FIRST configuration attaining the
+ * minimum value.  Bit-identical to that reduction of pvb_composed_query's results, for every set it accepts.
+ * out_val [n_pts], out_grad [n_pts * 3]; out_cfg [n_pts] (the absolute configuration index c*) and out_which [n_pts]
+ * (the sub-SDF index) are optional; everything else as pvb_composed_query.  PVB_ERR_INVALID also when cfg_count < 1
+ * and n_pts > 0: there is no minimum over an empty set.  n_pts == 0 does nothing. */
+int pvb_composed_query_swept(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh, const float *xforms,
+                             int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                             const float *pts, int64_t n_pts, uint32_t mesh_mode,
+                             float *out_val, float *out_grad, int32_t *out_cfg, int32_t *out_which, void *stream);
+
 /* ---- the same query with the result slab stored to several destinations from the kernel epilogue ----
  * Multi-GPU re-assembly of a configuration-sharded RobotSDF result (model_to_sdf.py:117-125 returns the full
  * (|A|, N) tensors): every rank evaluates its slab [cfg_begin, cfg_begin + cfg_count) and writes it straight into

@@ -972,4 +972,52 @@ __device__ __forceinline__ float rs_sphere_lb(f3 p, float cx, float cy, float cz
     return fmaf(d2 * rsqrt_approx(d2), kRsBoundScale, -sph_rad);
 }
 
+// ----------------------------------------------------------------------------
+// Swept queries (robot_swept_kernel / composed_swept_kernel, pvb_composed_query_swept): the minimum over a slab of
+// configurations at every point.  The result is the per-configuration result (value, gradient, which) of the
+// configuration c* such that (value, c, which) is lexicographically smallest: c* is the FIRST configuration attaining
+// the minimum value, and which is that configuration's own argmin.
+
+// The lexicographic order of two configurations' results at one point: a before b.  Configurations are distinct, so
+// the sub-SDF index never decides.
+__device__ __forceinline__ bool swept_before(float va, int ca, float vb, int cb) {
+    return va < vb || (va == vb && ca < cb);
+}
+
+// The running result of one point.  cfg < 0: nothing folded yet.
+struct SweptBest { float val; f3 grad; int cfg; int which; };
+
+// Fold the result of a configuration (or the winner of a tile of configurations) into the point's running result.
+// Configurations arrive in ascending order, so a later one replaces the running result only when STRICTLY smaller.
+__device__ __forceinline__ void swept_fold(SweptBest &b, float val, f3 grad, int cfg, int which) {
+    if (b.cfg < 0 || val < b.val) { b.val = val; b.grad = grad; b.cfg = cfg; b.which = which; }
+}
+
+// One lane of robot_swept_kernel: one (configuration, point) pair, its links visited nearest-sphere first (`pred`)
+// and then in index order.  The prune threshold is the smaller of the lane's own running value and `bp`, the point's
+// best value over the configurations of earlier tiles: a link is skipped only when a lower bound of its value is
+// STRICTLY above the threshold, so it can neither be this configuration's argmin nor beat an earlier configuration --
+// links whose value ties are always evaluated, and the visiting order never changes c* or which.
+//   lb: the bounding-sphere bounds (rs_sphere_lb; +inf for slots beyond n_sdf, which are never visited once a link has
+//   been evaluated, since values are finite); link(si, thr, o): transform the point into link si's frame, return false
+//   when its exact AABB bound (margin included) is strictly above thr, else evaluate it into o = (value, link-frame
+//   gradient).
+// The result is (best, bg, bs): this configuration's per-configuration result whenever best <= bp; when best > bp it
+// may differ from it, but then the configuration cannot win (its true minimum is above bp as well).  bs < 0: every
+// link was pruned (best = +inf > bp).
+template <class Link>
+__device__ __forceinline__ void rs_swept_pair(const float (&lb)[8], int pred, float bp, const Link &link, float &best,
+                                              f3 &bg, int &bs) {
+    best = PVB_INF; bg = mk3(0.f, 0.f, 0.f); bs = -1;
+    auto visit = [&](const int si) {
+        float4 o;
+        if (!link(si, fminf(best, bp), o)) return;
+        if (bs < 0 || o.x < best || (o.x == best && si < bs)) { best = o.x; bg = mk3(o.y, o.z, o.w); bs = si; }
+    };
+    if (!(lb[pred] > bp)) visit(pred);
+#pragma unroll
+    for (int si = 0; si < 8; ++si)
+        if (si != pred && !(lb[si] > fminf(best, bp))) visit(si);
+}
+
 }  // namespace pvb

@@ -868,6 +868,42 @@ composed_paired_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, 
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// Swept query, every sub-SDF set the composed query accepts (meshes, PVB_GRID_OOB_GT, 9-128 sub-SDFs): the minimum
+// over the configurations cfg_begin .. cfg_begin + cfg_count - 1 at every point, in the order of swept_fold
+// (pvb_device.cuh).  One thread per point walks the configurations in ascending order through composed_point with the
+// jitter index of the absolute configuration, as composed_paired_kernel does, so every configuration's result is the
+// per-configuration query's bit for bit.  out_cfg: the absolute configuration of the result.
+template <bool kMesh, bool kExt, int MAXS>
+__global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
+composed_swept_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
+                      int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_pts,
+                      uint32_t mesh_mode, float *__restrict__ out_val, float *__restrict__ out_grad,
+                      int *__restrict__ out_cfg, int *__restrict__ out_which, int nearest_first, float margin_max) {
+    NodeStage st; st.smem = nullptr; st.n = 0;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_pts; i += stride) {
+        const f3 p = load_point(pts, i);
+        SweptBest b;
+        b.val = PVB_INF; b.grad = mk3(0.f, 0.f, 0.f); b.cfg = -1; b.which = -1;
+        for (int c = 0; c < cfg_count; ++c) {
+            const int cfg = cfg_begin + c;
+            auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) {
+                const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
+                r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
+            };
+            const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st, p, mesh_mode,
+                                                              (uint64_t)cfg * (uint64_t)n_pts + (uint64_t)i,
+                                                              nearest_first, margin_max);
+            swept_fold(b, o.val, o.grad, cfg, o.which);
+        }
+        out_val[i] = b.val;
+        out_grad[3 * i] = b.grad.x; out_grad[3 * i + 1] = b.grad.y; out_grad[3 * i + 2] = b.grad.z;
+        if (out_cfg) out_cfg[i] = b.cfg;
+        if (out_which) out_which[i] = b.which;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // Configuration-major variant for RobotSDF-style batches (many joint configurations, shared points).
 //
 // Lanes of a warp are 32 CONFIGURATIONS of the same point instead of 32 points of the same configuration:
@@ -1631,6 +1667,128 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
             }
         }
         if constexpr (kCoop) __syncthreads(); else __syncwarp();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Swept query on the sets robot_serial_kernel takes (<= 8 GRID links with the bounding-box rule, nearest or
+// trilinear, or primitives): the minimum over the configuration slab at every point (swept_fold, pvb_device.cuh),
+// without materialising the cfg_count x n_pts cross product.
+//   * A block owns blk_pts consecutive points and walks the slab's configuration tiles (rs_tile) in ascending order.
+//     Per tile it stages the transforms and the object-frame sphere centres once, as robot_serial_kernel does, and its
+//     point groups (LC lanes = the tile's configurations of one point) take the block's points in turn.
+//   * Each point's running result (value, link-frame gradient, configuration, link) stays in shared memory across the
+//     tiles.  A lane prunes against the smaller of its own running value and the point's best from earlier tiles
+//     (rs_swept_pair): (configuration, link) pairs that cannot beat an earlier configuration are skipped as well.
+//   * After the pair, a lexicographic (value, configuration) shuffle reduction within the point group names the
+//     tile's winner, which folds itself into the point's result.
+//   * The gradient is rotated back once per point, at the end, with the winner's transform: the same
+//     composed_rotate_back on the same operands as the per-configuration query.  Outputs are written once per point.
+// Transform, bounds, lookups and primitives are those of robot_serial_kernel, so every configuration's candidate is
+// its per-configuration result bit for bit whenever it can win.
+constexpr int kSwMaxPts = 128;                    // points per block at most (blk_pts: 32, 64 or 128)
+
+struct __align__(16) SwSmem {
+    float4 xf[kRbCfg][3 * kRsMaxS + 1];
+    float4 sph[kRbCfg][3 * kRsMaxS / 4 + 1];
+    SweptBest best[kSwMaxPts];                    // cfg relative to cfg_begin
+};
+
+template <bool kExt>
+__global__ void __launch_bounds__(kRbCfg * kRsWarps, PVB_RS_MINB)
+robot_swept_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, const float *__restrict__ xforms,
+                   int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, int n_pts, int blk_pts,
+                   float *__restrict__ out_val, float *__restrict__ out_grad, int *__restrict__ out_cfg,
+                   int *__restrict__ out_which) {
+    __shared__ SwSmem sm;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long base = (long long)blockIdx.x * blk_pts;
+    const int npb = (int)min((long long)blk_pts, (long long)n_pts - base);     // points of this block
+    for (int j = threadIdx.x; j < npb; j += blockDim.x) {
+        sm.best[j].val = PVB_INF; sm.best[j].cfg = -1;
+    }
+    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const int n_tiles = (cfg_count >> 5) + __popc((unsigned)(cfg_count & 31));
+    for (int t = 0; t < n_tiles; ++t) {
+        int c0, lc_log2;
+        rs_tile(cfg_count, t, c0, lc_log2);
+        const int LC = 1 << lc_log2, sub_log2 = 5 - lc_log2;
+        const int cl = lane & (LC - 1), sub = lane >> lc_log2;
+        __syncthreads();                                     // the previous tile's staging is no longer read
+        for (int item = threadIdx.x; item < LC * n_sdf; item += blockDim.x) {
+            const int ci = item & (LC - 1), si = item >> lc_log2;
+            const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg_begin + c0 + ci) * 16);
+            sm.xf[ci][3 * si] = __ldg(row); sm.xf[ci][3 * si + 1] = __ldg(row + 1); sm.xf[ci][3 * si + 2] = __ldg(row + 2);
+        }
+        __syncthreads();
+        for (int item = threadIdx.x; item < LC * kRsMaxS; item += blockDim.x) {
+            const int ci = item & (LC - 1), si = item >> lc_log2;
+            const f3 co = si < n_sdf ? rs_sphere_centre(pk.d[si], sm.xf[ci][3 * si], sm.xf[ci][3 * si + 1],
+                                                        sm.xf[ci][3 * si + 2])
+                                     : mk3(0.f, 0.f, 0.f);
+            float *c = reinterpret_cast<float *>(&sm.sph[ci][0]) + 3 * si;
+            c[0] = co.x; c[1] = co.y; c[2] = co.z;
+        }
+        __syncthreads();
+        const int groups = kRsWarps << sub_log2;             // point groups of the block
+        const int gid = (warp << sub_log2) + sub;
+#pragma unroll 1
+        for (int j0 = 0; j0 < npb; j0 += groups) {
+            const int j = j0 + gid;
+            const bool on = j < npb;
+            if (!__any_sync(0xffffffffu, on)) break;         // uniform per warp: the warp's groups are all past the end
+            const f3 p = on ? load_point(pts, base + j) : mk3(0.f, 0.f, 0.f);
+            float cen[3 * kRsMaxS];
+#pragma unroll
+            for (int k = 0; k < 3 * kRsMaxS / 4; ++k) {
+                const float4 c4 = sm.sph[cl][k];
+                cen[4 * k] = c4.x; cen[4 * k + 1] = c4.y; cen[4 * k + 2] = c4.z; cen[4 * k + 3] = c4.w;
+            }
+            float lb[kRsMaxS], key[kRsMaxS];
+#pragma unroll
+            for (int si = 0; si < kRsMaxS; ++si) {
+                lb[si] = rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], pk.sph_rad[si]);
+                key[si] = rs_bound_key(lb[si], low3_off, si);
+            }
+            const int pred = __shfl_sync(0xffffffffu, rs_nearest(key, n_sdf), sub << lc_log2);
+            const float bp = on ? sm.best[j].val : PVB_INF;
+            auto link = [&](const int si, const float thr, float4 &o) -> bool {
+                const pvb_sdf_desc &d = pk.d[si];
+                const float4 r0 = sm.xf[cl][3 * si], r1 = sm.xf[cl][3 * si + 1], r2 = sm.xf[cl][3 * si + 2];
+                const f3 q = composed_xform(r0, r1, r2, p);
+                const float tm = thr + pk.visit_margin[si];
+                if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
+                o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
+                    : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
+                                                               : robot_lookup(d, q);
+                return true;
+            };
+            float best;
+            f3 bg;
+            int bs;
+            rs_swept_pair(lb, pred, bp, link, best, bg, bs);
+            // the tile's winner for this point: lexicographic (value, configuration) over the LC lanes of the group
+            float wv = best;
+            int wl = cl;
+            for (int off = 1; off < LC; off <<= 1) {
+                const float ov = __shfl_xor_sync(0xffffffffu, wv, off);
+                const int ol = __shfl_xor_sync(0xffffffffu, wl, off);
+                if (swept_before(ov, ol, wv, wl)) { wv = ov; wl = ol; }
+            }
+            if (on && cl == wl) swept_fold(sm.best[j], best, bg, c0 + cl, bs);
+        }
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < npb; j += blockDim.x) {
+        const SweptBest b = sm.best[j];
+        const int cfg = cfg_begin + b.cfg;
+        const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)max(b.which, 0) * n_cfg + cfg) * 16);
+        const f3 go = composed_rotate_back(__ldg(row), __ldg(row + 1), __ldg(row + 2), b.grad);
+        const long long i = base + j;
+        out_val[i] = b.val;
+        out_grad[3 * i] = go.x; out_grad[3 * i + 1] = go.y; out_grad[3 * i + 2] = go.z;
+        if (out_cfg) out_cfg[i] = cfg;
+        if (out_which) out_which[i] = b.which;
     }
 }
 
@@ -2596,6 +2754,88 @@ extern "C" int pvb_composed_query_paired(const pvb_sdf_desc *descs, int32_t n_sd
     const int rc = needs_mesh ? (any_ext ? PVB_PAIRED(true, true) : PVB_PAIRED(true, false))
                               : (any_ext ? PVB_PAIRED(false, true) : PVB_PAIRED(false, false));
 #undef PVB_PAIRED
+    return rc;
+}
+
+// Launch robot_swept_kernel.  Points per block: as many as keep >= 2 waves of resident blocks, so that the tile
+// staging is shared by up to 128 points without leaving SMs idle at 10^5 points.
+static int launch_robot_swept(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
+                              int cfg_count, const float *pts, long long n_pts, float *out_val, float *out_grad,
+                              int *out_cfg, int *out_which, bool ext, cudaStream_t stream) {
+    RobotPack<kRsMaxS> pack;
+    memset(&pack, 0, sizeof(pack));
+    for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
+    for (int si = 0; si < kRsMaxS; ++si) {
+        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
+        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
+    }
+    const long long slots = (long long)sm_count() * PVB_RS_MINB;
+    int blk_pts = kSwMaxPts;
+    while (blk_pts > 32 && n_pts < 2 * slots * blk_pts) blk_pts >>= 1;
+    const long long gx = (n_pts + blk_pts - 1) / blk_pts;
+    timing_mark(0, stream);
+    if (ext)
+        robot_swept_kernel<true><<<(unsigned)gx, kRbCfg * kRsWarps, 0, stream>>>(
+            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts, blk_pts, out_val, out_grad, out_cfg,
+            out_which);
+    else
+        robot_swept_kernel<false><<<(unsigned)gx, kRbCfg * kRsWarps, 0, stream>>>(
+            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts, blk_pts, out_val, out_grad, out_cfg,
+            out_which);
+    timing_mark(1, stream);
+    PVB_CHECK_LAUNCH("pvb_composed_query_swept(robot)");
+    return PVB_OK;
+}
+
+template <bool kMesh, bool kExt, int MAXS>
+static int launch_swept(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
+                        int cfg_count, const float *pts, long long n_pts, uint32_t mesh_mode, float *out_val,
+                        float *out_grad, int *out_cfg, int *out_which, cudaStream_t stream) {
+    DescPack<MAXS> pack;
+    memcpy(pack.d, descs, sizeof(pvb_sdf_desc) * (size_t)n_sdf);
+    fill_order(pack, n_sdf);
+    // the same switch as launch_composed: nearest-bound-first evaluation of mesh sub-SDFs
+    static const int nearest_first = [] { const char *e = getenv("PVB_COMP_NEAREST_FIRST"); return e ? atoi(e) : 1; }();
+    float margin_max = 0.f;
+    for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
+    timing_mark(0, stream);
+    composed_swept_kernel<kMesh, kExt, MAXS><<<grid_for(n_pts, kCompThreads, 8), kCompThreads, 0, stream>>>(
+        pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, mesh_mode, out_val, out_grad, out_cfg,
+        out_which, nearest_first, margin_max);
+    timing_mark(1, stream);
+    PVB_CHECK_LAUNCH("pvb_composed_query_swept");
+    return PVB_OK;
+}
+
+extern "C" int pvb_composed_query_swept(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,
+                                        const float *xforms, int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                                        const float *pts, int64_t n_pts, uint32_t mesh_mode, float *out_val,
+                                        float *out_grad, int32_t *out_cfg, int32_t *out_which, void *stream) {
+    bool any_ext;
+    const int bad = composed_check_args("pvb_composed_query_swept", descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count,
+                                        pts, n_pts, out_val, out_grad, any_ext);
+    if (bad) return bad;
+    if (n_pts == 0) return PVB_OK;
+    if (cfg_count < 1) {
+        pvb_set_error("pvb_composed_query_swept: no minimum over an empty configuration slab (cfg_count=%d)", cfg_count);
+        return PVB_ERR_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    // robot_serial_kernel's sets take the fused kernel: <= 8 GRID links with the bounding-box rule or primitives
+    bool fused = !needs_mesh && n_sdf <= kRsMaxS && n_pts < (1ll << 31);
+    for (int i = 0; i < n_sdf && fused; ++i)
+        fused = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    if (fused)
+        return launch_robot_swept(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_val, out_grad,
+                                  out_cfg, out_which, any_ext, s);
+#define PVB_SWEPT(MESH, TRI)                                                                                       \
+    (n_sdf <= 16 ? launch_swept<MESH, TRI, 16>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,       \
+                                                mesh_mode, out_val, out_grad, out_cfg, out_which, s)                 \
+                 : launch_swept<MESH, TRI, 128>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,      \
+                                                 mesh_mode, out_val, out_grad, out_cfg, out_which, s))
+    const int rc = needs_mesh ? (any_ext ? PVB_SWEPT(true, true) : PVB_SWEPT(true, false))
+                              : (any_ext ? PVB_SWEPT(false, true) : PVB_SWEPT(false, false));
+#undef PVB_SWEPT
     return rc;
 }
 

@@ -169,6 +169,13 @@ class RobotSDF(sdf.ObjectFrameSDF):
         (ComposedSDF.paired)."""
         return self.sdf.paired(points_in_object_frame)
 
+    def swept(self, points_in_object_frame, return_argmin=False):
+        """The minimum over every installed joint configuration at every point (the SDF of the swept volume):
+        points [*B, N, 3] in the robot frame -> (values [*B, N], gradients [*B, N, 3]) and, with return_argmin, the
+        first configuration attaining it (flat index into A) and its link, a position in `sdf_to_link_name`
+        (ComposedSDF.swept)."""
+        return self.sdf.swept(points_in_object_frame, return_argmin=return_argmin)
+
     def surface_bounding_box(self, **kwargs):
         return self.sdf.surface_bounding_box(**kwargs)
 

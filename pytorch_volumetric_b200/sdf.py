@@ -823,6 +823,87 @@ class ComposedSDF(ObjectFrameSDF):
         gg = nat.deliver(gg, out_device, dtype)
         return vv.reshape(pts_shape[:-1]), gg.reshape(*pts_shape[:-1], 3)
 
+    #: configurations per `_generic_query` chunk of the unfused swept fold (bounds its cfg_chunk x P temporaries)
+    swept_generic_chunk = 64
+
+    def query_swept(self, points_in_object_frame, cfg_begin=0, cfg_count=None, return_which=False):
+        """Swept form of `query`: at every point, the result of the configuration of the slab
+        [cfg_begin, cfg_begin + cfg_count) with the smallest value -- the first such configuration on ties -- without
+        the cfg_count-fold cross product.  Bit-identical to that reduction of query(..., return_which=True): (value,
+        configuration, sub-SDF index) minimised lexicographically.  Returns flat (P,) / (P, 3) fp32 tensors on the GPU,
+        and with return_which also the int32 absolute configuration index and sub-SDF index."""
+        S = len(self.sdfs)
+        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
+        if cfg_count is None:
+            cfg_count = n_cfg - cfg_begin
+        shape = tuple(points_in_object_frame.shape)
+        if shape[-1:] != (3,):
+            raise ValueError(f"swept query: points {shape} must be [..., 3]")
+        if cfg_count < 1 and math.prod(shape[:-1]) > 0:
+            raise ValueError(f"swept query: no minimum over an empty configuration slab (cfg_count={cfg_count})")
+        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
+        with torch.cuda.device(device):
+            p = nat.as_f32_points(points_in_object_frame, device)
+            P = p.shape[0]
+            descs_arr, needs_mesh = self._native_descs(device)
+            if descs_arr is None:
+                return self._generic_swept(p, cfg_begin, cfg_count, n_cfg, return_which)
+            xf = self._xforms_on(device)
+            val = torch.empty(P, dtype=torch.float32, device=device)
+            grad = torch.empty(P, 3, dtype=torch.float32, device=device)
+            cfg = torch.empty(P, dtype=torch.int32, device=device) if return_which else None
+            which = torch.empty(P, dtype=torch.int32, device=device) if return_which else None
+            nat.check(nat.lib().pvb_composed_query_swept(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg,
+                                                         cfg_begin, cfg_count, nat.ptr(p), P, nat.PVB_MESH_DEFAULT,
+                                                         nat.ptr(val), nat.ptr(grad), nat.ptr(cfg), nat.ptr(which),
+                                                         nat.stream_ptr(device)), "pvb_composed_query_swept")
+        return (val, grad, cfg, which) if return_which else (val, grad)
+
+    def _generic_swept(self, p, cfg_begin, cfg_count, n_cfg, return_which):
+        """query_swept for sub-SDFs without native descriptors: configuration chunks through `_generic_query` in
+        ascending order; within a chunk the first configuration attaining the minimum, across chunks a strictly
+        smaller value -- the same (value, configuration, sub-SDF) order as the fused kernels."""
+        P = p.shape[0]
+        best = torch.full((P,), float("inf"), dtype=torch.float32, device=p.device)
+        bgrad = torch.zeros(P, 3, dtype=torch.float32, device=p.device)
+        bcfg = torch.full((P,), -1, dtype=torch.int32, device=p.device)
+        bwhich = torch.full((P,), -1, dtype=torch.int32, device=p.device)
+        for c0 in range(cfg_begin, cfg_begin + (cfg_count if P > 0 else 0), self.swept_generic_chunk):
+            cc = min(self.swept_generic_chunk, cfg_begin + cfg_count - c0)
+            v, g, w = self._generic_query(p, c0, cc, n_cfg, True)
+            v, g, w = v.reshape(cc, P), g.reshape(cc, P, 3), w.reshape(cc, P)
+            first = (v == v.amin(dim=0)).int().argmax(dim=0)          # first configuration attaining the minimum
+            cv = v.gather(0, first[None])[0]
+            better = (cv < best) | (bcfg < 0)
+            best = torch.where(better, cv, best)
+            bgrad = torch.where(better[:, None], g.gather(0, first[None, :, None].expand(1, P, 3))[0], bgrad)
+            bcfg = torch.where(better, (first + c0).to(torch.int32), bcfg)
+            bwhich = torch.where(better, w.gather(0, first[None])[0], bwhich)
+        return (best, bgrad, bcfg, bwhich) if return_which else (best, bgrad)
+
+    def swept(self, points_in_object_frame, return_argmin=False):
+        """The minimum over every installed configuration at every point (the SDF of the swept volume of a
+        trajectory or a set of poses): points [*B, N, 3] give (values [*B, N], gradients [*B, N, 3]) in the points'
+        dtype and on their device.  Entry i is configuration c*'s result at point i, c* the first configuration
+        attaining the minimum value: bit-identical to __call__ followed by that reduction over the configuration
+        dimensions, without materialising the |A| x N cross product.  With return_argmin, also the configuration
+        index c* (int64, flat row-major into A) and the sub-SDF index, each [*B, N].  Without a configuration batch
+        it is __call__ (configuration 0).  Not a reference operator (an extension); raises ValueError before any
+        device work when the points are not [..., 3]."""
+        pts_shape = tuple(points_in_object_frame.shape)
+        if len(pts_shape) < 1 or pts_shape[-1] != 3:
+            raise ValueError(f"swept query: points {pts_shape} must be [..., 3]")
+        out = self.query_swept(points_in_object_frame, return_which=return_argmin)
+        dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
+        out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
+        vv = nat.deliver(out[0], out_device, dtype).reshape(pts_shape[:-1])
+        gg = nat.deliver(out[1], out_device, dtype).reshape(*pts_shape[:-1], 3)
+        if not return_argmin:
+            return vv, gg
+        cfg = nat.deliver(out[2], out_device, torch.int64).reshape(pts_shape[:-1])
+        which = nat.deliver(out[3], out_device, torch.int64).reshape(pts_shape[:-1])
+        return vv, gg, cfg, which
+
     def query_into(self, points_in_object_frame, targets, cfg_begin=0, cfg_count=None):
         """`query` whose result slab is stored by the kernel epilogue into several full-size result buffers at once
         (pvb_composed_query_multi): `targets` is a list of (val, grad) pairs, each a float32 tensor or a raw device
