@@ -227,6 +227,26 @@ int pvb_composed_query_swept(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
                              const float *pts, int64_t n_pts, uint32_t mesh_mode,
                              float *out_val, float *out_grad, int32_t *out_cfg, int32_t *out_which, void *stream);
 
+/* ---- EXTENSION: clearance query, the minimum over the points of a segment for every configuration ----
+ * The reference has no such operator; its equivalent is the minimum over the point dimension of ComposedSDF.__call__'s
+ * result (sdf.py:392-433), which materialises 16 * cfg_count * n_seg * seg_len bytes.  pts DEVICE [n_seg][seg_len][3]:
+ * segment b is pts[b].  For configuration cfg_begin + c and segment b, the result is the per-configuration result
+ * (pvb_composed_query: value, gradient, which) at the point i* of the segment that minimises (value, i)
+ * lexicographically: the FIRST point of the segment attaining the minimum value.  -0 and +0 compare equal; a NaN value
+ * ranks above every number (+inf included), so i* is a NaN point only when every point of the segment is NaN, and then
+ * the first one.  Bit-identical to that reduction of pvb_composed_query's results over the flat points, for every set
+ * it accepts.
+ * keys DEVICE scratch of cfg_count * n_seg entries (the library initialises it).  out_val [cfg_count * n_seg],
+ * out_grad [cfg_count * n_seg * 3], configuration-major (entry c * n_seg + b); out_point (i*, the index within the
+ * segment) and out_which (the sub-SDF index) are optional; everything else as pvb_composed_query.  PVB_ERR_INVALID also
+ * when seg_len == 0 with cfg_count >= 1 and n_seg >= 1 (no minimum over an empty segment), when cfg_count < 1 with
+ * points, and when seg_len >= 2^31.  n_seg == 0 does nothing. */
+int pvb_composed_query_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh, const float *xforms,
+                                 int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                                 const float *pts, int64_t n_seg, int64_t seg_len, uint32_t mesh_mode,
+                                 uint64_t *keys, float *out_val, float *out_grad,
+                                 int32_t *out_point, int32_t *out_which, void *stream);
+
 /* ---- the same query with the result slab stored to several destinations from the kernel epilogue ----
  * Multi-GPU re-assembly of a configuration-sharded RobotSDF result (model_to_sdf.py:117-125 returns the full
  * (|A|, N) tensors): every rank evaluates its slab [cfg_begin, cfg_begin + cfg_count) and writes it straight into

@@ -1020,4 +1020,27 @@ __device__ __forceinline__ void rs_swept_pair(const float (&lb)[8], int pred, fl
         if (si != pred && !(lb[si] > fminf(best, bp))) visit(si);
 }
 
+// ----------------------------------------------------------------------------
+// Clearance queries (robot_clearance_kernel / composed_clearance_kernel / clearance_finish_kernel,
+// pvb_composed_query_clearance): for every configuration and every segment of points, the per-configuration result at
+// the point i* that minimises (value, i) lexicographically -- the FIRST point of the segment attaining the minimum.
+//
+// A candidate (value v, point i of its segment) becomes one 64-bit key: an order-preserving image of v in the high
+// word, i in the low word.  The unsigned order of keys is exactly the (value, i) order, so a 64-bit atomicMin over keys
+// is an exact reduction whose result does not depend on the order in which candidates arrive (block count, block
+// scheduling, SM count).  -0 is mapped to +0 first, so that the two compare equal as they do in torch; every NaN maps to
+// the largest pattern, so a NaN value ranks above every number (+inf included), and ~0 ("no candidate yet") decodes to
+// NaN.
+__device__ __forceinline__ uint64_t clearance_key(float v, uint32_t i) {
+    const uint32_t b = (uint32_t)__float_as_int(v == 0.f ? 0.f : v);
+    const uint32_t h = v != v ? 0xffffffffu : ((b & 0x80000000u) ? ~b : (b | 0x80000000u));
+    return ((uint64_t)h << 32) | i;
+}
+
+// The value of a key (+0 for a zero of either sign; a NaN for every NaN and for ~0).
+__device__ __forceinline__ float clearance_key_value(uint64_t k) {
+    const uint32_t h = (uint32_t)(k >> 32);
+    return __int_as_float((int)((h & 0x80000000u) ? (h & 0x7fffffffu) : ~h));
+}
+
 }  // namespace pvb

@@ -904,6 +904,90 @@ composed_swept_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// Clearance query, every sub-SDF set the composed query accepts (meshes, PVB_GRID_OOB_GT, 9-128 sub-SDFs): for every
+// configuration c of the slab and every segment b of seg_len points, the smallest clearance_key (pvb_device.cuh) over
+// the segment's points, left in keys[c * n_seg + b] (which holds ~0 on entry).  One thread per (configuration, point)
+// pair t = c * n_pts + i runs composed_point with the absolute configuration and the flat point index, the jitter
+// inputs of the per-configuration query.  The lanes of a warp cover consecutive pairs, so lanes of the same key form
+// runs: a segmented shuffle reduction leaves each run's minimum in its first lane, which issues one atomicMin.
+template <bool kMesh, bool kExt, int MAXS>
+__global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
+composed_clearance_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
+                          int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_seg,
+                          long long seg_len, uint32_t mesh_mode, unsigned long long *__restrict__ keys,
+                          int nearest_first, float margin_max) {
+    NodeStage st; st.smem = nullptr; st.n = 0;
+    const int lane = threadIdx.x & 31;
+    const long long n_pts = n_seg * seg_len, total = (long long)cfg_count * n_pts;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    // warp-uniform loop: every lane takes part in the shuffles below
+    for (long long base = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31); base < total; base += stride) {
+        const long long t = base + lane;
+        unsigned long long k = ~0ull;
+        long long tgt = -1;
+        if (t < total) {
+            long long c, i;
+            paired_index(t, n_pts, c, i);
+            const long long b = i / seg_len;
+            const int cfg = cfg_begin + (int)c;
+            auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) {
+                const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
+                r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
+            };
+            const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st,
+                                                              load_point(pts, i), mesh_mode,
+                                                              (uint64_t)cfg * (uint64_t)n_pts + (uint64_t)i,
+                                                              nearest_first, margin_max);
+            k = clearance_key(o.val, (uint32_t)(i - b * seg_len));
+            tgt = c * n_seg + b;
+        }
+        // after step `off`, lane l holds the minimum over lanes l .. l + 2 off - 1 of its own run
+        for (int off = 1; off < 32; off <<= 1) {
+            const unsigned long long ok = __shfl_down_sync(0xffffffffu, k, off);
+            const long long ot = __shfl_down_sync(0xffffffffu, tgt, off);
+            if (lane + off < 32 && ot == tgt && ok < k) k = ok;
+        }
+        const long long prev = __shfl_up_sync(0xffffffffu, tgt, 1);
+        if (tgt >= 0 && (lane == 0 || prev != tgt)) atomicMin(keys + tgt, k);
+    }
+}
+
+// The result of a clearance query: one thread per (configuration c, segment b) decodes the point i* of its key and
+// evaluates that single pair with composed_point -- the same descriptors, absolute configuration and flat point index
+// as the per-configuration query -- into the value, world gradient, i* and sub-SDF.  Whichever kernel produced the
+// key, its value is this pair's per-configuration value (robot_clearance_kernel's visits give composed_point's bits
+// for every link kind: tests/test_clearance_cpu.py).
+template <bool kMesh, bool kExt, int MAXS>
+__global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
+clearance_finish_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
+                        int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_seg,
+                        long long seg_len, uint32_t mesh_mode, const unsigned long long *__restrict__ keys,
+                        float *__restrict__ out_val, float *__restrict__ out_grad, int *__restrict__ out_point,
+                        int *__restrict__ out_which, int nearest_first, float margin_max) {
+    NodeStage st; st.smem = nullptr; st.n = 0;
+    const long long n_pts = n_seg * seg_len, total = (long long)cfg_count * n_seg;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += stride) {
+        long long c, b;
+        paired_index(t, n_seg, c, b);
+        const int ip = (int)(uint32_t)keys[t];
+        const long long i = b * seg_len + ip;
+        const int cfg = cfg_begin + (int)c;
+        auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) {
+            const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
+            r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
+        };
+        const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st, load_point(pts, i),
+                                                          mesh_mode, (uint64_t)cfg * (uint64_t)n_pts + (uint64_t)i,
+                                                          nearest_first, margin_max);
+        out_val[t] = o.val;
+        out_grad[3 * t] = o.grad.x; out_grad[3 * t + 1] = o.grad.y; out_grad[3 * t + 2] = o.grad.z;
+        if (out_point) out_point[t] = ip;
+        if (out_which) out_which[t] = o.which;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // Configuration-major variant for RobotSDF-style batches (many joint configurations, shared points).
 //
 // Lanes of a warp are 32 CONFIGURATIONS of the same point instead of 32 points of the same configuration:
@@ -1789,6 +1873,125 @@ robot_swept_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, con
         out_grad[3 * i] = go.x; out_grad[3 * i + 1] = go.y; out_grad[3 * i + 2] = go.z;
         if (out_cfg) out_cfg[i] = cfg;
         if (out_which) out_which[i] = b.which;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Clearance query on the sets robot_serial_kernel takes (<= 8 GRID links with the bounding-box rule, nearest or
+// trilinear, or primitives): for every configuration of the slab and every segment of seg_len points, the smallest
+// clearance_key (pvb_device.cuh) over the segment, left in keys[c * n_seg + b] (~0 on entry); clearance_finish_kernel
+// turns it into the result.  Nothing per pair leaves the SM.
+//   * Orientation and tiles of robot_serial_kernel: grid row blockIdx.y is configuration tile rs_tile(blockIdx.y), its
+//     transforms and sphere centres staged once per block; lanes are the LC configurations of one point, and a warp
+//     holds 32 / LC point groups.
+//   * Work unit: (tile, chunk), a chunk being `chunk` consecutive points of ONE segment; blocks stride over the chunks.
+//     The point groups of the block take the chunk's points in turn.
+//   * Each lane keeps its configuration's running key over the points it has seen.  It evaluates a point through
+//     rs_swept_pair with bp = min(its running value, the seed): a (point, link) pair is skipped only when a lower bound
+//     of its value is STRICTLY above a value that some point of the segment attains, so ties are always evaluated, and
+//     a candidate can only be inexact when its value is above bp -- then it loses to the key that attains bp.
+//   * Seed: at the start of a chunk each lane reads its (configuration, segment) key from global memory -- the best
+//     that earlier blocks have found -- and prunes against its value (a NaN or ~0 key: no pruning).
+//   * End of a chunk: the lanes holding the same configuration (the point groups of a warp, then the 8 warps) reduce
+//     their keys, and one atomicMin per configuration leaves the block.
+struct __align__(16) ClSmem {
+    float4 xf[kRbCfg][3 * kRsMaxS + 1];
+    float4 sph[kRbCfg][3 * kRsMaxS / 4 + 1];
+    unsigned long long red[kRsWarps][kRbCfg];
+};
+
+template <bool kExt>
+__global__ void __launch_bounds__(kRbCfg * kRsWarps, PVB_RS_MINB)
+robot_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, const float *__restrict__ xforms,
+                       int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_seg,
+                       int seg_len, int chunk, int chunks_per_seg, unsigned long long *__restrict__ keys) {
+    __shared__ ClSmem sm;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int c0, lc_log2;
+    rs_tile(cfg_count, blockIdx.y, c0, lc_log2);
+    const int LC = 1 << lc_log2, sub_log2 = 5 - lc_log2;
+    const int cl = lane & (LC - 1), sub = lane >> lc_log2;
+    for (int item = threadIdx.x; item < LC * n_sdf; item += blockDim.x) {
+        const int ci = item & (LC - 1), si = item >> lc_log2;
+        const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg_begin + c0 + ci) * 16);
+        sm.xf[ci][3 * si] = __ldg(row); sm.xf[ci][3 * si + 1] = __ldg(row + 1); sm.xf[ci][3 * si + 2] = __ldg(row + 2);
+    }
+    __syncthreads();
+    for (int item = threadIdx.x; item < LC * kRsMaxS; item += blockDim.x) {
+        const int ci = item & (LC - 1), si = item >> lc_log2;
+        const f3 co = si < n_sdf ? rs_sphere_centre(pk.d[si], sm.xf[ci][3 * si], sm.xf[ci][3 * si + 1],
+                                                    sm.xf[ci][3 * si + 2])
+                                 : mk3(0.f, 0.f, 0.f);
+        float *c = reinterpret_cast<float *>(&sm.sph[ci][0]) + 3 * si;
+        c[0] = co.x; c[1] = co.y; c[2] = co.z;
+    }
+    __syncthreads();
+    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const int groups = kRsWarps << sub_log2;                 // point groups of the block
+    const int gid = (warp << sub_log2) + sub;
+    const long long n_work = n_seg * chunks_per_seg;
+    for (long long w = blockIdx.x; w < n_work; w += gridDim.x) {
+        const long long b = w / chunks_per_seg;
+        const int i0 = (int)(w - b * chunks_per_seg) * chunk;
+        const int len = min(chunk, seg_len - i0);
+        const long long pt0 = b * seg_len + i0;
+        unsigned long long *const kp = keys + (size_t)(c0 + cl) * n_seg + b;
+        const unsigned long long seed_key = __ldcg(kp);
+        const float seed = clearance_key_value(seed_key);
+        unsigned long long run = ~0ull;                      // this lane's running key
+        float rv = PVB_INF;                                  // and its value
+#pragma unroll 1
+        for (int j0 = 0; j0 < len; j0 += groups) {
+            const int j = j0 + gid;
+            const bool on = j < len;
+            if (!__any_sync(0xffffffffu, on)) break;         // uniform per warp: the warp's groups are all past the end
+            const f3 p = on ? load_point(pts, pt0 + j) : mk3(0.f, 0.f, 0.f);
+            float cen[3 * kRsMaxS];
+#pragma unroll
+            for (int k = 0; k < 3 * kRsMaxS / 4; ++k) {
+                const float4 c4 = sm.sph[cl][k];
+                cen[4 * k] = c4.x; cen[4 * k + 1] = c4.y; cen[4 * k + 2] = c4.z; cen[4 * k + 3] = c4.w;
+            }
+            float lb[kRsMaxS], key[kRsMaxS];
+#pragma unroll
+            for (int si = 0; si < kRsMaxS; ++si) {
+                lb[si] = rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], pk.sph_rad[si]);
+                key[si] = rs_bound_key(lb[si], low3_off, si);
+            }
+            const int pred = __shfl_sync(0xffffffffu, rs_nearest(key, n_sdf), sub << lc_log2);
+            auto link = [&](const int si, const float thr, float4 &o) -> bool {
+                const pvb_sdf_desc &d = pk.d[si];
+                const float4 r0 = sm.xf[cl][3 * si], r1 = sm.xf[cl][3 * si + 1], r2 = sm.xf[cl][3 * si + 2];
+                const f3 q = composed_xform(r0, r1, r2, p);
+                const float tm = thr + pk.visit_margin[si];
+                if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
+                o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
+                    : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
+                                                               : robot_lookup(d, q);
+                return true;
+            };
+            float best;
+            f3 bg;
+            int bs;
+            rs_swept_pair(lb, pred, fminf(rv, seed), link, best, bg, bs);
+            if (on && bs >= 0) {
+                const unsigned long long k = clearance_key(best, (uint32_t)(i0 + j));
+                if (k < run) { run = k; rv = best; }
+            }
+        }
+        // the configuration's minimum over the block: the point groups of this warp, then the warps
+        for (int off = LC; off < 32; off <<= 1) {
+            const unsigned long long o = __shfl_xor_sync(0xffffffffu, run, off);
+            run = o < run ? o : run;
+        }
+        if (sub == 0) sm.red[warp][cl] = run;
+        __syncthreads();
+        if (threadIdx.x < LC) {                              // warp 0, point group 0: cl == threadIdx.x
+            unsigned long long m = sm.red[0][cl];
+            for (int v = 1; v < kRsWarps; ++v) m = sm.red[v][cl] < m ? sm.red[v][cl] : m;
+            if (m < seed_key) atomicMin(kp, m);
+        }
+        __syncthreads();                                     // red is rewritten by the next chunk
     }
 }
 
@@ -2836,6 +3039,133 @@ extern "C" int pvb_composed_query_swept(const pvb_sdf_desc *descs, int32_t n_sdf
     const int rc = needs_mesh ? (any_ext ? PVB_SWEPT(true, true) : PVB_SWEPT(true, false))
                               : (any_ext ? PVB_SWEPT(false, true) : PVB_SWEPT(false, false));
 #undef PVB_SWEPT
+    return rc;
+}
+
+// Launch robot_clearance_kernel.  Chunk size from the sizes alone: the longest chunk (at least 64 points, or the whole
+// segment) that still gives >= 4 waves of resident blocks over the tiles x segments x chunks, so that blocks of later
+// waves start from the keys of earlier ones.
+static int launch_robot_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
+                                  int cfg_count, const float *pts, long long n_seg, long long seg_len,
+                                  unsigned long long *keys, bool ext, cudaStream_t stream) {
+    RobotPack<kRsMaxS> pack;
+    memset(&pack, 0, sizeof(pack));
+    for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
+    for (int si = 0; si < kRsMaxS; ++si) {
+        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
+        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
+    }
+    const int gy = (cfg_count >> 5) + __builtin_popcount((unsigned)(cfg_count & 31));
+    const long long want = 4ll * sm_count() * PVB_RS_MINB;          // blocks for 4 waves
+    long long per_seg = (want + (long long)gy * n_seg - 1) / ((long long)gy * n_seg);
+    if (per_seg > (seg_len + 63) / 64) per_seg = (seg_len + 63) / 64;
+    if (per_seg < 1) per_seg = 1;
+    const long long chunk = (seg_len + per_seg - 1) / per_seg;
+    const long long chunks_per_seg = (seg_len + chunk - 1) / chunk;
+    const long long n_work = n_seg * chunks_per_seg;
+    const unsigned gx = (unsigned)(n_work < INT32_MAX ? n_work : INT32_MAX);
+    dim3 grid(gx, (unsigned)gy);
+    timing_mark(0, stream);
+    if (ext)
+        robot_clearance_kernel<true><<<grid, kRbCfg * kRsWarps, 0, stream>>>(
+            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, (int)seg_len, (int)chunk,
+            (int)chunks_per_seg, keys);
+    else
+        robot_clearance_kernel<false><<<grid, kRbCfg * kRsWarps, 0, stream>>>(
+            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, (int)seg_len, (int)chunk,
+            (int)chunks_per_seg, keys);
+    timing_mark(1, stream);
+    PVB_CHECK_LAUNCH("pvb_composed_query_clearance(robot)");
+    return PVB_OK;
+}
+
+// The keys of composed_clearance_kernel (unless `fused`: robot_clearance_kernel already left them), then
+// clearance_finish_kernel.
+template <bool kMesh, bool kExt, int MAXS>
+static int launch_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
+                            int cfg_count, const float *pts, long long n_seg, long long seg_len, uint32_t mesh_mode,
+                            unsigned long long *keys, bool fused, float *out_val, float *out_grad, int *out_point,
+                            int *out_which, cudaStream_t stream) {
+    DescPack<MAXS> pack;
+    memcpy(pack.d, descs, sizeof(pvb_sdf_desc) * (size_t)n_sdf);
+    fill_order(pack, n_sdf);
+    // the same switch as launch_composed: nearest-bound-first evaluation of mesh sub-SDFs
+    static const int nearest_first = [] { const char *e = getenv("PVB_COMP_NEAREST_FIRST"); return e ? atoi(e) : 1; }();
+    float margin_max = 0.f;
+    for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
+    if (!fused) {
+        composed_clearance_kernel<kMesh, kExt, MAXS>
+            <<<grid_for((long long)cfg_count * n_seg * seg_len, kCompThreads, 8), kCompThreads, 0, stream>>>(
+                pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, mesh_mode, keys, nearest_first,
+                margin_max);
+        PVB_CHECK_LAUNCH("pvb_composed_query_clearance");
+    }
+    clearance_finish_kernel<kMesh, kExt, MAXS>
+        <<<grid_for((long long)cfg_count * n_seg, kCompThreads, 8), kCompThreads, 0, stream>>>(
+            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, mesh_mode, keys, out_val, out_grad,
+            out_point, out_which, nearest_first, margin_max);
+    PVB_CHECK_LAUNCH("pvb_composed_query_clearance(finish)");
+    return PVB_OK;
+}
+
+extern "C" int pvb_composed_query_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,
+                                            const float *xforms, int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                                            const float *pts, int64_t n_seg, int64_t seg_len, uint32_t mesh_mode,
+                                            uint64_t *keys, float *out_val, float *out_grad, int32_t *out_point,
+                                            int32_t *out_which, void *stream) {
+    const char *fn = "pvb_composed_query_clearance";
+    if (n_seg < 0 || seg_len < 0 || seg_len >= (1ll << 31) || (seg_len > 0 && n_seg > INT64_MAX / seg_len) ||
+        (cfg_count > 0 && n_seg > INT64_MAX / cfg_count)) {
+        pvb_set_error("%s: invalid argument (n_seg=%lld seg_len=%lld cfg_count=%d; seg_len < 2^31)", fn,
+                      (long long)n_seg, (long long)seg_len, cfg_count);
+        return PVB_ERR_INVALID;
+    }
+    const long long n_pts = n_seg * seg_len;
+    bool any_ext;
+    const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_val,
+                                        out_grad, any_ext);
+    if (bad) return bad;
+    if (n_seg == 0) return PVB_OK;
+    if (cfg_count < 1) {
+        if (n_pts == 0) return PVB_OK;
+        pvb_set_error("%s: no minimum over an empty configuration slab (cfg_count=%d)", fn, cfg_count);
+        return PVB_ERR_INVALID;
+    }
+    if (seg_len == 0) {
+        pvb_set_error("%s: no minimum over an empty segment (seg_len=0, n_seg=%lld)", fn, (long long)n_seg);
+        return PVB_ERR_INVALID;
+    }
+    if (!keys) {
+        pvb_set_error("%s: invalid argument (keys is null)", fn);
+        return PVB_ERR_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    unsigned long long *k = reinterpret_cast<unsigned long long *>(keys);
+    if (cudaMemsetAsync(k, 0xff, sizeof(uint64_t) * (size_t)cfg_count * (size_t)n_seg, s) != cudaSuccess) {
+        pvb_set_error("%s: cudaMemsetAsync(keys) failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+        return PVB_ERR_CUDA;
+    }
+    // robot_serial_kernel's sets take the fused kernel: <= 8 GRID links with the bounding-box rule or primitives, and
+    // one grid row per configuration tile
+    bool fused = !needs_mesh && n_sdf <= kRsMaxS &&
+                 (cfg_count >> 5) + __builtin_popcount((unsigned)(cfg_count & 31)) <= 65535;
+    for (int i = 0; i < n_sdf && fused; ++i)
+        fused = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    if (fused) {
+        const int rc = launch_robot_clearance(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
+                                              k, any_ext, s);
+        if (rc) return rc;
+    }
+#define PVB_CLEARANCE(MESH, TRI)                                                                                   \
+    (n_sdf <= 16 ? launch_clearance<MESH, TRI, 16>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg,   \
+                                                    seg_len, mesh_mode, k, fused, out_val, out_grad, out_point,     \
+                                                    out_which, s)                                                   \
+                 : launch_clearance<MESH, TRI, 128>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg,  \
+                                                     seg_len, mesh_mode, k, fused, out_val, out_grad, out_point,    \
+                                                     out_which, s))
+    const int rc = needs_mesh ? (any_ext ? PVB_CLEARANCE(true, true) : PVB_CLEARANCE(true, false))
+                              : (any_ext ? PVB_CLEARANCE(false, true) : PVB_CLEARANCE(false, false));
+#undef PVB_CLEARANCE
     return rc;
 }
 

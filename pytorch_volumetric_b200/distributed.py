@@ -347,7 +347,7 @@ class PeerResult:
                 self.nat.check(self.nat.lib().pvb_ipc_free(self._local), "pvb_ipc_free")
 
 
-def sharded_robot_query(robot_sdf, points, gather=True, group=None, result=None, paired=False):
+def sharded_robot_query(robot_sdf, points, gather=True, group=None, result=None, paired=False, clearance=False):
     """RobotSDF over this rank's contiguous slab of the (flattened) configuration batch.
 
     The output slab (cfg_count, P) is a contiguous block of the (|A|, P) result, so re-assembly is a plain
@@ -356,12 +356,26 @@ def sharded_robot_query(robot_sdf, points, gather=True, group=None, result=None,
     the returned tensors are views of one of `result`'s two slots and stay valid until the second-next query into
     it (see PeerResult for the cross-rank ordering this relies on).
     paired=True: RobotSDF.paired sharded the same way -- points [*A, *B, N, 3], and this rank evaluates its
-    configurations on their own points[begin:end] only; gather must be True or False."""
+    configurations on their own points[begin:end] only; gather must be True or False.
+    clearance=True: RobotSDF.clearance sharded the same way -- points [*B, N, 3], this rank's slab is
+    (cfg_count, prod(B)) and the re-assembled result ([A,] *B) / (..., 3); gather must be True or False."""
     rank, world = _world(group)
     comp = robot_sdf.sdf
     n_cfg = 1 if comp.tsf_batch is None else math.prod(list(comp.tsf_batch))
     begin, end = shard_range(n_cfg, rank, world)
     batch = tuple(comp.tsf_batch) if comp.tsf_batch is not None else ()
+    if paired and clearance:
+        raise ValueError("paired and clearance queries cannot be combined")
+    if clearance:
+        if isinstance(gather, str):
+            raise ValueError("clearance queries re-assemble with gather=True or gather=False only")
+        n_seg, _ = comp._clearance_segments(tuple(points.shape))
+        if end > begin:
+            val, grad = comp.query_clearance(points, cfg_begin=begin, cfg_count=end - begin)
+        else:                               # more ranks than configurations: this rank's slab is empty
+            dev = torch.device("cuda", torch.cuda.current_device())
+            val, grad = torch.empty(0, device=dev), torch.empty(0, 3, device=dev)
+        return _slab_result(val, grad, begin, end, n_cfg, n_seg, batch, tuple(points.shape[:-2]), gather, group)
     if paired:
         if isinstance(gather, str):
             raise ValueError("paired queries re-assemble with gather=True or gather=False only")

@@ -176,6 +176,13 @@ class RobotSDF(sdf.ObjectFrameSDF):
         (ComposedSDF.swept)."""
         return self.sdf.swept(points_in_object_frame, return_argmin=return_argmin)
 
+    def clearance(self, points_in_object_frame, return_argmin=False):
+        """For every installed joint configuration, the minimum over the points of every segment (the robot's
+        clearance to a cloud): points [*B, N, 3] in the robot frame -> (values [*A, *B], gradients [*A, *B, 3]) and,
+        with return_argmin, the first point attaining it (index into N) and its link, a position in
+        `sdf_to_link_name` (ComposedSDF.clearance)."""
+        return self.sdf.clearance(points_in_object_frame, return_argmin=return_argmin)
+
     def surface_bounding_box(self, **kwargs):
         return self.sdf.surface_bounding_box(**kwargs)
 

@@ -904,6 +904,109 @@ class ComposedSDF(ObjectFrameSDF):
         which = nat.deliver(out[3], out_device, torch.int64).reshape(pts_shape[:-1])
         return vv, gg, cfg, which
 
+    #: configurations per `_generic_query` chunk of the unfused clearance query (bounds its cfg_chunk x P temporaries)
+    clearance_generic_chunk = 64
+
+    @staticmethod
+    def _clearance_segments(shape):
+        """(n_seg, seg_len) of points [*B, N, 3]; ValueError when they are not [..., N, 3]."""
+        if len(shape) < 2 or shape[-1] != 3:
+            raise ValueError(f"clearance query: points {shape} must be [..., N, 3]")
+        return math.prod(shape[:-2]), shape[-2]
+
+    def query_clearance(self, points_in_object_frame, cfg_begin=0, cfg_count=None, return_which=False):
+        """Clearance form of `query`: points [*B, N, 3] are n_seg = prod(B) segments of N points; for configuration
+        cfg_begin + c and segment b, the per-configuration result at the FIRST point of the segment attaining the
+        minimum value, without the cfg_count-fold cross product.  Bit-identical to that reduction of
+        query(..., return_which=True) over the flat points: (value, point) minimised lexicographically, -0 == +0, a NaN
+        value above every number.  Returns flat (cfg_count * n_seg,) / (cfg_count * n_seg, 3) fp32 tensors on the GPU,
+        configuration-major, and with return_which also the int32 point index within the segment and sub-SDF index."""
+        S = len(self.sdfs)
+        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
+        if cfg_count is None:
+            cfg_count = n_cfg - cfg_begin
+        n_seg, seg_len = self._clearance_segments(tuple(points_in_object_frame.shape))
+        if n_seg > 0 and seg_len == 0 and cfg_count > 0:
+            raise ValueError("clearance query: no minimum over an empty segment (N = 0)")
+        if cfg_count < 1 and n_seg * seg_len > 0:
+            raise ValueError(f"clearance query: no minimum over an empty configuration slab (cfg_count={cfg_count})")
+        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
+        with torch.cuda.device(device):
+            p = nat.as_f32_points(points_in_object_frame, device)
+            descs_arr, needs_mesh = self._native_descs(device)
+            if descs_arr is None:
+                return self._generic_clearance(p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which)
+            xf = self._xforms_on(device)
+            R = max(cfg_count, 0) * n_seg
+            keys = torch.empty(R, dtype=torch.int64, device=device)
+            val = torch.empty(R, dtype=torch.float32, device=device)
+            grad = torch.empty(R, 3, dtype=torch.float32, device=device)
+            point = torch.empty(R, dtype=torch.int32, device=device) if return_which else None
+            which = torch.empty(R, dtype=torch.int32, device=device) if return_which else None
+            nat.check(nat.lib().pvb_composed_query_clearance(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg,
+                                                             cfg_begin, cfg_count, nat.ptr(p), n_seg, seg_len,
+                                                             nat.PVB_MESH_DEFAULT, nat.ptr(keys), nat.ptr(val),
+                                                             nat.ptr(grad), nat.ptr(point), nat.ptr(which),
+                                                             nat.stream_ptr(device)), "pvb_composed_query_clearance")
+        return (val, grad, point, which) if return_which else (val, grad)
+
+    @staticmethod
+    def _clearance_keys(v):
+        """The kernels' clearance_key (pvb_device.cuh) of values v [..., N] and their index along the last dimension,
+        as int64 in the same order (the unsigned key minus 2^63): its minimum names the first point attaining the
+        minimum value, with -0 == +0 and a NaN value above every number."""
+        v = torch.where(v == 0, torch.zeros_like(v), v)
+        b = v.view(torch.int32).to(torch.int64) & 0xFFFFFFFF
+        h = torch.where(b >= 1 << 31, 0xFFFFFFFF - b, b + (1 << 31))
+        h = torch.where(torch.isnan(v), torch.full_like(h, 0xFFFFFFFF), h)
+        i = torch.arange(v.shape[-1], device=v.device, dtype=torch.int64)
+        return ((h - (1 << 31)) << 32) | i
+
+    def _generic_clearance(self, p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which):
+        """query_clearance for sub-SDFs without native descriptors: configuration chunks through `_generic_query`,
+        each reduced over the points of every segment by the kernels' key order."""
+        R = max(cfg_count, 0) * n_seg
+        val = torch.empty(R, dtype=torch.float32, device=p.device)
+        grad = torch.empty(R, 3, dtype=torch.float32, device=p.device)
+        point = torch.empty(R, dtype=torch.int32, device=p.device)
+        which = torch.empty(R, dtype=torch.int32, device=p.device)
+        for c0 in range(cfg_begin, cfg_begin + (cfg_count if R > 0 else 0), self.clearance_generic_chunk):
+            cc = min(self.clearance_generic_chunk, cfg_begin + cfg_count - c0)
+            v, g, w = self._generic_query(p, c0, cc, n_cfg, True)
+            v, g, w = v.reshape(cc, n_seg, seg_len), g.reshape(cc, n_seg, seg_len, 3), w.reshape(cc, n_seg, seg_len)
+            i = (self._clearance_keys(v).amin(dim=-1) & 0xFFFFFFFF)[..., None]
+            out = slice((c0 - cfg_begin) * n_seg, (c0 - cfg_begin + cc) * n_seg)
+            val[out] = v.gather(-1, i).reshape(-1)
+            grad[out] = g.gather(-2, i[..., None].expand(cc, n_seg, 1, 3)).reshape(-1, 3)
+            point[out] = i.reshape(-1).to(torch.int32)
+            which[out] = w.gather(-1, i).reshape(-1)
+        return (val, grad, point, which) if return_which else (val, grad)
+
+    def clearance(self, points_in_object_frame, return_argmin=False):
+        """For every installed configuration, the minimum over the points of every segment (the clearance of the
+        configuration to a cloud): points [*B, N, 3] give (values [*A, *B], gradients [*A, *B, 3]) in the points'
+        dtype and on their device, A the configuration batch.  Entry [a, b] is configuration a's result at the first
+        point of points[b] attaining the minimum value: bit-identical to __call__ followed by that reduction over the
+        point dimension, without materialising the |A| x N cross product.  With return_argmin, also that point's index
+        into N (int64) and the sub-SDF index, each [*A, *B].  Without a configuration batch the result is [*B].  Not a
+        reference operator (an extension); raises ValueError before any device work when the points are not
+        [..., N, 3] or N = 0 with segments to reduce."""
+        pts_shape = tuple(points_in_object_frame.shape)
+        n_seg, seg_len = self._clearance_segments(pts_shape)
+        if n_seg > 0 and seg_len == 0:
+            raise ValueError("clearance query: no minimum over an empty segment (N = 0)")
+        out = self.query_clearance(points_in_object_frame, return_which=return_argmin)
+        shape = (*(self.tsf_batch or ()), *pts_shape[:-2])
+        dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
+        out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
+        vv = nat.deliver(out[0], out_device, dtype).reshape(shape)
+        gg = nat.deliver(out[1], out_device, dtype).reshape(*shape, 3)
+        if not return_argmin:
+            return vv, gg
+        point = nat.deliver(out[2], out_device, torch.int64).reshape(shape)
+        which = nat.deliver(out[3], out_device, torch.int64).reshape(shape)
+        return vv, gg, point, which
+
     def query_into(self, points_in_object_frame, targets, cfg_begin=0, cfg_count=None):
         """`query` whose result slab is stored by the kernel epilogue into several full-size result buffers at once
         (pvb_composed_query_multi): `targets` is a list of (val, grad) pairs, each a float32 tensor or a raw device
