@@ -793,7 +793,10 @@ __device__ __forceinline__ ComposedOut composed_point(const pvb_sdf_desc *descs,
                 const bool bounded = (d.kind == PVB_KIND_GRID || (kExt && d.kind != PVB_KIND_MESH))
                                          ? (d.flags & PVB_GRID_PRUNE_OK) != 0
                                          : (d.kind == PVB_KIND_MESH && (d.flags & PVB_MESH_CLOSED) && (mesh_mode & PVB_MESH_SIGNED));
-                key[s] = bounded ? composed_aabb_lb2(d, composed_xform(r0, r1, r2, p)) : -1.f;
+                const float lb2 = bounded ? composed_aabb_lb2(d, composed_xform(r0, r1, r2, p)) : -1.f;
+                // a closed mesh is bounded only from OUTSIDE its box (composed_consider): inside it, its value may be
+                // as deep as the mesh itself, far below -prune_margin, so a query in the box has no bound
+                key[s] = (d.kind == PVB_KIND_MESH && !(lb2 > 0.f)) ? -1.f : lb2;
             }
             while (todo) {
                 int s = -1;

@@ -755,7 +755,10 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
                         const bool bounded = (d.kind == PVB_KIND_GRID || (kExt && d.kind != PVB_KIND_MESH))
                                                  ? (d.flags & PVB_GRID_PRUNE_OK) != 0
                                                  : (d.kind == PVB_KIND_MESH && (d.flags & PVB_MESH_CLOSED) && (mesh_mode & PVB_MESH_SIGNED));
-                        key[s] = bounded ? composed_aabb_lb2(d, composed_xform(r0, r1, r2, p[0])) : -1.f;
+                        const float lb2 = bounded ? composed_aabb_lb2(d, composed_xform(r0, r1, r2, p[0])) : -1.f;
+                        // a closed mesh is bounded only from OUTSIDE its box (composed_consider): inside it, its value may be
+                        // as deep as the mesh itself, far below -prune_margin, so a query in the box has no bound
+                        key[s] = (d.kind == PVB_KIND_MESH && !(lb2 > 0.f)) ? -1.f : lb2;
                     }
                     while (todo) {
                         int s = -1;

@@ -723,17 +723,20 @@ class ComposedSDF(ObjectFrameSDF):
         return slice(i * total_to_slice, (i + 1) * total_to_slice)
 
     # -- fused path ---------------------------------------------------------------
+    #: most sub-SDFs one fused-kernel launch takes (pvb_composed_query* refuse more)
+    max_fused_sdfs = 128
+
     def _native_descs(self, device):
+        """(descriptor array, needs_mesh) for the fused kernels, or (None, False) when the set must take the generic
+        per-sub-SDF path: some sub-SDF has no native descriptor, or there are more than `max_fused_sdfs` of them."""
         key = (device, tuple(id(s) for s in self.sdfs))
         hit = self._desc_cache.get(key)
         if hit is None:
-            descs = [s.native_desc(device) for s in self.sdfs]
-            if any(d is None for d in descs):
+            descs = None if len(self.sdfs) > self.max_fused_sdfs else [s.native_desc(device) for s in self.sdfs]
+            if descs is None or any(d is None for d in descs):
                 hit = (None, False, None)
             else:
                 needs_mesh = any(d.kind == nat.PVB_KIND_MESH or (d.flags & nat.PVB_GRID_OOB_GT) for d in descs)
-                if len(descs) > 128:
-                    raise ValueError("ComposedSDF: at most 128 sub-SDFs are supported by the fused kernel")
                 hit = (nat.desc_array(descs), needs_mesh, descs)
             self._desc_cache = {key: hit}
         return hit[0], hit[1]
@@ -1024,7 +1027,8 @@ class ComposedSDF(ObjectFrameSDF):
             P = p.shape[0]
             descs_arr, needs_mesh = self._native_descs(device)
             if descs_arr is None:
-                raise NotImplementedError("query_into needs sub-SDFs with native descriptors (mesh / cached / sphere)")
+                raise NotImplementedError("query_into needs the fused kernels: at most 128 sub-SDFs, all with native "
+                                          "descriptors")
             arr = (nat.OutTarget * len(targets))()
             for t, (tv, tg) in enumerate(targets):
                 for buf, per in ((tv, 1), (tg, 3)):
@@ -1054,7 +1058,7 @@ class ComposedSDF(ObjectFrameSDF):
             P = p.shape[0]
             descs_arr, needs_mesh = self._native_descs(device)
             if descs_arr is None:
-                raise NotImplementedError("query_at needs sub-SDFs with native descriptors (mesh / cached / sphere)")
+                raise NotImplementedError("query_at needs the fused kernels: at most 128 sub-SDFs, all with native descriptors")
             xf = self._xforms_on(device)
             nat.check(nat.lib().pvb_composed_query(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg, cfg_begin,
                                                    cfg_count, nat.ptr(p), P, nat.PVB_MESH_DEFAULT,
@@ -1075,7 +1079,8 @@ class ComposedSDF(ObjectFrameSDF):
             P = p.shape[0]
             descs_arr, needs_mesh = self._native_descs(device)
             if descs_arr is None:
-                raise NotImplementedError("query_multicast needs sub-SDFs with native descriptors")
+                raise NotImplementedError("query_multicast needs the fused kernels: at most 128 sub-SDFs, all with native "
+                                          "descriptors")
             xf = self._xforms_on(device)
             nat.check(nat.lib().pvb_composed_query_multicast(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg, cfg_begin,
                                                              cfg_count, nat.ptr(p), P, nat.PVB_MESH_DEFAULT,

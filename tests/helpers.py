@@ -109,17 +109,53 @@ def _aabb_rule(bb, q):
     return dist, (delta / dist if dist > 0 else delta)
 
 
+def _primitive_alternatives(spec, q):
+    """(value, sub-frame gradient, gradient slack) pairs of a BOX / CYLINDER spec at q (3,): the fp64 result, plus
+    the other axis of the inside rule wherever two of its terms are within 1e-5 (fp32 rounding may pick either).  The
+    slack is the fp32 conditioning of the outside gradient w / |w| near the surface and of the radial direction near
+    a cylinder's axis (tests/test_gpu_primitive.py)."""
+    import primitive_ref as pr
+    q = np.asarray(q, dtype=np.float64)
+    scale = 3e-7 * np.abs(q).max()
+    if spec["kind"] == "box":
+        v, g = pr.box_ref(spec["half"], q[None])
+        v, g = float(v[0]), g[0]
+        slack = scale / max(abs(v), 1e-30) if v > -1e-6 else 0.0
+        out = [(v, g, slack)]
+        if v <= 0:
+            e = np.abs(q) - np.asarray(spec["half"])
+            for k in np.nonzero(e >= e.max() - 1e-5)[0]:
+                gk = np.zeros(3)
+                gk[k] = 1.0 if q[k] >= 0 else -1.0
+                out.append((v, gk, slack))
+        return out
+    v, g = pr.cylinder_ref(spec["radius"], spec["half_length"], q[None])
+    v, g = float(v[0]), g[0]
+    rho = float(np.hypot(q[0], q[1]))
+    slack = scale / max(min(abs(v) if v > -1e-6 else np.inf, rho), 1e-30)
+    out = [(v, g, slack)]
+    dr, dz = rho - spec["radius"], abs(q[2]) - spec["half_length"]
+    if v <= 0 and abs(dr - dz) < 1e-5:
+        ux, uy = (q[0] / rho, q[1] / rho) if rho > 0 else (1.0, 0.0)
+        out += [(v, np.array([ux, uy, 0.0]), slack), (v, np.array([0.0, 0.0, 1.0 if q[2] >= 0 else -1.0]), slack)]
+    return out
+
+
 def flip_candidates(specs, M, p):
-    """All (value, object-frame gradient) pairs the reference's rules can produce for point p (3,) under the
-    object->sub-frame matrices M (S,4,4, fp64) when every link-frame coordinate within FLIP_BAND of a cell boundary
-    (or 1e-6 m of the range edge) is allowed to fall on either side."""
+    """All (value, object-frame gradient, sub-SDF, gradient slack) the reference's rules can produce for point p (3,)
+    under the object->sub-frame matrices M (S,4,4, fp64) when every link-frame coordinate within FLIP_BAND of a cell
+    boundary (or 1e-6 m of the range edge) is allowed to fall on either side, and a primitive's inside rule may pick
+    either of two near-equal axes.  The slack is added to the gradient tolerance of that candidate."""
     out = []
     for s, spec in enumerate(specs):
         R, t = M[s, :3, :3], M[s, :3, 3]
         q = R @ p + t
         if spec["kind"] == "sphere":
             r = np.linalg.norm(q)
-            out.append((r - spec["radius"], (q / (r + 1e-12)) @ R, s))
+            out.append((r - spec["radius"], (q / (r + 1e-12)) @ R, s, 0.0))
+            continue
+        if spec["kind"] in ("box", "cylinder"):
+            out += [(v, g @ R, s, slack) for v, g, slack in _primitive_alternatives(spec, q)]
             continue
         lo, hi, val, grad = spec["lo"], spec["hi"], spec["val"], spec["grad"]
         n = np.array(val.shape)
@@ -140,10 +176,10 @@ def flip_candidates(specs, M, p):
             for kx in opts[0]:
                 for ky in opts[1]:
                     for kz in opts[2]:
-                        out.append((val[kx, ky, kz], grad[kx, ky, kz] @ R, s))
+                        out.append((val[kx, ky, kz], grad[kx, ky, kz] @ R, s, 0.0))
         if maybe_out:
             d, g = _aabb_rule(spec["bb"], q)
-            out.append((d, g @ R, s))
+            out.append((d, g @ R, s, 0.0))
     return out
 
 
@@ -162,15 +198,15 @@ def classify_composed(v_gpu, g_gpu, v_ref, g_ref, specs, mats, pts, tol=1e-5):
         cands = flip_candidates(specs, mats[:, a], pts[i])
         # a valid output is min over sub-SDFs of ONE alternative each: it lies between the two extreme choices
         per_s = {}
-        for cv, _cg, s_ in cands:
+        for cv, _cg, s_, _sl in cands:
             lo_hi = per_s.setdefault(s_, [cv, cv])
             lo_hi[0], lo_hi[1] = min(lo_hi[0], cv), max(lo_hi[1], cv)
         lower = min(v[0] for v in per_s.values())
         upper = min(v[1] for v in per_s.values())
         ok = False
         if lower - tol <= v_gpu[a, i] <= upper + tol:
-            for cv, cg, _s in cands:
-                if abs(cv - v_gpu[a, i]) <= tol and np.abs(cg - g_gpu[a, i]).max() <= tol:
+            for cv, cg, _s, slack in cands:
+                if abs(cv - v_gpu[a, i]) <= tol and np.abs(cg - g_gpu[a, i]).max() <= tol + slack:
                     ok = True
                     break
         if not ok:
