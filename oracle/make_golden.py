@@ -13,7 +13,7 @@ TEST INFRASTRUCTURE.  Two kinds of fixtures:
    dependencies).  They pin oracle/port.py (tests/test_oracle_pinning.py) and serve as golden vectors for
    the CUDA path (tests/test_gpu_mesh.py, test_gpu_cached.py, test_gpu_composed.py, test_gpu_chamfer_sample.py).
 
-Run:  PVB_REFERENCE_SRC=<checkout> python -m oracle.make_golden [voxel|robot_r008]
+Run:  PVB_REFERENCE_SRC=<checkout> python -m oracle.make_golden [voxel|robot_r008|chamfer_pairwise]
 """
 import atexit
 import os
@@ -212,6 +212,42 @@ def make_reference_vectors():
         np.savez_compressed(os.path.join(GOLD, f"ref_chamfer_{name}.npz"), pts_world=pts_world.numpy(),
                             w2o=w2o.numpy(), err0=err0.numpy(), w2o_p=w2o_p.numpy(), err1=err1.numpy())
         print(name, "chamfer: err0 max", float(err0.max()), "err1 mean", float(err1.mean()))
+    make_chamfer_pairwise_vectors(pv, pk, tmp)
+
+
+def make_chamfer_pairwise_vectors(pv, pk, tmp):
+    """pairwise_distance_chamfer (chamfer.py:20-59) with B_world_to_link_tfs given (|A| = 5, |B| = 3: the view
+    re-chunks the flat data) and None, and PlausibleDiversity (chamfer.py:130-195) one-way and bidirectional with
+    |T_est_inv| = 4, |T_p| = 6, on the probe mesh and 200 points near its surface -> ref_chamfer_pairwise.npz."""
+    obj = pv.MeshObjectFactory(os.path.join(REF, MESHES["probe"]))
+    pts, _, _ = pv.sample_mesh_points(obj, name="probe", num_points=200, seed=4,
+                                      dbpath=os.path.join(tmp, "mpp_probe.pkl"), clean_cache=True)
+    g = torch.Generator().manual_seed(21)
+    pts = (pts + 0.002 * torch.randn(pts.shape, generator=g)).float()
+    torch.manual_seed(22)
+    gt = pk.Transform3d(pos=torch.randn(3) * 0.1, rot=pk.random_rotation())
+    A = gt.sample_perturbations(5, radian_sigma=0.2, translation_sigma=0.02)
+    Bw = gt.sample_perturbations(3, radian_sigma=0.2, translation_sigma=0.02).inverse()
+    np.random.seed(23)
+    err_given = pv.pairwise_distance_chamfer(A, Bw, obj_factory=obj, model_points_eval=pts)
+    np.random.seed(24)
+    err_none = pv.pairwise_distance_chamfer(A, None, obj_factory=obj, model_points_eval=pts)
+    T_est_inv = gt.sample_perturbations(4, radian_sigma=0.2, translation_sigma=0.02).inverse().get_matrix()
+    T_p = gt.sample_perturbations(6, radian_sigma=0.2, translation_sigma=0.02).get_matrix()
+    pd = pv.PlausibleDiversity(obj, model_points_eval=pts)
+    np.random.seed(25)
+    r1 = pd(T_est_inv, T_p)
+    np.random.seed(26)
+    r2 = pd(T_est_inv, T_p, bidirectional=True)
+    np.savez_compressed(os.path.join(GOLD, "ref_chamfer_pairwise.npz"), pts=pts.numpy(),
+                        A=A.get_matrix().numpy(), B_w2l=Bw.get_matrix().numpy(), err_given=err_given.numpy(),
+                        err_none=err_none.numpy(), T_est_inv=T_est_inv.numpy(), T_p=T_p.numpy(),
+                        pd_plausibility=float(r1.plausibility), pd_coverage=float(r1.coverage),
+                        pd_best_est=r1.most_plausible_per_estimated.indices.numpy(),
+                        pd_best_pl=r1.most_covered_per_plausible.indices.numpy(),
+                        pd2_plausibility=float(r2.plausibility), pd2_coverage=float(r2.coverage))
+    print("chamfer pairwise:", tuple(err_given.shape), tuple(err_none.shape), float(r1.plausibility),
+          float(r2.coverage))
 
 
 def make_robot_r008_vectors(pv, pk, tmp):
@@ -314,6 +350,11 @@ if __name__ == "__main__":
         import pytorch_volumetric as pv
         import pytorch_kinematics as pk
         make_robot_r008_vectors(pv, pk, scratch_dir())
+    elif len(sys.argv) > 1 and sys.argv[1] == "chamfer_pairwise":
+        import_reference()
+        import pytorch_volumetric as pv
+        import pytorch_kinematics as pk
+        make_chamfer_pairwise_vectors(pv, pk, scratch_dir())
     else:
         make_meshes()
         make_reference_vectors()

@@ -2231,16 +2231,35 @@ __global__ void fk_serial_kernel(const __grid_constant__ FkPlan plan, const floa
 }
 
 // =================================================================== chamfer
-// grid = (tiles, n_tf).  Each block: transform its points with W_b, unsigned
-// distance (no sign pass: the value is squared, chamfer.py:92), block-reduce
-// (scale*d)^2 into one partial; a second tiny kernel sums the partials in a
-// fixed order (deterministic) and divides by N.
+// grid = (tiles, transforms).  Each block: transform its points with W_b, unsigned distance (no sign pass: the value
+// is squared, chamfer.py:92), sd = scale*d.  Thread t of block k sums fmaf(sd, sd, acc) over the points
+// i = k*256 + t, i + stride, ... in that order; the block sums its 8 warps in order into one partial, and
+// chamfer_finish_kernel adds the partials in fp64 in a fixed order and divides by N.  Every step of the sum is in a
+// fixed order, so the result is a function of the inputs and the grid size only.
+// A binned cloud (mesh, >= kSortMinPoints points) is walked in binned order for tree-walk locality, but the order
+// within a Morton cell is set by the atomics of sort_scatter_kernel.  So that pass only stores sd (coalesced, at its
+// binned position) and chamfer_sum_kernel then sums that scratch through the inverse permutation, with the unbinned
+// assignment and order above: binned and unbinned results are equal bit for bit.
 constexpr int kChamThreads = 256;
+constexpr int kChamSdPass = 4;      // transforms per binned pass: 4 floats per point fit the 16-byte result staging
 
+__device__ __forceinline__ void chamfer_block_partial(float acc, float *s_red, float *partial_slot) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float s = 0.f;
+        for (int w = 0; w < kChamThreads / 32; ++w) s += s_red[w];
+        *partial_slot = s;
+    }
+}
+
+// sorted == nullptr: sums into partial.  Otherwise (binned order): stores sd to sd_out[blockIdx.y * n_pts + j].
 __global__ void __launch_bounds__(kChamThreads)
 chamfer_partial_kernel(const pvb_sdf_desc obj, const float *__restrict__ w2o, const float *__restrict__ pts,
                        long long n_pts, const float4 *__restrict__ sorted, float scale, int n_stage_max,
-                       float *__restrict__ partial) {
+                       float *__restrict__ partial, float *__restrict__ sd_out) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ uint64_t bar;
     __shared__ float s_red[kChamThreads / 32];
@@ -2277,17 +2296,29 @@ chamfer_partial_kernel(const pvb_sdf_desc obj, const float *__restrict__ w2o, co
             d = primitive_eval(obj, q).val;
         }
         const float sd = scale * d;
-        acc = fmaf(sd, sd, acc);
+        if (sorted)
+            sd_out[(size_t)blockIdx.y * n_pts + j] = sd;
+        else
+            acc = fmaf(sd, sd, acc);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float s = 0.f;
-        for (int w = 0; w < kChamThreads / 32; ++w) s += s_red[w];
-        partial[(size_t)blockIdx.y * gridDim.x + blockIdx.x] = s;
+    if (sorted) return;
+    chamfer_block_partial(acc, s_red, partial + (size_t)blockIdx.y * gridDim.x + blockIdx.x);
+}
+
+// the unbinned kernel's sum over the scratch of a binned pass (same grid, same assignment and order): point i's sd
+// is at its binned position inv[i]
+__global__ void __launch_bounds__(kChamThreads)
+chamfer_sum_kernel(const float *__restrict__ sd, const uint32_t *__restrict__ inv, long long n_pts,
+                   float *__restrict__ partial) {
+    __shared__ float s_red[kChamThreads / 32];
+    const float *row = sd + (size_t)blockIdx.y * n_pts;
+    float acc = 0.f;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < n_pts; j += stride) {
+        const float s = __ldg(row + __ldg(inv + j));
+        acc = fmaf(s, s, acc);
     }
+    chamfer_block_partial(acc, s_red, partial + (size_t)blockIdx.y * gridDim.x + blockIdx.x);
 }
 
 __global__ void chamfer_finish_kernel(const float *__restrict__ partial, int n_blk, long long n_pts,
@@ -3455,12 +3486,27 @@ extern "C" int pvb_chamfer(const pvb_sdf_desc *obj, const float *world_to_object
         sq = sort_queries(obj, pts, n_pts, world_to_object, sort_workspace,
                           (size_t)(sort_workspace_bytes < 0 ? 0 : sort_workspace_bytes), (cudaStream_t)stream, &rc);
     if (rc != PVB_OK) return rc;
-    dim3 grid((unsigned)n_blk, (unsigned)n_tf);
     timing_mark(0, (cudaStream_t)stream);
-    chamfer_partial_kernel<<<grid, kChamThreads, (size_t)n_stage * 128, (cudaStream_t)stream>>>(
-        *obj, world_to_object, pts, n_pts, sq.sorted, scale, n_stage, workspace);
+    if (!sq.sorted) {
+        chamfer_partial_kernel<<<dim3((unsigned)n_blk, (unsigned)n_tf), kChamThreads, (size_t)n_stage * 128,
+                                 (cudaStream_t)stream>>>(*obj, world_to_object, pts, n_pts, nullptr, scale, n_stage,
+                                                         workspace, nullptr);
+        PVB_CHECK_LAUNCH("pvb_chamfer(partial)");
+    } else {
+        // binned: scaled distances of kChamSdPass transforms at a time in the result staging (16 B per point), then
+        // the unbinned kernel's fixed-order sum over them
+        float *sd = reinterpret_cast<float *>(sq.stage);
+        for (int b0 = 0; b0 < n_tf; b0 += kChamSdPass) {
+            const dim3 grid((unsigned)n_blk, (unsigned)(n_tf - b0 < kChamSdPass ? n_tf - b0 : kChamSdPass));
+            chamfer_partial_kernel<<<grid, kChamThreads, (size_t)n_stage * 128, (cudaStream_t)stream>>>(
+                *obj, world_to_object + (size_t)b0 * 16, pts, n_pts, sq.sorted, scale, n_stage, nullptr, sd);
+            PVB_CHECK_LAUNCH("pvb_chamfer(partial)");
+            chamfer_sum_kernel<<<grid, kChamThreads, 0, (cudaStream_t)stream>>>(sd, sq.inv, n_pts,
+                                                                               workspace + (size_t)b0 * n_blk);
+            PVB_CHECK_LAUNCH("pvb_chamfer(sum)");
+        }
+    }
     timing_mark(1, (cudaStream_t)stream);
-    PVB_CHECK_LAUNCH("pvb_chamfer(partial)");
     chamfer_finish_kernel<<<n_tf, 32, 0, (cudaStream_t)stream>>>(workspace, n_blk, n_pts, out);
     PVB_CHECK_LAUNCH("pvb_chamfer(finish)");
     return PVB_OK;
