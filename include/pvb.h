@@ -247,6 +247,22 @@ int pvb_composed_query_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, int32
                                  uint64_t *keys, float *out_val, float *out_grad,
                                  int32_t *out_point, int32_t *out_which, void *stream);
 
+/* ---- EXTENSION: paired clearance query, every configuration against its own points ----
+ * The reference has no such operator; its equivalent is the per-configuration clearance over each configuration's own
+ * cloud, pvb_composed_query_clearance(pts[c], cfg_begin + c, 1) for every c.  pts DEVICE [cfg_count][n_seg][seg_len][3]:
+ * segment b of configuration cfg_begin + c is pts[c][b].  Entry c * n_seg + b of every output is bit-identical to entry
+ * b of that per-configuration call (value, gradient, point i* within the segment, sub-SDF), mesh ray jitter included:
+ * the jitter index of pts[c][b][i] is (cfg_begin + c) * n_seg * seg_len + b * seg_len + i, as in the paired and the
+ * per-configuration query.  Equivalently, the first-point (value, i) minimum of pvb_composed_query_paired's results over
+ * each segment; -0 == +0 and a NaN value ranks above every number, as in pvb_composed_query_clearance.
+ * Arguments and refusals are those of pvb_composed_query_clearance (keys: device scratch of cfg_count * n_seg entries
+ * that the library initialises), plus PVB_ERR_INVALID when cfg_count * n_seg * seg_len overflows int64. */
+int pvb_composed_query_paired_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,
+                                        const float *xforms, int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                                        const float *pts, int64_t n_seg, int64_t seg_len, uint32_t mesh_mode,
+                                        uint64_t *keys, float *out_val, float *out_grad,
+                                        int32_t *out_point, int32_t *out_which, void *stream);
+
 /* ---- the same query with the result slab stored to several destinations from the kernel epilogue ----
  * Multi-GPU re-assembly of a configuration-sharded RobotSDF result (model_to_sdf.py:117-125 returns the full
  * (|A|, N) tensors): every rank evaluates its slab [cfg_begin, cfg_begin + cfg_count) and writes it straight into

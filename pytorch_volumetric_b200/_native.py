@@ -142,6 +142,12 @@ _SIGNATURES = {
                                                     ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32,
                                                     ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                                     ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "pvb_composed_query_paired_clearance": (ctypes.c_int, [ctypes.POINTER(SdfDesc), ctypes.c_int32, ctypes.c_int32,
+                                                           ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                                           ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,
+                                                           ctypes.c_int64, ctypes.c_uint32, ctypes.c_void_p,
+                                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                                           ctypes.c_void_p, ctypes.c_void_p]),
     "pvb_composed_query_multi": (ctypes.c_int, [ctypes.POINTER(SdfDesc), ctypes.c_int32, ctypes.c_int32,
                                                 ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                                 ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint32, ctypes.c_void_p,

@@ -913,12 +913,16 @@ composed_swept_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
 // pair t = c * n_pts + i runs composed_point with the absolute configuration and the flat point index, the jitter
 // inputs of the per-configuration query.  The lanes of a warp cover consecutive pairs, so lanes of the same key form
 // runs: a segmented shuffle reduction leaves each run's minimum in its first lane, which issues one atomicMin.
-template <bool kMesh, bool kExt, int MAXS>
-__global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
-composed_clearance_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
-                          int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_seg,
-                          long long seg_len, uint32_t mesh_mode, unsigned long long *__restrict__ keys,
-                          int nearest_first, float margin_max) {
+// kPaired (composed_paired_clearance_kernel, pvb_composed_query_paired_clearance): configuration c has its own points,
+// the point of pair t is pts[t] instead of pts[i]; the jitter index stays cfg * n_pts + i, that of the
+// per-configuration query on pts[c].  (The flag sits on the inlined body, so that composed_clearance_kernel keeps its
+// name and its code.)
+template <bool kMesh, bool kExt, int MAXS, bool kPaired>
+__device__ __forceinline__ void clearance_pairs(const DescPack<MAXS> &descs, int n_sdf, const float *__restrict__ xforms,
+                                                int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts,
+                                                long long n_seg, long long seg_len, uint32_t mesh_mode,
+                                                unsigned long long *__restrict__ keys, int nearest_first,
+                                                float margin_max) {
     NodeStage st; st.smem = nullptr; st.n = 0;
     const int lane = threadIdx.x & 31;
     const long long n_pts = n_seg * seg_len, total = (long long)cfg_count * n_pts;
@@ -938,7 +942,7 @@ composed_clearance_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sd
                 r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
             };
             const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st,
-                                                              load_point(pts, i), mesh_mode,
+                                                              load_point(pts, kPaired ? t : i), mesh_mode,
                                                               (uint64_t)cfg * (uint64_t)n_pts + (uint64_t)i,
                                                               nearest_first, margin_max);
             k = clearance_key(o.val, (uint32_t)(i - b * seg_len));
@@ -955,18 +959,41 @@ composed_clearance_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sd
     }
 }
 
+template <bool kMesh, bool kExt, int MAXS>
+__global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
+composed_clearance_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
+                          int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_seg,
+                          long long seg_len, uint32_t mesh_mode, unsigned long long *__restrict__ keys,
+                          int nearest_first, float margin_max) {
+    clearance_pairs<kMesh, kExt, MAXS, false>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
+                                              mesh_mode, keys, nearest_first, margin_max);
+}
+
+template <bool kMesh, bool kExt, int MAXS>
+__global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
+composed_paired_clearance_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf,
+                                 const float *__restrict__ xforms, int n_cfg, int cfg_begin, int cfg_count,
+                                 const float *__restrict__ pts, long long n_seg, long long seg_len, uint32_t mesh_mode,
+                                 unsigned long long *__restrict__ keys, int nearest_first, float margin_max) {
+    clearance_pairs<kMesh, kExt, MAXS, true>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
+                                             mesh_mode, keys, nearest_first, margin_max);
+}
+
 // The result of a clearance query: one thread per (configuration c, segment b) decodes the point i* of its key and
 // evaluates that single pair with composed_point -- the same descriptors, absolute configuration and flat point index
 // as the per-configuration query -- into the value, world gradient, i* and sub-SDF.  Whichever kernel produced the
 // key, its value is this pair's per-configuration value (robot_clearance_kernel's visits give composed_point's bits
-// for every link kind: tests/test_clearance_cpu.py).
-template <bool kMesh, bool kExt, int MAXS>
-__global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
-clearance_finish_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
-                        int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_seg,
-                        long long seg_len, uint32_t mesh_mode, const unsigned long long *__restrict__ keys,
-                        float *__restrict__ out_val, float *__restrict__ out_grad, int *__restrict__ out_point,
-                        int *__restrict__ out_which, int nearest_first, float margin_max) {
+// for every link kind: tests/test_clearance_cpu.py).  kPaired (paired_clearance_finish_kernel): the point of (c, b) is
+// pts[c * n_pts + i], as in composed_paired_clearance_kernel.
+template <bool kMesh, bool kExt, int MAXS, bool kPaired>
+__device__ __forceinline__ void clearance_finish(const DescPack<MAXS> &descs, int n_sdf,
+                                                 const float *__restrict__ xforms, int n_cfg, int cfg_begin,
+                                                 int cfg_count, const float *__restrict__ pts, long long n_seg,
+                                                 long long seg_len, uint32_t mesh_mode,
+                                                 const unsigned long long *__restrict__ keys,
+                                                 float *__restrict__ out_val, float *__restrict__ out_grad,
+                                                 int *__restrict__ out_point, int *__restrict__ out_which,
+                                                 int nearest_first, float margin_max) {
     NodeStage st; st.smem = nullptr; st.n = 0;
     const long long n_pts = n_seg * seg_len, total = (long long)cfg_count * n_seg;
     const long long stride = (long long)gridDim.x * blockDim.x;
@@ -980,14 +1007,40 @@ clearance_finish_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf,
             const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
             r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
         };
-        const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st, load_point(pts, i),
-                                                          mesh_mode, (uint64_t)cfg * (uint64_t)n_pts + (uint64_t)i,
+        const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st,
+                                                          load_point(pts, kPaired ? c * n_pts + i : i), mesh_mode,
+                                                          (uint64_t)cfg * (uint64_t)n_pts + (uint64_t)i,
                                                           nearest_first, margin_max);
         out_val[t] = o.val;
         out_grad[3 * t] = o.grad.x; out_grad[3 * t + 1] = o.grad.y; out_grad[3 * t + 2] = o.grad.z;
         if (out_point) out_point[t] = ip;
         if (out_which) out_which[t] = o.which;
     }
+}
+
+template <bool kMesh, bool kExt, int MAXS>
+__global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
+clearance_finish_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, const float *__restrict__ xforms,
+                        int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_seg,
+                        long long seg_len, uint32_t mesh_mode, const unsigned long long *__restrict__ keys,
+                        float *__restrict__ out_val, float *__restrict__ out_grad, int *__restrict__ out_point,
+                        int *__restrict__ out_which, int nearest_first, float margin_max) {
+    clearance_finish<kMesh, kExt, MAXS, false>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
+                                               mesh_mode, keys, out_val, out_grad, out_point, out_which,
+                                               nearest_first, margin_max);
+}
+
+template <bool kMesh, bool kExt, int MAXS>
+__global__ void __launch_bounds__(kCompThreads, (kMesh ? PVB_COMPMESH_MINB : 1))
+paired_clearance_finish_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf,
+                               const float *__restrict__ xforms, int n_cfg, int cfg_begin, int cfg_count,
+                               const float *__restrict__ pts, long long n_seg, long long seg_len, uint32_t mesh_mode,
+                               const unsigned long long *__restrict__ keys, float *__restrict__ out_val,
+                               float *__restrict__ out_grad, int *__restrict__ out_point, int *__restrict__ out_which,
+                               int nearest_first, float margin_max) {
+    clearance_finish<kMesh, kExt, MAXS, true>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
+                                              mesh_mode, keys, out_val, out_grad, out_point, out_which, nearest_first,
+                                              margin_max);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1995,6 +2048,114 @@ robot_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf,
             if (m < seed_key) atomicMin(kp, m);
         }
         __syncthreads();                                     // red is rewritten by the next chunk
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Paired clearance query on the sets robot_serial_kernel takes: configuration c against its OWN points, pts
+// [cfg_count][n_seg][seg_len][3].  For every configuration of the slab and every segment b of its points, the smallest
+// clearance_key over the segment, left in keys[c * n_seg + b] (~0 on entry); paired_clearance_finish_kernel turns it
+// into the result.  robot_clearance_kernel cannot serve here: its lanes are the configurations of one shared point.
+//   * Work unit: (configuration, segment, chunk of `chunk` consecutive points), owned by one warp.  Units are numbered
+//     chunk-major -- unit w is chunk w / (cfg_count * n_seg) of pair w % (cfg_count * n_seg) -- and the warps of a 1-D
+//     grid stride over them, so any cfg_count fits, and the later chunks of a segment start after its earlier ones.
+//   * The lanes are points of the unit's one configuration: its transform rows and sphere centres are staged once per
+//     unit in the warp's slot of shared memory, and every lane reads the same words (broadcasts).
+//   * Per lane: the 8 sphere bounds, then rs_swept_pair with the lane's own nearest link first (the visiting order
+//     never changes a result) and bp = min(running value, seed), the seed being the pair's key read when the unit
+//     starts.  A (point, link) pair is skipped only when its bound is STRICTLY above a value the segment attains.
+//   * After every step of 32 points the running value is the minimum over the warp: every lane holds the same
+//     configuration and segment, so each prunes against the best point the warp has seen (5 shuffles per step).
+//   * End of unit: a warp key minimum, one atomicMin per unit.
+// (Measured on the 8-link arm, DESIGN.md §4: a whole block per unit -- shared staging, 8 warps on one chunk -- was 1.2x
+// to 3.8x slower, most at 64 points per configuration where 192 of its 256 threads idle; without the per-step warp
+// minimum the unit was 1.12-1.27x slower at 4096 x 2048 and 65 536 x 64.)
+struct __align__(16) PclSmem {
+    float4 xf[kRsWarps][3 * kRsMaxS];
+    float4 sph[kRsWarps][3 * kRsMaxS / 4];
+};
+
+template <bool kExt>
+__global__ void __launch_bounds__(kRbCfg * kRsWarps, PVB_RS_MINB)
+robot_paired_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf,
+                              const float *__restrict__ xforms, int n_cfg, int cfg_begin, int cfg_count,
+                              const float *__restrict__ pts, long long n_seg, int seg_len, int chunk, long long n_units,
+                              unsigned long long *__restrict__ keys) {
+    __shared__ PclSmem sm;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const long long pairs = (long long)cfg_count * n_seg;
+    // uniform per warp: every lane takes part in the shuffles
+    for (long long w = (long long)blockIdx.x * kRsWarps + warp; w < n_units; w += (long long)gridDim.x * kRsWarps) {
+        const long long k = w / pairs, cb = w - k * pairs;   // chunk index; c * n_seg + b
+        const int cfg = cfg_begin + (int)(cb / n_seg);
+        const int i0 = (int)k * chunk;
+        const int len = min(chunk, seg_len - i0);
+        const long long pt0 = cb * seg_len + i0;             // pts[c][b][i0]
+        __syncwarp();                                        // the previous unit's staging is no longer read
+        if (lane < 3 * n_sdf) {
+            const int si = lane / 3;
+            sm.xf[warp][lane] = __ldg(reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg) * 16) +
+                                      (lane - 3 * si));
+        }
+        __syncwarp();
+        if (lane < kRsMaxS) {
+            const f3 co = lane < n_sdf ? rs_sphere_centre(pk.d[lane], sm.xf[warp][3 * lane], sm.xf[warp][3 * lane + 1],
+                                                          sm.xf[warp][3 * lane + 2])
+                                       : mk3(0.f, 0.f, 0.f);
+            float *c = reinterpret_cast<float *>(&sm.sph[warp][0]) + 3 * lane;
+            c[0] = co.x; c[1] = co.y; c[2] = co.z;
+        }
+        __syncwarp();
+        unsigned long long *const kp = keys + cb;
+        const unsigned long long seed_key = __ldcg(kp);
+        const float seed = clearance_key_value(seed_key);
+        unsigned long long run = ~0ull;                      // this lane's running key
+        float rv = PVB_INF;                                  // the warp's running value
+#pragma unroll 1
+        for (int j0 = 0; j0 < len; j0 += 32) {
+            const int j = j0 + lane;
+            const bool on = j < len;
+            const f3 p = on ? load_point(pts, pt0 + j) : mk3(0.f, 0.f, 0.f);
+            float cen[3 * kRsMaxS];
+#pragma unroll
+            for (int q = 0; q < 3 * kRsMaxS / 4; ++q) {
+                const float4 c4 = sm.sph[warp][q];
+                cen[4 * q] = c4.x; cen[4 * q + 1] = c4.y; cen[4 * q + 2] = c4.z; cen[4 * q + 3] = c4.w;
+            }
+            float lb[kRsMaxS], key[kRsMaxS];
+#pragma unroll
+            for (int si = 0; si < kRsMaxS; ++si) {
+                lb[si] = rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], pk.sph_rad[si]);
+                key[si] = rs_bound_key(lb[si], low3_off, si);
+            }
+            auto link = [&](const int si, const float thr, float4 &o) -> bool {
+                const pvb_sdf_desc &d = pk.d[si];
+                const float4 r0 = sm.xf[warp][3 * si], r1 = sm.xf[warp][3 * si + 1], r2 = sm.xf[warp][3 * si + 2];
+                const f3 q = composed_xform(r0, r1, r2, p);
+                const float tm = thr + pk.visit_margin[si];
+                if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
+                o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
+                    : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
+                                                               : robot_lookup(d, q);
+                return true;
+            };
+            float best;
+            f3 bg;
+            int bs;
+            // lanes past the end prune everything that has a bound (bp = -inf); their result is not used
+            rs_swept_pair(lb, rs_nearest(key, n_sdf), on ? fminf(rv, seed) : -PVB_INF, link, best, bg, bs);
+            if (on && bs >= 0) {
+                const unsigned long long kk = clearance_key(best, (uint32_t)(i0 + j));
+                if (kk < run) { run = kk; rv = best; }
+            }
+            for (int off = 16; off > 0; off >>= 1) rv = fminf(rv, __shfl_xor_sync(0xffffffffu, rv, off));
+        }
+        for (int off = 16; off > 0; off >>= 1) {
+            const unsigned long long o = __shfl_xor_sync(0xffffffffu, run, off);
+            run = o < run ? o : run;
+        }
+        if (lane == 0 && run < seed_key) atomicMin(kp, run);
     }
 }
 
@@ -3114,8 +3275,9 @@ static int launch_robot_clearance(const pvb_sdf_desc *descs, int n_sdf, const fl
 }
 
 // The keys of composed_clearance_kernel (unless `fused`: robot_clearance_kernel already left them), then
-// clearance_finish_kernel.
-template <bool kMesh, bool kExt, int MAXS>
+// clearance_finish_kernel.  kPaired: their paired forms, composed_paired_clearance_kernel (unless
+// robot_paired_clearance_kernel left the keys) and paired_clearance_finish_kernel.
+template <bool kMesh, bool kExt, int MAXS, bool kPaired = false>
 static int launch_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                             int cfg_count, const float *pts, long long n_seg, long long seg_len, uint32_t mesh_mode,
                             unsigned long long *keys, bool fused, float *out_val, float *out_grad, int *out_point,
@@ -3128,13 +3290,13 @@ static int launch_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *x
     float margin_max = 0.f;
     for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
     if (!fused) {
-        composed_clearance_kernel<kMesh, kExt, MAXS>
+        (kPaired ? composed_paired_clearance_kernel<kMesh, kExt, MAXS> : composed_clearance_kernel<kMesh, kExt, MAXS>)
             <<<grid_for((long long)cfg_count * n_seg * seg_len, kCompThreads, 8), kCompThreads, 0, stream>>>(
                 pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, mesh_mode, keys, nearest_first,
                 margin_max);
         PVB_CHECK_LAUNCH("pvb_composed_query_clearance");
     }
-    clearance_finish_kernel<kMesh, kExt, MAXS>
+    (kPaired ? paired_clearance_finish_kernel<kMesh, kExt, MAXS> : clearance_finish_kernel<kMesh, kExt, MAXS>)
         <<<grid_for((long long)cfg_count * n_seg, kCompThreads, 8), kCompThreads, 0, stream>>>(
             pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, mesh_mode, keys, out_val, out_grad,
             out_point, out_which, nearest_first, margin_max);
@@ -3200,6 +3362,103 @@ extern "C" int pvb_composed_query_clearance(const pvb_sdf_desc *descs, int32_t n
     const int rc = needs_mesh ? (any_ext ? PVB_CLEARANCE(true, true) : PVB_CLEARANCE(true, false))
                               : (any_ext ? PVB_CLEARANCE(false, true) : PVB_CLEARANCE(false, false));
 #undef PVB_CLEARANCE
+    return rc;
+}
+
+// Launch robot_paired_clearance_kernel.  Chunk size from the sizes alone: the longest chunk (whole steps of a warp,
+// at least 64 points, or the whole segment) that still gives >= 4 waves of resident units, so that the later chunks of
+// a segment start from the keys of its earlier ones.
+static int launch_robot_paired_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg,
+                                         int cfg_begin, int cfg_count, const float *pts, long long n_seg,
+                                         long long seg_len, unsigned long long *keys, bool ext, cudaStream_t stream) {
+    RobotPack<kRsMaxS> pack;
+    memset(&pack, 0, sizeof(pack));
+    for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
+    for (int si = 0; si < kRsMaxS; ++si) {
+        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
+        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
+    }
+    const long long pairs = (long long)cfg_count * n_seg;
+    const long long want = 4ll * sm_count() * PVB_RS_MINB * kRsWarps;    // warp units for 4 waves
+    long long per_seg = (want + pairs - 1) / pairs;
+    if (per_seg > (seg_len + 63) / 64) per_seg = (seg_len + 63) / 64;
+    if (per_seg < 1) per_seg = 1;
+    long long chunk = (seg_len + per_seg - 1) / per_seg;
+    chunk = (chunk + 31) / 32 * 32;                                      // whole steps of the warp
+    if (chunk > seg_len) chunk = seg_len;
+    const long long n_units = pairs * ((seg_len + chunk - 1) / chunk);
+    const long long blocks = (n_units + kRsWarps - 1) / kRsWarps;
+    const unsigned gx = (unsigned)(blocks < INT32_MAX ? blocks : INT32_MAX);
+    timing_mark(0, stream);
+    if (ext)
+        robot_paired_clearance_kernel<true><<<gx, kRbCfg * kRsWarps, 0, stream>>>(
+            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, (int)seg_len, (int)chunk, n_units, keys);
+    else
+        robot_paired_clearance_kernel<false><<<gx, kRbCfg * kRsWarps, 0, stream>>>(
+            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, (int)seg_len, (int)chunk, n_units, keys);
+    timing_mark(1, stream);
+    PVB_CHECK_LAUNCH("pvb_composed_query_paired_clearance(robot)");
+    return PVB_OK;
+}
+
+extern "C" int pvb_composed_query_paired_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,
+                                                   const float *xforms, int32_t n_cfg, int32_t cfg_begin,
+                                                   int32_t cfg_count, const float *pts, int64_t n_seg, int64_t seg_len,
+                                                   uint32_t mesh_mode, uint64_t *keys, float *out_val, float *out_grad,
+                                                   int32_t *out_point, int32_t *out_which, void *stream) {
+    const char *fn = "pvb_composed_query_paired_clearance";
+    if (n_seg < 0 || seg_len < 0 || seg_len >= (1ll << 31) || (seg_len > 0 && n_seg > INT64_MAX / seg_len) ||
+        (cfg_count > 0 && n_seg > INT64_MAX / cfg_count) ||
+        (cfg_count > 0 && n_seg * seg_len > INT64_MAX / cfg_count)) {
+        pvb_set_error("%s: invalid argument (n_seg=%lld seg_len=%lld cfg_count=%d; seg_len < 2^31, "
+                      "cfg_count * n_seg * seg_len < 2^63)", fn, (long long)n_seg, (long long)seg_len, cfg_count);
+        return PVB_ERR_INVALID;
+    }
+    const long long n_pts = n_seg * seg_len;                 // points per configuration
+    bool any_ext;
+    const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_val,
+                                        out_grad, any_ext);
+    if (bad) return bad;
+    if (n_seg == 0) return PVB_OK;
+    if (cfg_count < 1) {
+        if (n_pts == 0) return PVB_OK;
+        pvb_set_error("%s: no minimum over an empty configuration slab (cfg_count=%d)", fn, cfg_count);
+        return PVB_ERR_INVALID;
+    }
+    if (seg_len == 0) {
+        pvb_set_error("%s: no minimum over an empty segment (seg_len=0, n_seg=%lld)", fn, (long long)n_seg);
+        return PVB_ERR_INVALID;
+    }
+    if (!keys) {
+        pvb_set_error("%s: invalid argument (keys is null)", fn);
+        return PVB_ERR_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    unsigned long long *k = reinterpret_cast<unsigned long long *>(keys);
+    if (cudaMemsetAsync(k, 0xff, sizeof(uint64_t) * (size_t)cfg_count * (size_t)n_seg, s) != cudaSuccess) {
+        pvb_set_error("%s: cudaMemsetAsync(keys) failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+        return PVB_ERR_CUDA;
+    }
+    // robot_serial_kernel's sets take the fused kernel: <= 8 GRID links with the bounding-box rule or primitives (its
+    // 1-D grid has no limit on cfg_count)
+    bool fused = !needs_mesh && n_sdf <= kRsMaxS;
+    for (int i = 0; i < n_sdf && fused; ++i)
+        fused = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    if (fused) {
+        const int rc = launch_robot_paired_clearance(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg,
+                                                     seg_len, k, any_ext, s);
+        if (rc) return rc;
+    }
+#define PVB_PCLEARANCE(MESH, TRI)                                                                                  \
+    (n_sdf <= 16 ? launch_clearance<MESH, TRI, 16, true>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,   \
+                                                          n_seg, seg_len, mesh_mode, k, fused, out_val, out_grad,   \
+                                                          out_point, out_which, s)                                  \
+                 : launch_clearance<MESH, TRI, 128, true>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,  \
+                                                           n_seg, seg_len, mesh_mode, k, fused, out_val, out_grad,  \
+                                                           out_point, out_which, s))
+    const int rc = needs_mesh ? (any_ext ? PVB_PCLEARANCE(true, true) : PVB_PCLEARANCE(true, false))
+                              : (any_ext ? PVB_PCLEARANCE(false, true) : PVB_PCLEARANCE(false, false));
+#undef PVB_PCLEARANCE
     return rc;
 }
 

@@ -183,6 +183,12 @@ class RobotSDF(sdf.ObjectFrameSDF):
         `sdf_to_link_name` (ComposedSDF.clearance)."""
         return self.sdf.clearance(points_in_object_frame, return_argmin=return_argmin)
 
+    def paired_clearance(self, points_in_object_frame, return_argmin=False):
+        """Every installed joint configuration against its own cloud: points [*A, *B, N, 3] in the robot frame ->
+        (values [*A, *B], gradients [*A, *B, 3]) and, with return_argmin, the first point attaining the minimum (index
+        into N) and its link, a position in `sdf_to_link_name` (ComposedSDF.paired_clearance)."""
+        return self.sdf.paired_clearance(points_in_object_frame, return_argmin=return_argmin)
+
     def surface_bounding_box(self, **kwargs):
         return self.sdf.surface_bounding_box(**kwargs)
 

@@ -965,17 +965,23 @@ class ComposedSDF(ObjectFrameSDF):
         i = torch.arange(v.shape[-1], device=v.device, dtype=torch.int64)
         return ((h - (1 << 31)) << 32) | i
 
-    def _generic_clearance(self, p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which):
+    def _generic_clearance(self, p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which, paired=False):
         """query_clearance for sub-SDFs without native descriptors: configuration chunks through `_generic_query`,
-        each reduced over the points of every segment by the kernels' key order."""
+        each reduced over the points of every segment by the kernels' key order.  paired: p holds cfg_count blocks of
+        n_seg * seg_len points, block c for configuration cfg_begin + c only (query_paired_clearance)."""
         R = max(cfg_count, 0) * n_seg
         val = torch.empty(R, dtype=torch.float32, device=p.device)
         grad = torch.empty(R, 3, dtype=torch.float32, device=p.device)
         point = torch.empty(R, dtype=torch.int32, device=p.device)
         which = torch.empty(R, dtype=torch.int32, device=p.device)
+        n_pts = n_seg * seg_len
         for c0 in range(cfg_begin, cfg_begin + (cfg_count if R > 0 else 0), self.clearance_generic_chunk):
             cc = min(self.clearance_generic_chunk, cfg_begin + cfg_count - c0)
-            v, g, w = self._generic_query(p, c0, cc, n_cfg, True)
+            if paired:
+                own = p[(c0 - cfg_begin) * n_pts:(c0 - cfg_begin + cc) * n_pts]
+                v, g, w = self._generic_query(own, c0, cc, n_cfg, True, paired=True)
+            else:
+                v, g, w = self._generic_query(p, c0, cc, n_cfg, True)
             v, g, w = v.reshape(cc, n_seg, seg_len), g.reshape(cc, n_seg, seg_len, 3), w.reshape(cc, n_seg, seg_len)
             i = (self._clearance_keys(v).amin(dim=-1) & 0xFFFFFFFF)[..., None]
             out = slice((c0 - cfg_begin) * n_seg, (c0 - cfg_begin + cc) * n_seg)
@@ -1000,6 +1006,86 @@ class ComposedSDF(ObjectFrameSDF):
             raise ValueError("clearance query: no minimum over an empty segment (N = 0)")
         out = self.query_clearance(points_in_object_frame, return_which=return_argmin)
         shape = (*(self.tsf_batch or ()), *pts_shape[:-2])
+        dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
+        out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
+        vv = nat.deliver(out[0], out_device, dtype).reshape(shape)
+        gg = nat.deliver(out[1], out_device, dtype).reshape(*shape, 3)
+        if not return_argmin:
+            return vv, gg
+        point = nat.deliver(out[2], out_device, torch.int64).reshape(shape)
+        which = nat.deliver(out[3], out_device, torch.int64).reshape(shape)
+        return vv, gg, point, which
+
+    def query_paired_clearance(self, points_in_object_frame, cfg_begin=0, cfg_count=None, return_which=False):
+        """Paired form of `query_clearance`: configuration cfg_begin + c against its own points only.  The points
+        reshape to [cfg_count, n_seg, N, 3], N = points.shape[-2]; entry c * n_seg + b of the result is
+        query_clearance(points[c], cfg_begin=cfg_begin + c, cfg_count=1)[b], bit for bit in all four outputs, mesh
+        ray jitter included -- equivalently the first-point (value, point) minimum of query_paired(...,
+        return_which=True) over each segment.  Returns flat (cfg_count * n_seg,) / (cfg_count * n_seg, 3) fp32
+        tensors on the GPU, configuration-major, and with return_which also the int32 point index within the segment
+        and sub-SDF index."""
+        S = len(self.sdfs)
+        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
+        if cfg_count is None:
+            cfg_count = n_cfg - cfg_begin
+        shape = tuple(points_in_object_frame.shape)
+        lead, seg_len = self._clearance_segments(shape)
+        if (lead % cfg_count) if cfg_count > 0 else lead:
+            raise ValueError(f"paired clearance query: points {shape} do not split into {cfg_count} blocks of "
+                             f"[n_seg, N, 3]")
+        n_seg = lead // cfg_count if cfg_count > 0 else 0
+        if n_seg > 0 and seg_len == 0:
+            raise ValueError("paired clearance query: no minimum over an empty segment (N = 0)")
+        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
+        with torch.cuda.device(device):
+            p = nat.as_f32_points(points_in_object_frame, device)
+            descs_arr, needs_mesh = self._native_descs(device)
+            if descs_arr is None:
+                return self._generic_paired_clearance(p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which)
+            xf = self._xforms_on(device)
+            R = max(cfg_count, 0) * n_seg
+            keys = torch.empty(R, dtype=torch.int64, device=device)
+            val = torch.empty(R, dtype=torch.float32, device=device)
+            grad = torch.empty(R, 3, dtype=torch.float32, device=device)
+            point = torch.empty(R, dtype=torch.int32, device=device) if return_which else None
+            which = torch.empty(R, dtype=torch.int32, device=device) if return_which else None
+            nat.check(nat.lib().pvb_composed_query_paired_clearance(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg,
+                                                                    cfg_begin, cfg_count, nat.ptr(p), n_seg, seg_len,
+                                                                    nat.PVB_MESH_DEFAULT, nat.ptr(keys), nat.ptr(val),
+                                                                    nat.ptr(grad), nat.ptr(point), nat.ptr(which),
+                                                                    nat.stream_ptr(device)),
+                      "pvb_composed_query_paired_clearance")
+        return (val, grad, point, which) if return_which else (val, grad)
+
+    def _generic_paired_clearance(self, p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which):
+        """query_paired_clearance for sub-SDFs without native descriptors (or more than `max_fused_sdfs`):
+        configuration chunks through `_generic_query(..., paired=True)`, reduced by `_clearance_keys` -- the order of
+        the fused route."""
+        return self._generic_clearance(p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which, paired=True)
+
+    def paired_clearance(self, points_in_object_frame, return_argmin=False):
+        """Every installed configuration against its own cloud: points [*A, *B, N, 3], A the configuration batch, give
+        (values [*A, *B], gradients [*A, *B, 3]) in the points' dtype and on their device.  Entry [a, b] is
+        configuration a's result at the first point of points[a, b] attaining the minimum value: bit-identical to
+        paired() followed by that reduction over N, and to clearance(points[a]) of configuration a alone, without
+        |A| times the work of clearance() over every cloud.  With return_argmin, also that point's index into N and
+        the sub-SDF index, int64 [*A, *B].  Without a configuration batch it is clearance().  Not a reference
+        operator (an extension); raises ValueError before any device work when the leading dimensions of the points
+        are not A, when they are not [..., N, 3], or when N = 0 with segments to reduce."""
+        if self.tsf_batch is None:
+            return self.clearance(points_in_object_frame, return_argmin=return_argmin)
+        batch = tuple(int(a) for a in self.tsf_batch)
+        pts_shape = tuple(points_in_object_frame.shape)
+        if len(pts_shape) < len(batch) + 2 or pts_shape[-1] != 3:
+            raise ValueError(f"paired clearance query: points {pts_shape} must be [*A, ..., N, 3] with the "
+                             f"configuration batch A = {batch} leading")
+        if pts_shape[:len(batch)] != batch:
+            raise ValueError(f"paired clearance query: points {pts_shape} must have the configuration batch "
+                             f"A = {batch} leading")
+        if math.prod(pts_shape[:-2]) > 0 and pts_shape[-2] == 0:
+            raise ValueError("paired clearance query: no minimum over an empty segment (N = 0)")
+        out = self.query_paired_clearance(points_in_object_frame, return_which=return_argmin)
+        shape = pts_shape[:-2]
         dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
         out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
         vv = nat.deliver(out[0], out_device, dtype).reshape(shape)
