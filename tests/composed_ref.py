@@ -7,9 +7,15 @@ A sub-SDF is described by a spec:
   helpers.grid_spec(cached)   nearest-voxel CachedSDF with the bounding-box rule (table lookup + helpers._aabb_rule)
   primitive_spec(desc)        SphereSDF / BoxSDF / CylinderSDF descriptor (tests/primitive_ref.py)
   mesh_spec(port_mesh)        a closed mesh through the oracle's closest point and crossing parity (oracle.port)
+  trilinear_spec(cached)      trilinear CachedSDF: the interpolant in range, the bounding-box rule outside it
+                              (tests/grid_ref.py)
+  grid_gt_spec(cached, mesh)  nearest-voxel CachedSDF with OutOfBoundsStrategy.LOOKUP_GT_SDF: the signed fp64 mesh
+                              (tests/mesh_ref.MeshRef) outside the range
 Test infrastructure only."""
 import numpy as np
 
+import grid_ref
+import helpers
 import primitive_ref as pr
 from helpers import classify_mesh_mismatch, ray_noise
 
@@ -30,6 +36,28 @@ def mesh_spec(port_mesh, seed=0):
     """Spec of a closed mesh (oracle.port.MeshPort).  The sign of a closed mesh does not depend on the ray direction
     off the surface, so any seeded ray noise stands in for the reference's random draw."""
     return {"kind": "mesh", "port": port_mesh, "seed": seed}
+
+
+def trilinear_spec(cached):
+    return {"kind": "trilinear", "ref": grid_ref.Grid.of(cached)}
+
+
+def grid_gt_spec(cached, mesh):
+    """mesh: the tests/mesh_ref.MeshRef of the CachedSDF's ground-truth mesh (closed: its sign does not depend on the
+    point's index in the call)."""
+    s = helpers.grid_spec(cached)
+    s.update(kind="grid_gt", ref=grid_ref.Grid.of(cached), mesh=mesh)
+    return s
+
+
+def grid_gt_eval(spec, q):
+    r = spec["ref"].nearest(q)
+    v, g = r["value"].copy(), r["grad"].copy()
+    out = ~r["inb"]
+    if out.any():
+        m = spec["mesh"].query(q[out])
+        v[out], g[out] = m["value"], m["grad"]
+    return v, g
 
 
 def grid_eval(spec, q):
@@ -63,6 +91,11 @@ def evaluate(spec, q):
         return grid_eval(spec, q)
     if kind == "mesh":
         return mesh_eval(spec, q)
+    if kind == "trilinear":
+        r = spec["ref"].trilinear(q)
+        return r["value"], r["grad"]
+    if kind == "grid_gt":
+        return grid_gt_eval(spec, q)
     if kind == "box":
         return pr.box_ref(spec["half"], q)
     if kind == "cylinder":

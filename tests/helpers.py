@@ -83,7 +83,10 @@ def classify_mesh_mismatch(d_gpu, g_gpu, d_ref, g_ref, tol=1e-5, coord_scale=0.1
 #         link-frame point across a cell boundary it sits on (|frac - 0.5| < FLIP_BAND cells) or across the edge of
 #         the cached range, and the output equals the entry of that neighbouring cell / the other side's rule;
 #   (ii)  the |d| = 1e-3 shell of sdf.py:162 or a closest-feature tie (same distance, another gradient) of a mesh;
-#   (iii) an argmin tie between sub-SDFs (values within the tolerance, the other one's gradient reported).
+#   (iii) an argmin tie between sub-SDFs (values within the tolerance, the other one's gradient reported);
+#   (iv)  a trilinear cell-face flip: the link-frame point lies within FLIP_BAND cells of an interior cell face of a
+#         trilinear grid, and the gradient is that of another cell touching the face (the interpolant is continuous
+#         there, its gradient is not).
 # Anything else is unexplained and fails the test.
 FLIP_BAND = 1.5e-4      # cells; rounding of the S*|A| rigid transforms: ~3 ulp of |q| over the cell size
 
@@ -157,6 +160,9 @@ def flip_candidates(specs, M, p):
         if spec["kind"] in ("box", "cylinder"):
             out += [(v, g @ R, s, slack) for v, g, slack in _primitive_alternatives(spec, q)]
             continue
+        if spec["kind"] == "trilinear":
+            out += _trilinear_alternatives(spec["ref"], q, R, s)
+            continue
         lo, hi, val, grad = spec["lo"], spec["hi"], spec["val"], spec["grad"]
         n = np.array(val.shape)
         res = (hi - lo) / (n - 1)
@@ -177,9 +183,41 @@ def flip_candidates(specs, M, p):
                 for ky in opts[1]:
                     for kz in opts[2]:
                         out.append((val[kx, ky, kz], grad[kx, ky, kz] @ R, s, 0.0))
-        if maybe_out:
+        if maybe_out and spec["kind"] == "grid_gt":
+            m = spec["mesh"].query(q[None])
+            tie = bool(m["tie_face"][0] | m["tie_normal"][0] | m["shell_edge"][0] | m["sign_margin"][0])
+            slack = 2.0 if tie else float(mesh_grad_bound(m["scale"], m["cond"])[0])
+            out.append((float(m["value"][0]), m["grad"][0] @ R, s, slack))
+        elif maybe_out:
             d, g = _aabb_rule(spec["bb"], q)
             out.append((d, g @ R, s, 0.0))
+    return out
+
+
+def mesh_grad_bound(scale, cond):
+    import mesh_ref
+    return mesh_ref.grad_bound(scale, cond)
+
+
+def _trilinear_alternatives(ref, q, R, s):
+    """Candidates of a trilinear grid (tests/grid_ref.Grid) at q (3,): the interpolant with the gradient of every cell
+    touching a cell face within FLIP_BAND of q, and the bounding-box rule near the range's edge.  The slack is the
+    gradient bound of grid_ref."""
+    import grid_ref
+    out = []
+    r = ref.trilinear(q[None], band=FLIP_BAND)
+    if r["inb"][0] or np.all((q >= ref.lo - 1e-6) & (q <= ref.hi + 1e-6)):
+        qc = np.clip(q, ref.lo64, ref.hi64)
+        rc = ref.trilinear(qc[None], band=FLIP_BAND) if not r["inb"][0] else r
+        slack = float(rc["gbound"][0].max())
+        v = float(rc["value"][0])
+        out.append((v, rc["grad"][0] @ R, s, slack))
+        for g in rc["alt"][:, 0]:
+            if np.isfinite(g).all():
+                out.append((v, g @ R, s, slack))
+    if not r["inb"][0] or np.any((q < ref.lo + 1e-6) | (q > ref.hi - 1e-6)):
+        d, g = grid_ref.box_rule(ref.bb32, q[None])
+        out.append((float(d[0]), g[0] @ R, s, 0.0))
     return out
 
 
