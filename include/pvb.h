@@ -263,6 +263,31 @@ int pvb_composed_query_paired_clearance(const pvb_sdf_desc *descs, int32_t n_sdf
                                         uint64_t *keys, float *out_val, float *out_grad,
                                         int32_t *out_point, int32_t *out_which, void *stream);
 
+/* ---- EXTENSION: self-clearance query, every configuration's smallest distance between its own sub-SDFs ----
+ * The reference has no such operator.  M_s(a) = xforms[s * n_cfg + a] (object -> sub-frame, as every composed query
+ * reads it) and W_s(a) = inv_xforms[s * n_cfg + a], the same layout (sub-frame -> object frame; the caller computes
+ * it, ComposedSDF caches _affine_inverse(M)).  link_pts DEVICE [n_sdf][K][3]: K points of every sub-SDF in its own
+ * frame.  allowed HOST uint8_t[n_sdf]: bit j of row i lets the points of i be tested against sub-SDF j; the diagonal
+ * is ignored.  For configuration cfg_begin + c: over every i, every allowed j and every k, the minimum of
+ * sdf_j(M_j(a) x) with x = W_i(a) link_pts[i][k] posed by the arithmetic of pvb_transform_points_paired.  The minimum
+ * is taken over (value, i, k) lexicographically; for that point the first allowed j attaining the value wins (the
+ * composition's first-index rule); -0 == +0 and a NaN value ranks above every number, as in
+ * pvb_composed_query_clearance.  out_val [cfg_count], out_grad [cfg_count * 3] (the object-frame gradient
+ * pvb_composed_query_paired of the allowed sub-composition reports at x); optional out_src (i), out_point (k),
+ * out_which (j).  A configuration without an allowed pair gets +inf, a zero gradient and indices -1.  Bit-identical to
+ * the composition route: per source i, its points posed by pvb_transform_points_paired with W_i, then
+ * pvb_composed_query_paired_clearance on the allowed sub-SDFs and their transform rows, reduced over i by (value, i).
+ * keys: device scratch of cfg_count entries that the library initialises.
+ * Serves the sets pvb_composed_query_paired_clearance runs fused: at most 8 GRID sub-SDFs with the bounding-box rule
+ * (nearest or trilinear) or primitives.  PVB_ERR_INVALID for every other set (mesh, LOOKUP_GT_SDF grids, more than 8
+ * sub-SDFs: callers compose the route above), for K < 1 or K >= 2^24, bits of allowed beyond n_sdf, cfg_count < 1,
+ * null inv_xforms, allowed or keys, and the argument checks of pvb_composed_query. */
+int pvb_composed_query_self_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,
+                                      const float *inv_xforms, int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                                      const float *link_pts, int64_t K, const uint8_t *allowed, uint64_t *keys,
+                                      float *out_val, float *out_grad, int32_t *out_src, int32_t *out_point,
+                                      int32_t *out_which, void *stream);
+
 /* ---- the same query with the result slab stored to several destinations from the kernel epilogue ----
  * Multi-GPU re-assembly of a configuration-sharded RobotSDF result (model_to_sdf.py:117-125 returns the full
  * (|A|, N) tensors): every rank evaluates its slab [cfg_begin, cfg_begin + cfg_count) and writes it straight into

@@ -1046,4 +1046,57 @@ __device__ __forceinline__ float clearance_key_value(uint64_t k) {
     return __int_as_float((int)((h & 0x80000000u) ? (h & 0x7fffffffu) : ~h));
 }
 
+// ----------------------------------------------------------------------------
+// Self-clearance queries (robot_self_clearance_kernel / self_clearance_finish_kernel,
+// pvb_composed_query_self_clearance): for configuration a, over every source sub-SDF i, every sub-SDF j that row i of
+// the mask allows (bit j; the diagonal is cleared) and every link point k of i, the minimum of sdf_j(M_j(a) x) with
+// x = W_i(a) link_pts[i][k] posed by composed_xform.  The minimum is taken over (value, i, k) lexicographically, and
+// for that point the first allowed j attaining the value wins.
+//
+// One key per configuration: the value as in clearance_key, (i << 24) | k in the low word (k < 2^24, i < 8), so the
+// unsigned order of keys is exactly the (value, i, k) order and every source of a configuration prunes against the
+// best value any of them has reached.
+__device__ __forceinline__ uint64_t self_clearance_key(float v, int i, int k) {
+    return clearance_key(v, ((uint32_t)i << 24) | (uint32_t)k);
+}
+
+struct SelfClearanceOut { float val; f3 grad; int src; int point; int which; };
+
+// The result of one configuration from its key: (i, k) decoded, x posed again, then every allowed sub-SDF of row i
+// evaluated at x in index order (first index on ties) and the winner's gradient rotated back -- what
+// composed_point of the composition of the allowed sub-SDFs gives at x.  ~0 (no allowed pair): +inf, 0, -1.
+//   load_xf(s, r0, r1, r2) / load_inv(s, ...): rows of M_s / W_s of this configuration; load_pt(i, k): the link point;
+//   eval(s, q): (value, sub-frame gradient) of sub-SDF s at q in its frame
+template <class LoadXf, class LoadInv, class LoadPt, class Eval>
+__device__ __forceinline__ SelfClearanceOut self_clearance_finish_one(uint64_t key, const unsigned char *masks,
+                                                                      int n_sdf, const LoadXf &load_xf,
+                                                                      const LoadInv &load_inv, const LoadPt &load_pt,
+                                                                      const Eval &eval) {
+    SelfClearanceOut o;
+    if (key == ~0ull) {
+        o.val = PVB_INF; o.grad = mk3(0.f, 0.f, 0.f); o.src = -1; o.point = -1; o.which = -1;
+        return o;
+    }
+    const uint32_t low = (uint32_t)key;
+    const int i = (int)(low >> 24), k = (int)(low & 0xffffffu);
+    float4 w0, w1, w2;
+    load_inv(i, w0, w1, w2);
+    const f3 x = composed_xform(w0, w1, w2, load_pt(i, k));
+    const unsigned mask = masks[i];
+    float best = PVB_INF;
+    f3 bg = mk3(0.f, 0.f, 0.f);
+    int bs = -1;
+    for (int s = 0; s < n_sdf; ++s) {
+        if (!((mask >> s) & 1u)) continue;
+        float4 r0, r1, r2;
+        load_xf(s, r0, r1, r2);
+        const float4 e = eval(s, composed_xform(r0, r1, r2, x));
+        if (bs < 0 || e.x < best) { best = e.x; bg = mk3(e.y, e.z, e.w); bs = s; }
+    }
+    float4 r0, r1, r2;
+    load_xf(max(bs, 0), r0, r1, r2);
+    o.val = best; o.grad = composed_rotate_back(r0, r1, r2, bg); o.src = i; o.point = k; o.which = bs;
+    return o;
+}
+
 }  // namespace pvb

@@ -2159,6 +2159,165 @@ robot_paired_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// Self-clearance query on the sets robot_paired_clearance_kernel takes (pvb_device.cuh: self_clearance_key): for every
+// configuration of the slab, the smallest self_clearance_key over its sources' link points against their allowed
+// sub-SDFs, left in keys[c] (~0 on entry); self_clearance_finish_kernel turns it into the result.
+//   * Work unit: (configuration, source sub-SDF i, chunk of `chunk` consecutive link points of i), owned by one warp.
+//     Only sources with a non-empty row are numbered (rows.src); units are numbered chunk-major -- unit w is chunk
+//     w / (cfg_count * n_src) of (configuration, source) w % (cfg_count * n_src) -- and the warps of a 1-D grid stride
+//     over them.
+//   * The lanes are link points of the unit's one configuration: its transform rows, W_i's three rows and the sphere
+//     centres are staged once per unit in the warp's slot of shared memory.  A lane loads link_pts[i][k] (the same for
+//     every configuration: L2-resident) and poses it with composed_xform.
+//   * Masked links get a bound of +inf AND are refused inside the visit: rs_swept_pair visits its first link whenever
+//     the bound is not strictly above bp, and bp is +inf until a value has been reached.
+//   * Pruning, the per-step warp minimum and the one atomicMin per unit are robot_paired_clearance_kernel's, against
+//     the configuration's one key: every source prunes against the best value any source of it has reached.
+struct SclRows {
+    unsigned char src[kRsMaxS];     // the sources with a non-empty row, ascending
+    unsigned char mask[kRsMaxS];    // by sub-SDF index: bit j allows (i, j); the diagonal is cleared
+};
+
+struct __align__(16) SclSmem {
+    float4 xf[kRsWarps][3 * kRsMaxS];
+    float4 inv[kRsWarps][4];
+    float4 sph[kRsWarps][3 * kRsMaxS / 4];
+};
+
+template <bool kExt>
+__global__ void __launch_bounds__(kRbCfg * kRsWarps, PVB_RS_MINB)
+robot_self_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf,
+                            const float *__restrict__ xforms, const float *__restrict__ inv_xforms, int n_cfg,
+                            int cfg_begin, int cfg_count, const float *__restrict__ link_pts, int K,
+                            const __grid_constant__ SclRows rows, int n_src, int chunk, long long n_units,
+                            unsigned long long *__restrict__ keys) {
+    __shared__ SclSmem sm;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const long long pairs = (long long)cfg_count * n_src;
+    // uniform per warp: every lane takes part in the shuffles
+    for (long long w = (long long)blockIdx.x * kRsWarps + warp; w < n_units; w += (long long)gridDim.x * kRsWarps) {
+        const long long kc = w / pairs, r = w - kc * pairs;  // chunk index; c * n_src + source position
+        const int c = (int)(r / n_src);
+        const int i = rows.src[r - (long long)c * n_src];
+        const unsigned mask = rows.mask[i];
+        const int cfg = cfg_begin + c;
+        const int k0 = (int)kc * chunk;
+        const int len = min(chunk, K - k0);
+        __syncwarp();                                        // the previous unit's staging is no longer read
+        if (lane < 3 * n_sdf) {
+            const int si = lane / 3;
+            sm.xf[warp][lane] = __ldg(reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg) * 16) +
+                                      (lane - 3 * si));
+        } else if (lane >= 3 * kRsMaxS && lane < 3 * kRsMaxS + 3) {
+            sm.inv[warp][lane - 3 * kRsMaxS] =
+                __ldg(reinterpret_cast<const float4 *>(inv_xforms + ((size_t)i * n_cfg + cfg) * 16) +
+                      (lane - 3 * kRsMaxS));
+        }
+        __syncwarp();
+        if (lane < kRsMaxS) {
+            const f3 co = lane < n_sdf ? rs_sphere_centre(pk.d[lane], sm.xf[warp][3 * lane], sm.xf[warp][3 * lane + 1],
+                                                          sm.xf[warp][3 * lane + 2])
+                                       : mk3(0.f, 0.f, 0.f);
+            float *cc = reinterpret_cast<float *>(&sm.sph[warp][0]) + 3 * lane;
+            cc[0] = co.x; cc[1] = co.y; cc[2] = co.z;
+        }
+        __syncwarp();
+        unsigned long long *const kp = keys + c;
+        const unsigned long long seed_key = __ldcg(kp);
+        const float seed = clearance_key_value(seed_key);
+        const float4 w0 = sm.inv[warp][0], w1 = sm.inv[warp][1], w2 = sm.inv[warp][2];
+        unsigned long long run = ~0ull;                      // this lane's running key
+        float rv = PVB_INF;                                  // the warp's running value
+#pragma unroll 1
+        for (int j0 = 0; j0 < len; j0 += 32) {
+            const int j = j0 + lane;
+            const bool on = j < len;
+            const f3 p = composed_xform(w0, w1, w2,
+                                        on ? load_point(link_pts, (long long)i * K + k0 + j) : mk3(0.f, 0.f, 0.f));
+            float cen[3 * kRsMaxS];
+#pragma unroll
+            for (int q = 0; q < 3 * kRsMaxS / 4; ++q) {
+                const float4 c4 = sm.sph[warp][q];
+                cen[4 * q] = c4.x; cen[4 * q + 1] = c4.y; cen[4 * q + 2] = c4.z; cen[4 * q + 3] = c4.w;
+            }
+            float lb[kRsMaxS], key[kRsMaxS];
+#pragma unroll
+            for (int si = 0; si < kRsMaxS; ++si) {
+                lb[si] = ((mask >> si) & 1u) ? rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2],
+                                                            pk.sph_rad[si])
+                                             : PVB_INF;
+                key[si] = rs_bound_key(lb[si], low3_off, si);
+            }
+            auto link = [&](const int si, const float thr, float4 &o) -> bool {
+                if (!((mask >> si) & 1u)) return false;
+                const pvb_sdf_desc &d = pk.d[si];
+                const float4 r0 = sm.xf[warp][3 * si], r1 = sm.xf[warp][3 * si + 1], r2 = sm.xf[warp][3 * si + 2];
+                const f3 q = composed_xform(r0, r1, r2, p);
+                const float tm = thr + pk.visit_margin[si];
+                if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
+                o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
+                    : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
+                                                               : robot_lookup(d, q);
+                return true;
+            };
+            float best;
+            f3 bg;
+            int bs;
+            // lanes past the end prune everything that has a bound (bp = -inf) and refuse the rest; unused
+            rs_swept_pair(lb, rs_nearest(key, n_sdf), on ? fminf(rv, seed) : -PVB_INF, link, best, bg, bs);
+            if (on && bs >= 0) {
+                const unsigned long long kk = self_clearance_key(best, i, k0 + j);
+                if (kk < run) { run = kk; rv = best; }
+            }
+            for (int off = 16; off > 0; off >>= 1) rv = fminf(rv, __shfl_xor_sync(0xffffffffu, rv, off));
+        }
+        for (int off = 16; off > 0; off >>= 1) {
+            const unsigned long long o = __shfl_xor_sync(0xffffffffu, run, off);
+            run = o < run ? o : run;
+        }
+        if (lane == 0 && run < seed_key) atomicMin(kp, run);
+    }
+}
+
+// The result of a self-clearance query: one thread per configuration, self_clearance_finish_one (pvb_device.cuh) with
+// the visit arithmetic of robot_self_clearance_kernel.  Whichever route produced the key, the output is what the
+// composition route's finish (composed_point of the allowed sub-composition at the posed point) gives, bit for bit.
+template <bool kExt>
+__global__ void __launch_bounds__(kCompThreads)
+self_clearance_finish_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf,
+                             const float *__restrict__ xforms, const float *__restrict__ inv_xforms, int n_cfg,
+                             int cfg_begin, int cfg_count, const float *__restrict__ link_pts, int K,
+                             const __grid_constant__ SclRows rows, const unsigned long long *__restrict__ keys,
+                             float *__restrict__ out_val, float *__restrict__ out_grad, int *__restrict__ out_src,
+                             int *__restrict__ out_point, int *__restrict__ out_which) {
+    const int stride = gridDim.x * blockDim.x;
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < cfg_count; c += stride) {
+        const int cfg = cfg_begin + c;
+        auto rows_of = [&](const float *m, int s, float4 &r0, float4 &r1, float4 &r2) {
+            const float4 *row = reinterpret_cast<const float4 *>(m + ((size_t)s * n_cfg + cfg) * 16);
+            r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
+        };
+        auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) { rows_of(xforms, s, r0, r1, r2); };
+        auto load_inv = [&](int s, float4 &r0, float4 &r1, float4 &r2) { rows_of(inv_xforms, s, r0, r1, r2); };
+        auto load_pt = [&](int i, int k) { return load_point(link_pts, (long long)i * K + k); };
+        auto eval = [&](int s, f3 q) -> float4 {
+            const pvb_sdf_desc &d = pk.d[s];
+            return (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
+                   : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
+                                                              : robot_lookup(d, q);
+        };
+        const SelfClearanceOut o = self_clearance_finish_one(__ldcg(keys + c), rows.mask, n_sdf, load_xf, load_inv,
+                                                             load_pt, eval);
+        out_val[c] = o.val;
+        out_grad[3 * c] = o.grad.x; out_grad[3 * c + 1] = o.grad.y; out_grad[3 * c + 2] = o.grad.z;
+        if (out_src) out_src[c] = o.src;
+        if (out_point) out_point[c] = o.point;
+        if (out_which) out_which[c] = o.which;
+    }
+}
+
 // ========================================================== voxel containers
 // VoxelGrid / ExpandingVoxelGrid / voxel_down_sample (voxel.py:42-171) and the value-range view they sit on
 // (TorchMultidimView: sdf.py:264, voxel.py:55-64): the reference reads, writes and lists voxels with boolean-mask
@@ -3460,6 +3619,113 @@ extern "C" int pvb_composed_query_paired_clearance(const pvb_sdf_desc *descs, in
                               : (any_ext ? PVB_PCLEARANCE(false, true) : PVB_PCLEARANCE(false, false));
 #undef PVB_PCLEARANCE
     return rc;
+}
+
+// Launch robot_self_clearance_kernel (when some row is not empty), then self_clearance_finish_kernel.  Chunk size as
+// in launch_robot_paired_clearance: the longest chunk (whole steps of a warp, at least 64 points, or all K) that still
+// gives >= 4 waves of resident units.
+static int launch_self_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, const float *inv_xforms,
+                                 int n_cfg, int cfg_begin, int cfg_count, const float *link_pts, int K,
+                                 const SclRows &rows, int n_src, unsigned long long *keys, float *out_val,
+                                 float *out_grad, int *out_src, int *out_point, int *out_which, bool ext,
+                                 cudaStream_t stream) {
+    RobotPack<kRsMaxS> pack;
+    memset(&pack, 0, sizeof(pack));
+    for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
+    for (int si = 0; si < kRsMaxS; ++si) {
+        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
+        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
+    }
+    if (n_src > 0) {
+        const long long pairs = (long long)cfg_count * n_src;
+        const long long want = 4ll * sm_count() * PVB_RS_MINB * kRsWarps;    // warp units for 4 waves
+        long long per_src = (want + pairs - 1) / pairs;
+        if (per_src > (K + 63) / 64) per_src = (K + 63) / 64;
+        if (per_src < 1) per_src = 1;
+        long long chunk = (K + per_src - 1) / per_src;
+        chunk = (chunk + 31) / 32 * 32;                                      // whole steps of the warp
+        if (chunk > K) chunk = K;
+        const long long n_units = pairs * ((K + chunk - 1) / chunk);
+        const long long blocks = (n_units + kRsWarps - 1) / kRsWarps;
+        const unsigned gx = (unsigned)(blocks < INT32_MAX ? blocks : INT32_MAX);
+        timing_mark(0, stream);
+        if (ext)
+            robot_self_clearance_kernel<true><<<gx, kRbCfg * kRsWarps, 0, stream>>>(
+                pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, K, rows, n_src, (int)chunk,
+                n_units, keys);
+        else
+            robot_self_clearance_kernel<false><<<gx, kRbCfg * kRsWarps, 0, stream>>>(
+                pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, K, rows, n_src, (int)chunk,
+                n_units, keys);
+        timing_mark(1, stream);
+        PVB_CHECK_LAUNCH("pvb_composed_query_self_clearance");
+    }
+    const unsigned gf = (unsigned)grid_for(cfg_count, kCompThreads, 8);
+    if (ext)
+        self_clearance_finish_kernel<true><<<gf, kCompThreads, 0, stream>>>(
+            pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, K, rows, keys, out_val, out_grad,
+            out_src, out_point, out_which);
+    else
+        self_clearance_finish_kernel<false><<<gf, kCompThreads, 0, stream>>>(
+            pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, K, rows, keys, out_val, out_grad,
+            out_src, out_point, out_which);
+    PVB_CHECK_LAUNCH("pvb_composed_query_self_clearance(finish)");
+    return PVB_OK;
+}
+
+extern "C" int pvb_composed_query_self_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,
+                                                 const float *inv_xforms, int32_t n_cfg, int32_t cfg_begin,
+                                                 int32_t cfg_count, const float *link_pts, int64_t K,
+                                                 const uint8_t *allowed, uint64_t *keys, float *out_val,
+                                                 float *out_grad, int32_t *out_src, int32_t *out_point,
+                                                 int32_t *out_which, void *stream) {
+    const char *fn = "pvb_composed_query_self_clearance";
+    if (K < 1 || K >= (1ll << 24) || !inv_xforms || !allowed) {
+        pvb_set_error("%s: invalid argument (K=%lld; 1 <= K < 2^24, inv_xforms and allowed not null)", fn,
+                      (long long)K);
+        return PVB_ERR_INVALID;
+    }
+    bool any_ext;
+    const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, link_pts,
+                                        (int64_t)n_sdf * K, out_val, out_grad, any_ext);
+    if (bad) return bad;
+    if (cfg_count < 1) {
+        pvb_set_error("%s: no minimum over an empty configuration slab (cfg_count=%d)", fn, cfg_count);
+        return PVB_ERR_INVALID;
+    }
+    // the sets robot_paired_clearance_kernel takes: <= 8 GRID links with the bounding-box rule, or primitives
+    bool fused = n_sdf <= kRsMaxS;
+    for (int i = 0; i < n_sdf && fused; ++i)
+        fused = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    if (!fused) {
+        pvb_set_error("%s: the fused query takes at most %d grid (bounding-box rule) or primitive sub-SDFs, no mesh or "
+                      "LOOKUP_GT_SDF grid (n_sdf=%d); compose the per-source paired clearance queries instead", fn,
+                      kRsMaxS, n_sdf);
+        return PVB_ERR_INVALID;
+    }
+    SclRows rows;
+    memset(&rows, 0, sizeof(rows));
+    int n_src = 0;
+    for (int i = 0; i < n_sdf; ++i) {
+        if (allowed[i] >> n_sdf) {
+            pvb_set_error("%s: allowed row %d has bits beyond n_sdf=%d (0x%02x)", fn, i, n_sdf, allowed[i]);
+            return PVB_ERR_INVALID;
+        }
+        rows.mask[i] = (unsigned char)(allowed[i] & ~(1u << i));
+        if (rows.mask[i]) rows.src[n_src++] = (unsigned char)i;
+    }
+    if (!keys) {
+        pvb_set_error("%s: invalid argument (keys is null)", fn);
+        return PVB_ERR_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    unsigned long long *k = reinterpret_cast<unsigned long long *>(keys);
+    if (cudaMemsetAsync(k, 0xff, sizeof(uint64_t) * (size_t)cfg_count, s) != cudaSuccess) {
+        pvb_set_error("%s: cudaMemsetAsync(keys) failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+        return PVB_ERR_CUDA;
+    }
+    return launch_self_clearance(descs, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, (int)K, rows,
+                                 n_src, k, out_val, out_grad, out_src, out_point, out_which, any_ext, s);
 }
 
 extern "C" int pvb_composed_query_multi(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,

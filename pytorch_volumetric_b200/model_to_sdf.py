@@ -45,6 +45,31 @@ def _primitive_sdf(vis):
     return sdf.SphereSDF(radius)
 
 
+def _primitive_surface(link_sdf, n, rng):
+    """[n, 3] fp64 area-uniform samples of the surface of a BoxSDF, CylinderSDF or SphereSDF, in its own frame."""
+    if isinstance(link_sdf, sdf.SphereSDF):
+        d = rng.normal(size=(n, 3))
+        return float(link_sdf.radius) * d / np.linalg.norm(d, axis=1, keepdims=True)
+    u = rng.uniform(-1.0, 1.0, size=(n, 3))
+    if isinstance(link_sdf, sdf.BoxSDF):
+        h = np.asarray(link_sdf._half, dtype=np.float64)
+        area = np.array([h[1] * h[2], h[0] * h[2], h[0] * h[1]])        # face pair normal to x, y, z
+        axis = rng.choice(3, size=n, p=area / area.sum())
+        out = u * h
+        rows = np.arange(n)
+        out[rows, axis] = np.where(rng.uniform(size=n) < 0.5, -1.0, 1.0) * h[axis]
+        return out
+    if isinstance(link_sdf, sdf.CylinderSDF):
+        r, hl = float(link_sdf.radius), 0.5 * float(link_sdf.length)
+        side, cap = 2.0 * np.pi * r * 2.0 * hl, np.pi * r * r          # side, one cap
+        region = rng.choice(3, size=n, p=np.array([side, cap, cap]) / (side + 2.0 * cap))
+        phi = rng.uniform(0.0, 2.0 * np.pi, size=n)
+        rho = np.where(region == 0, r, r * np.sqrt(rng.uniform(size=n)))
+        z = np.where(region == 0, u[:, 2] * hl, np.where(region == 1, hl, -hl))
+        return np.stack([rho * np.cos(phi), rho * np.sin(phi), z], axis=1)
+    raise ValueError(f"no analytic surface for {type(link_sdf).__name__}")
+
+
 class RobotSDF(sdf.ObjectFrameSDF):
     """SDF of an articulated robot in its base frame.
 
@@ -75,13 +100,18 @@ class RobotSDF(sdf.ObjectFrameSDF):
         visuals = list(_mesh_visuals(chain, self.frame_names, primitive_visuals))
         self.sdf_to_link_name = [name for name, _ in visuals]
         link_sdfs = []
+        self._link_factories = []          # the MeshObjectFactory of every mesh link, None for primitives
         for name, vis in visuals:
             logger.info("%s offset %s", name, vis.offset)
             if vis.geom_type != "mesh":
                 link_sdfs.append(_primitive_sdf(vis))
+                self._link_factories.append(None)
                 continue
             mesh_file, mesh_scale = vis.geom_param[0], vis.geom_param[1]
-            link_sdfs.append(link_sdf_cls(sdf.MeshObjectFactory(mesh_file, scale=mesh_scale, path_prefix=path_prefix)))
+            factory = sdf.MeshObjectFactory(mesh_file, scale=mesh_scale, path_prefix=path_prefix)
+            link_sdfs.append(link_sdf_cls(factory))
+            self._link_factories.append(factory)
+        self._surface_points = {}
         # visual origin of every mesh inside its link frame, stacked link-major
         self.offset_transforms = Transform3d(
             matrix=torch.cat([matrix_of(vis.offset) for _, vis in visuals]).to(device=self.device, dtype=self.dtype))
@@ -188,6 +218,50 @@ class RobotSDF(sdf.ObjectFrameSDF):
         (values [*A, *B], gradients [*A, *B, 3]) and, with return_argmin, the first point attaining the minimum (index
         into N) and its link, a position in `sdf_to_link_name` (ComposedSDF.paired_clearance)."""
         return self.sdf.paired_clearance(points_in_object_frame, return_argmin=return_argmin)
+
+    def link_surface_points(self, num_points=256, seed=0):
+        """[S, num_points, 3] points on the surface of every link, each in its link's own (mesh or primitive) frame,
+        in the robot's dtype and on its device; cached per (num_points, seed).  Mesh links: sample_mesh_points on the
+        link's mesh (kept in memory, never written to a cache file); box, cylinder and sphere links: seeded
+        area-uniform samples of the analytic surface."""
+        hit = self._surface_points.get((num_points, seed))
+        if hit is None:
+            per_link = []
+            for s, (link_sdf, factory) in enumerate(zip(self.sdf.sdfs, self._link_factories)):
+                if factory is not None:
+                    pts = sdf.sample_mesh_points(factory, num_points, seed=seed, name=factory.name, device=self.device,
+                                                 cache={})[0]
+                else:
+                    pts = torch.from_numpy(_primitive_surface(link_sdf, num_points, np.random.default_rng([seed, s])))
+                per_link.append(pts.to(device=self.device, dtype=self.dtype))
+            hit = self._surface_points[(num_points, seed)] = torch.stack(per_link)
+        return hit
+
+    def self_collision_pairs(self):
+        """The default `allowed` matrix of self_clearance, [S, S] bool: with m(s) the number of movable joints from the
+        root up to link s's frame, the pair (i, j) is tested when |m(i) - m(j)| >= 2.  That leaves out links on the same
+        rigid body (one frame, or frames joined by fixed joints) and links one joint apart, which touch by design.
+        Defined for serial chains; other structures pass `allowed` explicitly."""
+        movable, m_of = 0, {}
+        for fname in self.frame_names:
+            frame = self.chain.find_frame(fname)
+            if frame.joint.joint_type != "fixed":
+                movable += 1
+            m_of.setdefault(frame.link.name, movable)
+        m = torch.tensor([m_of[name] for name in self.sdf_to_link_name])
+        return (m[:, None] - m[None, :]).abs() >= 2
+
+    def self_clearance(self, link_points=None, allowed=None, return_argmin=False):
+        """For every installed joint configuration, the smallest distance between the robot's own links: link_points
+        [S, K, 3] (default: link_surface_points()) are posed with their links and tested against the links `allowed`
+        [S, S] lets them (default: self_collision_pairs()).  Returns (values [*A], robot-frame gradients [*A, 3]) and,
+        with return_argmin, the source link, point and target link, int64 [*A]; a negative value is a
+        self-collision.  See ComposedSDF.self_clearance."""
+        if link_points is None:
+            link_points = self.link_surface_points()
+        if allowed is None:
+            allowed = self.self_collision_pairs()
+        return self.sdf.self_clearance(link_points, allowed, return_argmin=return_argmin)
 
     def surface_bounding_box(self, **kwargs):
         return self.sdf.surface_bounding_box(**kwargs)

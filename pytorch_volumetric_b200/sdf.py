@@ -707,6 +707,7 @@ class ComposedSDF(ObjectFrameSDF):
         self.obj_frame_to_link_frame = tsf
         self._link_to_obj = None
         self._xf_dev = {}
+        self._inv_xf_dev = {}
         self.tsf_batch = batch_dim
         if tsf is not None:
             S = len(self.sdfs)
@@ -747,6 +748,15 @@ class ComposedSDF(ObjectFrameSDF):
             xf = matrix_of(self.obj_frame_to_link_frame).detach().to(device=device, dtype=torch.float32).contiguous()
             self._xf_dev = {device: xf}
         return xf
+
+    def _inv_xforms_on(self, device):
+        """W = _affine_inverse(M) of the fp32 transforms `_xforms_on` returns: sub-frame -> object frame, [S * A, 4, 4]
+        fp32 on `device`, computed once per installed transform set."""
+        inv = self._inv_xf_dev.get(device)
+        if inv is None:
+            inv = _affine_inverse(self._xforms_on(device)).contiguous()
+            self._inv_xf_dev = {device: inv}
+        return inv
 
     def query(self, points_in_object_frame, cfg_begin=0, cfg_count=None, return_which=False):
         """__call__ restricted to the configuration slab [cfg_begin, cfg_begin + cfg_count) (multi-GPU sharding
@@ -1095,6 +1105,138 @@ class ComposedSDF(ObjectFrameSDF):
         point = nat.deliver(out[2], out_device, torch.int64).reshape(shape)
         which = nat.deliver(out[3], out_device, torch.int64).reshape(shape)
         return vv, gg, point, which
+
+    def _self_clearance_args(self, link_points, allowed):
+        """(K, allowed rows as S lists of bools with the diagonal cleared) of a self-clearance query; ValueError when
+        link_points is not [S, K, 3] with 1 <= K < 2^24 or allowed is not an [S, S] bool matrix."""
+        S = len(self.sdfs)
+        shape = tuple(link_points.shape)
+        if len(shape) != 3 or shape[0] != S or shape[2] != 3 or not 1 <= shape[1] < (1 << 24):
+            raise ValueError(f"self-clearance query: link_points {shape} must be [S, K, 3] with S = {S} sub-SDFs and "
+                             f"1 <= K < 2^24")
+        a = allowed if torch.is_tensor(allowed) else torch.as_tensor(np.asarray(allowed))
+        if a.dtype != torch.bool or tuple(a.shape) != (S, S):
+            raise ValueError(f"self-clearance query: allowed must be an [S, S] = [{S}, {S}] bool matrix, got "
+                             f"{tuple(a.shape)} {a.dtype}")
+        rows = a.detach().cpu().tolist()
+        for i in range(S):
+            rows[i][i] = False
+        return shape[1], rows
+
+    def _self_clearance_fused(self, device):
+        """Whether pvb_composed_query_self_clearance takes this set: native descriptors, at most 8 sub-SDFs, no mesh and
+        no LOOKUP_GT_SDF grid (the sets robot_paired_clearance_kernel takes)."""
+        descs_arr, needs_mesh = self._native_descs(device)
+        return descs_arr is not None and len(self.sdfs) <= 8 and not needs_mesh
+
+    def query_self_clearance(self, link_points, allowed, cfg_begin=0, cfg_count=None, return_which=False):
+        """Self-clearance of configurations [cfg_begin, cfg_begin + cfg_count): for configuration a, the smallest
+        sdf_j(M_j(a) x) over every source sub-SDF i, every j that `allowed[i, j]` lets i be tested against (the
+        diagonal is ignored) and every point x = W_i(a) link_points[i, k], W_i = _affine_inverse(M_i) -- points that
+        belong to sub-SDF i, given in its own frame, posed with it.  The minimum is taken over (value, i, k)
+        lexicographically, and for that point the first allowed j attaining the value wins; -0 == +0 and a NaN value
+        ranks above every number.  The gradient is the object-frame gradient query_paired of the allowed
+        sub-composition reports at x.  A configuration without an allowed pair gets +inf, a zero gradient and indices
+        -1.
+
+        The definition is the composition route (`_composed_self_clearance`): for every source i, its points posed by
+        pvb_transform_points_paired and query_paired_clearance of the composition of its allowed sub-SDFs.  Sets of
+        at most 8 grid (bounding-box rule) or primitive sub-SDFs run fused in one kernel and its finish
+        (pvb_composed_query_self_clearance), bit-identical to that route; every other set takes the route itself.
+
+        link_points [S, K, 3], 1 <= K < 2^24; allowed [S, S] bool.  Returns flat (cfg_count,) / (cfg_count, 3) fp32
+        tensors on the GPU, and with return_which also int32 source sub-SDF i, point k and sub-SDF j.  Raises
+        ValueError before any device work on wrong shapes or an empty slab."""
+        S = len(self.sdfs)
+        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
+        if cfg_count is None:
+            cfg_count = n_cfg - cfg_begin
+        K, rows = self._self_clearance_args(link_points, allowed)
+        if cfg_count < 1 or cfg_begin < 0 or cfg_begin + cfg_count > n_cfg:
+            raise ValueError(f"self-clearance query: empty or invalid configuration slab [{cfg_begin}, +{cfg_count}) "
+                             f"of {n_cfg}")
+        device = nat.compute_device(link_points.device if torch.is_tensor(link_points) else None)
+        with torch.cuda.device(device):
+            p = nat.as_f32_points(link_points, device)
+            if not self._self_clearance_fused(device):
+                return self._composed_self_clearance(p, K, rows, cfg_begin, cfg_count, return_which)
+            descs_arr, _ = self._native_descs(device)
+            xf, inv = self._xforms_on(device), self._inv_xforms_on(device)
+            masks = (ctypes.c_uint8 * S)(*[sum(1 << j for j in range(S) if rows[i][j]) for i in range(S)])
+            keys = torch.empty(cfg_count, dtype=torch.int64, device=device)
+            val = torch.empty(cfg_count, dtype=torch.float32, device=device)
+            grad = torch.empty(cfg_count, 3, dtype=torch.float32, device=device)
+            src, point, which = (torch.empty(cfg_count, dtype=torch.int32, device=device) if return_which else None
+                                 for _ in range(3))
+            nat.check(nat.lib().pvb_composed_query_self_clearance(descs_arr, S, nat.ptr(xf), nat.ptr(inv), n_cfg,
+                                                                  cfg_begin, cfg_count, nat.ptr(p), K, masks,
+                                                                  nat.ptr(keys), nat.ptr(val), nat.ptr(grad),
+                                                                  nat.ptr(src), nat.ptr(point), nat.ptr(which),
+                                                                  nat.stream_ptr(device)),
+                      "pvb_composed_query_self_clearance")
+        return (val, grad, src, point, which) if return_which else (val, grad)
+
+    def _composed_self_clearance(self, p, K, rows, cfg_begin, cfg_count, return_which):
+        """query_self_clearance by composition, the definition of its result: for every source i with an allowed
+        row, link_points[i] posed by W_i of the slab (pvb_transform_points_paired), then
+        query_paired_clearance(..., return_which=True) of ComposedSDF([sdfs[j] for allowed j], their transform rows),
+        its sub-SDF index mapped back; then the minimum over i by (value, i)."""
+        S = len(self.sdfs)
+        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
+        device = p.device
+        xf = self._xforms_on(device).reshape(S, n_cfg, 4, 4)
+        inv = self._inv_xforms_on(device).reshape(S, n_cfg, 4, 4)
+        lp = p.reshape(S, K, 3)
+        per_src = []
+        for i in range(S):
+            js = [j for j in range(S) if rows[i][j]]
+            if not js:
+                continue
+            w_i = inv[i, cfg_begin:cfg_begin + cfg_count].contiguous()
+            own = lp[i].expand(cfg_count, K, 3).contiguous()
+            x = torch.empty(cfg_count, K, 3, dtype=torch.float32, device=device)
+            nat.check(nat.lib().pvb_transform_points_paired(nat.ptr(w_i), cfg_count, nat.ptr(own), K, nat.ptr(x),
+                                                            nat.stream_ptr(device)), "pvb_transform_points_paired")
+            sub = ComposedSDF([self.sdfs[j] for j in js], None)
+            sub.set_transforms(Transform3d(matrix=xf[js].reshape(len(js) * n_cfg, 4, 4)), batch_dim=(n_cfg,))
+            v, g, pt, w = sub.query_paired_clearance(x, cfg_begin=cfg_begin, cfg_count=cfg_count, return_which=True)
+            w = torch.tensor(js, dtype=torch.int32, device=device)[w.long()]
+            per_src.append((i, v, g, pt, w))
+        if not per_src:
+            val = torch.full((cfg_count,), float("inf"), dtype=torch.float32, device=device)
+            grad = torch.zeros(cfg_count, 3, dtype=torch.float32, device=device)
+            idx = [torch.full((cfg_count,), -1, dtype=torch.int32, device=device) for _ in range(3)]
+            return (val, grad, *idx) if return_which else (val, grad)
+        v = torch.stack([r[1] for r in per_src], dim=1)                                   # [cfg_count, n_src]
+        pos = (self._clearance_keys(v).amin(dim=-1) & 0xFFFFFFFF)[:, None]                 # first source on ties
+        val = v.gather(1, pos).reshape(-1)
+        grad = torch.stack([r[2] for r in per_src], dim=1).gather(1, pos[..., None].expand(cfg_count, 1, 3))
+        grad = grad.reshape(-1, 3)
+        if not return_which:
+            return val, grad
+        srcs = torch.tensor([r[0] for r in per_src], dtype=torch.int32, device=device)[pos.reshape(-1)]
+        point = torch.stack([r[3] for r in per_src], dim=1).gather(1, pos).reshape(-1)
+        which = torch.stack([r[4] for r in per_src], dim=1).gather(1, pos).reshape(-1)
+        return val, grad, srcs, point, which
+
+    def self_clearance(self, link_points, allowed, return_argmin=False):
+        """For every installed configuration, the smallest distance between its own sub-SDFs: link_points [S, K, 3]
+        holds K points of every sub-SDF in its own frame (its surface, say), and allowed [S, S] bool says which
+        sub-SDFs the points of each one are tested against (the diagonal is ignored).  Returns (values [*A],
+        gradients [*A, 3]) in link_points' dtype on the composition's device -- 0-d / [3] without a configuration
+        batch -- and with return_argmin also the source sub-SDF i, point k and sub-SDF j, int64 [*A].  Negative
+        values mean the two sub-SDFs intersect.  The semantics, tie rule and routes are those of
+        `query_self_clearance`; a configuration without an allowed pair gets +inf and indices -1.  Not a reference
+        operator (an extension); raises ValueError before any device work on wrong shapes."""
+        shape = () if self.tsf_batch is None else tuple(int(a) for a in self.tsf_batch)
+        out = self.query_self_clearance(link_points, allowed, return_which=return_argmin)
+        dtype = link_points.dtype if torch.is_tensor(link_points) else torch.float
+        out_device = matrix_of(self.obj_frame_to_link_frame).device
+        vv = nat.deliver(out[0], out_device, dtype).reshape(shape)
+        gg = nat.deliver(out[1], out_device, dtype).reshape(*shape, 3)
+        if not return_argmin:
+            return vv, gg
+        return (vv, gg) + tuple(nat.deliver(t, out_device, torch.int64).reshape(shape) for t in out[2:])
 
     def query_into(self, points_in_object_frame, targets, cfg_begin=0, cfg_count=None):
         """`query` whose result slab is stored by the kernel epilogue into several full-size result buffers at once
