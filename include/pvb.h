@@ -288,6 +288,31 @@ int pvb_composed_query_self_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, 
                                       float *out_val, float *out_grad, int32_t *out_src, int32_t *out_point,
                                       int32_t *out_which, void *stream);
 
+/* ---- EXTENSION: collision-cost query, a hinge cost over a cloud and its twist gradient for every configuration ----
+ * The reference has no such operator.  pts DEVICE [n_seg][seg_len][3] (object frame): segment b is pts[b].  For
+ * configuration a = cfg_begin + c, segment b and margin m, with (d, g, s) the per-configuration result of
+ * pvb_composed_query at point p (value, object-frame gradient, first sub-SDF attaining the value):
+ *   out_cost[c * n_seg + b]                 = sum over p of max(0, m - d)^2   (0 for an empty segment)
+ *   out_twist[((c * n_seg + b) * n_sdf + s) * 6 + k], k = 0..5
+ *                                            = sum over the p with argmin s and d < m of 2 (m - d) (g, p x g),
+ * the derivative of the cost when sub-SDF s alone moves by an object-frame twist (v, w) about the origin (its material
+ * points moving at v + w x p).  Every (d, g, s) that enters a sum is bit-identical to pvb_composed_query's; a pair is
+ * skipped only when a lower bound of its value is >= m.  The sums are deterministic: no atomics, and the order of every
+ * (configuration, segment) sum depends on seg_len alone (pvb_device.cuh collision_cost_chunk), so a slab reproduces
+ * the rows of a larger call bit for bit; they are not bit-identical to a composition of pvb_composed_query.
+ * workspace DEVICE, at least pvb_collision_cost_workspace(n_sdf, cfg_count, n_seg, seg_len) bytes, 4-byte aligned
+ * (may be NULL when that is 0); pvb_collision_cost_workspace returns -1 for negative sizes or an overflow.
+ * Serves the sets pvb_composed_query_self_clearance serves: at most 8 GRID sub-SDFs with the bounding-box rule
+ * (nearest or trilinear) or primitives.  PVB_ERR_INVALID for every other set (mesh, LOOKUP_GT_SDF grids, more than 8
+ * sub-SDFs: callers compose pvb_composed_query), for a margin that is not finite, cfg_count < 1 with points,
+ * seg_len >= 2^31, a workspace that is too small, null outputs with segments and configurations, and the argument
+ * checks of pvb_composed_query.  n_seg == 0 does nothing. */
+int64_t pvb_collision_cost_workspace(int32_t n_sdf, int32_t cfg_count, int64_t n_seg, int64_t seg_len);
+int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms, int32_t n_cfg,
+                                      int32_t cfg_begin, int32_t cfg_count, const float *pts, int64_t n_seg,
+                                      int64_t seg_len, float margin, void *workspace, int64_t workspace_bytes,
+                                      float *out_cost, float *out_twist, void *stream);
+
 /* ---- the same query with the result slab stored to several destinations from the kernel epilogue ----
  * Multi-GPU re-assembly of a configuration-sharded RobotSDF result (model_to_sdf.py:117-125 returns the full
  * (|A|, N) tensors): every rank evaluates its slab [cfg_begin, cfg_begin + cfg_count) and writes it straight into

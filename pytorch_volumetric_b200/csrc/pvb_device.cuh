@@ -1099,4 +1099,58 @@ __device__ __forceinline__ SelfClearanceOut self_clearance_finish_one(uint64_t k
     return o;
 }
 
+// ----------------------------------------------------------------------------
+// Collision-cost queries (robot_collision_cost_kernel / collision_cost_finish_kernel,
+// pvb_composed_query_collision_cost): for configuration a and segment b of the points, with margin m,
+//   cost[a, b]        = sum_n max(0, m - d)^2
+//   twist[a, b, s, :] = sum over the points n whose argmin sub-SDF is s and d < m of
+//                       (2 (m - d) g, 2 (m - d) (p x g))
+// where (d, g, s) is the per-configuration result (value, object-frame gradient, first sub-SDF attaining it) at p.
+//
+// A segment of seg_len points is summed in chunks of collision_cost_chunk(seg_len) consecutive points.  The chunk
+// depends on seg_len alone (whole multiples of 512 points, at most 256 chunks per segment; a shorter segment is one
+// chunk), and so does the order of every sum: within a chunk, the points j = w, w + 8, w + 16, ... in ascending order
+// per accumulator w = 0..7 (fp32), then the 8 accumulators in order (fp64, rounded to fp32 once per chunk), then the
+// chunks in order (fp64).  No configuration tile, slab offset, grid size or SM count enters it.
+constexpr int kCcWarps = 8;                       // accumulators per chunk: the warps of a block
+__host__ __device__ inline long long collision_cost_chunk(long long seg_len) {
+    const long long c = 512 * ((seg_len + 512 * 256 - 1) / (512 * 256));
+    return c < seg_len ? c : (seg_len > 0 ? seg_len : 1);
+}
+__host__ __device__ inline long long collision_cost_chunks(long long seg_len) {
+    return seg_len > 0 ? (seg_len + collision_cost_chunk(seg_len) - 1) / collision_cost_chunk(seg_len) : 0;
+}
+
+// a b - c d to within about one ulp of the result (Kahan's difference of products, two fused multiply-adds): the
+// moment p x g cancels when p is nearly parallel to g, and the plain difference would then carry an error of the
+// order of u |p| |g| instead of u |p x g|
+__device__ __forceinline__ float cc_diff_of_products(float a, float b, float c, float d) {
+    const float w = c * d;
+    const float e = fmaf(-c, d, w);
+    return fmaf(a, b, -w) + e;
+}
+
+// The terms of one contributing pair (d < m): cost (m - d)^2, then 2 (m - d) g and 2 (m - d) (p x g).
+struct CollisionTerm { float cost; float tw[6]; };
+__device__ __forceinline__ CollisionTerm collision_cost_term(float m, float d, f3 g, f3 p) {
+    const float h = m - d, t = 2.f * h;
+    CollisionTerm o;
+    o.cost = h * h;
+    o.tw[0] = t * g.x; o.tw[1] = t * g.y; o.tw[2] = t * g.z;
+    o.tw[3] = t * cc_diff_of_products(p.y, g.z, p.z, g.y);
+    o.tw[4] = t * cc_diff_of_products(p.z, g.x, p.x, g.z);
+    o.tw[5] = t * cc_diff_of_products(p.x, g.y, p.y, g.x);
+    return o;
+}
+
+// Whether a point can contribute for a configuration at all: some link's lower bound is below m.  A NaN bound (a
+// transform that is not an isometry) or -inf (a link without a valid bound) always passes; the +inf bound of a slot
+// beyond n_sdf never does.
+__device__ __forceinline__ bool collision_cost_near(const float (&lb)[8], float m) {
+    bool near = false;
+#pragma unroll
+    for (int si = 0; si < 8; ++si) near |= !(lb[si] >= m);
+    return near;
+}
+
 }  // namespace pvb

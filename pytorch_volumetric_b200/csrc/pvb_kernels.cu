@@ -68,7 +68,8 @@ static int sm_count() {
 // id; returns false when the runtime refuses.
 enum { kSlotMesh = 0, kSlotGridTma, kSlotCfgMajor, kSlotCfgMajorMulti, kSlotChamfer, kSlotRobot, kSlotRobotMulti,
        kSlotRobotMc, kSlotRobotWide, kSlotRobotWideMulti, kSlotRobotWideMc, kSlotSerial, kSlotSerialMulti, kSlotSerialMc,
-       kSlotSerialExt, kSlotSerialExtMulti, kSlotSerialExtMc, kSlotCfgMajorExt, kSlotCfgMajorExtMulti, kSlotCount };
+       kSlotSerialExt, kSlotSerialExtMulti, kSlotSerialExtMc, kSlotCfgMajorExt, kSlotCfgMajorExtMulti,
+       kSlotCollisionCost, kSlotCollisionCostExt, kSlotCount };
 template <typename K>
 static bool ensure_smem(K kernel, int slot, int bytes) {
     static unsigned char done[kSlotCount][kMaxDevices] = {{0}};
@@ -2318,6 +2319,149 @@ self_clearance_finish_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int 
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// Collision-cost query on the sets robot_serial_kernel takes (pvb_device.cuh: collision_cost_term): for every
+// configuration of the slab, every segment and every chunk of the segment (collision_cost_chunk), the chunk's partial
+// sums -- cost and the 6 n_sdf twist components -- left in partial[((c * n_seg + b) * chunks_per_seg + kc) * E + e],
+// E = 1 + 6 n_sdf (e = 0: cost; 1 + 6 s + k: component k of sub-SDF s).  collision_cost_finish_kernel adds the chunks.
+//   * Orientation of robot_clearance_kernel: the lanes are 32 configurations of one shared point, whose transform rows
+//     and sphere centres the block stages once per work unit.  Tiles are always 32 configurations wide (tile t starts
+//     at slab configuration 32 t; lanes past cfg_count evaluate the slab's last configuration and are never stored),
+//     so that no configuration's summation order depends on the slab.
+//   * Work unit: (tile, segment, chunk), one block; units are numbered tile-fastest (the tiles of a chunk read the same
+//     points) and the blocks of a 1-D grid stride over them.  Warp w takes the chunk's points w, w + 8, ... in order.
+//   * A point is skipped by the whole warp when no lane has a link whose sphere bound is below m; otherwise each lane
+//     runs rs_swept_pair with bp = m: a link is skipped only when a lower bound of its value is above min(running
+//     value, m), so whenever the configuration's value at the point is below m, (d, g, s) is its per-configuration
+//     result bit for bit (the gradient rotated back with the winner's rows, as robot_serial_kernel does).
+//   * Accumulators: the cost in a register, the twist sums in the lane's column of its warp's slab of shared memory,
+//     acc[warp][1 + 6 s + k][lane] (row stride 33: conflict-free for the end-of-unit reads down a column).  8 x 6
+//     registers per lane would be the alternative; a contributing lane touches only its argmin link's 6 slots.
+//   * End of unit: one thread per (configuration, slot) adds the 8 warps' values in order in fp64 and stores the
+//     partial rounded to fp32.  No atomics anywhere: the result does not depend on the grid or on block scheduling.
+struct __align__(16) CcSmem {
+    float4 xf[kRbCfg][3 * kRsMaxS + 1];
+    float4 sph[kRbCfg][3 * kRsMaxS / 4 + 1];
+};
+constexpr int kCcLaneStride = kRbCfg + 1;
+// CcSmem, then the accumulators: kCcWarps x (1 + 6 n_sdf) rows of kCcLaneStride floats
+static int cc_smem_bytes(int n_sdf) {
+    return (int)sizeof(CcSmem) + kCcWarps * (1 + 6 * n_sdf) * kCcLaneStride * (int)sizeof(float);
+}
+
+template <bool kExt>
+__global__ void __launch_bounds__(kRbCfg * kCcWarps, 3)
+robot_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, const float *__restrict__ xforms,
+                            int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ pts, long long n_seg,
+                            int seg_len, int chunk, int chunks_per_seg, float margin, long long n_units,
+                            float *__restrict__ partial) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    CcSmem &sm = *reinterpret_cast<CcSmem *>(smem_raw);
+    float *const acc_all = reinterpret_cast<float *>(smem_raw + sizeof(CcSmem));
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int E = 1 + 6 * n_sdf;
+    float *const acc = acc_all + warp * E * kCcLaneStride + lane;       // this lane's column
+    const int n_tiles = (cfg_count + 31) >> 5;
+    const int low3_off = ~7 | (n_sdf >> 30);                           // as in robot_serial_kernel: ~7, not foldable
+    const float m = margin;
+    for (long long u = blockIdx.x; u < n_units; u += gridDim.x) {
+        const long long sc = u / n_tiles;                               // segment * chunks_per_seg + chunk
+        const int c0 = (int)(u - sc * n_tiles) << 5;
+        const long long b = sc / chunks_per_seg;
+        const int kc = (int)(sc - b * chunks_per_seg);
+        const int i0 = kc * chunk;
+        const int len = min(chunk, seg_len - i0);
+        const long long pt0 = b * seg_len + i0;
+        __syncthreads();                                                // the previous unit is no longer read
+        for (int item = threadIdx.x; item < kRbCfg * n_sdf; item += blockDim.x) {
+            const int ci = item & 31, si = item >> 5;
+            const int cfg = cfg_begin + min(c0 + ci, cfg_count - 1);
+            const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg) * 16);
+            sm.xf[ci][3 * si] = __ldg(row); sm.xf[ci][3 * si + 1] = __ldg(row + 1); sm.xf[ci][3 * si + 2] = __ldg(row + 2);
+        }
+        for (int e = 0; e < E; ++e) acc[e * kCcLaneStride] = 0.f;
+        __syncthreads();
+        for (int item = threadIdx.x; item < kRbCfg * kRsMaxS; item += blockDim.x) {
+            const int ci = item & 31, si = item >> 5;
+            const f3 co = si < n_sdf ? rs_sphere_centre(pk.d[si], sm.xf[ci][3 * si], sm.xf[ci][3 * si + 1],
+                                                        sm.xf[ci][3 * si + 2])
+                                     : mk3(0.f, 0.f, 0.f);
+            float *c = reinterpret_cast<float *>(&sm.sph[ci][0]) + 3 * si;
+            c[0] = co.x; c[1] = co.y; c[2] = co.z;
+        }
+        __syncthreads();
+        float cost = 0.f;
+#pragma unroll 1
+        for (int j = warp; j < len; j += kCcWarps) {                    // uniform per warp
+            const f3 p = load_point(pts, pt0 + j);
+            float cen[3 * kRsMaxS];
+#pragma unroll
+            for (int k = 0; k < 3 * kRsMaxS / 4; ++k) {
+                const float4 c4 = sm.sph[lane][k];
+                cen[4 * k] = c4.x; cen[4 * k + 1] = c4.y; cen[4 * k + 2] = c4.z; cen[4 * k + 3] = c4.w;
+            }
+            float lb[kRsMaxS], key[kRsMaxS];
+#pragma unroll
+            for (int si = 0; si < kRsMaxS; ++si) {
+                lb[si] = rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], pk.sph_rad[si]);
+                key[si] = rs_bound_key(lb[si], low3_off, si);
+            }
+            if (!__any_sync(0xffffffffu, collision_cost_near(lb, m))) continue;
+            const int pred = __shfl_sync(0xffffffffu, rs_nearest(key, n_sdf), 0);
+            auto link = [&](const int si, const float thr, float4 &o) -> bool {
+                const pvb_sdf_desc &d = pk.d[si];
+                const float4 r0 = sm.xf[lane][3 * si], r1 = sm.xf[lane][3 * si + 1], r2 = sm.xf[lane][3 * si + 2];
+                const f3 q = composed_xform(r0, r1, r2, p);
+                const float tm = thr + pk.visit_margin[si];
+                if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
+                o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
+                    : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
+                                                               : robot_lookup(d, q);
+                return true;
+            };
+            float best;
+            f3 bg;
+            int bs;
+            rs_swept_pair(lb, pred, m, link, best, bg, bs);
+            if (bs >= 0 && best < m) {
+                const f3 g = composed_rotate_back(sm.xf[lane][3 * bs], sm.xf[lane][3 * bs + 1], sm.xf[lane][3 * bs + 2],
+                                                  bg);
+                const CollisionTerm t = collision_cost_term(m, best, g, p);
+                cost += t.cost;
+                float *const a = acc + (1 + 6 * bs) * kCcLaneStride;
+#pragma unroll
+                for (int k = 0; k < 6; ++k) a[k * kCcLaneStride] += t.tw[k];
+            }
+        }
+        acc[0] = cost;
+        __syncthreads();
+        const int active = min(kRbCfg, cfg_count - c0);
+        for (int item = threadIdx.x; item < active * E; item += blockDim.x) {
+            const int ci = item / E, e = item - ci * E;
+            double s = 0.0;
+            for (int w = 0; w < kCcWarps; ++w) s += (double)acc_all[(w * E + e) * kCcLaneStride + ci];
+            partial[(((size_t)(c0 + ci) * n_seg + b) * chunks_per_seg + kc) * E + e] = (float)s;
+        }
+    }
+}
+
+// The result of a collision-cost query: one thread per (configuration, segment, slot) adds the chunks' partials in
+// order in fp64.  Without chunks (seg_len == 0) every output is 0.
+__global__ void __launch_bounds__(kCompThreads)
+collision_cost_finish_kernel(const float *__restrict__ partial, long long n_rows, int chunks_per_seg, int E,
+                             float *__restrict__ out_cost, float *__restrict__ out_twist) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n_rows * E; t += stride) {
+        const long long r = t / E;
+        const int e = (int)(t - r * E);
+        const float *src = partial + (size_t)r * chunks_per_seg * E + e;
+        double s = 0.0;
+        for (int kc = 0; kc < chunks_per_seg; ++kc) s += (double)__ldg(src + (size_t)kc * E);
+        if (e == 0) out_cost[r] = (float)s;
+        else out_twist[(size_t)r * (E - 1) + (e - 1)] = (float)s;
+    }
+}
+
 // ========================================================== voxel containers
 // VoxelGrid / ExpandingVoxelGrid / voxel_down_sample (voxel.py:42-171) and the value-range view they sit on
 // (TorchMultidimView: sdf.py:264, voxel.py:55-64): the reference reads, writes and lists voxels with boolean-mask
@@ -3726,6 +3870,111 @@ extern "C" int pvb_composed_query_self_clearance(const pvb_sdf_desc *descs, int3
     }
     return launch_self_clearance(descs, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, (int)K, rows,
                                  n_src, k, out_val, out_grad, out_src, out_point, out_which, any_ext, s);
+}
+
+// Bytes of partial sums a collision-cost query needs: one fp32 row of 1 + 6 n_sdf per (configuration, segment, chunk);
+// -1 for negative sizes or an overflow.
+static long long collision_cost_bytes(int n_sdf, long long cfg_count, long long n_seg, long long seg_len) {
+    if (n_sdf < 1 || cfg_count < 0 || n_seg < 0 || seg_len < 0) return -1;
+    const long long row = 4ll * (1 + 6 * (long long)n_sdf);
+    const long long cps = collision_cost_chunks(seg_len);
+    long long n = cfg_count;
+    for (const long long f : {n_seg, cps, row}) {
+        if (f != 0 && n > INT64_MAX / f) return -1;
+        n *= f;
+    }
+    return n;
+}
+
+extern "C" int64_t pvb_collision_cost_workspace(int32_t n_sdf, int32_t cfg_count, int64_t n_seg, int64_t seg_len) {
+    return collision_cost_bytes(n_sdf, cfg_count, n_seg, seg_len);
+}
+
+// robot_collision_cost_kernel over every (tile, segment, chunk) unit, then collision_cost_finish_kernel.
+static int launch_collision_cost(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
+                                 int cfg_count, const float *pts, long long n_seg, long long seg_len, float margin,
+                                 float *partial, float *out_cost, float *out_twist, bool ext, cudaStream_t stream) {
+    const char *fn = "pvb_composed_query_collision_cost";
+    RobotPack<kRsMaxS> pack;
+    memset(&pack, 0, sizeof(pack));
+    for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
+    for (int si = 0; si < kRsMaxS; ++si) {
+        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
+        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
+    }
+    const int E = 1 + 6 * n_sdf;
+    const long long chunk = collision_cost_chunk(seg_len), cps = collision_cost_chunks(seg_len);
+    if (cps > 0) {
+        auto k = ext ? robot_collision_cost_kernel<true> : robot_collision_cost_kernel<false>;
+        if (!ensure_smem(k, ext ? kSlotCollisionCostExt : kSlotCollisionCost, cc_smem_bytes(kRsMaxS))) {
+            pvb_set_error("%s: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed", fn);
+            return PVB_ERR_CUDA;
+        }
+        const long long n_units = (long long)((cfg_count + 31) >> 5) * n_seg * cps;
+        const unsigned gx = (unsigned)(n_units < INT32_MAX ? n_units : INT32_MAX);
+        timing_mark(0, stream);
+        k<<<gx, kRbCfg * kCcWarps, cc_smem_bytes(n_sdf), stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,
+                                                                   n_seg, (int)seg_len, (int)chunk, (int)cps, margin,
+                                                                   n_units, partial);
+        timing_mark(1, stream);
+        PVB_CHECK_LAUNCH("pvb_composed_query_collision_cost");
+    }
+    const long long rows = (long long)cfg_count * n_seg;
+    collision_cost_finish_kernel<<<grid_for(rows * E, kCompThreads, 8), kCompThreads, 0, stream>>>(
+        partial, rows, (int)cps, E, out_cost, out_twist);
+    PVB_CHECK_LAUNCH("pvb_composed_query_collision_cost(finish)");
+    return PVB_OK;
+}
+
+extern "C" int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,
+                                                 int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                                                 const float *pts, int64_t n_seg, int64_t seg_len, float margin,
+                                                 void *workspace, int64_t workspace_bytes, float *out_cost,
+                                                 float *out_twist, void *stream) {
+    const char *fn = "pvb_composed_query_collision_cost";
+    if (n_seg < 0 || seg_len < 0 || seg_len >= (1ll << 31) || (seg_len > 0 && n_seg > INT64_MAX / seg_len) ||
+        (cfg_count > 0 && n_seg > INT64_MAX / cfg_count)) {
+        pvb_set_error("%s: invalid argument (n_seg=%lld seg_len=%lld cfg_count=%d; seg_len < 2^31)", fn,
+                      (long long)n_seg, (long long)seg_len, cfg_count);
+        return PVB_ERR_INVALID;
+    }
+    if (!(margin - margin == 0.f)) {                 // NaN or +-inf
+        pvb_set_error("%s: the margin must be finite (margin=%g)", fn, (double)margin);
+        return PVB_ERR_INVALID;
+    }
+    const long long n_pts = n_seg * seg_len;
+    bool any_ext;
+    const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_cost,
+                                        out_twist, any_ext);
+    if (bad) return bad;
+    if (n_seg == 0) return PVB_OK;
+    if (cfg_count < 1) {
+        if (n_pts == 0) return PVB_OK;
+        pvb_set_error("%s: no configurations to sum for (cfg_count=%d) with points", fn, cfg_count);
+        return PVB_ERR_INVALID;
+    }
+    if (!out_cost || !out_twist) {                   // empty segments still get their zeros
+        pvb_set_error("%s: invalid argument (out_cost or out_twist is null)", fn);
+        return PVB_ERR_INVALID;
+    }
+    // the sets robot_serial_kernel takes: <= 8 GRID links with the bounding-box rule, or primitives
+    bool fused = n_sdf <= kRsMaxS;
+    for (int i = 0; i < n_sdf && fused; ++i)
+        fused = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    if (!fused) {
+        pvb_set_error("%s: the fused query takes at most %d grid (bounding-box rule) or primitive sub-SDFs, no mesh or "
+                      "LOOKUP_GT_SDF grid (n_sdf=%d); compose it from pvb_composed_query instead", fn, kRsMaxS, n_sdf);
+        return PVB_ERR_INVALID;
+    }
+    const long long need = collision_cost_bytes(n_sdf, cfg_count, n_seg, seg_len);
+    if (need < 0 || (need > 0 && (!workspace || workspace_bytes < need || ((uintptr_t)workspace & 3)))) {
+        pvb_set_error("%s: the workspace must hold pvb_collision_cost_workspace() = %lld bytes, 4-byte aligned "
+                      "(got %lld bytes)", fn, need, (long long)workspace_bytes);
+        return PVB_ERR_INVALID;
+    }
+    return launch_collision_cost(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, margin,
+                                 reinterpret_cast<float *>(workspace), out_cost, out_twist, any_ext,
+                                 (cudaStream_t)stream);
 }
 
 extern "C" int pvb_composed_query_multi(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,

@@ -6,6 +6,7 @@ output shapes and state semantics.  `chain` is duck-typed on the pytorch_kinemat
 kinematics.py; every query is a single pvb_composed_query launch.
 """
 import logging
+import math
 import typing
 
 import numpy as np
@@ -153,6 +154,7 @@ class RobotSDF(sdf.ObjectFrameSDF):
     def set_joint_configuration(self, joint_config=None):
         """Install joint values of shape [*A, n_joints]; A (possibly empty) becomes the leading shape of results."""
         n_joints = len(self.joint_names)
+        self._twists = None                   # joint twists of the installed configurations (collision_cost)
         if joint_config is None:
             joint_config = torch.zeros(n_joints, device=self.device, dtype=self.dtype)
         batched = joint_config.dim() > 1
@@ -262,6 +264,67 @@ class RobotSDF(sdf.ObjectFrameSDF):
         if allowed is None:
             allowed = self.self_collision_pairs()
         return self.sdf.self_clearance(link_points, allowed, return_argmin=return_argmin)
+
+    def joint_twists(self):
+        """[|A|, J, 6] fp64, J in `joint_names` order: (v_j, w_j) of every movable joint under the installed
+        configurations, the robot-frame twist about the origin that a unit rate of q_j gives everything it moves.
+        Revolute and continuous joints: w_j = R_f axis_j and v_j = -w_j x t_f, with (R_f, t_f) the pose of joint j's
+        frame after its motion; prismatic joints: v_j = R_f axis_j, w_j = 0.  From the chain's forward_kinematics,
+        computed on first use and kept until the configuration changes."""
+        if self._twists is None:
+            q = self.q.reshape(-1, len(self.joint_names))
+            poses = self.chain.forward_kinematics(q, end_only=False)
+            rows = []
+            for fname in self.frame_names:
+                frame = self.chain.find_frame(fname)
+                jt = frame.joint.joint_type
+                if jt == "fixed":
+                    continue
+                pose = matrix_of(poses[frame.link.name]).to(torch.float64)
+                axis = torch.as_tensor(frame.joint.axis, dtype=torch.float64, device=pose.device)
+                d = pose[:, :3, :3] @ (axis / axis.norm())
+                if jt == "prismatic":
+                    rows.append(torch.cat([d, torch.zeros_like(d)], dim=-1))
+                else:
+                    rows.append(torch.cat([-torch.linalg.cross(d, pose[:, :3, 3], dim=-1), d], dim=-1))
+            self._twists = torch.stack(rows, dim=1) if rows else torch.zeros(q.shape[0], 0, 6, dtype=torch.float64)
+        return self._twists
+
+    def joint_moves_link(self):
+        """[J, S] bool: joint j moves link s when j's frame comes at or before s's frame in the chain's frame order
+        (get_frame_names(exclude_fixed=False)) -- a serial chain, as self_collision_pairs assumes."""
+        pos = {}
+        for k, fname in enumerate(self.frame_names):
+            pos.setdefault(self.chain.find_frame(fname).link.name, k)
+        joints = [k for k, fname in enumerate(self.frame_names)
+                  if self.chain.find_frame(fname).joint.joint_type != "fixed"]
+        links = [pos[name] for name in self.sdf_to_link_name]
+        return torch.tensor([[j <= s for s in links] for j in joints], dtype=torch.bool).reshape(len(joints),
+                                                                                                  len(links))
+
+    def collision_cost(self, points_in_object_frame, margin):
+        """For every installed joint configuration and every segment of points [*B, N, 3] in the robot frame, the soft
+        collision cost sum_p max(0, margin - d)^2 over the points within `margin` of the robot, and its derivative
+        with respect to the joint values: returns (cost [*A, *B], joint_grad [*A, *B, J]) in the points' dtype and on
+        their device, J in `joint_names` order.  dC/dq_j = sum over the links s that joint j moves of
+        twist_grad[s] . (v_j, w_j): ComposedSDF.collision_cost's twist gradient through `joint_twists`, with the link
+        gradients the query reports (for cached links, their gradient tables).  Not autograd: the gradient is an
+        output of the query."""
+        cost, twist = self.sdf.collision_cost(points_in_object_frame, margin)
+        grad = self.joint_gradient(twist, self.joint_twists(), self.joint_moves_link())
+        return cost, grad.to(cost.dtype)
+
+    @staticmethod
+    def joint_gradient(twist, joint_twists, moves):
+        """The Jacobian transpose of a serial chain: twist gradients [A, *B, S, 6] (configuration-major, A flat or
+        not), joint twists [A, J, 6] and the [J, S] move mask give [A, *B, J] in fp64, dC/dq_j = sum_s moves[j, s]
+        twist[..., s, :] . joint_twists[a, j, :]."""
+        jt = joint_twists.to(device=twist.device, dtype=torch.float64)
+        tw = twist.to(torch.float64)
+        lead = tw.shape[:-2]
+        tw = tw.reshape(jt.shape[0], math.prod(lead) // jt.shape[0], *tw.shape[-2:])
+        grad = torch.einsum("absk,js,ajk->abj", tw, moves.to(device=tw.device, dtype=torch.float64), jt)
+        return grad.reshape(*lead, jt.shape[1])
 
     def surface_bounding_box(self, **kwargs):
         return self.sdf.surface_bounding_box(**kwargs)

@@ -1238,6 +1238,109 @@ class ComposedSDF(ObjectFrameSDF):
             return vv, gg
         return (vv, gg) + tuple(nat.deliver(t, out_device, torch.int64).reshape(shape) for t in out[2:])
 
+    @staticmethod
+    def _collision_cost_margin(margin):
+        """The margin rounded to fp32 (every route computes with that value), as a Python float; ValueError unless it
+        is one number that stays finite in fp32."""
+        try:
+            m = float(np.float32(float(margin)))
+        except (TypeError, ValueError, RuntimeError):
+            raise ValueError(f"collision-cost query: the margin must be one finite number, got {margin!r}") from None
+        if not math.isfinite(m):
+            raise ValueError(f"collision-cost query: the margin must be finite, got {m}")
+        return m
+
+    def query_collision_cost(self, points_in_object_frame, margin, cfg_begin=0, cfg_count=None):
+        """Collision cost of configurations [cfg_begin, cfg_begin + cfg_count) against points [*B, N, 3], n_seg =
+        prod(B) segments of N points.  For configuration a, segment b and margin m (rounded to fp32), with (d, g, s) what
+        query(..., return_which=True) gives at point p (value, object-frame gradient, first sub-SDF attaining it):
+        cost = sum_p max(0, m - d)^2, and for every sub-SDF s, twist[s] = sum over the p with argmin s and d < m of
+        (2 (m - d) g, 2 (m - d) (p x g)) -- the derivative of the cost when sub-SDF s alone moves by an object-frame
+        twist (v, w) about the origin.  A segment without points costs 0.
+
+        Sets of at most 8 grid (bounding-box rule) or primitive sub-SDFs run in one fused kernel
+        (pvb_composed_query_collision_cost); every other set is composed from `query` in chunks of
+        `clearance_generic_chunk` configurations and reduced in torch.  Both are deterministic, and the fused route's
+        rows do not depend on the slab: a configuration split reproduces the full call bit for bit.  Returns flat
+        (cfg_count * n_seg,) / (cfg_count * n_seg, S, 6) fp32 tensors on the GPU, configuration-major.  Raises
+        ValueError before any device work on malformed points, a margin that is not finite, or a slab without
+        configurations when there are points."""
+        S = len(self.sdfs)
+        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
+        if cfg_count is None:
+            cfg_count = n_cfg - cfg_begin
+        m = self._collision_cost_margin(margin)
+        shape = tuple(points_in_object_frame.shape)
+        if len(shape) < 2 or shape[-1] != 3:
+            raise ValueError(f"collision-cost query: points {shape} must be [..., N, 3]")
+        n_seg, seg_len = math.prod(shape[:-2]), shape[-2]
+        if cfg_begin < 0 or cfg_count < 0 or cfg_begin + cfg_count > n_cfg or (cfg_count < 1 and n_seg * seg_len > 0):
+            raise ValueError(f"collision-cost query: invalid configuration slab [{cfg_begin}, +{cfg_count}) of {n_cfg}")
+        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
+        with torch.cuda.device(device):
+            p = nat.as_f32_points(points_in_object_frame, device)
+            R = cfg_count * n_seg
+            if not self._self_clearance_fused(device):
+                return self._composed_collision_cost(p, m, cfg_begin, cfg_count, n_seg, seg_len)
+            descs_arr, _ = self._native_descs(device)
+            xf = self._xforms_on(device)
+            cost = torch.empty(R, dtype=torch.float32, device=device)
+            twist = torch.empty(R, S, 6, dtype=torch.float32, device=device)
+            lib = nat.lib()
+            need = lib.pvb_collision_cost_workspace(S, cfg_count, n_seg, seg_len)
+            ws = torch.empty(max(need, 0) // 4, dtype=torch.float32, device=device)
+            nat.check(lib.pvb_composed_query_collision_cost(descs_arr, S, nat.ptr(xf), n_cfg, cfg_begin, cfg_count,
+                                                            nat.ptr(p), n_seg, seg_len, m,
+                                                            nat.ptr(ws) if need > 0 else None, need, nat.ptr(cost),
+                                                            nat.ptr(twist), nat.stream_ptr(device)),
+                      "pvb_composed_query_collision_cost")
+        return cost, twist
+
+    def _composed_collision_cost(self, p, m, cfg_begin, cfg_count, n_seg, seg_len):
+        """query_collision_cost by composition, for the sets the fused kernel refuses: query(..., return_which=True)
+        on chunks of `clearance_generic_chunk` configurations, the terms in fp64, grouped by sub-SDF with one mask and
+        one sum per sub-SDF (torch's sums are deterministic; scatter_add / index_add on CUDA are not)."""
+        S = len(self.sdfs)
+        R = cfg_count * n_seg
+        cost = torch.zeros(R, dtype=torch.float32, device=p.device)
+        twist = torch.zeros(R, S, 6, dtype=torch.float32, device=p.device)
+        if R == 0 or seg_len == 0:
+            return cost, twist
+        pts = p.double().reshape(n_seg, seg_len, 3)
+        for c0 in range(cfg_begin, cfg_begin + cfg_count, self.clearance_generic_chunk):
+            cc = min(self.clearance_generic_chunk, cfg_begin + cfg_count - c0)
+            v, g, w = self.query(p, cfg_begin=c0, cfg_count=cc, return_which=True)
+            v, g, w = v.reshape(cc, n_seg, seg_len), g.reshape(cc, n_seg, seg_len, 3), w.reshape(cc, n_seg, seg_len)
+            h = (m - v.double()).clamp_min(0.0)                     # 0 exactly where d >= m
+            g = g.double()
+            terms = torch.cat([g, torch.linalg.cross(pts.expand_as(g), g, dim=-1)], dim=-1) * (2.0 * h)[..., None]
+            out = slice((c0 - cfg_begin) * n_seg, (c0 - cfg_begin + cc) * n_seg)
+            cost[out] = (h * h).sum(dim=-1).reshape(-1).float()
+            for s in range(S):
+                twist[out, s] = (terms * (w == s)[..., None]).sum(dim=-2).reshape(-1, 6).float()
+        return cost, twist
+
+    def collision_cost(self, points_in_object_frame, margin):
+        """For every installed configuration and every segment of points [*B, N, 3], the soft collision cost
+        sum_p max(0, margin - d)^2 over the points within `margin` of the composition, and its twist gradient per
+        sub-SDF: returns (cost [*A, *B], twist_grad [*A, *B, S, 6]) in the points' dtype and on their device, A the
+        configuration batch (no A without one).  twist_grad[..., s, :] = (dC/dv_s, dC/dw_s), the derivative of the cost
+        when sub-SDF s alone moves by an object-frame twist (v, w) about the origin; a point contributes to the
+        sub-SDF that attains its minimum, with the gradient `__call__` reports there.  Margins <= 0 count penetration
+        only; a segment with N = 0 costs 0.  Semantics and routes are those of `query_collision_cost`.  Not a
+        reference operator (an extension); raises ValueError before any device work on malformed points or a margin
+        that is not finite."""
+        pts_shape = tuple(points_in_object_frame.shape)
+        if len(pts_shape) < 2 or pts_shape[-1] != 3:
+            raise ValueError(f"collision-cost query: points {pts_shape} must be [..., N, 3]")
+        m = self._collision_cost_margin(margin)
+        cost, twist = self.query_collision_cost(points_in_object_frame, m)
+        shape = (*(self.tsf_batch or ()), *pts_shape[:-2])
+        dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
+        out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
+        return (nat.deliver(cost, out_device, dtype).reshape(shape),
+                nat.deliver(twist, out_device, dtype).reshape(*shape, len(self.sdfs), 6))
+
     def query_into(self, points_in_object_frame, targets, cfg_begin=0, cfg_count=None):
         """`query` whose result slab is stored by the kernel epilogue into several full-size result buffers at once
         (pvb_composed_query_multi): `targets` is a list of (val, grad) pairs, each a float32 tensor or a raw device
