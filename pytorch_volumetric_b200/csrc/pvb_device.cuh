@@ -975,6 +975,54 @@ __device__ __forceinline__ float rs_sphere_lb(f3 p, float cx, float cy, float cz
     return fmaf(d2 * rsqrt_approx(d2), kRsBoundScale, -sph_rad);
 }
 
+// Everything that is not "in range, fp32 index estimate certain" -- the exact index of a point inside a cell
+// boundary's uncertainty band, or the point-to-AABB rule of an out-of-range point -- out of line and through a
+// pointer to the descriptor in parameter space: rare, and 32 inlined copies of it (4 points x 8 unrolled links) were
+// two thirds of the kernel's code.
+__device__ __noinline__ float4 robot_lookup_slow(const pvb_sdf_desc *dp, float qx, float qy, float qz) {
+    const pvb_sdf_desc &d = *dp;
+    NodeStage st; st.smem = nullptr; st.n = 0;
+    const SdfOut o = grid_eval<false, true>(d, st, mk3(qx, qy, qz), 0u, 0ull, nullptr);
+    return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
+}
+
+// In-range + certain: the record of the nearest voxel, same arithmetic as grid_eval.
+__device__ __forceinline__ float4 robot_lookup(const pvb_sdf_desc &g, f3 p) {
+    const float kMagic = 12582912.f;   // 1.5 * 2^23
+    const float qx = (p.x - g.min32[0]) * g.inv_res32[0];
+    const float qy = (p.y - g.min32[1]) * g.inv_res32[1];
+    const float qz = (p.z - g.min32[2]) * g.inv_res32[2];
+    const float mx = __fadd_rn(qx, kMagic), my = __fadd_rn(qy, kMagic), mz = __fadd_rn(qz, kMagic);
+    const int kx = __float_as_int(mx) - 0x4B400000, ky = __float_as_int(my) - 0x4B400000,
+              kz = __float_as_int(mz) - 0x4B400000;
+    const bool certain = (fabsf(qx - __fsub_rn(mx, kMagic)) <= g.idx_certain[0]) &
+                         (fabsf(qy - __fsub_rn(my, kMagic)) <= g.idx_certain[1]) &
+                         (fabsf(qz - __fsub_rn(mz, kMagic)) <= g.idx_certain[2]);
+    const bool inb = (p.x >= g.valid_lo[0]) & (p.x <= g.valid_hi[0]) & (p.y >= g.valid_lo[1]) &
+                     (p.y <= g.valid_hi[1]) & (p.z >= g.valid_lo[2]) & (p.z <= g.valid_hi[2]);
+    if (inb & certain)      // the index is exact and inside the table: no clamp needed
+        return __ldg(reinterpret_cast<const float4 *>(g.table) + ((kx * g.dims[1] + ky) * g.dims[2] + kz));
+    return robot_lookup_slow(&g, p.x, p.y, p.z);
+}
+
+// PVB_GRID_TRILINEAR link: the interpolant of grid_trilinear_eval in range; out of range the
+// point-to-AABB rule, which is the same for both modes, out of line as above.
+__device__ __forceinline__ float4 robot_lookup_trilinear(const pvb_sdf_desc &g, f3 p) {
+    if (grid_in_range(g, p)) {
+        const SdfOut o = grid_trilinear_interp(g, p);
+        return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
+    }
+    return robot_lookup_slow(&g, p.x, p.y, p.z);
+}
+
+// SPHERE / BOX / CYLINDER link: primitive_eval, the arithmetic of every other kernel.  Out of line,
+// like robot_lookup_slow: 9 inlined copies (the first visit + 8 unrolled links) would nearly double the code of the
+// kernel's extension instantiations, which trilinear robots run too.
+__device__ __noinline__ float4 robot_primitive(const pvb_sdf_desc *dp, float qx, float qy, float qz) {
+    const SdfOut o = primitive_eval(*dp, mk3(qx, qy, qz));
+    return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
+}
+
 // ----------------------------------------------------------------------------
 // Swept queries (robot_swept_kernel / composed_swept_kernel, pvb_composed_query_swept): the minimum over a slab of
 // configurations at every point.  The result is the per-configuration result (value, gradient, which) of the
@@ -1021,6 +1069,46 @@ __device__ __forceinline__ void rs_swept_pair(const float (&lb)[8], int pred, fl
 #pragma unroll
     for (int si = 0; si < 8; ++si)
         if (si != pred && !(lb[si] > fminf(best, bp))) visit(si);
+}
+
+// One link of the robot-family kernels evaluated at q in its frame: analytic primitive, trilinear interpolant or
+// nearest voxel (kExt = false: nearest voxel only).
+template <bool kExt>
+__device__ __forceinline__ float4 rs_link_eval(const pvb_sdf_desc &d, f3 q) {
+    return (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
+           : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
+                                                      : robot_lookup(d, q);
+}
+
+// The `link` of rs_swept_pair in the robot-family kernels: p carried into the link's frame by its rows r0..r2; false
+// when thr + visit_margin is negative or the exact AABB bound is above it, else the link evaluated into o.
+template <bool kExt>
+__device__ __forceinline__ bool rs_link_visit(const pvb_sdf_desc &d, float visit_margin, const float4 &r0,
+                                              const float4 &r1, const float4 &r2, f3 p, float thr, float4 &o) {
+    const f3 q = composed_xform(r0, r1, r2, p);
+    const float tm = thr + visit_margin;
+    if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
+    o = rs_link_eval<kExt>(d, q);
+    return true;
+}
+
+// The bounds of point p from the 8 links' bounding spheres (rs_sphere_lb) and their nearest-link keys (rs_bound_key),
+// from one staged row of sphere centres ({x, y, z} of the 8 links back to back: 6 float4).  A link whose mask bit is
+// clear gets +inf.
+__device__ __forceinline__ void rs_point_bounds(const float4 *sph, const float *sph_rad, f3 p, int low3_off,
+                                                unsigned mask, float (&lb)[8], float (&key)[8]) {
+    float cen[24];
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+        const float4 c4 = sph[j];
+        cen[4 * j] = c4.x; cen[4 * j + 1] = c4.y; cen[4 * j + 2] = c4.z; cen[4 * j + 3] = c4.w;
+    }
+#pragma unroll
+    for (int si = 0; si < 8; ++si) {
+        lb[si] = ((mask >> si) & 1u) ? rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], sph_rad[si])
+                                     : PVB_INF;
+        key[si] = rs_bound_key(lb[si], low3_off, si);
+    }
 }
 
 // ----------------------------------------------------------------------------

@@ -1275,54 +1275,6 @@ __device__ __forceinline__ void st_mc_f32(float *mc, float v) {
     asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(mc), "f"(v) : "memory");
 }
 
-// Everything that is not "in range, fp32 index estimate certain" -- the exact index of a point inside a cell
-// boundary's uncertainty band, or the point-to-AABB rule of an out-of-range point -- out of line and through a
-// pointer to the descriptor in parameter space: rare, and 32 inlined copies of it (4 points x 8 unrolled links) were
-// two thirds of the kernel's code.
-__device__ __noinline__ float4 robot_lookup_slow(const pvb_sdf_desc *dp, float qx, float qy, float qz) {
-    const pvb_sdf_desc &d = *dp;
-    NodeStage st; st.smem = nullptr; st.n = 0;
-    const SdfOut o = grid_eval<false, true>(d, st, mk3(qx, qy, qz), 0u, 0ull, nullptr);
-    return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
-}
-
-// In-range + certain: the record of the nearest voxel, same arithmetic as grid_eval (pvb_device.cuh).
-__device__ __forceinline__ float4 robot_lookup(const pvb_sdf_desc &g, f3 p) {
-    const float kMagic = 12582912.f;   // 1.5 * 2^23
-    const float qx = (p.x - g.min32[0]) * g.inv_res32[0];
-    const float qy = (p.y - g.min32[1]) * g.inv_res32[1];
-    const float qz = (p.z - g.min32[2]) * g.inv_res32[2];
-    const float mx = __fadd_rn(qx, kMagic), my = __fadd_rn(qy, kMagic), mz = __fadd_rn(qz, kMagic);
-    const int kx = __float_as_int(mx) - 0x4B400000, ky = __float_as_int(my) - 0x4B400000,
-              kz = __float_as_int(mz) - 0x4B400000;
-    const bool certain = (fabsf(qx - __fsub_rn(mx, kMagic)) <= g.idx_certain[0]) &
-                         (fabsf(qy - __fsub_rn(my, kMagic)) <= g.idx_certain[1]) &
-                         (fabsf(qz - __fsub_rn(mz, kMagic)) <= g.idx_certain[2]);
-    const bool inb = (p.x >= g.valid_lo[0]) & (p.x <= g.valid_hi[0]) & (p.y >= g.valid_lo[1]) &
-                     (p.y <= g.valid_hi[1]) & (p.z >= g.valid_lo[2]) & (p.z <= g.valid_hi[2]);
-    if (inb & certain)      // the index is exact and inside the table: no clamp needed
-        return __ldg(reinterpret_cast<const float4 *>(g.table) + ((kx * g.dims[1] + ky) * g.dims[2] + kz));
-    return robot_lookup_slow(&g, p.x, p.y, p.z);
-}
-
-// PVB_GRID_TRILINEAR link: the interpolant of grid_trilinear_eval (pvb_device.cuh) in range; out of range the
-// point-to-AABB rule, which is the same for both modes, out of line as above.
-__device__ __forceinline__ float4 robot_lookup_trilinear(const pvb_sdf_desc &g, f3 p) {
-    if (grid_in_range(g, p)) {
-        const SdfOut o = grid_trilinear_interp(g, p);
-        return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
-    }
-    return robot_lookup_slow(&g, p.x, p.y, p.z);
-}
-
-// SPHERE / BOX / CYLINDER link: primitive_eval (pvb_device.cuh), the arithmetic of every other kernel.  Out of line,
-// like robot_lookup_slow: 9 inlined copies (the first visit + 8 unrolled links) would nearly double the code of the
-// kernel's extension instantiations, which trilinear robots run too.
-__device__ __noinline__ float4 robot_primitive(const pvb_sdf_desc *dp, float qx, float qy, float qz) {
-    const SdfOut o = primitive_eval(*dp, mk3(qx, qy, qz));
-    return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
-}
-
 // kDest: 0 = out_val / out_grad, 1 = every (val, grad) pair of tg, 2 = tg.val[0] / tg.grad[0] are multicast addresses
 template <int MAXS, bool kUnroll, int kDest>
 __global__ void __launch_bounds__(kRbCfg * kRbWarps, kUnroll ? PVB_ROBOT_MINB : 3)
@@ -1612,11 +1564,16 @@ constexpr int kRsGradStride = 3 * kRsChunk + 1;   // 25
 #define PVB_RS_MINB 4
 #endif
 
-struct __align__(16) RsSmem {
+// The configuration tile of the block-level robot-family kernels: per configuration (lane), its transform rows and the
+// object-frame centres of its links' bounding spheres.
+struct __align__(16) RsTile {
     float4 xf[kRbCfg][3 * kRsMaxS + 1];
-    // object-frame centres of the lane's bounding spheres, {x, y, z} of the 8 links back to back: 6 LDS.128 (24
-    // wavefronts) per point instead of one 16-byte record per link (32); + 1 float4: odd row stride, conflict-free
+    // {x, y, z} of the 8 links back to back: 6 LDS.128 (24 wavefronts) per point instead of one 16-byte record per link
+    // (32); + 1 float4: odd row stride, conflict-free
     float4 sph[kRbCfg][3 * kRsMaxS / 4 + 1];
+};
+
+struct __align__(16) RsSmem : RsTile {
     // per-warp staging, LC rows x (8 * 32/LC values + 1) resp. (24 * 32/LC gradient floats + 1): at most 32 x 9 / 32 x 25
     float sv[kRsWarps][kRbCfg][kRsValStride];
     float sg[kRsWarps][kRbCfg][kRsGradStride];
@@ -1704,18 +1661,8 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
             const f3 p = on ? load_point(pts, pt) : mk3(0.f, 0.f, 0.f);     // the same for the LC lanes of a point group
             // ---- lower bounds of every link's value from its bounding sphere (rs_sphere_lb): value_s >= lb_s.
             // radius = inf (bound not valid) gives -inf, a NaN centre (not an isometry) NaN: never rejected.
-            float cen[3 * kRsMaxS];
-#pragma unroll
-            for (int j = 0; j < 3 * kRsMaxS / 4; ++j) {
-                const float4 c4 = sm.sph[cl][j];
-                cen[4 * j] = c4.x; cen[4 * j + 1] = c4.y; cen[4 * j + 2] = c4.z; cen[4 * j + 3] = c4.w;
-            }
             float lb[kRsMaxS], key[kRsMaxS];
-#pragma unroll
-            for (int si = 0; si < kRsMaxS; ++si) {
-                lb[si] = rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], pk.sph_rad[si]);
-                key[si] = rs_bound_key(lb[si], low3_off, si);       // link index in the 3 low mantissa bits
-            }
+            rs_point_bounds(sm.sph[cl], pk.sph_rad, p, low3_off, 0xffu, lb, key);
             // one visiting order per point group: its first lane's nearest sphere (neighbouring configurations agree;
             // rs_nearest in pvb_device.cuh: any link is a valid first visit, the order never changes a result)
             const int pred = __shfl_sync(0xffffffffu, rs_nearest(key, n_sdf), sub << lc_log2);
@@ -1732,6 +1679,8 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
                     const float thr = best + pk.visit_margin[si];
                     if (thr < 0.f || composed_aabb_lb2(d, q) > thr * thr) return;
                 }
+                // (the three-way choice of rs_link_eval, written out: through the helper, ptxas allocates the kExt
+                // instantiations' registers differently)
                 const float4 o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
                                  : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
                                                                             : robot_lookup(d, q);
@@ -1829,9 +1778,7 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
 // its per-configuration result bit for bit whenever it can win.
 constexpr int kSwMaxPts = 128;                    // points per block at most (blk_pts: 32, 64 or 128)
 
-struct __align__(16) SwSmem {
-    float4 xf[kRbCfg][3 * kRsMaxS + 1];
-    float4 sph[kRbCfg][3 * kRsMaxS / 4 + 1];
+struct __align__(16) SwSmem : RsTile {
     SweptBest best[kSwMaxPts];                    // cfg relative to cfg_begin
 };
 
@@ -1879,30 +1826,14 @@ robot_swept_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, con
             const bool on = j < npb;
             if (!__any_sync(0xffffffffu, on)) break;         // uniform per warp: the warp's groups are all past the end
             const f3 p = on ? load_point(pts, base + j) : mk3(0.f, 0.f, 0.f);
-            float cen[3 * kRsMaxS];
-#pragma unroll
-            for (int k = 0; k < 3 * kRsMaxS / 4; ++k) {
-                const float4 c4 = sm.sph[cl][k];
-                cen[4 * k] = c4.x; cen[4 * k + 1] = c4.y; cen[4 * k + 2] = c4.z; cen[4 * k + 3] = c4.w;
-            }
             float lb[kRsMaxS], key[kRsMaxS];
-#pragma unroll
-            for (int si = 0; si < kRsMaxS; ++si) {
-                lb[si] = rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], pk.sph_rad[si]);
-                key[si] = rs_bound_key(lb[si], low3_off, si);
-            }
+            rs_point_bounds(sm.sph[cl], pk.sph_rad, p, low3_off, 0xffu, lb, key);
             const int pred = __shfl_sync(0xffffffffu, rs_nearest(key, n_sdf), sub << lc_log2);
             const float bp = on ? sm.best[j].val : PVB_INF;
             auto link = [&](const int si, const float thr, float4 &o) -> bool {
                 const pvb_sdf_desc &d = pk.d[si];
                 const float4 r0 = sm.xf[cl][3 * si], r1 = sm.xf[cl][3 * si + 1], r2 = sm.xf[cl][3 * si + 2];
-                const f3 q = composed_xform(r0, r1, r2, p);
-                const float tm = thr + pk.visit_margin[si];
-                if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
-                o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
-                    : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
-                                                               : robot_lookup(d, q);
-                return true;
+                return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
             };
             float best;
             f3 bg;
@@ -1951,9 +1882,7 @@ robot_swept_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, con
 //     that earlier blocks have found -- and prunes against its value (a NaN or ~0 key: no pruning).
 //   * End of a chunk: the lanes holding the same configuration (the point groups of a warp, then the 8 warps) reduce
 //     their keys, and one atomicMin per configuration leaves the block.
-struct __align__(16) ClSmem {
-    float4 xf[kRbCfg][3 * kRsMaxS + 1];
-    float4 sph[kRbCfg][3 * kRsMaxS / 4 + 1];
+struct __align__(16) ClSmem : RsTile {
     unsigned long long red[kRsWarps][kRbCfg];
 };
 
@@ -2003,29 +1932,13 @@ robot_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf,
             const bool on = j < len;
             if (!__any_sync(0xffffffffu, on)) break;         // uniform per warp: the warp's groups are all past the end
             const f3 p = on ? load_point(pts, pt0 + j) : mk3(0.f, 0.f, 0.f);
-            float cen[3 * kRsMaxS];
-#pragma unroll
-            for (int k = 0; k < 3 * kRsMaxS / 4; ++k) {
-                const float4 c4 = sm.sph[cl][k];
-                cen[4 * k] = c4.x; cen[4 * k + 1] = c4.y; cen[4 * k + 2] = c4.z; cen[4 * k + 3] = c4.w;
-            }
             float lb[kRsMaxS], key[kRsMaxS];
-#pragma unroll
-            for (int si = 0; si < kRsMaxS; ++si) {
-                lb[si] = rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], pk.sph_rad[si]);
-                key[si] = rs_bound_key(lb[si], low3_off, si);
-            }
+            rs_point_bounds(sm.sph[cl], pk.sph_rad, p, low3_off, 0xffu, lb, key);
             const int pred = __shfl_sync(0xffffffffu, rs_nearest(key, n_sdf), sub << lc_log2);
             auto link = [&](const int si, const float thr, float4 &o) -> bool {
                 const pvb_sdf_desc &d = pk.d[si];
                 const float4 r0 = sm.xf[cl][3 * si], r1 = sm.xf[cl][3 * si + 1], r2 = sm.xf[cl][3 * si + 2];
-                const f3 q = composed_xform(r0, r1, r2, p);
-                const float tm = thr + pk.visit_margin[si];
-                if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
-                o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
-                    : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
-                                                               : robot_lookup(d, q);
-                return true;
+                return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
             };
             float best;
             f3 bg;
@@ -2118,28 +2031,12 @@ robot_paired_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int
             const int j = j0 + lane;
             const bool on = j < len;
             const f3 p = on ? load_point(pts, pt0 + j) : mk3(0.f, 0.f, 0.f);
-            float cen[3 * kRsMaxS];
-#pragma unroll
-            for (int q = 0; q < 3 * kRsMaxS / 4; ++q) {
-                const float4 c4 = sm.sph[warp][q];
-                cen[4 * q] = c4.x; cen[4 * q + 1] = c4.y; cen[4 * q + 2] = c4.z; cen[4 * q + 3] = c4.w;
-            }
             float lb[kRsMaxS], key[kRsMaxS];
-#pragma unroll
-            for (int si = 0; si < kRsMaxS; ++si) {
-                lb[si] = rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], pk.sph_rad[si]);
-                key[si] = rs_bound_key(lb[si], low3_off, si);
-            }
+            rs_point_bounds(sm.sph[warp], pk.sph_rad, p, low3_off, 0xffu, lb, key);
             auto link = [&](const int si, const float thr, float4 &o) -> bool {
                 const pvb_sdf_desc &d = pk.d[si];
                 const float4 r0 = sm.xf[warp][3 * si], r1 = sm.xf[warp][3 * si + 1], r2 = sm.xf[warp][3 * si + 2];
-                const f3 q = composed_xform(r0, r1, r2, p);
-                const float tm = thr + pk.visit_margin[si];
-                if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
-                o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
-                    : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
-                                                               : robot_lookup(d, q);
-                return true;
+                return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
             };
             float best;
             f3 bg;
@@ -2237,31 +2134,13 @@ robot_self_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n
             const bool on = j < len;
             const f3 p = composed_xform(w0, w1, w2,
                                         on ? load_point(link_pts, (long long)i * K + k0 + j) : mk3(0.f, 0.f, 0.f));
-            float cen[3 * kRsMaxS];
-#pragma unroll
-            for (int q = 0; q < 3 * kRsMaxS / 4; ++q) {
-                const float4 c4 = sm.sph[warp][q];
-                cen[4 * q] = c4.x; cen[4 * q + 1] = c4.y; cen[4 * q + 2] = c4.z; cen[4 * q + 3] = c4.w;
-            }
             float lb[kRsMaxS], key[kRsMaxS];
-#pragma unroll
-            for (int si = 0; si < kRsMaxS; ++si) {
-                lb[si] = ((mask >> si) & 1u) ? rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2],
-                                                            pk.sph_rad[si])
-                                             : PVB_INF;
-                key[si] = rs_bound_key(lb[si], low3_off, si);
-            }
+            rs_point_bounds(sm.sph[warp], pk.sph_rad, p, low3_off, mask, lb, key);
             auto link = [&](const int si, const float thr, float4 &o) -> bool {
                 if (!((mask >> si) & 1u)) return false;
                 const pvb_sdf_desc &d = pk.d[si];
                 const float4 r0 = sm.xf[warp][3 * si], r1 = sm.xf[warp][3 * si + 1], r2 = sm.xf[warp][3 * si + 2];
-                const f3 q = composed_xform(r0, r1, r2, p);
-                const float tm = thr + pk.visit_margin[si];
-                if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
-                o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
-                    : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
-                                                               : robot_lookup(d, q);
-                return true;
+                return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
             };
             float best;
             f3 bg;
@@ -2303,12 +2182,7 @@ self_clearance_finish_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int 
         auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) { rows_of(xforms, s, r0, r1, r2); };
         auto load_inv = [&](int s, float4 &r0, float4 &r1, float4 &r2) { rows_of(inv_xforms, s, r0, r1, r2); };
         auto load_pt = [&](int i, int k) { return load_point(link_pts, (long long)i * K + k); };
-        auto eval = [&](int s, f3 q) -> float4 {
-            const pvb_sdf_desc &d = pk.d[s];
-            return (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
-                   : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
-                                                              : robot_lookup(d, q);
-        };
+        auto eval = [&](int s, f3 q) { return rs_link_eval<kExt>(pk.d[s], q); };
         const SelfClearanceOut o = self_clearance_finish_one(__ldcg(keys + c), rows.mask, n_sdf, load_xf, load_inv,
                                                              load_pt, eval);
         out_val[c] = o.val;
@@ -2339,14 +2213,10 @@ self_clearance_finish_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int 
 //     registers per lane would be the alternative; a contributing lane touches only its argmin link's 6 slots.
 //   * End of unit: one thread per (configuration, slot) adds the 8 warps' values in order in fp64 and stores the
 //     partial rounded to fp32.  No atomics anywhere: the result does not depend on the grid or on block scheduling.
-struct __align__(16) CcSmem {
-    float4 xf[kRbCfg][3 * kRsMaxS + 1];
-    float4 sph[kRbCfg][3 * kRsMaxS / 4 + 1];
-};
 constexpr int kCcLaneStride = kRbCfg + 1;
-// CcSmem, then the accumulators: kCcWarps x (1 + 6 n_sdf) rows of kCcLaneStride floats
+// RsTile, then the accumulators: kCcWarps x (1 + 6 n_sdf) rows of kCcLaneStride floats
 static int cc_smem_bytes(int n_sdf) {
-    return (int)sizeof(CcSmem) + kCcWarps * (1 + 6 * n_sdf) * kCcLaneStride * (int)sizeof(float);
+    return (int)sizeof(RsTile) + kCcWarps * (1 + 6 * n_sdf) * kCcLaneStride * (int)sizeof(float);
 }
 
 template <bool kExt>
@@ -2356,8 +2226,8 @@ robot_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n
                             int seg_len, int chunk, int chunks_per_seg, float margin, long long n_units,
                             float *__restrict__ partial) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    CcSmem &sm = *reinterpret_cast<CcSmem *>(smem_raw);
-    float *const acc_all = reinterpret_cast<float *>(smem_raw + sizeof(CcSmem));
+    RsTile &sm = *reinterpret_cast<RsTile *>(smem_raw);
+    float *const acc_all = reinterpret_cast<float *>(smem_raw + sizeof(RsTile));
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int E = 1 + 6 * n_sdf;
     float *const acc = acc_all + warp * E * kCcLaneStride + lane;       // this lane's column
@@ -2394,30 +2264,14 @@ robot_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n
 #pragma unroll 1
         for (int j = warp; j < len; j += kCcWarps) {                    // uniform per warp
             const f3 p = load_point(pts, pt0 + j);
-            float cen[3 * kRsMaxS];
-#pragma unroll
-            for (int k = 0; k < 3 * kRsMaxS / 4; ++k) {
-                const float4 c4 = sm.sph[lane][k];
-                cen[4 * k] = c4.x; cen[4 * k + 1] = c4.y; cen[4 * k + 2] = c4.z; cen[4 * k + 3] = c4.w;
-            }
             float lb[kRsMaxS], key[kRsMaxS];
-#pragma unroll
-            for (int si = 0; si < kRsMaxS; ++si) {
-                lb[si] = rs_sphere_lb(p, cen[3 * si], cen[3 * si + 1], cen[3 * si + 2], pk.sph_rad[si]);
-                key[si] = rs_bound_key(lb[si], low3_off, si);
-            }
+            rs_point_bounds(sm.sph[lane], pk.sph_rad, p, low3_off, 0xffu, lb, key);
             if (!__any_sync(0xffffffffu, collision_cost_near(lb, m))) continue;
             const int pred = __shfl_sync(0xffffffffu, rs_nearest(key, n_sdf), 0);
             auto link = [&](const int si, const float thr, float4 &o) -> bool {
                 const pvb_sdf_desc &d = pk.d[si];
                 const float4 r0 = sm.xf[lane][3 * si], r1 = sm.xf[lane][3 * si + 1], r2 = sm.xf[lane][3 * si + 2];
-                const f3 q = composed_xform(r0, r1, r2, p);
-                const float tm = thr + pk.visit_margin[si];
-                if (tm < 0.f || composed_aabb_lb2(d, q) > tm * tm) return false;
-                o = (kExt && d.kind != PVB_KIND_GRID)         ? robot_primitive(&d, q.x, q.y, q.z)
-                    : (kExt && (d.flags & PVB_GRID_TRILINEAR)) ? robot_lookup_trilinear(d, q)
-                                                               : robot_lookup(d, q);
-                return true;
+                return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
             };
             float best;
             f3 bg;
@@ -3198,9 +3052,9 @@ static int launch_robot(const pvb_sdf_desc *descs, int n_sdf, const float *xform
 
 // Launch robot_serial_kernel (<= 8 GRID sub-SDFs with the bounding-box rule or primitives; `ext`: some of them
 // PVB_GRID_TRILINEAR or primitives).
-static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
-                               int cfg_count, const float *pts, long long n_pts, int vec, float *out_val,
-                               float *out_grad, int *out_which, const OutTargets *tg, bool ext, cudaStream_t stream) {
+// The pack of the robot-family kernels (robot_serial_kernel and the forms built on its tiles): the links in index
+// order with their bound constants (rs_link_consts); slots beyond n_sdf get radius -inf, i.e. a bound of +inf.
+static RobotPack<kRsMaxS> rs_pack(const pvb_sdf_desc *descs, int n_sdf) {
     RobotPack<kRsMaxS> pack;
     memset(&pack, 0, sizeof(pack));
     for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
@@ -3208,6 +3062,22 @@ static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float
         if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
         else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
     }
+    return pack;
+}
+
+// The links the robot-family kernels evaluate: GRID sub-SDFs with the bounding-box rule (nearest or trilinear) and
+// primitives; no mesh and no LOOKUP_GT_SDF grid.
+static bool rs_links_ok(const pvb_sdf_desc *descs, int n_sdf) {
+    for (int i = 0; i < n_sdf; ++i)
+        if (descs[i].kind == PVB_KIND_GRID ? (descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind == PVB_KIND_MESH)
+            return false;
+    return true;
+}
+
+static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
+                               int cfg_count, const float *pts, long long n_pts, int vec, float *out_val,
+                               float *out_grad, int *out_which, const OutTargets *tg, bool ext, cudaStream_t stream) {
+    const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
     const int kind = !tg ? 0 : (tg->mc ? 2 : 1);
     auto k0 = ext ? robot_serial_kernel<0, true> : robot_serial_kernel<0, false>;
     auto k1 = ext ? robot_serial_kernel<1, true> : robot_serial_kernel<1, false>;
@@ -3310,9 +3180,7 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
     static const int robot_kernel = [] { const char *e = getenv("PVB_ROBOT_KERNEL"); return e ? atoi(e) : 2; }();
     // every sub-SDF a GRID with the bounding-box rule (nearest or trilinear) or a primitive: the robot kernels'
     // precondition (primitives and trilinear grids then need the serial kernel, see serial_taken)
-    bool all_grid = !needs_mesh && n_sdf <= 16 && n_pts < (1ll << 31);
-    for (int i = 0; i < n_sdf && all_grid; ++i)
-        all_grid = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    const bool all_grid = !needs_mesh && n_sdf <= 16 && n_pts < (1ll << 31) && rs_links_ok(descs, n_sdf);
     // the point-serial kernel has no fill problem (remainder configurations run in lane-split tiles): any batch of
     // PVB_ROBOT_MIN_CFG or more configurations takes it
     static const int serial_min_cfg = [] { const char *e = getenv("PVB_ROBOT_MIN_CFG"); return e ? atoi(e) : 8; }();
@@ -3463,13 +3331,7 @@ extern "C" int pvb_composed_query_paired(const pvb_sdf_desc *descs, int32_t n_sd
 static int launch_robot_swept(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                               int cfg_count, const float *pts, long long n_pts, float *out_val, float *out_grad,
                               int *out_cfg, int *out_which, bool ext, cudaStream_t stream) {
-    RobotPack<kRsMaxS> pack;
-    memset(&pack, 0, sizeof(pack));
-    for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
-    for (int si = 0; si < kRsMaxS; ++si) {
-        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
-        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
-    }
+    const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
     const long long slots = (long long)sm_count() * PVB_RS_MINB;
     int blk_pts = kSwMaxPts;
     while (blk_pts > 32 && n_pts < 2 * slots * blk_pts) blk_pts >>= 1;
@@ -3523,9 +3385,7 @@ extern "C" int pvb_composed_query_swept(const pvb_sdf_desc *descs, int32_t n_sdf
     }
     cudaStream_t s = (cudaStream_t)stream;
     // robot_serial_kernel's sets take the fused kernel: <= 8 GRID links with the bounding-box rule or primitives
-    bool fused = !needs_mesh && n_sdf <= kRsMaxS && n_pts < (1ll << 31);
-    for (int i = 0; i < n_sdf && fused; ++i)
-        fused = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    const bool fused = !needs_mesh && n_sdf <= kRsMaxS && n_pts < (1ll << 31) && rs_links_ok(descs, n_sdf);
     if (fused)
         return launch_robot_swept(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_val, out_grad,
                                   out_cfg, out_which, any_ext, s);
@@ -3546,13 +3406,7 @@ extern "C" int pvb_composed_query_swept(const pvb_sdf_desc *descs, int32_t n_sdf
 static int launch_robot_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                                   int cfg_count, const float *pts, long long n_seg, long long seg_len,
                                   unsigned long long *keys, bool ext, cudaStream_t stream) {
-    RobotPack<kRsMaxS> pack;
-    memset(&pack, 0, sizeof(pack));
-    for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
-    for (int si = 0; si < kRsMaxS; ++si) {
-        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
-        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
-    }
+    const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
     const int gy = (cfg_count >> 5) + __builtin_popcount((unsigned)(cfg_count & 31));
     const long long want = 4ll * sm_count() * PVB_RS_MINB;          // blocks for 4 waves
     long long per_seg = (want + (long long)gy * n_seg - 1) / ((long long)gy * n_seg);
@@ -3646,10 +3500,9 @@ extern "C" int pvb_composed_query_clearance(const pvb_sdf_desc *descs, int32_t n
     }
     // robot_serial_kernel's sets take the fused kernel: <= 8 GRID links with the bounding-box rule or primitives, and
     // one grid row per configuration tile
-    bool fused = !needs_mesh && n_sdf <= kRsMaxS &&
-                 (cfg_count >> 5) + __builtin_popcount((unsigned)(cfg_count & 31)) <= 65535;
-    for (int i = 0; i < n_sdf && fused; ++i)
-        fused = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    const bool fused = !needs_mesh && n_sdf <= kRsMaxS &&
+                       (cfg_count >> 5) + __builtin_popcount((unsigned)(cfg_count & 31)) <= 65535 &&
+                       rs_links_ok(descs, n_sdf);
     if (fused) {
         const int rc = launch_robot_clearance(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
                                               k, any_ext, s);
@@ -3674,13 +3527,7 @@ extern "C" int pvb_composed_query_clearance(const pvb_sdf_desc *descs, int32_t n
 static int launch_robot_paired_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg,
                                          int cfg_begin, int cfg_count, const float *pts, long long n_seg,
                                          long long seg_len, unsigned long long *keys, bool ext, cudaStream_t stream) {
-    RobotPack<kRsMaxS> pack;
-    memset(&pack, 0, sizeof(pack));
-    for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
-    for (int si = 0; si < kRsMaxS; ++si) {
-        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
-        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
-    }
+    const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
     const long long pairs = (long long)cfg_count * n_seg;
     const long long want = 4ll * sm_count() * PVB_RS_MINB * kRsWarps;    // warp units for 4 waves
     long long per_seg = (want + pairs - 1) / pairs;
@@ -3744,9 +3591,7 @@ extern "C" int pvb_composed_query_paired_clearance(const pvb_sdf_desc *descs, in
     }
     // robot_serial_kernel's sets take the fused kernel: <= 8 GRID links with the bounding-box rule or primitives (its
     // 1-D grid has no limit on cfg_count)
-    bool fused = !needs_mesh && n_sdf <= kRsMaxS;
-    for (int i = 0; i < n_sdf && fused; ++i)
-        fused = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    const bool fused = !needs_mesh && n_sdf <= kRsMaxS && rs_links_ok(descs, n_sdf);
     if (fused) {
         const int rc = launch_robot_paired_clearance(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg,
                                                      seg_len, k, any_ext, s);
@@ -3773,13 +3618,7 @@ static int launch_self_clearance(const pvb_sdf_desc *descs, int n_sdf, const flo
                                  const SclRows &rows, int n_src, unsigned long long *keys, float *out_val,
                                  float *out_grad, int *out_src, int *out_point, int *out_which, bool ext,
                                  cudaStream_t stream) {
-    RobotPack<kRsMaxS> pack;
-    memset(&pack, 0, sizeof(pack));
-    for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
-    for (int si = 0; si < kRsMaxS; ++si) {
-        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
-        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
-    }
+    const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
     if (n_src > 0) {
         const long long pairs = (long long)cfg_count * n_src;
         const long long want = 4ll * sm_count() * PVB_RS_MINB * kRsWarps;    // warp units for 4 waves
@@ -3838,9 +3677,7 @@ extern "C" int pvb_composed_query_self_clearance(const pvb_sdf_desc *descs, int3
         return PVB_ERR_INVALID;
     }
     // the sets robot_paired_clearance_kernel takes: <= 8 GRID links with the bounding-box rule, or primitives
-    bool fused = n_sdf <= kRsMaxS;
-    for (int i = 0; i < n_sdf && fused; ++i)
-        fused = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    const bool fused = n_sdf <= kRsMaxS && rs_links_ok(descs, n_sdf);
     if (!fused) {
         pvb_set_error("%s: the fused query takes at most %d grid (bounding-box rule) or primitive sub-SDFs, no mesh or "
                       "LOOKUP_GT_SDF grid (n_sdf=%d); compose the per-source paired clearance queries instead", fn,
@@ -3895,13 +3732,7 @@ static int launch_collision_cost(const pvb_sdf_desc *descs, int n_sdf, const flo
                                  int cfg_count, const float *pts, long long n_seg, long long seg_len, float margin,
                                  float *partial, float *out_cost, float *out_twist, bool ext, cudaStream_t stream) {
     const char *fn = "pvb_composed_query_collision_cost";
-    RobotPack<kRsMaxS> pack;
-    memset(&pack, 0, sizeof(pack));
-    for (int si = 0; si < n_sdf; ++si) { pack.d[si] = descs[si]; pack.orig[si] = si; }
-    for (int si = 0; si < kRsMaxS; ++si) {
-        if (si < n_sdf) rs_link_consts(descs[si], pack.sph_rad[si], pack.visit_margin[si]);
-        else pack.sph_rad[si] = -PVB_INF;       // empty slot: bound +inf
-    }
+    const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
     const int E = 1 + 6 * n_sdf;
     const long long chunk = collision_cost_chunk(seg_len), cps = collision_cost_chunks(seg_len);
     if (cps > 0) {
@@ -3958,9 +3789,7 @@ extern "C" int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int3
         return PVB_ERR_INVALID;
     }
     // the sets robot_serial_kernel takes: <= 8 GRID links with the bounding-box rule, or primitives
-    bool fused = n_sdf <= kRsMaxS;
-    for (int i = 0; i < n_sdf && fused; ++i)
-        fused = descs[i].kind == PVB_KIND_GRID ? !(descs[i].flags & PVB_GRID_OOB_GT) : descs[i].kind != PVB_KIND_MESH;
+    const bool fused = n_sdf <= kRsMaxS && rs_links_ok(descs, n_sdf);
     if (!fused) {
         pvb_set_error("%s: the fused query takes at most %d grid (bounding-box rule) or primitive sub-SDFs, no mesh or "
                       "LOOKUP_GT_SDF grid (n_sdf=%d); compose it from pvb_composed_query instead", fn, kRsMaxS, n_sdf);

@@ -10,49 +10,15 @@
 #include <random>
 #include <vector>
 
-#include "cuda_runtime.h"
-#include "../../pytorch_volumetric_b200/csrc/pvb_device.cuh"
+// The link visits (lookups included) and sphere bounds are the kernels' own: rs_link_visit, rs_link_eval and
+// rs_point_bounds of pvb_device.cuh.
+#include "hostsim_robot.h"
 
-using namespace pvb;
-
-static inline void load_rows(const float *xforms, int n_cfg, int s, int cfg, float4 &r0, float4 &r1, float4 &r2) {
-    const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
-    r0 = row[0]; r1 = row[1]; r2 = row[2];
-}
-
-// robot_clearance_kernel's evaluation of a link: primitive, trilinear or nearest-voxel lookup (the same arithmetic as
-// robot_primitive / robot_lookup_trilinear / robot_lookup)
-static inline float4 eval_link(const pvb_sdf_desc &d, f3 q) {
-    NodeStage st; st.smem = nullptr; st.n = 0;
-    SdfOut o;
-    if (d.kind != PVB_KIND_GRID) o = primitive_eval(d, q);
-    else if (d.flags & PVB_GRID_TRILINEAR) o = grid_trilinear_eval(d, q);
-    else o = grid_eval<false, true>(d, st, q, 0u, 0ull, nullptr);
-    return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
-}
-
-struct Consts {
-    float sph_rad[8], visit_margin[8];
-    Consts(const pvb_sdf_desc *descs, int n_sdf) {
-        for (int s = 0; s < 8; ++s) {
-            if (s < n_sdf) rs_link_consts(descs[s], sph_rad[s], visit_margin[s]);
-            else { sph_rad[s] = -PVB_INF; visit_margin[s] = 0.f; }
-        }
-    }
-};
-
-static void bounds(const pvb_sdf_desc *descs, int n_sdf, const Consts &k, const float *xforms, int n_cfg, int cfg, f3 p,
-                   float (&lb)[8], float (&key)[8]) {
-    for (int s = 0; s < 8; ++s) {
-        f3 cen = mk3(0.f, 0.f, 0.f);
-        if (s < n_sdf) {
-            float4 r0, r1, r2;
-            load_rows(xforms, n_cfg, s, cfg, r0, r1, r2);
-            cen = rs_sphere_centre(descs[s], r0, r1, r2);
-        }
-        lb[s] = rs_sphere_lb(p, cen.x, cen.y, cen.z, k.sph_rad[s]);
-        key[s] = rs_bound_key(lb[s], ~7, s);
-    }
+static void bounds(const pvb_sdf_desc *descs, int n_sdf, const RsConsts &k, const float *xforms, int n_cfg, int cfg,
+                   f3 p, float (&lb)[8], float (&key)[8]) {
+    float4 sph[6];
+    rs_centres(descs, n_sdf, xforms, n_cfg, cfg, sph);
+    rs_point_bounds(sph, k.sph_rad, p, ~7, 0xffu, lb, key);
 }
 
 // chunk: points per chunk (>= seg_len: whole segments); unit_order 0 ascending, 1 descending, 2 shuffled by
@@ -62,7 +28,7 @@ extern "C" void simclear_fused(const pvb_sdf_desc *descs, int n_sdf, const float
                                int cfg_count, const float *pts, long long n_seg, int seg_len, int chunk,
                                int unit_order, int shuffle_seed, int seeded, int first, int lanes_reversed,
                                uint64_t *keys, long long *n_evals) {
-    const Consts k(descs, n_sdf);
+    const RsConsts k(descs, n_sdf);
     for (long long t = 0; t < (long long)cfg_count * n_seg; ++t) keys[t] = ~0ull;
     const int n_tiles = (cfg_count >> 5) + __builtin_popcount((unsigned)(cfg_count & 31));
     const int per_seg = (seg_len + chunk - 1) / chunk;
@@ -100,10 +66,7 @@ extern "C" void simclear_fused(const pvb_sdf_desc *descs, int n_sdf, const float
                     auto link = [&](const int si, const float thr, float4 &o) -> bool {
                         float4 r0, r1, r2;
                         load_rows(xforms, n_cfg, si, cfg, r0, r1, r2);
-                        const f3 q = composed_xform(r0, r1, r2, p);
-                        const float tm = thr + k.visit_margin[si];
-                        if (tm < 0.f || composed_aabb_lb2(descs[si], q) > tm * tm) return false;
-                        o = eval_link(descs[si], q);
+                        if (!rs_link_visit<true>(descs[si], k.visit_margin[si], r0, r1, r2, p, thr, o)) return false;
                         ++evals;
                         return true;
                     };
@@ -186,7 +149,7 @@ extern "C" void simclear_finish(const pvb_sdf_desc *descs, int n_sdf, const unsi
 extern "C" void simclear_serial_pairs(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg,
                                       const float *pts, long long n_pts, int first, float *out_val, float *out_grad,
                                       int *out_which) {
-    const Consts k(descs, n_sdf);
+    const RsConsts k(descs, n_sdf);
 #pragma omp parallel for schedule(dynamic, 64)
     for (long long t = 0; t < (long long)n_cfg * n_pts; ++t) {
         const int cfg = (int)(t / n_pts);
@@ -206,7 +169,7 @@ extern "C" void simclear_serial_pairs(const pvb_sdf_desc *descs, int n_sdf, cons
                 const float thr = best + k.visit_margin[si];
                 if (thr < 0.f || composed_aabb_lb2(descs[si], q) > thr * thr) return;
             }
-            const float4 o = eval_link(descs[si], q);
+            const float4 o = rs_link_eval<true>(descs[si], q);
             if (is_first || o.x < best || (o.x == best && si < bs)) { best = o.x; bg = mk3(o.y, o.z, o.w); bs = si; }
         };
         visit(pred, true);

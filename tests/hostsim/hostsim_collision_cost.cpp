@@ -13,26 +13,9 @@
 #include <random>
 #include <vector>
 
-#include "cuda_runtime.h"
-#include "../../pytorch_volumetric_b200/csrc/pvb_device.cuh"
-
-using namespace pvb;
-
-static inline void load_rows(const float *xforms, int n_cfg, int s, int cfg, float4 &r0, float4 &r1, float4 &r2) {
-    const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
-    r0 = row[0]; r1 = row[1]; r2 = row[2];
-}
-
-// robot_collision_cost_kernel's evaluation of a link: primitive, trilinear or nearest-voxel lookup (the arithmetic of
-// robot_primitive / robot_lookup_trilinear / robot_lookup)
-static inline float4 eval_link(const pvb_sdf_desc &d, f3 q) {
-    NodeStage st; st.smem = nullptr; st.n = 0;
-    SdfOut o;
-    if (d.kind != PVB_KIND_GRID) o = primitive_eval(d, q);
-    else if (d.flags & PVB_GRID_TRILINEAR) o = grid_trilinear_eval(d, q);
-    else o = grid_eval<false, true>(d, st, q, 0u, 0ull, nullptr);
-    return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
-}
+// The link visits (lookups included) and sphere bounds are the kernels' own: rs_link_visit, rs_link_eval and
+// rs_point_bounds of pvb_device.cuh.
+#include "hostsim_robot.h"
 
 // chunk: points per chunk (0: collision_cost_chunk(seg_len), the kernel's rule); n_acc: accumulators per unit (8 in the
 // kernel); lanes: configurations per tile (32 in the kernel); unit_order 0 ascending, 1 descending, 2 shuffled by
@@ -44,11 +27,7 @@ extern "C" void simcc_fused(const pvb_sdf_desc *descs, int n_sdf, const float *x
                             int n_acc, int lanes, int unit_order, int shuffle_seed, int first, float *out_cost,
                             float *out_twist, unsigned char *visited, float *pair_val, float *pair_grad,
                             int *pair_which, long long *n_evals) {
-    float sph_rad[8], visit_margin[8];
-    for (int s = 0; s < 8; ++s) {
-        if (s < n_sdf) rs_link_consts(descs[s], sph_rad[s], visit_margin[s]);
-        else { sph_rad[s] = -PVB_INF; visit_margin[s] = 0.f; }
-    }
+    const RsConsts links(descs, n_sdf);
     const int E = 1 + 6 * n_sdf;
     if (chunk <= 0) chunk = (int)collision_cost_chunk(seg_len);
     const int cps = seg_len > 0 ? (seg_len + chunk - 1) / chunk : 0;
@@ -79,18 +58,11 @@ extern "C" void simcc_fused(const pvb_sdf_desc *descs, int n_sdf, const float *x
                 bool any = false;
                 for (int cl = 0; cl < lanes; ++cl) {
                     const int cfg = cfg_begin + std::min(c0 + cl, cfg_count - 1);
+                    float4 sph[6];
                     float lb[8], key[8];
-                    for (int s = 0; s < 8; ++s) {
-                        f3 cen = mk3(0.f, 0.f, 0.f);
-                        if (s < n_sdf) {
-                            float4 r0, r1, r2;
-                            load_rows(xforms, n_cfg, s, cfg, r0, r1, r2);
-                            cen = rs_sphere_centre(descs[s], r0, r1, r2);
-                        }
-                        lb[s] = rs_sphere_lb(p, cen.x, cen.y, cen.z, sph_rad[s]);
-                        key[s] = rs_bound_key(lb[s], ~7, s);
-                        lbs[cl][s] = lb[s]; keys[cl][s] = key[s];
-                    }
+                    rs_centres(descs, n_sdf, xforms, n_cfg, cfg, sph);
+                    rs_point_bounds(sph, links.sph_rad, p, ~7, 0xffu, lb, key);
+                    for (int s = 0; s < 8; ++s) { lbs[cl][s] = lb[s]; keys[cl][s] = key[s]; }
                     any |= collision_cost_near(lb, m);
                 }
                 if (!any) continue;                             // the whole warp skips the point
@@ -107,12 +79,8 @@ extern "C" void simcc_fused(const pvb_sdf_desc *descs, int n_sdf, const float *x
                     auto link = [&](const int si, const float thr, float4 &o) -> bool {
                         float4 r0, r1, r2;
                         load_rows(xforms, n_cfg, si, cfg, r0, r1, r2);
-                        const f3 q = composed_xform(r0, r1, r2, p);
-                        const float tm = thr + visit_margin[si];
-                        if (tm < 0.f || composed_aabb_lb2(descs[si], q) > tm * tm) return false;
-                        o = eval_link(descs[si], q);
+                        if (!rs_link_visit<true>(descs[si], links.visit_margin[si], r0, r1, r2, p, thr, o)) return false;
                         evals += cl < active;           // lanes past the slab are not counted
-
                         return true;
                     };
                     float best;

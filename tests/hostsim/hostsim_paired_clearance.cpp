@@ -11,26 +11,9 @@
 #include <random>
 #include <vector>
 
-#include "cuda_runtime.h"
-#include "../../pytorch_volumetric_b200/csrc/pvb_device.cuh"
-
-using namespace pvb;
-
-static inline void load_rows(const float *xforms, int n_cfg, int s, int cfg, float4 &r0, float4 &r1, float4 &r2) {
-    const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
-    r0 = row[0]; r1 = row[1]; r2 = row[2];
-}
-
-// the kernel's evaluation of a link: primitive, trilinear or nearest-voxel lookup (the same arithmetic as
-// robot_primitive / robot_lookup_trilinear / robot_lookup)
-static inline float4 eval_link(const pvb_sdf_desc &d, f3 q) {
-    NodeStage st; st.smem = nullptr; st.n = 0;
-    SdfOut o;
-    if (d.kind != PVB_KIND_GRID) o = primitive_eval(d, q);
-    else if (d.flags & PVB_GRID_TRILINEAR) o = grid_trilinear_eval(d, q);
-    else o = grid_eval<false, true>(d, st, q, 0u, 0ull, nullptr);
-    return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
-}
+// The link visits (lookups included) and sphere bounds are the kernels' own: rs_link_visit, rs_link_eval and
+// rs_point_bounds of pvb_device.cuh.
+#include "hostsim_robot.h"
 
 // chunk: points per unit (>= seg_len: whole segments); lanes: threads per unit (32: a warp, 256: a block); share: the
 // running value is the minimum over each warp of the unit after every step; unit_order 0 ascending, 1 descending, 2
@@ -40,11 +23,7 @@ extern "C" void simpcl_fused(const pvb_sdf_desc *descs, int n_sdf, const float *
                              int cfg_count, const float *pts, long long n_seg, int seg_len, int chunk, int lanes,
                              int share, int unit_order, int shuffle_seed, int seeded, int first, int steps_reversed,
                              uint64_t *keys, long long *n_evals) {
-    float sph_rad[8], visit_margin[8];
-    for (int s = 0; s < 8; ++s) {
-        if (s < n_sdf) rs_link_consts(descs[s], sph_rad[s], visit_margin[s]);
-        else { sph_rad[s] = -PVB_INF; visit_margin[s] = 0.f; }
-    }
+    const RsConsts links(descs, n_sdf);
     const long long pairs = (long long)cfg_count * n_seg;
     for (long long t = 0; t < pairs; ++t) keys[t] = ~0ull;
     const int per_seg = (seg_len + chunk - 1) / chunk;
@@ -60,15 +39,8 @@ extern "C" void simpcl_fused(const pvb_sdf_desc *descs, int n_sdf, const float *
         const int len = std::min(chunk, seg_len - i0);
         const long long pt0 = cb * seg_len + i0;
         // the unit's staging: sphere centres of its one configuration
-        f3 cen[8];
-        for (int s = 0; s < 8; ++s) {
-            cen[s] = mk3(0.f, 0.f, 0.f);
-            if (s < n_sdf) {
-                float4 r0, r1, r2;
-                load_rows(xforms, n_cfg, s, cfg, r0, r1, r2);
-                cen[s] = rs_sphere_centre(descs[s], r0, r1, r2);
-            }
-        }
+        float4 sph[6];
+        rs_centres(descs, n_sdf, xforms, n_cfg, cfg, sph);
         const uint64_t seed_key = seeded ? keys[cb] : ~0ull;
         const float seed = clearance_key_value(seed_key);
         std::vector<uint64_t> run(lanes, ~0ull);
@@ -82,17 +54,11 @@ extern "C" void simpcl_fused(const pvb_sdf_desc *descs, int n_sdf, const float *
                 const long long i = pt0 + j;
                 const f3 p = mk3(pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]);
                 float lb[8], key[8];
-                for (int s = 0; s < 8; ++s) {
-                    lb[s] = rs_sphere_lb(p, cen[s].x, cen[s].y, cen[s].z, sph_rad[s]);
-                    key[s] = rs_bound_key(lb[s], ~7, s);
-                }
+                rs_point_bounds(sph, links.sph_rad, p, ~7, 0xffu, lb, key);
                 auto link = [&](const int si, const float thr, float4 &o) -> bool {
                     float4 r0, r1, r2;
                     load_rows(xforms, n_cfg, si, cfg, r0, r1, r2);
-                    const f3 q = composed_xform(r0, r1, r2, p);
-                    const float tm = thr + visit_margin[si];
-                    if (tm < 0.f || composed_aabb_lb2(descs[si], q) > tm * tm) return false;
-                    o = eval_link(descs[si], q);
+                    if (!rs_link_visit<true>(descs[si], links.visit_margin[si], r0, r1, r2, p, thr, o)) return false;
                     ++evals;
                     return true;
                 };

@@ -12,26 +12,9 @@
 #include <random>
 #include <vector>
 
-#include "cuda_runtime.h"
-#include "../../pytorch_volumetric_b200/csrc/pvb_device.cuh"
-
-using namespace pvb;
-
-static inline void load_rows(const float *xforms, int n_cfg, int s, int cfg, float4 &r0, float4 &r1, float4 &r2) {
-    const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
-    r0 = row[0]; r1 = row[1]; r2 = row[2];
-}
-
-// the kernels' evaluation of a link: primitive, trilinear or nearest-voxel lookup (the same arithmetic as
-// robot_primitive / robot_lookup_trilinear / robot_lookup)
-static inline float4 eval_link(const pvb_sdf_desc &d, f3 q) {
-    NodeStage st; st.smem = nullptr; st.n = 0;
-    SdfOut o;
-    if (d.kind != PVB_KIND_GRID) o = primitive_eval(d, q);
-    else if (d.flags & PVB_GRID_TRILINEAR) o = grid_trilinear_eval(d, q);
-    else o = grid_eval<false, true>(d, st, q, 0u, 0ull, nullptr);
-    return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
-}
+// The link visits (lookups included) and sphere bounds are the kernels' own: rs_link_visit, rs_link_eval and
+// rs_point_bounds of pvb_device.cuh.
+#include "hostsim_robot.h"
 
 extern "C" uint64_t simscl_key(float v, int i, int k) { return self_clearance_key(v, i, k); }
 
@@ -56,11 +39,7 @@ extern "C" void simscl_fused(const pvb_sdf_desc *descs, int n_sdf, const float *
                              int n_cfg, int cfg_begin, int cfg_count, const float *link_pts, int K,
                              const unsigned char *masks, int chunk, int lanes, int share, int unit_order,
                              int shuffle_seed, int seeded, int first, uint64_t *keys, long long *visits) {
-    float sph_rad[8], visit_margin[8];
-    for (int s = 0; s < 8; ++s) {
-        if (s < n_sdf) rs_link_consts(descs[s], sph_rad[s], visit_margin[s]);
-        else { sph_rad[s] = -PVB_INF; visit_margin[s] = 0.f; }
-    }
+    const RsConsts links(descs, n_sdf);
     for (int c = 0; c < cfg_count; ++c) keys[c] = ~0ull;
     for (int q = 0; q < 64; ++q) visits[q] = 0;
     std::vector<int> src;
@@ -79,15 +58,8 @@ extern "C" void simscl_fused(const pvb_sdf_desc *descs, int n_sdf, const float *
         const unsigned mask = masks[i];
         const int k0 = (int)kc * chunk;
         const int len = std::min(chunk, K - k0);
-        f3 cen[8];
-        for (int s = 0; s < 8; ++s) {
-            cen[s] = mk3(0.f, 0.f, 0.f);
-            if (s < n_sdf) {
-                float4 r0, r1, r2;
-                load_rows(xforms, n_cfg, s, cfg, r0, r1, r2);
-                cen[s] = rs_sphere_centre(descs[s], r0, r1, r2);
-            }
-        }
+        float4 sph[6];
+        rs_centres(descs, n_sdf, xforms, n_cfg, cfg, sph);
         float4 w0, w1, w2;
         load_rows(inv_xforms, n_cfg, i, cfg, w0, w1, w2);
         const uint64_t seed_key = seeded ? keys[c] : ~0ull;
@@ -100,18 +72,12 @@ extern "C" void simscl_fused(const pvb_sdf_desc *descs, int n_sdf, const float *
                 const float *lp = link_pts + 3 * ((size_t)i * K + k);
                 const f3 p = composed_xform(w0, w1, w2, mk3(lp[0], lp[1], lp[2]));
                 float lb[8], key[8];
-                for (int s = 0; s < 8; ++s) {
-                    lb[s] = ((mask >> s) & 1u) ? rs_sphere_lb(p, cen[s].x, cen[s].y, cen[s].z, sph_rad[s]) : PVB_INF;
-                    key[s] = rs_bound_key(lb[s], ~7, s);
-                }
+                rs_point_bounds(sph, links.sph_rad, p, ~7, mask, lb, key);
                 auto link = [&](const int si, const float thr, float4 &o) -> bool {
                     if (!((mask >> si) & 1u)) return false;
                     float4 r0, r1, r2;
                     load_rows(xforms, n_cfg, si, cfg, r0, r1, r2);
-                    const f3 q = composed_xform(r0, r1, r2, p);
-                    const float tm = thr + visit_margin[si];
-                    if (tm < 0.f || composed_aabb_lb2(descs[si], q) > tm * tm) return false;
-                    o = eval_link(descs[si], q);
+                    if (!rs_link_visit<true>(descs[si], links.visit_margin[si], r0, r1, r2, p, thr, o)) return false;
                     ++visits[i * 8 + si];
                     return true;
                 };
@@ -154,7 +120,7 @@ extern "C" void simscl_finish(const pvb_sdf_desc *descs, int n_sdf, const float 
             return mk3(lp[0], lp[1], lp[2]);
         };
         const SelfClearanceOut o = self_clearance_finish_one(keys[c], masks, n_sdf, load_xf, load_inv, load_pt,
-                                                             [&](int s, f3 q) { return eval_link(descs[s], q); });
+                                                             [&](int s, f3 q) { return rs_link_eval<true>(descs[s], q); });
         out_val[c] = o.val;
         out_grad[3 * c] = o.grad.x; out_grad[3 * c + 1] = o.grad.y; out_grad[3 * c + 2] = o.grad.z;
         out_src[c] = o.src; out_point[c] = o.point; out_which[c] = o.which;

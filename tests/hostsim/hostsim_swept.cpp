@@ -3,37 +3,16 @@
 // configuration tiles of rs_tile in ascending order, rs_swept_pair for every lane of a tile with the point's best from
 // earlier tiles, the lexicographic winner of the tile (swept_before) and swept_fold, the rotation back at the end.
 // simswept_generic is the per-thread work of composed_swept_kernel.  Test infrastructure only.
-#include "cuda_runtime.h"
-#include "../../pytorch_volumetric_b200/csrc/pvb_device.cuh"
-
-using namespace pvb;
-
-static inline void load_rows(const float *xforms, int n_cfg, int s, int cfg, float4 &r0, float4 &r1, float4 &r2) {
-    const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
-    r0 = row[0]; r1 = row[1]; r2 = row[2];
-}
-
-// robot_swept_kernel's evaluation of a link: primitive, trilinear or nearest-voxel lookup (the same arithmetic as
-// robot_primitive / robot_lookup_trilinear / robot_lookup)
-static inline float4 eval_link(const pvb_sdf_desc &d, f3 q) {
-    NodeStage st; st.smem = nullptr; st.n = 0;
-    SdfOut o;
-    if (d.kind != PVB_KIND_GRID) o = primitive_eval(d, q);
-    else if (d.flags & PVB_GRID_TRILINEAR) o = grid_trilinear_eval(d, q);
-    else o = grid_eval<false, true>(d, st, q, 0u, 0ull, nullptr);
-    return make_float4(o.val, o.grad.x, o.grad.y, o.grad.z);
-}
+// The link visits (lookups included) and sphere bounds are the kernels' own: rs_link_visit, rs_link_eval and
+// rs_point_bounds of pvb_device.cuh.
+#include "hostsim_robot.h"
 
 // first >= 0: every point group visits link `first` first instead of its nearest sphere (any link is a valid first
 // visit); lanes_reversed: the tile's lanes are folded from the last to the first (the winner does not depend on it).
 extern "C" void simswept_fused(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                                int cfg_count, const float *pts, long long n_pts, int first, int lanes_reversed,
                                float *out_val, float *out_grad, int *out_cfg, int *out_which, long long *n_evals) {
-    float sph_rad[8], visit_margin[8];
-    for (int s = 0; s < 8; ++s) {
-        if (s < n_sdf) rs_link_consts(descs[s], sph_rad[s], visit_margin[s]);
-        else { sph_rad[s] = -PVB_INF; visit_margin[s] = 0.f; }
-    }
+    const RsConsts links(descs, n_sdf);
     const int low3_off = ~7;
     const int n_tiles = (cfg_count >> 5) + __builtin_popcount((unsigned)(cfg_count & 31));
     long long evals = 0;
@@ -55,37 +34,20 @@ extern "C" void simswept_fused(const pvb_sdf_desc *descs, int n_sdf, const float
             for (int k = 0; k < LC; ++k) {
                 const int cl = lanes_reversed ? LC - 1 - k : k;
                 const int cfg = cfg_begin + c0 + cl;
+                float4 sph[6];
                 float lb[8], key[8];
-                for (int s = 0; s < 8; ++s) {
-                    f3 cen = mk3(0.f, 0.f, 0.f);
-                    if (s < n_sdf) {
-                        float4 r0, r1, r2;
-                        load_rows(xforms, n_cfg, s, cfg, r0, r1, r2);
-                        cen = rs_sphere_centre(descs[s], r0, r1, r2);
-                    }
-                    lb[s] = rs_sphere_lb(p, cen.x, cen.y, cen.z, sph_rad[s]);
-                    key[s] = rs_bound_key(lb[s], low3_off, s);
-                }
+                rs_centres(descs, n_sdf, xforms, n_cfg, cfg, sph);
+                rs_point_bounds(sph, links.sph_rad, p, low3_off, 0xffu, lb, key);
                 if (pred < 0) {         // the point group's first lane (configuration c0) names the first visit
-                    float key0[8];
-                    for (int s = 0; s < 8; ++s) {
-                        f3 cen = mk3(0.f, 0.f, 0.f);
-                        if (s < n_sdf) {
-                            float4 r0, r1, r2;
-                            load_rows(xforms, n_cfg, s, cfg_begin + c0, r0, r1, r2);
-                            cen = rs_sphere_centre(descs[s], r0, r1, r2);
-                        }
-                        key0[s] = rs_bound_key(rs_sphere_lb(p, cen.x, cen.y, cen.z, sph_rad[s]), low3_off, s);
-                    }
+                    float lb0[8], key0[8];
+                    rs_centres(descs, n_sdf, xforms, n_cfg, cfg_begin + c0, sph);
+                    rs_point_bounds(sph, links.sph_rad, p, low3_off, 0xffu, lb0, key0);
                     pred = first >= 0 ? first : rs_nearest(key0, n_sdf);
                 }
                 auto link = [&](const int si, const float thr, float4 &o) -> bool {
                     float4 r0, r1, r2;
                     load_rows(xforms, n_cfg, si, cfg, r0, r1, r2);
-                    const f3 q = composed_xform(r0, r1, r2, p);
-                    const float tm = thr + visit_margin[si];
-                    if (tm < 0.f || composed_aabb_lb2(descs[si], q) > tm * tm) return false;
-                    o = eval_link(descs[si], q);
+                    if (!rs_link_visit<true>(descs[si], links.visit_margin[si], r0, r1, r2, p, thr, o)) return false;
                     ++ev;
                     return true;
                 };

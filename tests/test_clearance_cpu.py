@@ -39,6 +39,7 @@ def _simlib():
     if _sim is None:
         root = os.path.dirname(os.path.dirname(_SIM_DIR))
         sources = [os.path.join(_SIM_DIR, "hostsim_clearance.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
+                   os.path.join(_SIM_DIR, "hostsim_robot.h"),
                    os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
                    os.path.join(root, "include", "pvb.h")]
         if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
