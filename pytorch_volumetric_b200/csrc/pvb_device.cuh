@@ -868,6 +868,21 @@ __device__ __forceinline__ void rs_tile(int cfg_count, int t, int &c0, int &lc_l
     }
 }
 
+// Launch limits of the robot-family kernels, shared by the host's route choice and the CPU tier.
+// Grid rows: robot_serial_kernel and robot_clearance_kernel run one grid row per rs_tile tile, robot_query_kernel and
+// composed_cfgmajor_kernel one per 32 configurations, and gridDim.y is at most 65535.
+constexpr int kRsMaxGridRows = 65535;
+__host__ __device__ inline int rs_tile_count(int cfg_count) {
+    const int r = cfg_count & 31;
+    return (cfg_count >> 5) + (r & 1) + ((r >> 1) & 1) + ((r >> 2) & 1) + ((r >> 3) & 1) + ((r >> 4) & 1);
+}
+// Points: robot_serial_kernel and robot_query_kernel index the points with int.  A step's end reaches
+// n_pts + kRsIntPtsSpan - 1, the span being the points a block flushes at once in robot_serial_kernel's
+// multi-destination form (8 warps x 32 point groups x 8 points; robot_query_kernel's 32-point tile is less), so a batch
+// takes them only while that end stays below 2^31.
+constexpr long long kRsIntPtsSpan = 2048;
+__host__ __device__ inline bool rs_int_pts_ok(long long n_pts) { return n_pts <= 0x7fffffffll - (kRsIntPtsSpan - 1); }
+
 // A staging tile holds LC = 32 >> sub_log2 configuration rows of row_pts = (1 << (w_log2 + chunk_log2 + sub_log2)) points:
 // row_pts values and 3 row_pts gradient floats per row.  It leaves as LC * row_pts pieces of 16 bytes -- the first
 // LC * row_pts / 4 are values, the rest gradients -- numbered so that consecutive pieces are consecutive in a row.

@@ -3165,6 +3165,31 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
                                         n_pts, out_val, out_grad, any_ext);
     if (bad) return bad;
     if (n_pts == 0 || cfg_count == 0) return PVB_OK;
+    // The robot and configuration-major kernels run one grid row per configuration tile (rs_tile_count).  A slab of
+    // more tiles than a grid has rows runs as consecutive slabs, each of whole 32-configuration tiles but the last and
+    // balanced so that each takes the route the whole would (none of them a small remainder).  A configuration's row
+    // depends on nothing else of the slab, so the rows are bit for bit those of one call.
+    if (rs_tile_count(cfg_count) > kRsMaxGridRows) {
+        // at most kSlab configurations per slab: 65531 tiles of 32 and up to 4 remainder tiles fit in a grid
+        constexpr int kSlab = (kRsMaxGridRows - 4) * kRbCfg;
+        const int n_slab = (cfg_count - 1) / kSlab + 1;
+        const int step = ((cfg_count - 1) / n_slab / kRbCfg + 1) * kRbCfg;      // <= kSlab, whole tiles
+        for (long long b = 0; b < cfg_count; b += step) {
+            const int cnt = (int)(cfg_count - b < step ? cfg_count - b : step);
+            const size_t o = (size_t)b * (size_t)n_pts;
+            OutTargets sub{};
+            if (tg) {
+                sub = *tg;
+                for (int t = 0; t < sub.n; ++t) { sub.val[t] += o; sub.grad[t] += 3 * o; }
+            }
+            const int rc = composed_dispatch(descs, n_sdf, needs_mesh, xforms, n_cfg, cfg_begin + (int)b, cnt, pts, n_pts,
+                                             mesh_mode, out_val ? out_val + o : nullptr,
+                                             out_grad ? out_grad + 3 * o : nullptr, out_which ? out_which + o : nullptr,
+                                             tg ? &sub : nullptr, stream);
+            if (rc) return rc;
+        }
+        return PVB_OK;
+    }
     cudaStream_t s = (cudaStream_t)stream;
     auto aligned16 = [](const void *p) { return p == nullptr || ((uintptr_t)p % 16) == 0; };
     // 4-points-per-thread vector path needs 16-byte aligned rows: every configuration slab starts at c * n_pts
@@ -3180,12 +3205,12 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
     static const int robot_kernel = [] { const char *e = getenv("PVB_ROBOT_KERNEL"); return e ? atoi(e) : 2; }();
     // every sub-SDF a GRID with the bounding-box rule (nearest or trilinear) or a primitive: the robot kernels'
     // precondition (primitives and trilinear grids then need the serial kernel, see serial_taken)
-    const bool all_grid = !needs_mesh && n_sdf <= 16 && n_pts < (1ll << 31) && rs_links_ok(descs, n_sdf);
+    const bool all_grid = !needs_mesh && n_sdf <= 16 && rs_int_pts_ok(n_pts) && rs_links_ok(descs, n_sdf);
     // the point-serial kernel has no fill problem (remainder configurations run in lane-split tiles): any batch of
     // PVB_ROBOT_MIN_CFG or more configurations takes it
     static const int serial_min_cfg = [] { const char *e = getenv("PVB_ROBOT_MIN_CFG"); return e ? atoi(e) : 8; }();
     const bool serial_ok = robot_kernel >= 2 && n_sdf <= kRsMaxS && cfg_count >= serial_min_cfg &&
-                           cfg_count <= 65535 * kRbCfg;          // one grid row per 32-configuration tile
+                           rs_tile_count(cfg_count) <= kRsMaxGridRows;          // one grid row per tile
     // sets with trilinear or primitive links take the serial kernel where nearest sets would; robot_query_kernel (9-16
     // links) is nearest-voxel only, so otherwise they fall through to the configuration-major or point-major kernel
     const bool serial_taken = robot_kernel && cfg_major && all_grid && serial_ok;
@@ -3400,6 +3425,11 @@ extern "C" int pvb_composed_query_swept(const pvb_sdf_desc *descs, int32_t n_sdf
     return rc;
 }
 
+// The longest chunk of the clearance kernels: their point loops step j0 = 0, 32, 64, ... (robot_clearance_kernel: up to
+// 256) past the chunk's end in int, so a chunk as long as a segment of nearly 2^31 points would wrap.  The chunking
+// never changes a result (the keys name the first point attaining the minimum).
+constexpr long long kRsMaxChunk = 1ll << 30;
+
 // Launch robot_clearance_kernel.  Chunk size from the sizes alone: the longest chunk (at least 64 points, or the whole
 // segment) that still gives >= 4 waves of resident blocks over the tiles x segments x chunks, so that blocks of later
 // waves start from the keys of earlier ones.
@@ -3407,10 +3437,11 @@ static int launch_robot_clearance(const pvb_sdf_desc *descs, int n_sdf, const fl
                                   int cfg_count, const float *pts, long long n_seg, long long seg_len,
                                   unsigned long long *keys, bool ext, cudaStream_t stream) {
     const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
-    const int gy = (cfg_count >> 5) + __builtin_popcount((unsigned)(cfg_count & 31));
+    const int gy = rs_tile_count(cfg_count);
     const long long want = 4ll * sm_count() * PVB_RS_MINB;          // blocks for 4 waves
     long long per_seg = (want + (long long)gy * n_seg - 1) / ((long long)gy * n_seg);
     if (per_seg > (seg_len + 63) / 64) per_seg = (seg_len + 63) / 64;
+    if (per_seg < (seg_len + kRsMaxChunk - 1) / kRsMaxChunk) per_seg = (seg_len + kRsMaxChunk - 1) / kRsMaxChunk;
     if (per_seg < 1) per_seg = 1;
     const long long chunk = (seg_len + per_seg - 1) / per_seg;
     const long long chunks_per_seg = (seg_len + chunk - 1) / chunk;
@@ -3500,8 +3531,7 @@ extern "C" int pvb_composed_query_clearance(const pvb_sdf_desc *descs, int32_t n
     }
     // robot_serial_kernel's sets take the fused kernel: <= 8 GRID links with the bounding-box rule or primitives, and
     // one grid row per configuration tile
-    const bool fused = !needs_mesh && n_sdf <= kRsMaxS &&
-                       (cfg_count >> 5) + __builtin_popcount((unsigned)(cfg_count & 31)) <= 65535 &&
+    const bool fused = !needs_mesh && n_sdf <= kRsMaxS && rs_tile_count(cfg_count) <= kRsMaxGridRows &&
                        rs_links_ok(descs, n_sdf);
     if (fused) {
         const int rc = launch_robot_clearance(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
@@ -3532,6 +3562,7 @@ static int launch_robot_paired_clearance(const pvb_sdf_desc *descs, int n_sdf, c
     const long long want = 4ll * sm_count() * PVB_RS_MINB * kRsWarps;    // warp units for 4 waves
     long long per_seg = (want + pairs - 1) / pairs;
     if (per_seg > (seg_len + 63) / 64) per_seg = (seg_len + 63) / 64;
+    if (per_seg < (seg_len + kRsMaxChunk - 1) / kRsMaxChunk) per_seg = (seg_len + kRsMaxChunk - 1) / kRsMaxChunk;
     if (per_seg < 1) per_seg = 1;
     long long chunk = (seg_len + per_seg - 1) / per_seg;
     chunk = (chunk + 31) / 32 * 32;                                      // whole steps of the warp

@@ -116,6 +116,8 @@ extern "C" float sim_hash_normal(uint32_t seed, unsigned long long idx, uint32_t
 
 // index arithmetic of robot_serial_kernel
 extern "C" void sim_rs_tile(int cfg_count, int t, int *c0, int *lc_log2) { rs_tile(cfg_count, t, *c0, *lc_log2); }
+extern "C" int sim_rs_tile_count(int cfg_count) { return rs_tile_count(cfg_count); }
+extern "C" int sim_rs_int_pts_ok(long long n_pts) { return rs_int_pts_ok(n_pts) ? 1 : 0; }
 extern "C" void sim_rs_flush_piece(int c, int chunk_log2, int sub_log2, int w_log2, int *is_val, int *row, int *part) {
     bool v;
     rs_flush_piece(c, chunk_log2, sub_log2, w_log2, v, *row, *part);

@@ -425,6 +425,71 @@ def test_robot_serial_tiles_and_flush_pieces_cover_everything_once(built_lib):
                 assert (val == 1).all() and (grad == 1).all(), (w_log2, chunk_log2, sub_log2)
 
 
+INT_MAX = 2 ** 31 - 1
+
+
+def _robot_int_extreme(n_pts):
+    """The largest int intermediate robot_serial_kernel (pvb_kernels.cu) and robot_query_kernel form from n_pts, over
+    every tile shape (LC = 32..1 lanes per point), step size (4 / 8 points) and flush mode (per warp / per block of 8
+    warps): the step count's rounding n_pts + pts_per_step - 1, the tile ends tile_base + row_pts and pt_base +
+    pts_per_step of every warp the super-step loop runs (inactive ones included), the last point index, and
+    robot_query_kernel's 32-point tiles."""
+    worst = n_pts + 31                                                       # (n_pts + kRbTilePts - 1) / kRbTilePts
+    worst = max(worst, -(-n_pts // 32) * 32)                                 # tile * 32 + 32 of its last tile
+    for chunk_log2 in (2, 3):
+        for sub_log2 in range(6):
+            pps = (1 << chunk_log2) << sub_log2                              # points a warp finishes per step
+            n_chunks = -(-n_pts // pps)
+            n_super = -(-n_chunks // 8)
+            last_chunk = 8 * n_super - 1                                     # sup * 8 + warp, every warp
+            for coop in (False, True):
+                tile_end = (n_super * 8 * pps) if coop else (last_chunk + 1) * pps
+                worst = max(worst, n_pts + pps - 1, tile_end, last_chunk * pps + pps - 1, n_chunks + 7)
+    return worst
+
+
+def test_robot_int_point_guard_is_exact(built_lib):
+    """rs_int_pts_ok (pvb_device.cuh), the guard that sends a batch to the int-indexed robot kernels: every point count
+    it accepts keeps every int intermediate of robot_serial_kernel and robot_query_kernel at or below INT_MAX, and the
+    first count it refuses is the first that would wrap -- the guard is exact, not merely safe."""
+    import ctypes
+    L = hs.lib()
+    ok = lambda n: bool(L.sim_rs_int_pts_ok(ctypes.c_longlong(n)))
+    limit = 2 ** 31 - 2048
+    assert ok(limit) and not ok(limit + 1)
+    assert _robot_int_extreme(limit) <= INT_MAX < _robot_int_extreme(limit + 1)
+    for n in list(range(limit - 4200, limit + 4200)) + [0, 1, 255, 256, 2047, 2048, 2 ** 31 - 1, 2 ** 31, 2 ** 40]:
+        assert ok(n) == (n <= limit), n
+        if ok(n):
+            assert _robot_int_extreme(n) <= INT_MAX, n
+
+
+def test_robot_tile_count_at_the_grid_row_limit(built_lib):
+    """rs_tile_count (pvb_device.cuh), the grid rows robot_serial_kernel and robot_clearance_kernel launch: the tiles
+    rs_tile enumerates, on both sides of 65535 rows (2 097 120 = 65535 x 32 configurations, and the counts just below it
+    whose remainder splits into more than one tile)."""
+    import ctypes
+    L = hs.lib()
+    counts = list(range(65530 * 32, 65537 * 32)) + [1, 31, 32, 33, 2 ** 31 - 1]
+    for c in counts:
+        n = L.sim_rs_tile_count(c)
+        assert n == (c >> 5) + bin(c & 31).count("1"), c
+        if c in (1, 31, 32, 33, 65535 * 32 - 1, 65535 * 32 + 33):
+            seen, last = 0, -1
+            for t in range(n):
+                c0, lc = ctypes.c_int(), ctypes.c_int()
+                L.sim_rs_tile(c, t, ctypes.byref(c0), ctypes.byref(lc))
+                assert c0.value == last + 1 or (t == 0 and c0.value == 0), (c, t)
+                last = c0.value + (1 << lc.value) - 1
+                seen += 1 << lc.value
+            assert seen == c and last == c - 1, c
+    assert L.sim_rs_tile_count(65535 * 32) == 65535
+    assert L.sim_rs_tile_count(65535 * 32 + 1) == 65536
+    # the largest counts below 65535 x 32 that still need more than 65535 rows: remainders of 2+ binary digits
+    assert [c for c in range(65534 * 32, 65535 * 32) if L.sim_rs_tile_count(c) > 65535] == \
+        [c for c in range(65534 * 32, 65535 * 32) if bin(c & 31).count("1") >= 2]
+
+
 def test_robot_serial_nearest_sphere_key(built_lib):
     """rs_bound_key / rs_nearest (pvb_device.cuh): the link index rides in the 3 low mantissa bits of each sphere bound
     and the smallest key names the first link to visit.  Always a real link (0 <= pred < n_sdf), whatever mix of finite,
