@@ -14,10 +14,11 @@ sweeps when the caller wants the full result on every rank.
                         epilogue (NVLink traffic under the lookups) instead of a trailing all-gather
 """
 import ctypes
-import math
 
 import torch
 import torch.distributed as dist
+
+from .sdf import _config_count
 
 
 def shard_range(n, rank, world):
@@ -361,7 +362,7 @@ def sharded_robot_query(robot_sdf, points, gather=True, group=None, result=None,
     (cfg_count, prod(B)) and the re-assembled result ([A,] *B) / (..., 3); gather must be True or False."""
     rank, world = _world(group)
     comp = robot_sdf.sdf
-    n_cfg = 1 if comp.tsf_batch is None else math.prod(list(comp.tsf_batch))
+    n_cfg = _config_count(comp.tsf_batch)
     begin, end = shard_range(n_cfg, rank, world)
     batch = tuple(comp.tsf_batch) if comp.tsf_batch is not None else ()
     if paired and clearance:
@@ -380,10 +381,7 @@ def sharded_robot_query(robot_sdf, points, gather=True, group=None, result=None,
         if isinstance(gather, str):
             raise ValueError("paired queries re-assemble with gather=True or gather=False only")
         pts_shape = tuple(points.shape)
-        if len(pts_shape) < len(batch) + 1 or pts_shape[:len(batch)] != tuple(int(a) for a in batch) \
-                or pts_shape[-1] != 3:
-            raise ValueError(f"paired query: points {pts_shape} must be [*A, ..., 3] with the configuration batch "
-                             f"A = {batch} leading")
+        comp._check_leading_batch(pts_shape, "paired query", "..., 3", 1)
         per_cfg = points.reshape(n_cfg, -1, 3)
         P = per_cfg.shape[1]
         val, grad = comp.query_paired(per_cfg[begin:end], cfg_begin=begin, cfg_count=end - begin)

@@ -498,6 +498,34 @@ def _result_like(points, lead, tensors_tails, out_device=None):
     return tuple(nat.deliver(t, dev, dtype).reshape(*lead, *tail) for t, tail in tensors_tails)
 
 
+def _config_count(tsf_batch):
+    """The number of configurations a composition's transforms hold: prod(tsf_batch), 1 without a batch (None)."""
+    return 1 if tsf_batch is None else math.prod(list(tsf_batch))
+
+
+class _query_points:
+    """`with _query_points(points) as (device, p)`: enter the device a query of `points` runs on -- theirs when they
+    are a CUDA tensor, else the current device -- with p the points as contiguous fp32 (M, 3) on it.  (A class rather
+    than a contextlib generator: it is entered on every query call.)"""
+    __slots__ = ("points", "guard")
+
+    def __init__(self, points):
+        self.points = points
+
+    def __enter__(self):
+        device = nat.compute_device(self.points.device if torch.is_tensor(self.points) else None)
+        self.guard = torch.cuda.device(device)
+        self.guard.__enter__()
+        try:
+            return device, nat.as_f32_points(self.points, device)
+        except BaseException:
+            self.guard.__exit__(None, None, None)
+            raise
+
+    def __exit__(self, *exc):
+        return self.guard.__exit__(*exc)
+
+
 class SphereSDF(ObjectFrameSDF):
     """SDF for a geometric primitive, the sphere centered at the origin"""
 
@@ -506,9 +534,7 @@ class SphereSDF(ObjectFrameSDF):
 
     def __call__(self, points_in_object_frame):
         lead = tuple(points_in_object_frame.shape[:-1])
-        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(points_in_object_frame, device)
+        with _query_points(points_in_object_frame) as (device, p):
             n = p.shape[0]
             val = torch.empty(n, dtype=torch.float32, device=device)
             grad = torch.empty(n, 3, dtype=torch.float32, device=device)
@@ -718,10 +744,43 @@ class ComposedSDF(ObjectFrameSDF):
                 raise ValueError(f"{S_tsf} transforms cannot be split over {S} SDFs")
 
     def ith_transform_slice(self, i):
-        if self.tsf_batch is None:
-            return slice(i, i + 1)
-        total_to_slice = math.prod(list(self.tsf_batch))
-        return slice(i * total_to_slice, (i + 1) * total_to_slice)
+        n_cfg = _config_count(self.tsf_batch)
+        return slice(i * n_cfg, (i + 1) * n_cfg)
+
+    def _slab(self, cfg_begin, cfg_count):
+        """(n_cfg, cfg_count) of the configuration slab [cfg_begin, cfg_begin + cfg_count) of the n_cfg installed
+        configurations; cfg_count None runs to the last one."""
+        n_cfg = _config_count(self.tsf_batch)
+        return n_cfg, n_cfg - cfg_begin if cfg_count is None else cfg_count
+
+    def _check_leading_batch(self, pts_shape, form, tail, n_tail, separate_mismatch=False):
+        """The shape rule of a paired form: points of shape pts_shape are [*A, <tail>], the configuration batch A
+        leading, then at least n_tail dimensions, the last of size 3.  Otherwise ValueError "<form>: points ... must
+        be [*A, <tail>] with the configuration batch A = ... leading"; with separate_mismatch, points with enough
+        dimensions but other leading ones get "<form>: points ... must have the configuration batch A = ... leading"
+        instead."""
+        batch = tuple(int(a) for a in self.tsf_batch or ())
+        fits = len(pts_shape) >= len(batch) + n_tail and pts_shape[-1:] == (3,)
+        leads = pts_shape[:len(batch)] == batch
+        if separate_mismatch and fits and not leads:
+            raise ValueError(f"{form}: points {pts_shape} must have the configuration batch A = {batch} leading")
+        if not (fits and leads):
+            raise ValueError(f"{form}: points {pts_shape} must be [*A, {tail}] with the configuration batch "
+                             f"A = {batch} leading")
+
+    @staticmethod
+    def _deliver(points, outs, shape, device=None):
+        """Flat query results as a public form returns them: values and gradients in the points' dtype (fp32 for
+        non-tensors), index outputs as int64, on `device` -- by default the points' device, CPU for non-tensors --
+        and each reshaped to `shape` followed by its own trailing dimensions."""
+        dtype = points.dtype if torch.is_tensor(points) else torch.float
+        if device is None:
+            device = points.device if torch.is_tensor(points) else "cpu"
+        res = []
+        for t in outs:      # a plain loop and argument-list reshapes: this runs on every call of every public form
+            d = nat.deliver(t, device, dtype if t.is_floating_point() else torch.int64)
+            res.append(d.reshape(shape) if t.dim() == 1 else d.reshape(*shape, *t.shape[1:]))
+        return tuple(res)
 
     # -- fused path ---------------------------------------------------------------
     #: most sub-SDFs one fused-kernel launch takes (pvb_composed_query* refuse more)
@@ -741,6 +800,14 @@ class ComposedSDF(ObjectFrameSDF):
                 hit = (nat.desc_array(descs), needs_mesh, descs)
             self._desc_cache = {key: hit}
         return hit[0], hit[1]
+
+    def _fused_descs(self, device, form):
+        """`_native_descs` of a form only the fused kernels run; NotImplementedError when the set is generic."""
+        descs_arr, needs_mesh = self._native_descs(device)
+        if descs_arr is None:
+            raise NotImplementedError(f"{form} needs the fused kernels: at most 128 sub-SDFs, all with native "
+                                      "descriptors")
+        return descs_arr, needs_mesh
 
     def _xforms_on(self, device):
         xf = self._xf_dev.get(device)
@@ -762,12 +829,8 @@ class ComposedSDF(ObjectFrameSDF):
         """__call__ restricted to the configuration slab [cfg_begin, cfg_begin + cfg_count) (multi-GPU sharding
         over configurations).  Returns flat (cfg_count * P,) / (cfg_count * P, 3) fp32 tensors on the GPU."""
         S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
-        if cfg_count is None:
-            cfg_count = n_cfg - cfg_begin
-        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(points_in_object_frame, device)
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
+        with _query_points(points_in_object_frame) as (device, p):
             P = p.shape[0]
             descs_arr, needs_mesh = self._native_descs(device)
             if descs_arr is None:
@@ -788,17 +851,13 @@ class ComposedSDF(ObjectFrameSDF):
         Bit-identical to query(points[c], cfg_begin=cfg_begin + c, cfg_count=1) for every c, mesh ray jitter
         included.  Returns flat (cfg_count * P,) / (cfg_count * P, 3) fp32 tensors on the GPU."""
         S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
-        if cfg_count is None:
-            cfg_count = n_cfg - cfg_begin
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
         shape = tuple(points_in_object_frame.shape)
         n = math.prod(shape[:-1])
         if shape[-1:] != (3,) or (n % cfg_count if cfg_count else n):
             raise ValueError(f"paired query: points {shape} do not split into {cfg_count} blocks of [P, 3]")
         P = n // cfg_count if cfg_count else 0
-        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(points_in_object_frame, device)
+        with _query_points(points_in_object_frame) as (device, p):
             descs_arr, needs_mesh = self._native_descs(device)
             if descs_arr is None:
                 return self._generic_query(p, cfg_begin, cfg_count, n_cfg, return_which, paired=True)
@@ -824,17 +883,9 @@ class ComposedSDF(ObjectFrameSDF):
         leading dimensions of the points are not A."""
         if self.tsf_batch is None:
             return self(points_in_object_frame)
-        batch = tuple(int(a) for a in self.tsf_batch)
         pts_shape = tuple(points_in_object_frame.shape)
-        if len(pts_shape) < len(batch) + 1 or pts_shape[:len(batch)] != batch or pts_shape[-1] != 3:
-            raise ValueError(f"paired query: points {pts_shape} must be [*A, ..., 3] with the configuration batch "
-                             f"A = {batch} leading")
-        vv, gg = self.query_paired(points_in_object_frame)
-        dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
-        out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
-        vv = nat.deliver(vv, out_device, dtype)
-        gg = nat.deliver(gg, out_device, dtype)
-        return vv.reshape(pts_shape[:-1]), gg.reshape(*pts_shape[:-1], 3)
+        self._check_leading_batch(pts_shape, "paired query", "..., 3", 1)
+        return self._deliver(points_in_object_frame, self.query_paired(points_in_object_frame), pts_shape[:-1])
 
     #: configurations per `_generic_query` chunk of the unfused swept fold (bounds its cfg_chunk x P temporaries)
     swept_generic_chunk = 64
@@ -846,17 +897,13 @@ class ComposedSDF(ObjectFrameSDF):
         configuration, sub-SDF index) minimised lexicographically.  Returns flat (P,) / (P, 3) fp32 tensors on the GPU,
         and with return_which also the int32 absolute configuration index and sub-SDF index."""
         S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
-        if cfg_count is None:
-            cfg_count = n_cfg - cfg_begin
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
         shape = tuple(points_in_object_frame.shape)
         if shape[-1:] != (3,):
             raise ValueError(f"swept query: points {shape} must be [..., 3]")
         if cfg_count < 1 and math.prod(shape[:-1]) > 0:
             raise ValueError(f"swept query: no minimum over an empty configuration slab (cfg_count={cfg_count})")
-        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(points_in_object_frame, device)
+        with _query_points(points_in_object_frame) as (device, p):
             P = p.shape[0]
             descs_arr, needs_mesh = self._native_descs(device)
             if descs_arr is None:
@@ -907,15 +954,7 @@ class ComposedSDF(ObjectFrameSDF):
         if len(pts_shape) < 1 or pts_shape[-1] != 3:
             raise ValueError(f"swept query: points {pts_shape} must be [..., 3]")
         out = self.query_swept(points_in_object_frame, return_which=return_argmin)
-        dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
-        out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
-        vv = nat.deliver(out[0], out_device, dtype).reshape(pts_shape[:-1])
-        gg = nat.deliver(out[1], out_device, dtype).reshape(*pts_shape[:-1], 3)
-        if not return_argmin:
-            return vv, gg
-        cfg = nat.deliver(out[2], out_device, torch.int64).reshape(pts_shape[:-1])
-        which = nat.deliver(out[3], out_device, torch.int64).reshape(pts_shape[:-1])
-        return vv, gg, cfg, which
+        return self._deliver(points_in_object_frame, out, pts_shape[:-1])
 
     #: configurations per `_generic_query` chunk of the unfused clearance query (bounds its cfg_chunk x P temporaries)
     clearance_generic_chunk = 64
@@ -934,21 +973,23 @@ class ComposedSDF(ObjectFrameSDF):
         query(..., return_which=True) over the flat points: (value, point) minimised lexicographically, -0 == +0, a NaN
         value above every number.  Returns flat (cfg_count * n_seg,) / (cfg_count * n_seg, 3) fp32 tensors on the GPU,
         configuration-major, and with return_which also the int32 point index within the segment and sub-SDF index."""
-        S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
-        if cfg_count is None:
-            cfg_count = n_cfg - cfg_begin
+        _, cfg_count = self._slab(cfg_begin, cfg_count)
         n_seg, seg_len = self._clearance_segments(tuple(points_in_object_frame.shape))
         if n_seg > 0 and seg_len == 0 and cfg_count > 0:
             raise ValueError("clearance query: no minimum over an empty segment (N = 0)")
         if cfg_count < 1 and n_seg * seg_len > 0:
             raise ValueError(f"clearance query: no minimum over an empty configuration slab (cfg_count={cfg_count})")
-        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(points_in_object_frame, device)
+        return self._clearance_query(points_in_object_frame, cfg_begin, cfg_count, n_seg, seg_len, return_which)
+
+    def _clearance_query(self, points, cfg_begin, cfg_count, n_seg, seg_len, return_which, paired=False):
+        """query_clearance (paired=False) or query_paired_clearance (paired=True) once their checks have passed: the
+        form's fused entry point, or `_generic_clearance` for the sets the fused kernels do not take."""
+        S, n_cfg = len(self.sdfs), _config_count(self.tsf_batch)
+        with _query_points(points) as (device, p):
             descs_arr, needs_mesh = self._native_descs(device)
             if descs_arr is None:
-                return self._generic_clearance(p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which)
+                return self._generic_clearance(p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which,
+                                               paired=paired)
             xf = self._xforms_on(device)
             R = max(cfg_count, 0) * n_seg
             keys = torch.empty(R, dtype=torch.int64, device=device)
@@ -956,11 +997,11 @@ class ComposedSDF(ObjectFrameSDF):
             grad = torch.empty(R, 3, dtype=torch.float32, device=device)
             point = torch.empty(R, dtype=torch.int32, device=device) if return_which else None
             which = torch.empty(R, dtype=torch.int32, device=device) if return_which else None
-            nat.check(nat.lib().pvb_composed_query_clearance(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg,
-                                                             cfg_begin, cfg_count, nat.ptr(p), n_seg, seg_len,
-                                                             nat.PVB_MESH_DEFAULT, nat.ptr(keys), nat.ptr(val),
-                                                             nat.ptr(grad), nat.ptr(point), nat.ptr(which),
-                                                             nat.stream_ptr(device)), "pvb_composed_query_clearance")
+            lib = nat.lib()
+            entry = lib.pvb_composed_query_paired_clearance if paired else lib.pvb_composed_query_clearance
+            nat.check(entry(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg, cfg_begin, cfg_count, nat.ptr(p),
+                            n_seg, seg_len, nat.PVB_MESH_DEFAULT, nat.ptr(keys), nat.ptr(val), nat.ptr(grad),
+                            nat.ptr(point), nat.ptr(which), nat.stream_ptr(device)), entry.__name__)
         return (val, grad, point, which) if return_which else (val, grad)
 
     @staticmethod
@@ -1015,16 +1056,7 @@ class ComposedSDF(ObjectFrameSDF):
         if n_seg > 0 and seg_len == 0:
             raise ValueError("clearance query: no minimum over an empty segment (N = 0)")
         out = self.query_clearance(points_in_object_frame, return_which=return_argmin)
-        shape = (*(self.tsf_batch or ()), *pts_shape[:-2])
-        dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
-        out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
-        vv = nat.deliver(out[0], out_device, dtype).reshape(shape)
-        gg = nat.deliver(out[1], out_device, dtype).reshape(*shape, 3)
-        if not return_argmin:
-            return vv, gg
-        point = nat.deliver(out[2], out_device, torch.int64).reshape(shape)
-        which = nat.deliver(out[3], out_device, torch.int64).reshape(shape)
-        return vv, gg, point, which
+        return self._deliver(points_in_object_frame, out, (*(self.tsf_batch or ()), *pts_shape[:-2]))
 
     def query_paired_clearance(self, points_in_object_frame, cfg_begin=0, cfg_count=None, return_which=False):
         """Paired form of `query_clearance`: configuration cfg_begin + c against its own points only.  The points
@@ -1034,10 +1066,7 @@ class ComposedSDF(ObjectFrameSDF):
         return_which=True) over each segment.  Returns flat (cfg_count * n_seg,) / (cfg_count * n_seg, 3) fp32
         tensors on the GPU, configuration-major, and with return_which also the int32 point index within the segment
         and sub-SDF index."""
-        S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
-        if cfg_count is None:
-            cfg_count = n_cfg - cfg_begin
+        _, cfg_count = self._slab(cfg_begin, cfg_count)
         shape = tuple(points_in_object_frame.shape)
         lead, seg_len = self._clearance_segments(shape)
         if (lead % cfg_count) if cfg_count > 0 else lead:
@@ -1046,32 +1075,8 @@ class ComposedSDF(ObjectFrameSDF):
         n_seg = lead // cfg_count if cfg_count > 0 else 0
         if n_seg > 0 and seg_len == 0:
             raise ValueError("paired clearance query: no minimum over an empty segment (N = 0)")
-        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(points_in_object_frame, device)
-            descs_arr, needs_mesh = self._native_descs(device)
-            if descs_arr is None:
-                return self._generic_paired_clearance(p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which)
-            xf = self._xforms_on(device)
-            R = max(cfg_count, 0) * n_seg
-            keys = torch.empty(R, dtype=torch.int64, device=device)
-            val = torch.empty(R, dtype=torch.float32, device=device)
-            grad = torch.empty(R, 3, dtype=torch.float32, device=device)
-            point = torch.empty(R, dtype=torch.int32, device=device) if return_which else None
-            which = torch.empty(R, dtype=torch.int32, device=device) if return_which else None
-            nat.check(nat.lib().pvb_composed_query_paired_clearance(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg,
-                                                                    cfg_begin, cfg_count, nat.ptr(p), n_seg, seg_len,
-                                                                    nat.PVB_MESH_DEFAULT, nat.ptr(keys), nat.ptr(val),
-                                                                    nat.ptr(grad), nat.ptr(point), nat.ptr(which),
-                                                                    nat.stream_ptr(device)),
-                      "pvb_composed_query_paired_clearance")
-        return (val, grad, point, which) if return_which else (val, grad)
-
-    def _generic_paired_clearance(self, p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which):
-        """query_paired_clearance for sub-SDFs without native descriptors (or more than `max_fused_sdfs`):
-        configuration chunks through `_generic_query(..., paired=True)`, reduced by `_clearance_keys` -- the order of
-        the fused route."""
-        return self._generic_clearance(p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which, paired=True)
+        return self._clearance_query(points_in_object_frame, cfg_begin, cfg_count, n_seg, seg_len, return_which,
+                                     paired=True)
 
     def paired_clearance(self, points_in_object_frame, return_argmin=False):
         """Every installed configuration against its own cloud: points [*A, *B, N, 3], A the configuration batch, give
@@ -1084,27 +1089,12 @@ class ComposedSDF(ObjectFrameSDF):
         are not A, when they are not [..., N, 3], or when N = 0 with segments to reduce."""
         if self.tsf_batch is None:
             return self.clearance(points_in_object_frame, return_argmin=return_argmin)
-        batch = tuple(int(a) for a in self.tsf_batch)
         pts_shape = tuple(points_in_object_frame.shape)
-        if len(pts_shape) < len(batch) + 2 or pts_shape[-1] != 3:
-            raise ValueError(f"paired clearance query: points {pts_shape} must be [*A, ..., N, 3] with the "
-                             f"configuration batch A = {batch} leading")
-        if pts_shape[:len(batch)] != batch:
-            raise ValueError(f"paired clearance query: points {pts_shape} must have the configuration batch "
-                             f"A = {batch} leading")
+        self._check_leading_batch(pts_shape, "paired clearance query", "..., N, 3", 2, separate_mismatch=True)
         if math.prod(pts_shape[:-2]) > 0 and pts_shape[-2] == 0:
             raise ValueError("paired clearance query: no minimum over an empty segment (N = 0)")
         out = self.query_paired_clearance(points_in_object_frame, return_which=return_argmin)
-        shape = pts_shape[:-2]
-        dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
-        out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
-        vv = nat.deliver(out[0], out_device, dtype).reshape(shape)
-        gg = nat.deliver(out[1], out_device, dtype).reshape(*shape, 3)
-        if not return_argmin:
-            return vv, gg
-        point = nat.deliver(out[2], out_device, torch.int64).reshape(shape)
-        which = nat.deliver(out[3], out_device, torch.int64).reshape(shape)
-        return vv, gg, point, which
+        return self._deliver(points_in_object_frame, out, pts_shape[:-2])
 
     def _self_clearance_args(self, link_points, allowed):
         """(K, allowed rows as S lists of bools with the diagonal cleared) of a self-clearance query; ValueError when
@@ -1148,16 +1138,12 @@ class ComposedSDF(ObjectFrameSDF):
         tensors on the GPU, and with return_which also int32 source sub-SDF i, point k and sub-SDF j.  Raises
         ValueError before any device work on wrong shapes or an empty slab."""
         S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
-        if cfg_count is None:
-            cfg_count = n_cfg - cfg_begin
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
         K, rows = self._self_clearance_args(link_points, allowed)
         if cfg_count < 1 or cfg_begin < 0 or cfg_begin + cfg_count > n_cfg:
             raise ValueError(f"self-clearance query: empty or invalid configuration slab [{cfg_begin}, +{cfg_count}) "
                              f"of {n_cfg}")
-        device = nat.compute_device(link_points.device if torch.is_tensor(link_points) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(link_points, device)
+        with _query_points(link_points) as (device, p):
             if not self._self_clearance_fused(device):
                 return self._composed_self_clearance(p, K, rows, cfg_begin, cfg_count, return_which)
             descs_arr, _ = self._native_descs(device)
@@ -1181,8 +1167,7 @@ class ComposedSDF(ObjectFrameSDF):
         row, link_points[i] posed by W_i of the slab (pvb_transform_points_paired), then
         query_paired_clearance(..., return_which=True) of ComposedSDF([sdfs[j] for allowed j], their transform rows),
         its sub-SDF index mapped back; then the minimum over i by (value, i)."""
-        S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
+        S, n_cfg = len(self.sdfs), _config_count(self.tsf_batch)
         device = p.device
         xf = self._xforms_on(device).reshape(S, n_cfg, 4, 4)
         inv = self._inv_xforms_on(device).reshape(S, n_cfg, 4, 4)
@@ -1230,13 +1215,7 @@ class ComposedSDF(ObjectFrameSDF):
         operator (an extension); raises ValueError before any device work on wrong shapes."""
         shape = () if self.tsf_batch is None else tuple(int(a) for a in self.tsf_batch)
         out = self.query_self_clearance(link_points, allowed, return_which=return_argmin)
-        dtype = link_points.dtype if torch.is_tensor(link_points) else torch.float
-        out_device = matrix_of(self.obj_frame_to_link_frame).device
-        vv = nat.deliver(out[0], out_device, dtype).reshape(shape)
-        gg = nat.deliver(out[1], out_device, dtype).reshape(*shape, 3)
-        if not return_argmin:
-            return vv, gg
-        return (vv, gg) + tuple(nat.deliver(t, out_device, torch.int64).reshape(shape) for t in out[2:])
+        return self._deliver(link_points, out, shape, device=matrix_of(self.obj_frame_to_link_frame).device)
 
     @staticmethod
     def _collision_cost_margin(margin):
@@ -1266,9 +1245,7 @@ class ComposedSDF(ObjectFrameSDF):
         ValueError before any device work on malformed points, a margin that is not finite, or a slab without
         configurations when there are points."""
         S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
-        if cfg_count is None:
-            cfg_count = n_cfg - cfg_begin
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
         m = self._collision_cost_margin(margin)
         shape = tuple(points_in_object_frame.shape)
         if len(shape) < 2 or shape[-1] != 3:
@@ -1276,9 +1253,7 @@ class ComposedSDF(ObjectFrameSDF):
         n_seg, seg_len = math.prod(shape[:-2]), shape[-2]
         if cfg_begin < 0 or cfg_count < 0 or cfg_begin + cfg_count > n_cfg or (cfg_count < 1 and n_seg * seg_len > 0):
             raise ValueError(f"collision-cost query: invalid configuration slab [{cfg_begin}, +{cfg_count}) of {n_cfg}")
-        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(points_in_object_frame, device)
+        with _query_points(points_in_object_frame) as (device, p):
             R = cfg_count * n_seg
             if not self._self_clearance_fused(device):
                 return self._composed_collision_cost(p, m, cfg_begin, cfg_count, n_seg, seg_len)
@@ -1334,12 +1309,8 @@ class ComposedSDF(ObjectFrameSDF):
         if len(pts_shape) < 2 or pts_shape[-1] != 3:
             raise ValueError(f"collision-cost query: points {pts_shape} must be [..., N, 3]")
         m = self._collision_cost_margin(margin)
-        cost, twist = self.query_collision_cost(points_in_object_frame, m)
-        shape = (*(self.tsf_batch or ()), *pts_shape[:-2])
-        dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
-        out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
-        return (nat.deliver(cost, out_device, dtype).reshape(shape),
-                nat.deliver(twist, out_device, dtype).reshape(*shape, len(self.sdfs), 6))
+        out = self.query_collision_cost(points_in_object_frame, m)
+        return self._deliver(points_in_object_frame, out, (*(self.tsf_batch or ()), *pts_shape[:-2]))
 
     def query_into(self, points_in_object_frame, targets, cfg_begin=0, cfg_count=None):
         """`query` whose result slab is stored by the kernel epilogue into several full-size result buffers at once
@@ -1347,19 +1318,12 @@ class ComposedSDF(ObjectFrameSDF):
         address of a buffer holding ALL n_cfg * P results -- typically this rank's buffer and the peer-mapped buffers
         of the other ranks (distributed.PeerResult).  The slab lands at element cfg_begin * P of every buffer."""
         S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
-        if cfg_count is None:
-            cfg_count = n_cfg - cfg_begin
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
         if not 1 <= len(targets) <= nat.MAX_TARGETS:
             raise ValueError(f"between 1 and {nat.MAX_TARGETS} targets per launch, got {len(targets)}")
-        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(points_in_object_frame, device)
+        with _query_points(points_in_object_frame) as (device, p):
             P = p.shape[0]
-            descs_arr, needs_mesh = self._native_descs(device)
-            if descs_arr is None:
-                raise NotImplementedError("query_into needs the fused kernels: at most 128 sub-SDFs, all with native "
-                                          "descriptors")
+            descs_arr, needs_mesh = self._fused_descs(device, "query_into")
             arr = (nat.OutTarget * len(targets))()
             for t, (tv, tg) in enumerate(targets):
                 for buf, per in ((tv, 1), (tg, 3)):
@@ -1380,16 +1344,10 @@ class ComposedSDF(ObjectFrameSDF):
         destination, the kernels' fastest store path -- what the copy-engine re-assembly (gather="dma") runs before it
         pushes the slab to the peers."""
         S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
-        if cfg_count is None:
-            cfg_count = n_cfg - cfg_begin
-        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(points_in_object_frame, device)
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
+        with _query_points(points_in_object_frame) as (device, p):
             P = p.shape[0]
-            descs_arr, needs_mesh = self._native_descs(device)
-            if descs_arr is None:
-                raise NotImplementedError("query_at needs the fused kernels: at most 128 sub-SDFs, all with native descriptors")
+            descs_arr, needs_mesh = self._fused_descs(device, "query_at")
             xf = self._xforms_on(device)
             nat.check(nat.lib().pvb_composed_query(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg, cfg_begin,
                                                    cfg_count, nat.ptr(p), P, nat.PVB_MESH_DEFAULT,
@@ -1401,17 +1359,10 @@ class ComposedSDF(ObjectFrameSDF):
         mc_grad are the multicast device addresses of the full (n_cfg * P) value / gradient buffers; one multimem.st
         per 16-byte chunk lands in every bound GPU's copy."""
         S = len(self.sdfs)
-        n_cfg = 1 if self.tsf_batch is None else math.prod(list(self.tsf_batch))
-        if cfg_count is None:
-            cfg_count = n_cfg - cfg_begin
-        device = nat.compute_device(points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else None)
-        with torch.cuda.device(device):
-            p = nat.as_f32_points(points_in_object_frame, device)
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
+        with _query_points(points_in_object_frame) as (device, p):
             P = p.shape[0]
-            descs_arr, needs_mesh = self._native_descs(device)
-            if descs_arr is None:
-                raise NotImplementedError("query_multicast needs the fused kernels: at most 128 sub-SDFs, all with native "
-                                          "descriptors")
+            descs_arr, needs_mesh = self._fused_descs(device, "query_multicast")
             xf = self._xforms_on(device)
             nat.check(nat.lib().pvb_composed_query_multicast(descs_arr, S, int(needs_mesh), nat.ptr(xf), n_cfg, cfg_begin,
                                                              cfg_count, nat.ptr(p), P, nat.PVB_MESH_DEFAULT,
@@ -1457,7 +1408,7 @@ class ComposedSDF(ObjectFrameSDF):
         if not (torch.is_tensor(points_in_object_frame) and points_in_object_frame.device.type == "cpu"
                 and points_in_object_frame.dtype == torch.float32 and self.tsf_batch is not None):
             return None
-        n_cfg = math.prod(list(self.tsf_batch))
+        n_cfg = _config_count(self.tsf_batch)
         P = points_in_object_frame.numel() // 3
         if n_cfg < 64 or 16 * n_cfg * P < self.host_result_pipeline_min_bytes:
             return None
@@ -1490,20 +1441,11 @@ class ComposedSDF(ObjectFrameSDF):
 
     def __call__(self, points_in_object_frame):
         pts_shape = tuple(points_in_object_frame.shape)
-        piped = self._host_result_pipeline(points_in_object_frame)
-        if piped is not None:
-            vv, gg = piped
-        else:
-            vv, gg = self.query(points_in_object_frame)
-            dtype = points_in_object_frame.dtype if torch.is_tensor(points_in_object_frame) else torch.float
-            out_device = points_in_object_frame.device if torch.is_tensor(points_in_object_frame) else "cpu"
-            vv = nat.deliver(vv, out_device, dtype)
-            gg = nat.deliver(gg, out_device, dtype)
-        if self.tsf_batch is not None:
-            # configuration batch dims first, then the query points' batch dims (sdf.py:428-431)
-            vv = vv.reshape(*self.tsf_batch, *pts_shape[:-1])
-            gg = gg.reshape(*self.tsf_batch, *pts_shape[:-1], 3)
-        return vv, gg
+        piped = self._host_result_pipeline(points_in_object_frame)      # fp32 on the host already, like its points
+        out = piped if piped is not None else self.query(points_in_object_frame)
+        # configuration batch dims first, then the query points' batch dims (sdf.py:428-431); flat without a batch
+        shape = (*self.tsf_batch, *pts_shape[:-1]) if self.tsf_batch is not None else (-1,)
+        return self._deliver(points_in_object_frame, out, shape)
 
 
 class OutOfBoundsStrategy(enum.Enum):
