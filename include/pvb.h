@@ -313,6 +313,41 @@ int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf, 
                                       int64_t seg_len, float margin, void *workspace, int64_t workspace_bytes,
                                       float *out_cost, float *out_twist, void *stream);
 
+/* ---- EXTENSION: self-collision-cost query, a hinge cost between every configuration's own links and its twists ----
+ * The reference has no such operator.  xforms, inv_xforms, link_pts and allowed as in
+ * pvb_composed_query_self_clearance.  The definition:
+ *   Inputs: a composition of S sub-SDFs with transforms M_s(a), and W_s = _affine_inverse(M_s); link_points [S, K, 3],
+ *   each row in its own sub-SDF's frame; allowed [S, S] bool (the diagonal is ignored); a margin m, rounded to fp32
+ *   exactly as _collision_cost_margin does.
+ *   For configuration a, every source i and every point k:
+ *   - x = W_i(a) . link_points[i, k], posed with composed_xform.  This is the same posed point as in
+ *     pvb_transform_points_paired and self_clearance.
+ *   - (d, g, j) is what query_paired(..., return_which=True) of the composition of row i's allowed sub-SDFs gives at x:
+ *     the value, the object-frame gradient, and the first allowed sub-SDF attaining the value.  These are the
+ *     per-point values _composed_self_clearance already uses.
+ *   - When d < m, with h = m - d and tau = 2h (g, x x g):
+ *     - cost[a] += h^2
+ *     - twist[a, j] += tau.  The target moves.  This is the same term and sign as collision_cost_term.
+ *     - twist[a, i] -= tau.  The source moves.  Its point travels with it, so d changes by +g . (v + w x x).
+ *   - twist[a, s] is therefore the derivative of the cost when sub-SDF s alone moves by an object-frame twist (v, w)
+ *     about the origin.  This is the convention of collision_cost, so RobotSDF.joint_gradient applies unchanged.
+ *   - A configuration with no allowed pair, or with no point below m, costs exactly 0 and has all-zero twists.
+ * out_cost [cfg_count] and out_twist [cfg_count * n_sdf * 6] (k = 0..5 of sub-SDF s at (c * n_sdf + s) * 6 + k) for
+ * configuration cfg_begin + c.  Every (d, g, j) that enters a sum is bit-identical to the per-point query's; a pair is
+ * skipped only when a lower bound of its value is >= m.  The sums are deterministic: no atomics, and their order
+ * depends on K, n_sdf and allowed alone (pvb_device.cuh), so repeated calls give identical bits and a slab reproduces
+ * the rows of a larger call; they are not bit-identical to a composition of per-source queries.  No workspace.
+ * Serves the sets pvb_composed_query_self_clearance serves: at most 8 GRID sub-SDFs with the bounding-box rule
+ * (nearest or trilinear) or primitives.  PVB_ERR_INVALID for every other set (mesh, LOOKUP_GT_SDF grids, more than 8
+ * sub-SDFs: callers compose the per-source paired queries), for K < 1 or K >= 2^24, bits of allowed beyond n_sdf, a
+ * margin that is not finite, cfg_count < 1, null inv_xforms, allowed or outputs, and the argument checks of
+ * pvb_composed_query. */
+int pvb_composed_query_self_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,
+                                           const float *inv_xforms, int32_t n_cfg, int32_t cfg_begin,
+                                           int32_t cfg_count, const float *link_pts, int64_t K,
+                                           const uint8_t *allowed, float margin, float *out_cost, float *out_twist,
+                                           void *stream);
+
 /* ---- the same query with the result slab stored to several destinations from the kernel epilogue ----
  * Multi-GPU re-assembly of a configuration-sharded RobotSDF result (model_to_sdf.py:117-125 returns the full
  * (|A|, N) tensors): every rank evaluates its slab [cfg_begin, cfg_begin + cfg_count) and writes it straight into

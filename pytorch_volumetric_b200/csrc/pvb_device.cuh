@@ -1256,4 +1256,29 @@ __device__ __forceinline__ bool collision_cost_near(const float (&lb)[8], float 
     return near;
 }
 
+// ----------------------------------------------------------------------------
+// Self-collision-cost queries (robot_self_collision_cost_kernel, pvb_composed_query_self_collision_cost).
+// Inputs: a composition of S sub-SDFs with transforms M_s(a), and W_s = _affine_inverse(M_s); link_points [S, K, 3],
+// each row in its own sub-SDF's frame; allowed [S, S] bool (the diagonal is ignored); a margin m, rounded to fp32
+// exactly as _collision_cost_margin does.  For configuration a, every source i and every point k:
+//   * x = W_i(a) . link_points[i, k], posed with composed_xform.  This is the same posed point as in
+//     pvb_transform_points_paired and self_clearance.
+//   * (d, g, j) is what query_paired(..., return_which=True) of the composition of row i's allowed sub-SDFs gives at
+//     x: the value, the object-frame gradient, and the first allowed sub-SDF attaining the value.  These are the
+//     per-point values _composed_self_clearance already uses.
+//   * When d < m, with h = m - d and tau = 2h (g, x x g):
+//       cost[a] += h^2
+//       twist[a, j] += tau.  The target moves.  This is the same term and sign as collision_cost_term.
+//       twist[a, i] -= tau.  The source moves.  Its point travels with it, so d changes by +g . (v + w x x).
+//   * twist[a, s] is therefore the derivative of the cost when sub-SDF s alone moves by an object-frame twist (v, w)
+//     about the origin.  This is the convention of collision_cost, so RobotSDF.joint_gradient applies unchanged.
+//   * A configuration with no allowed pair, or with no point below m, costs exactly 0 and has all-zero twists.
+//
+// Summation order (robot_self_collision_cost_kernel): one warp owns a configuration.  Lane l takes the points
+// k = l, l + 32, l + 64, ... of every source, sources in ascending index order, and adds each term into its own fp32
+// accumulators (cost, and the 6 S twist components); at the end the 32 lanes' accumulators are added in lane order in
+// fp64 and rounded to fp32 once.  The order depends on K, S and allowed alone: not on the slab, the grid or the SM
+// count, so repeated calls give identical bits and a slab reproduces the rows of the full call.
+constexpr int kSccLanes = 32;                     // lanes of a configuration's warp: its accumulators
+
 }  // namespace pvb

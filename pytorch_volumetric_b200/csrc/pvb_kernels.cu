@@ -2316,6 +2316,115 @@ collision_cost_finish_kernel(const float *__restrict__ partial, long long n_rows
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// Self-collision-cost query on the sets robot_self_clearance_kernel takes (pvb_device.cuh: the definition and the
+// summation order): for every configuration of the slab, cost and the 6 n_sdf twist components, stored once each.
+//   * Work unit: one configuration, owned by one warp; the warps of a 1-D grid stride over the slab.  No workspace
+//     and no finish kernel.
+//   * Staging as robot_self_clearance_kernel: the configuration's transform rows and sphere centres once, W_i's three
+//     rows once per source (sources with a non-empty row, ascending).  A lane loads link_pts[i][k] and poses it with
+//     composed_xform.
+//   * A 32-point step is skipped by the whole warp when no lane has an allowed link whose sphere bound is below m;
+//     otherwise each lane runs rs_swept_pair with bp = m, so every (d, g, j) below m is the per-point result of the
+//     allowed sub-composition bit for bit.  Masked links get a +inf bound and are refused inside the visit.
+//   * Accumulators: acc[warp][e][lane] (e = 0: cost; 1 + 6 s + k: component k of sub-SDF s), row stride
+//     kCcLaneStride, each lane owning its column; a contributing pair adds collision_cost_term to its target's slots
+//     and subtracts it from its source's.  End of configuration: lane e adds row e over the 32 lanes in order in fp64.
+//     No atomics anywhere.
+constexpr int kSccWarps = 4;
+struct __align__(16) SccSmem {
+    float4 xf[kSccWarps][3 * kRsMaxS];
+    float4 inv[kSccWarps][4];
+    float4 sph[kSccWarps][3 * kRsMaxS / 4];
+    float acc[kSccWarps][1 + 6 * kRsMaxS][kCcLaneStride];
+};
+
+template <bool kExt>
+__global__ void __launch_bounds__(kSccLanes * kSccWarps, 8)
+robot_self_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf,
+                                 const float *__restrict__ xforms, const float *__restrict__ inv_xforms, int n_cfg,
+                                 int cfg_begin, int cfg_count, const float *__restrict__ link_pts, int K,
+                                 const __grid_constant__ SclRows rows, int n_src, float margin,
+                                 float *__restrict__ out_cost, float *__restrict__ out_twist) {
+    __shared__ SccSmem sm;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const int E = 1 + 6 * n_sdf;
+    const float m = margin;
+    float *const acc = &sm.acc[warp][0][lane];                 // this lane's column
+    // uniform per warp: every lane takes part in the shuffles
+    for (int c = blockIdx.x * kSccWarps + warp; c < cfg_count; c += gridDim.x * kSccWarps) {
+        const int cfg = cfg_begin + c;
+        __syncwarp();                                        // the previous configuration is no longer read
+        if (lane < 3 * n_sdf) {
+            const int si = lane / 3;
+            sm.xf[warp][lane] = __ldg(reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg) * 16) +
+                                      (lane - 3 * si));
+        }
+        for (int e = 0; e < E; ++e) acc[e * kCcLaneStride] = 0.f;
+        __syncwarp();
+        if (lane < kRsMaxS) {
+            const f3 co = lane < n_sdf ? rs_sphere_centre(pk.d[lane], sm.xf[warp][3 * lane], sm.xf[warp][3 * lane + 1],
+                                                          sm.xf[warp][3 * lane + 2])
+                                       : mk3(0.f, 0.f, 0.f);
+            float *cc = reinterpret_cast<float *>(&sm.sph[warp][0]) + 3 * lane;
+            cc[0] = co.x; cc[1] = co.y; cc[2] = co.z;
+        }
+#pragma unroll 1
+        for (int t = 0; t < n_src; ++t) {
+            const int i = rows.src[t];
+            const unsigned mask = rows.mask[i];
+            __syncwarp();                                    // the previous source's W_i is no longer read
+            if (lane < 3)
+                sm.inv[warp][lane] =
+                    __ldg(reinterpret_cast<const float4 *>(inv_xforms + ((size_t)i * n_cfg + cfg) * 16) + lane);
+            __syncwarp();
+            const float4 w0 = sm.inv[warp][0], w1 = sm.inv[warp][1], w2 = sm.inv[warp][2];
+            float *const acc_i = acc + (1 + 6 * i) * kCcLaneStride;
+#pragma unroll 1
+            for (int j0 = 0; j0 < K; j0 += 32) {
+                const int k = j0 + lane;
+                const bool on = k < K;
+                const f3 p = composed_xform(w0, w1, w2,
+                                            on ? load_point(link_pts, (long long)i * K + k) : mk3(0.f, 0.f, 0.f));
+                float lb[kRsMaxS], key[kRsMaxS];
+                rs_point_bounds(sm.sph[warp], pk.sph_rad, p, low3_off, mask, lb, key);
+                if (!__any_sync(0xffffffffu, on && collision_cost_near(lb, m))) continue;
+                auto link = [&](const int si, const float thr, float4 &o) -> bool {
+                    if (!((mask >> si) & 1u)) return false;
+                    const pvb_sdf_desc &d = pk.d[si];
+                    const float4 r0 = sm.xf[warp][3 * si], r1 = sm.xf[warp][3 * si + 1], r2 = sm.xf[warp][3 * si + 2];
+                    return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
+                };
+                float best;
+                f3 bg;
+                int bs;
+                // lanes past the end prune everything that has a bound (bp = -inf) and refuse the rest; unused
+                rs_swept_pair(lb, rs_nearest(key, n_sdf), on ? m : -PVB_INF, link, best, bg, bs);
+                if (on && bs >= 0 && best < m) {
+                    const f3 g = composed_rotate_back(sm.xf[warp][3 * bs], sm.xf[warp][3 * bs + 1],
+                                                      sm.xf[warp][3 * bs + 2], bg);
+                    const CollisionTerm tm = collision_cost_term(m, best, g, p);
+                    acc[0] += tm.cost;
+                    float *const acc_j = acc + (1 + 6 * bs) * kCcLaneStride;
+#pragma unroll
+                    for (int q = 0; q < 6; ++q) {
+                        acc_j[q * kCcLaneStride] += tm.tw[q];
+                        acc_i[q * kCcLaneStride] -= tm.tw[q];
+                    }
+                }
+            }
+        }
+        __syncwarp();
+        for (int e = lane; e < E; e += 32) {
+            double s = 0.0;
+            for (int l = 0; l < kSccLanes; ++l) s += (double)sm.acc[warp][e][l];
+            if (e == 0) out_cost[c] = (float)s;
+            else out_twist[(size_t)c * (E - 1) + (e - 1)] = (float)s;
+        }
+    }
+}
+
 // ========================================================== voxel containers
 // VoxelGrid / ExpandingVoxelGrid / voxel_down_sample (voxel.py:42-171) and the value-range view they sit on
 // (TorchMultidimView: sdf.py:264, voxel.py:55-64): the reference reads, writes and lists voxels with boolean-mask
@@ -3835,6 +3944,65 @@ extern "C" int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int3
     return launch_collision_cost(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, margin,
                                  reinterpret_cast<float *>(workspace), out_cost, out_twist, any_ext,
                                  (cudaStream_t)stream);
+}
+
+extern "C" int pvb_composed_query_self_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,
+                                                      const float *inv_xforms, int32_t n_cfg, int32_t cfg_begin,
+                                                      int32_t cfg_count, const float *link_pts, int64_t K,
+                                                      const uint8_t *allowed, float margin, float *out_cost,
+                                                      float *out_twist, void *stream) {
+    const char *fn = "pvb_composed_query_self_collision_cost";
+    if (K < 1 || K >= (1ll << 24) || !inv_xforms || !allowed) {
+        pvb_set_error("%s: invalid argument (K=%lld; 1 <= K < 2^24, inv_xforms and allowed not null)", fn,
+                      (long long)K);
+        return PVB_ERR_INVALID;
+    }
+    if (!(margin - margin == 0.f)) {                 // NaN or +-inf
+        pvb_set_error("%s: the margin must be finite (margin=%g)", fn, (double)margin);
+        return PVB_ERR_INVALID;
+    }
+    bool any_ext;
+    const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, link_pts,
+                                        (int64_t)n_sdf * K, out_cost, out_twist, any_ext);
+    if (bad) return bad;
+    if (cfg_count < 1) {
+        pvb_set_error("%s: no cost over an empty configuration slab (cfg_count=%d)", fn, cfg_count);
+        return PVB_ERR_INVALID;
+    }
+    // the sets robot_self_clearance_kernel takes: <= 8 GRID links with the bounding-box rule, or primitives
+    const bool fused = n_sdf <= kRsMaxS && rs_links_ok(descs, n_sdf);
+    if (!fused) {
+        pvb_set_error("%s: the fused query takes at most %d grid (bounding-box rule) or primitive sub-SDFs, no mesh or "
+                      "LOOKUP_GT_SDF grid (n_sdf=%d); compose the per-source paired queries instead", fn, kRsMaxS,
+                      n_sdf);
+        return PVB_ERR_INVALID;
+    }
+    SclRows rows;
+    memset(&rows, 0, sizeof(rows));
+    int n_src = 0;
+    for (int i = 0; i < n_sdf; ++i) {
+        if (allowed[i] >> n_sdf) {
+            pvb_set_error("%s: allowed row %d has bits beyond n_sdf=%d (0x%02x)", fn, i, n_sdf, allowed[i]);
+            return PVB_ERR_INVALID;
+        }
+        rows.mask[i] = (unsigned char)(allowed[i] & ~(1u << i));
+        if (rows.mask[i]) rows.src[n_src++] = (unsigned char)i;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
+    const long long blocks = ((long long)cfg_count + kSccWarps - 1) / kSccWarps;
+    timing_mark(0, s);
+    if (any_ext)
+        robot_self_collision_cost_kernel<true><<<(unsigned)blocks, kSccLanes * kSccWarps, 0, s>>>(
+            pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, (int)K, rows, n_src, margin,
+            out_cost, out_twist);
+    else
+        robot_self_collision_cost_kernel<false><<<(unsigned)blocks, kSccLanes * kSccWarps, 0, s>>>(
+            pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, (int)K, rows, n_src, margin,
+            out_cost, out_twist);
+    timing_mark(1, s);
+    PVB_CHECK_LAUNCH("pvb_composed_query_self_collision_cost");
+    return PVB_OK;
 }
 
 extern "C" int pvb_composed_query_multi(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,

@@ -314,6 +314,21 @@ class RobotSDF(sdf.ObjectFrameSDF):
         grad = self.joint_gradient(twist, self.joint_twists(), self.joint_moves_link())
         return cost, grad.to(cost.dtype)
 
+    def self_collision_cost(self, margin, link_points=None, allowed=None):
+        """For every installed joint configuration, the soft self-collision cost between the robot's own links and its
+        derivative with respect to the joint values: link_points [S, K, 3] (default: link_surface_points()) are posed
+        with their links and tested against the links `allowed` [S, S] lets them (default: self_collision_pairs()),
+        and every point within `margin` adds max(0, margin - d)^2.  Returns (cost [*A], joint_grad [*A, J]), J in
+        `joint_names` order: ComposedSDF.self_collision_cost's twist gradient through joint_gradient(twist,
+        joint_twists(), joint_moves_link()).  Not autograd: the gradient is an output of the query."""
+        if link_points is None:
+            link_points = self.link_surface_points()
+        if allowed is None:
+            allowed = self.self_collision_pairs()
+        cost, twist = self.sdf.self_collision_cost(link_points, allowed, margin)
+        grad = self.joint_gradient(twist, self.joint_twists(), self.joint_moves_link())
+        return cost, grad.to(cost.dtype)
+
     @staticmethod
     def joint_gradient(twist, joint_twists, moves):
         """The Jacobian transpose of a serial chain: twist gradients [A, *B, S, 6] (configuration-major, A flat or

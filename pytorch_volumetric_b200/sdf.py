@@ -1312,6 +1312,110 @@ class ComposedSDF(ObjectFrameSDF):
         out = self.query_collision_cost(points_in_object_frame, m)
         return self._deliver(points_in_object_frame, out, (*(self.tsf_batch or ()), *pts_shape[:-2]))
 
+    def query_self_collision_cost(self, link_points, allowed, margin, cfg_begin=0, cfg_count=None):
+        """Self-collision cost of configurations [cfg_begin, cfg_begin + cfg_count) and its twist gradient per
+        sub-SDF.
+
+        Inputs: a composition of S sub-SDFs with transforms M_s(a), and W_s = _affine_inverse(M_s); link_points
+        [S, K, 3], each row in its own sub-SDF's frame; allowed [S, S] bool (the diagonal is ignored); a margin m,
+        rounded to fp32 exactly as _collision_cost_margin does.  For configuration a, every source i and every
+        point k:
+          - x = W_i(a) . link_points[i, k], posed with composed_xform.  This is the same posed point as in
+            pvb_transform_points_paired and self_clearance.
+          - (d, g, j) is what query_paired(..., return_which=True) of the composition of row i's allowed sub-SDFs
+            gives at x: the value, the object-frame gradient, and the first allowed sub-SDF attaining the value.  These
+            are the per-point values _composed_self_clearance already uses.
+          - When d < m, with h = m - d and tau = 2h (g, x x g):
+              - cost[a] += h^2
+              - twist[a, j] += tau.  The target moves.  This is the same term and sign as collision_cost_term.
+              - twist[a, i] -= tau.  The source moves.  Its point travels with it, so d changes by +g . (v + w x x).
+          - twist[a, s] is therefore the derivative of the cost when sub-SDF s alone moves by an object-frame twist
+            (v, w) about the origin.  This is the convention of collision_cost, so RobotSDF.joint_gradient applies
+            unchanged.
+          - A configuration with no allowed pair, or with no point below m, costs exactly 0 and has all-zero twists.
+
+        Sets of at most 8 grid (bounding-box rule) or primitive sub-SDFs run in one fused kernel
+        (pvb_composed_query_self_collision_cost); every other set takes the composition route
+        (`_composed_self_collision_cost`), against which the fused route is checked.  Both are deterministic, and the
+        fused route's rows do not depend on the slab: a configuration split reproduces the full call bit for bit.
+        Returns flat (cfg_count,) / (cfg_count, S, 6) fp32 tensors on the GPU.  Raises ValueError before any device
+        work on wrong shapes, a margin that is not finite, or an empty slab."""
+        S = len(self.sdfs)
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
+        K, rows = self._self_clearance_args(link_points, allowed)
+        m = self._collision_cost_margin(margin)
+        if cfg_count < 1 or cfg_begin < 0 or cfg_begin + cfg_count > n_cfg:
+            raise ValueError(f"self-collision-cost query: empty or invalid configuration slab [{cfg_begin}, "
+                             f"+{cfg_count}) of {n_cfg}")
+        with _query_points(link_points) as (device, p):
+            if not self._self_clearance_fused(device):
+                return self._composed_self_collision_cost(p, K, rows, m, cfg_begin, cfg_count)
+            descs_arr, _ = self._native_descs(device)
+            xf, inv = self._xforms_on(device), self._inv_xforms_on(device)
+            masks = (ctypes.c_uint8 * S)(*[sum(1 << j for j in range(S) if rows[i][j]) for i in range(S)])
+            cost = torch.empty(cfg_count, dtype=torch.float32, device=device)
+            twist = torch.empty(cfg_count, S, 6, dtype=torch.float32, device=device)
+            nat.check(nat.lib().pvb_composed_query_self_collision_cost(descs_arr, S, nat.ptr(xf), nat.ptr(inv), n_cfg,
+                                                                       cfg_begin, cfg_count, nat.ptr(p), K, masks, m,
+                                                                       nat.ptr(cost), nat.ptr(twist),
+                                                                       nat.stream_ptr(device)),
+                      "pvb_composed_query_self_collision_cost")
+        return cost, twist
+
+    def _composed_self_collision_cost(self, p, K, rows, m, cfg_begin, cfg_count):
+        """query_self_collision_cost by composition, the definition of its result: for every source i with an
+        allowed row and every chunk of `clearance_generic_chunk` configurations, link_points[i] posed by W_i
+        (pvb_transform_points_paired), then query_paired(..., return_which=True) of ComposedSDF([sdfs[j] for allowed
+        j], their transform rows), its sub-SDF index mapped back; the terms in fp64, one masked sum per target, and
+        the source's total subtracted (torch's sums are deterministic; scatter_add / index_add on CUDA are not)."""
+        S, n_cfg = len(self.sdfs), _config_count(self.tsf_batch)
+        device = p.device
+        xf = self._xforms_on(device).reshape(S, n_cfg, 4, 4)
+        inv = self._inv_xforms_on(device).reshape(S, n_cfg, 4, 4)
+        lp = p.reshape(S, K, 3)
+        cost = torch.zeros(cfg_count, dtype=torch.float64, device=device)
+        twist = torch.zeros(cfg_count, S, 6, dtype=torch.float64, device=device)
+        for i in range(S):
+            js = [j for j in range(S) if rows[i][j]]
+            if not js:
+                continue
+            sub = ComposedSDF([self.sdfs[j] for j in js], None)
+            sub.set_transforms(Transform3d(matrix=xf[js].reshape(len(js) * n_cfg, 4, 4)), batch_dim=(n_cfg,))
+            js_t = torch.tensor(js, dtype=torch.long, device=device)
+            for c0 in range(cfg_begin, cfg_begin + cfg_count, self.clearance_generic_chunk):
+                cc = min(self.clearance_generic_chunk, cfg_begin + cfg_count - c0)
+                w_i = inv[i, c0:c0 + cc].contiguous()
+                own = lp[i].expand(cc, K, 3).contiguous()
+                x = torch.empty(cc, K, 3, dtype=torch.float32, device=device)
+                nat.check(nat.lib().pvb_transform_points_paired(nat.ptr(w_i), cc, nat.ptr(own), K, nat.ptr(x),
+                                                                nat.stream_ptr(device)), "pvb_transform_points_paired")
+                v, g, w = sub.query_paired(x, cfg_begin=c0, cfg_count=cc, return_which=True)
+                v, g, w = v.reshape(cc, K).double(), g.reshape(cc, K, 3).double(), js_t[w.long()].reshape(cc, K)
+                h = (m - v).clamp_min(0.0)                          # 0 exactly where d >= m
+                xd = x.double()
+                tau = torch.cat([g, torch.linalg.cross(xd, g, dim=-1)], dim=-1) * (2.0 * h)[..., None]
+                rs = slice(c0 - cfg_begin, c0 - cfg_begin + cc)
+                cost[rs] += (h * h).sum(dim=-1)
+                for j in js:
+                    twist[rs, j] += (tau * (w == j)[..., None]).sum(dim=-2)
+                twist[rs, i] -= tau.sum(dim=-2)
+        return cost.float(), twist.float()
+
+    def self_collision_cost(self, link_points, allowed, margin):
+        """For every installed configuration, the soft self-collision cost between its own sub-SDFs and its twist
+        gradient per sub-SDF: link_points [S, K, 3] holds K points of every sub-SDF in its own frame (its surface,
+        say), allowed [S, S] bool says which sub-SDFs the points of each one are tested against (the diagonal is
+        ignored), and every posed point within `margin` of an allowed sub-SDF adds max(0, margin - d)^2.  Returns
+        (cost [*A], twist_grad [*A, S, 6]) in link_points' dtype on the composition's device -- 0-d / [S, 6] without a
+        configuration batch.  twist_grad[..., s, :] is the derivative of the cost when sub-SDF s alone moves by an
+        object-frame twist (v, w) about the origin: a term adds to its target and subtracts from its source, so
+        moving both together changes nothing.  The definition and routes are those of `query_self_collision_cost`.
+        Not a reference operator (an extension); raises ValueError before any device work on wrong shapes or a margin
+        that is not finite."""
+        shape = () if self.tsf_batch is None else tuple(int(a) for a in self.tsf_batch)
+        out = self.query_self_collision_cost(link_points, allowed, margin)
+        return self._deliver(link_points, out, shape, device=matrix_of(self.obj_frame_to_link_frame).device)
+
     def query_into(self, points_in_object_frame, targets, cfg_begin=0, cfg_count=None):
         """`query` whose result slab is stored by the kernel epilogue into several full-size result buffers at once
         (pvb_composed_query_multi): `targets` is a list of (val, grad) pairs, each a float32 tensor or a raw device
