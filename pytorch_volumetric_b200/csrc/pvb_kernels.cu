@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
+#include <type_traits>
 
 // ------------------------------------------------------------------ errors
 static thread_local char g_err[512] = "";
@@ -3080,36 +3081,70 @@ extern "C" int pvb_sphere_query(float radius, const float *pts, int64_t n, float
     return PVB_OK;
 }
 
-template <bool kMesh, int PTS, int MAXS, bool kExt>
-static int launch_composed(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
-                           int cfg_count, const float *pts, long long first_pt, long long n_pts, uint32_t mesh_mode,
-                           float *out_val, float *out_grad, int *out_which, const OutTargets *tg, cudaStream_t stream) {
-    const long long n_items = (n_pts - first_pt) / PTS;
-    if (n_items <= 0) return PVB_OK;
+// The sub-SDFs of the generic composed kernels in their visiting order (fill_order).
+template <int MAXS>
+static DescPack<MAXS> desc_pack(const pvb_sdf_desc *descs, int n_sdf) {
     DescPack<MAXS> pack;
     memcpy(pack.d, descs, sizeof(pvb_sdf_desc) * (size_t)n_sdf);
     fill_order(pack, n_sdf);
+    return pack;
+}
+
+// The scalar arguments every generic composed kernel takes after its outputs: whether mesh sub-SDFs are evaluated
+// nearest-bound-first (PVB_COMP_NEAREST_FIRST=0 restores the fixed bit-reversed order) and the largest prune margin.
+struct CompConsts {
+    int nearest_first;
+    float margin_max;
+};
+
+static CompConsts comp_consts(const pvb_sdf_desc *descs, int n_sdf) {
+    static const int nearest_first = [] { const char *e = getenv("PVB_COMP_NEAREST_FIRST"); return e ? atoi(e) : 1; }();
+    float margin_max = 0.f;
+    for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
+    return {nearest_first, margin_max};
+}
+
+// Calls f(kMesh, kExt, kMaxS), std::bool_constant / std::integral_constant values naming the instantiation of the
+// generic composed kernels that serves the set: with mesh sub-SDFs or not, with trilinear or primitive sub-SDFs or
+// not, and room for 16 or 128 sub-SDFs.
+template <typename F>
+static int comp_variant(bool mesh, bool ext, int n_sdf, F &&f) {
+    auto by_maxs = [&](auto kMesh, auto kExt) {
+        return n_sdf <= 16 ? f(kMesh, kExt, std::integral_constant<int, 16>{})
+                           : f(kMesh, kExt, std::integral_constant<int, 128>{});
+    };
+    auto by_ext = [&](auto kMesh) { return ext ? by_maxs(kMesh, std::true_type{}) : by_maxs(kMesh, std::false_type{}); };
+    return mesh ? by_ext(std::true_type{}) : by_ext(std::false_type{});
+}
+
+template <bool kMesh, int PTS, int MAXS, bool kExt>
+static int launch_composed(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
+                           int cfg_count, const float *pts, long long n_pts, uint32_t mesh_mode, float *out_val,
+                           float *out_grad, int *out_which, const OutTargets *tg, cudaStream_t stream) {
+    const long long n_items = n_pts / PTS;
+    if (n_items <= 0) return PVB_OK;
+    const DescPack<MAXS> pack = desc_pack<MAXS>(descs, n_sdf);
+    const CompConsts c = comp_consts(descs, n_sdf);
     const int gx = grid_for(n_items, kCompThreads, 8);
     int gy = cfg_count < 65535 ? cfg_count : 65535;
     const long long cap = (long long)sm_count() * 64;     // bound the block count for huge configuration batches
     if ((long long)gx * gy > cap) { gy = (int)(cap / gx); if (gy < 1) gy = 1; }
     dim3 grid((unsigned)gx, (unsigned)gy);
-    // mesh sub-SDFs: nearest-bound-first evaluation (PVB_COMP_NEAREST_FIRST=0 restores the fixed bit-reversed order)
-    static const int nearest_first = [] { const char *e = getenv("PVB_COMP_NEAREST_FIRST"); return e ? atoi(e) : 1; }();
-    float margin_max = 0.f;
-    for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
+    auto k = tg ? composed_query_kernel<kMesh, PTS, MAXS, true, kExt>
+                : composed_query_kernel<kMesh, PTS, MAXS, false, kExt>;
     timing_mark(0, stream);
-    if (tg)
-        composed_query_kernel<kMesh, PTS, MAXS, true, kExt><<<grid, kCompThreads, 0, stream>>>(
-            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, first_pt, n_pts, mesh_mode, nullptr, nullptr,
-            out_which, *tg, nearest_first, margin_max);
-    else
-        composed_query_kernel<kMesh, PTS, MAXS, false, kExt><<<grid, kCompThreads, 0, stream>>>(
-            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, first_pt, n_pts, mesh_mode, out_val, out_grad,
-            out_which, OutTargets{}, nearest_first, margin_max);
+    k<<<grid, kCompThreads, 0, stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, 0, n_pts, mesh_mode,
+                                         tg ? nullptr : out_val, tg ? nullptr : out_grad, out_which,
+                                         tg ? *tg : OutTargets{}, c.nearest_first, c.margin_max);
     timing_mark(1, stream);
     PVB_CHECK_LAUNCH("pvb_composed_query");
     return PVB_OK;
+}
+
+// Waves of resident blocks the point-form robot kernels aim their grid at.
+static int robot_waves() {
+    static const int waves = [] { const char *e = getenv("PVB_ROBOT_WAVES"); return e ? atoi(e) : 4; }();
+    return waves;
 }
 
 // Launch robot_query_kernel (all sub-SDFs GRID with the bounding-box rule, <= 16 of them).
@@ -3127,33 +3162,25 @@ static int launch_robot(const pvb_sdf_desc *descs, int n_sdf, const float *xform
     }
     for (int si = n_sdf; si < MAXS; ++si) pack.orig[si] = -1;
     const int kind = !tg ? 0 : (tg->mc ? 2 : 1);
-    auto k0 = robot_query_kernel<MAXS, kUnroll, 0>;
-    auto k1 = robot_query_kernel<MAXS, kUnroll, 1>;
-    auto k2 = robot_query_kernel<MAXS, kUnroll, 2>;
+    decltype(&robot_query_kernel<MAXS, kUnroll, 0>) const ks[3] = {
+        robot_query_kernel<MAXS, kUnroll, 0>, robot_query_kernel<MAXS, kUnroll, 1>, robot_query_kernel<MAXS, kUnroll, 2>};
     const int smem = (int)sizeof(RobotSmem<MAXS>);
     const int slot0 = kUnroll ? kSlotRobot : kSlotRobotWide;
-    if (!ensure_smem(k0, slot0, smem) || !ensure_smem(k1, slot0 + 1, smem) || !ensure_smem(k2, slot0 + 2, smem)) {
-        pvb_set_error("pvb_composed_query: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
-        return PVB_ERR_CUDA;
-    }
+    for (int d = 0; d < 3; ++d)
+        if (!ensure_smem(ks[d], slot0 + d, smem)) {
+            pvb_set_error("pvb_composed_query: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
+            return PVB_ERR_CUDA;
+        }
     const int gy = (cfg_count + kRbCfg - 1) / kRbCfg;
     const long long n_tiles = (n_pts + kRbTilePts - 1) / kRbTilePts;
-    static const int waves = [] { const char *e = getenv("PVB_ROBOT_WAVES"); return e ? atoi(e) : 4; }();
-    long long gx = ((long long)sm_count() * (kUnroll ? 4 : 3) * waves + gy - 1) / gy;
+    long long gx = ((long long)sm_count() * (kUnroll ? 4 : 3) * robot_waves() + gy - 1) / gy;
     if (gx > n_tiles) gx = n_tiles;
     if (gx < 1) gx = 1;
     dim3 grid((unsigned)gx, (unsigned)gy);
-    const OutTargets none{};
     timing_mark(0, stream);
-    if (kind == 0)
-        k0<<<grid, kRbCfg * kRbWarps, smem, stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts,
-                                                      vec, out_val, out_grad, out_which, none);
-    else if (kind == 1)
-        k1<<<grid, kRbCfg * kRbWarps, smem, stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts,
-                                                      vec, nullptr, nullptr, out_which, *tg);
-    else
-        k2<<<grid, kRbCfg * kRbWarps, smem, stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts,
-                                                      vec, nullptr, nullptr, out_which, *tg);
+    ks[kind]<<<grid, kRbCfg * kRbWarps, smem, stream>>>(
+        pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts, vec, tg ? nullptr : out_val,
+        tg ? nullptr : out_grad, out_which, tg ? *tg : OutTargets{});
     timing_mark(1, stream);
     PVB_CHECK_LAUNCH("pvb_composed_query(robot)");
     return PVB_OK;
@@ -3188,15 +3215,17 @@ static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float
                                float *out_grad, int *out_which, const OutTargets *tg, bool ext, cudaStream_t stream) {
     const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
     const int kind = !tg ? 0 : (tg->mc ? 2 : 1);
-    auto k0 = ext ? robot_serial_kernel<0, true> : robot_serial_kernel<0, false>;
-    auto k1 = ext ? robot_serial_kernel<1, true> : robot_serial_kernel<1, false>;
-    auto k2 = ext ? robot_serial_kernel<2, true> : robot_serial_kernel<2, false>;
+    decltype(&robot_serial_kernel<0, false>) const ks[3] = {
+        ext ? robot_serial_kernel<0, true> : robot_serial_kernel<0, false>,
+        ext ? robot_serial_kernel<1, true> : robot_serial_kernel<1, false>,
+        ext ? robot_serial_kernel<2, true> : robot_serial_kernel<2, false>};
     const int smem = (int)sizeof(RsSmem);
     const int slot0 = ext ? kSlotSerialExt : kSlotSerial;
-    if (!ensure_smem(k0, slot0, smem) || !ensure_smem(k1, slot0 + 1, smem) || !ensure_smem(k2, slot0 + 2, smem)) {
-        pvb_set_error("pvb_composed_query: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
-        return PVB_ERR_CUDA;
-    }
+    for (int d = 0; d < 3; ++d)
+        if (!ensure_smem(ks[d], slot0 + d, smem)) {
+            pvb_set_error("pvb_composed_query: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
+            return PVB_ERR_CUDA;
+        }
     // tiles: cfg_count / 32 of 32 configurations, then one per binary digit of the remainder (rs_tile)
     const int n_full = cfg_count >> 5, rem = cfg_count & 31;
     const int gy = n_full + __builtin_popcount((unsigned)rem);
@@ -3209,24 +3238,16 @@ static int launch_robot_serial(const pvb_sdf_desc *descs, int n_sdf, const float
     const long long slots = (long long)sm_count() * PVB_RS_MINB * kRsWarps;
     const int chunk_log2 = (kRsChunk == 4 || total_steps < (long long)fine_below * slots) ? 2 : 3;
     const long long n_chunks = (n_pts + (1 << chunk_log2) - 1) >> chunk_log2;     // steps of a 32-configuration tile
-    static const int waves = [] { const char *e = getenv("PVB_ROBOT_WAVES"); return e ? atoi(e) : 4; }();
-    long long gx = ((long long)sm_count() * PVB_RS_MINB * waves + gy - 1) / gy;
+    long long gx = ((long long)sm_count() * PVB_RS_MINB * robot_waves() + gy - 1) / gy;
     const long long gx_max = (n_chunks + kRsWarps - 1) / kRsWarps;
     if (gx > gx_max) gx = gx_max;
     if (gx < 1) gx = 1;
     const long long spw = chunk_log2;
     dim3 grid((unsigned)gx, (unsigned)gy);
-    const OutTargets none{};
     timing_mark(0, stream);
-    if (kind == 0)
-        k0<<<grid, kRbCfg * kRsWarps, smem, stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts,
-                                                      vec, (int)spw, out_val, out_grad, out_which, none);
-    else if (kind == 1)
-        k1<<<grid, kRbCfg * kRsWarps, smem, stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts,
-                                                      vec, (int)spw, nullptr, nullptr, out_which, *tg);
-    else
-        k2<<<grid, kRbCfg * kRsWarps, smem, stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts,
-                                                      vec, (int)spw, nullptr, nullptr, out_which, *tg);
+    ks[kind]<<<grid, kRbCfg * kRsWarps, smem, stream>>>(
+        pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts, vec, (int)spw, tg ? nullptr : out_val,
+        tg ? nullptr : out_grad, out_which, tg ? *tg : OutTargets{});
     timing_mark(1, stream);
     PVB_CHECK_LAUNCH("pvb_composed_query(robot-serial)");
     return PVB_OK;
@@ -3334,8 +3355,6 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
         }
     }
     const bool vec = !needs_mesh && aligned16(pts) && out_aligned && aligned16(out_which) && (n_pts % 4 == 0);
-    const long long n_vec = vec ? n_pts : 0;
-    int rc = PVB_OK;
     // lanes = configurations: only worthwhile when the 32-wide configuration tiles are well filled (25 configurations
     // per rank on 8 GPUs would idle 22 % of the lanes, and point-major is faster there)
     const int cm_tiles = (cfg_count + kCmCfg - 1) / kCmCfg;
@@ -3367,9 +3386,7 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
             pvb_set_error("pvb_composed_query: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
             return PVB_ERR_CUDA;
         }
-        DescPack<kCmMaxS> pack;
-        memcpy(pack.d, descs, sizeof(pvb_sdf_desc) * (size_t)n_sdf);
-        fill_order(pack, n_sdf);
+        const DescPack<kCmMaxS> pack = desc_pack<kCmMaxS>(descs, n_sdf);
         const int gy = (cfg_count + kCmCfg - 1) / kCmCfg;
         const long long n_tiles = (n_pts + kCmTilePts - 1) / kCmTilePts;
         long long gx = ((long long)sm_count() * 3 * 4 + gy - 1) / gy;     // ~4 waves of resident CTAs
@@ -3377,32 +3394,26 @@ static int composed_dispatch(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t n
         if (gx < 1) gx = 1;
         dim3 grid((unsigned)gx, (unsigned)gy);
         timing_mark(0, s);
-        if (tg)
-            km<<<grid, kCmCfg * kCmWarps, sizeof(CmSmem), s>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,
-                                                               n_pts, nullptr, nullptr, out_which, *tg);
-        else
-            kl<<<grid, kCmCfg * kCmWarps, sizeof(CmSmem), s>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,
-                                                               n_pts, out_val, out_grad, out_which, OutTargets{});
+        (tg ? km : kl)<<<grid, kCmCfg * kCmWarps, sizeof(CmSmem), s>>>(
+            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, tg ? nullptr : out_val,
+            tg ? nullptr : out_grad, out_which, tg ? *tg : OutTargets{});
         timing_mark(1, s);
         PVB_CHECK_LAUNCH("pvb_composed_query(cfg-major)");
         return PVB_OK;
     }
-#define PVB_COMP(MESH, PTS, FIRST, N, TRI)                                                                         \
-    (n_sdf <= 16 ? launch_composed<MESH, PTS, 16, TRI>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, FIRST,  \
-                                                       N, mesh_mode, out_val, out_grad, out_which, tg, s)          \
-                 : launch_composed<MESH, PTS, 128, TRI>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, FIRST, \
-                                                        N, mesh_mode, out_val, out_grad, out_which, tg, s))
-#define PVB_COMP_ANY(MESH, PTS, FIRST, N) (any_ext ? PVB_COMP(MESH, PTS, FIRST, N, true) : PVB_COMP(MESH, PTS, FIRST, N, false))
-    if (n_vec > 0) {
-        rc = PVB_COMP_ANY(false, PVB_COMP_PTS, 0, n_pts);
-    } else if (needs_mesh) {
-        rc = PVB_COMP_ANY(true, 1, 0, n_pts);
-    } else {
-        rc = PVB_COMP_ANY(false, 1, 0, n_pts);
-    }
-#undef PVB_COMP_ANY
-#undef PVB_COMP
-    return rc;
+    // point-major; the 4-points-per-thread vector rows exist for sets without meshes only (vec implies !needs_mesh)
+    return comp_variant(needs_mesh, any_ext, n_sdf, [&](auto kMesh, auto kExt, auto kMaxS) {
+        if constexpr (kMesh)
+            return launch_composed<true, 1, kMaxS, kExt>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,
+                                                         mesh_mode, out_val, out_grad, out_which, tg, s);
+        else if (vec)
+            return launch_composed<false, PVB_COMP_PTS, kMaxS, kExt>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count,
+                                                                     pts, n_pts, mesh_mode, out_val, out_grad,
+                                                                     out_which, tg, s);
+        else
+            return launch_composed<false, 1, kMaxS, kExt>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,
+                                                          mesh_mode, out_val, out_grad, out_which, tg, s);
+    });
 }
 
 extern "C" int pvb_composed_query(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh, const float *xforms,
@@ -3417,17 +3428,12 @@ template <bool kMesh, bool kExt, int MAXS>
 static int launch_paired(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                          const float *pts, long long n_pts, long long n_pairs, uint32_t mesh_mode, float *out_val,
                          float *out_grad, int *out_which, cudaStream_t stream) {
-    DescPack<MAXS> pack;
-    memcpy(pack.d, descs, sizeof(pvb_sdf_desc) * (size_t)n_sdf);
-    fill_order(pack, n_sdf);
-    // the same switch as launch_composed: nearest-bound-first evaluation of mesh sub-SDFs
-    static const int nearest_first = [] { const char *e = getenv("PVB_COMP_NEAREST_FIRST"); return e ? atoi(e) : 1; }();
-    float margin_max = 0.f;
-    for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
+    const DescPack<MAXS> pack = desc_pack<MAXS>(descs, n_sdf);
+    const CompConsts c = comp_consts(descs, n_sdf);
     timing_mark(0, stream);
     composed_paired_kernel<kMesh, kExt, MAXS><<<grid_for(n_pairs, kCompThreads, 8), kCompThreads, 0, stream>>>(
         pack, n_sdf, xforms, n_cfg, cfg_begin, pts, n_pts, n_pairs, mesh_mode, out_val, out_grad, out_which,
-        nearest_first, margin_max);
+        c.nearest_first, c.margin_max);
     timing_mark(1, stream);
     PVB_CHECK_LAUNCH("pvb_composed_query_paired");
     return PVB_OK;
@@ -3448,16 +3454,10 @@ extern "C" int pvb_composed_query_paired(const pvb_sdf_desc *descs, int32_t n_sd
         return PVB_ERR_INVALID;
     }
     const long long n_pairs = (long long)cfg_count * n_pts;
-    cudaStream_t s = (cudaStream_t)stream;
-#define PVB_PAIRED(MESH, TRI)                                                                                      \
-    (n_sdf <= 16 ? launch_paired<MESH, TRI, 16>(descs, n_sdf, xforms, n_cfg, cfg_begin, pts, n_pts, n_pairs,       \
-                                                 mesh_mode, out_val, out_grad, out_which, s)                         \
-                 : launch_paired<MESH, TRI, 128>(descs, n_sdf, xforms, n_cfg, cfg_begin, pts, n_pts, n_pairs,      \
-                                                  mesh_mode, out_val, out_grad, out_which, s))
-    const int rc = needs_mesh ? (any_ext ? PVB_PAIRED(true, true) : PVB_PAIRED(true, false))
-                              : (any_ext ? PVB_PAIRED(false, true) : PVB_PAIRED(false, false));
-#undef PVB_PAIRED
-    return rc;
+    return comp_variant(needs_mesh, any_ext, n_sdf, [&](auto kMesh, auto kExt, auto kMaxS) {
+        return launch_paired<kMesh, kExt, kMaxS>(descs, n_sdf, xforms, n_cfg, cfg_begin, pts, n_pts, n_pairs, mesh_mode,
+                                                 out_val, out_grad, out_which, (cudaStream_t)stream);
+    });
 }
 
 // Launch robot_swept_kernel.  Points per block: as many as keep >= 2 waves of resident blocks, so that the tile
@@ -3470,15 +3470,10 @@ static int launch_robot_swept(const pvb_sdf_desc *descs, int n_sdf, const float 
     int blk_pts = kSwMaxPts;
     while (blk_pts > 32 && n_pts < 2 * slots * blk_pts) blk_pts >>= 1;
     const long long gx = (n_pts + blk_pts - 1) / blk_pts;
+    auto k = ext ? robot_swept_kernel<true> : robot_swept_kernel<false>;
     timing_mark(0, stream);
-    if (ext)
-        robot_swept_kernel<true><<<(unsigned)gx, kRbCfg * kRsWarps, 0, stream>>>(
-            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts, blk_pts, out_val, out_grad, out_cfg,
-            out_which);
-    else
-        robot_swept_kernel<false><<<(unsigned)gx, kRbCfg * kRsWarps, 0, stream>>>(
-            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts, blk_pts, out_val, out_grad, out_cfg,
-            out_which);
+    k<<<(unsigned)gx, kRbCfg * kRsWarps, 0, stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, (int)n_pts,
+                                                      blk_pts, out_val, out_grad, out_cfg, out_which);
     timing_mark(1, stream);
     PVB_CHECK_LAUNCH("pvb_composed_query_swept(robot)");
     return PVB_OK;
@@ -3488,17 +3483,12 @@ template <bool kMesh, bool kExt, int MAXS>
 static int launch_swept(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                         int cfg_count, const float *pts, long long n_pts, uint32_t mesh_mode, float *out_val,
                         float *out_grad, int *out_cfg, int *out_which, cudaStream_t stream) {
-    DescPack<MAXS> pack;
-    memcpy(pack.d, descs, sizeof(pvb_sdf_desc) * (size_t)n_sdf);
-    fill_order(pack, n_sdf);
-    // the same switch as launch_composed: nearest-bound-first evaluation of mesh sub-SDFs
-    static const int nearest_first = [] { const char *e = getenv("PVB_COMP_NEAREST_FIRST"); return e ? atoi(e) : 1; }();
-    float margin_max = 0.f;
-    for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
+    const DescPack<MAXS> pack = desc_pack<MAXS>(descs, n_sdf);
+    const CompConsts c = comp_consts(descs, n_sdf);
     timing_mark(0, stream);
     composed_swept_kernel<kMesh, kExt, MAXS><<<grid_for(n_pts, kCompThreads, 8), kCompThreads, 0, stream>>>(
         pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, mesh_mode, out_val, out_grad, out_cfg,
-        out_which, nearest_first, margin_max);
+        out_which, c.nearest_first, c.margin_max);
     timing_mark(1, stream);
     PVB_CHECK_LAUNCH("pvb_composed_query_swept");
     return PVB_OK;
@@ -3523,21 +3513,93 @@ extern "C" int pvb_composed_query_swept(const pvb_sdf_desc *descs, int32_t n_sdf
     if (fused)
         return launch_robot_swept(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_val, out_grad,
                                   out_cfg, out_which, any_ext, s);
-#define PVB_SWEPT(MESH, TRI)                                                                                       \
-    (n_sdf <= 16 ? launch_swept<MESH, TRI, 16>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,       \
-                                                mesh_mode, out_val, out_grad, out_cfg, out_which, s)                 \
-                 : launch_swept<MESH, TRI, 128>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,      \
-                                                 mesh_mode, out_val, out_grad, out_cfg, out_which, s))
-    const int rc = needs_mesh ? (any_ext ? PVB_SWEPT(true, true) : PVB_SWEPT(true, false))
-                              : (any_ext ? PVB_SWEPT(false, true) : PVB_SWEPT(false, false));
-#undef PVB_SWEPT
-    return rc;
+    return comp_variant(needs_mesh, any_ext, n_sdf, [&](auto kMesh, auto kExt, auto kMaxS) {
+        return launch_swept<kMesh, kExt, kMaxS>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts,
+                                                mesh_mode, out_val, out_grad, out_cfg, out_which, s);
+    });
 }
 
 // The longest chunk of the clearance kernels: their point loops step j0 = 0, 32, 64, ... (robot_clearance_kernel: up to
 // 256) past the chunk's end in int, so a chunk as long as a segment of nearly 2^31 points would wrap.  The chunking
 // never changes a result (the keys name the first point attaining the minimum).
 constexpr long long kRsMaxChunk = 1ll << 30;
+
+// Argument rules of the clearance, self-clearance and collision-cost entry points (`fn` names the entry point in the
+// error message).  Each entry point applies them in its own order: the first that fails decides the error.
+
+// Segment sizes: seg_len < 2^31, n_seg * seg_len and cfg_count * n_seg below 2^63, and (`paired`: one point set per
+// configuration) cfg_count * n_seg * seg_len below 2^63.
+static int check_segments(const char *fn, long long n_seg, long long seg_len, int cfg_count, bool paired) {
+    if (n_seg < 0 || seg_len < 0 || seg_len >= (1ll << 31) || (seg_len > 0 && n_seg > INT64_MAX / seg_len) ||
+        (cfg_count > 0 && n_seg > INT64_MAX / cfg_count) ||
+        (paired && cfg_count > 0 && n_seg * seg_len > INT64_MAX / cfg_count)) {
+        if (paired)
+            pvb_set_error("%s: invalid argument (n_seg=%lld seg_len=%lld cfg_count=%d; seg_len < 2^31, "
+                          "cfg_count * n_seg * seg_len < 2^63)", fn, n_seg, seg_len, cfg_count);
+        else
+            pvb_set_error("%s: invalid argument (n_seg=%lld seg_len=%lld cfg_count=%d; seg_len < 2^31)", fn, n_seg,
+                          seg_len, cfg_count);
+        return PVB_ERR_INVALID;
+    }
+    return PVB_OK;
+}
+
+// The link points of the self forms: K per link with 1 <= K < 2^24, the inverse transforms and the allowed rows.
+static int check_link_points(const char *fn, long long K, const float *inv_xforms, const uint8_t *allowed) {
+    if (K < 1 || K >= (1ll << 24) || !inv_xforms || !allowed) {
+        pvb_set_error("%s: invalid argument (K=%lld; 1 <= K < 2^24, inv_xforms and allowed not null)", fn, K);
+        return PVB_ERR_INVALID;
+    }
+    return PVB_OK;
+}
+
+static int check_margin(const char *fn, float margin) {
+    if (!(margin - margin == 0.f)) {                 // NaN or +-inf
+        pvb_set_error("%s: the margin must be finite (margin=%g)", fn, (double)margin);
+        return PVB_ERR_INVALID;
+    }
+    return PVB_OK;
+}
+
+// The forms without a generic route take robot_serial_kernel's sets only: <= 8 GRID links with the bounding-box rule,
+// or primitives.  `instead` is the advice the refusal closes with.
+static int check_fused_only(const char *fn, const pvb_sdf_desc *descs, int n_sdf, const char *instead) {
+    if (n_sdf > kRsMaxS || !rs_links_ok(descs, n_sdf)) {
+        pvb_set_error("%s: the fused query takes at most %d grid (bounding-box rule) or primitive sub-SDFs, no mesh or "
+                      "LOOKUP_GT_SDF grid (n_sdf=%d); %s instead", fn, kRsMaxS, n_sdf, instead);
+        return PVB_ERR_INVALID;
+    }
+    return PVB_OK;
+}
+
+// The rows of the self forms from allowed[i] (bit j allows the pair (i, j)): the diagonal cleared, and the sources
+// with a non-empty row in ascending order (n_src of them).
+static int scl_rows(const char *fn, const uint8_t *allowed, int n_sdf, SclRows &rows, int &n_src) {
+    memset(&rows, 0, sizeof(rows));
+    n_src = 0;
+    for (int i = 0; i < n_sdf; ++i) {
+        if (allowed[i] >> n_sdf) {
+            pvb_set_error("%s: allowed row %d has bits beyond n_sdf=%d (0x%02x)", fn, i, n_sdf, allowed[i]);
+            return PVB_ERR_INVALID;
+        }
+        rows.mask[i] = (unsigned char)(allowed[i] & ~(1u << i));
+        if (rows.mask[i]) rows.src[n_src++] = (unsigned char)i;
+    }
+    return PVB_OK;
+}
+
+// The n minimum keys of a clearance form start all-ones: no point reached yet.
+static int reset_keys(const char *fn, uint64_t *keys, size_t n, cudaStream_t stream) {
+    if (!keys) {
+        pvb_set_error("%s: invalid argument (keys is null)", fn);
+        return PVB_ERR_INVALID;
+    }
+    if (cudaMemsetAsync(keys, 0xff, sizeof(uint64_t) * n, stream) != cudaSuccess) {
+        pvb_set_error("%s: cudaMemsetAsync(keys) failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+        return PVB_ERR_CUDA;
+    }
+    return PVB_OK;
+}
 
 // Launch robot_clearance_kernel.  Chunk size from the sizes alone: the longest chunk (at least 64 points, or the whole
 // segment) that still gives >= 4 waves of resident blocks over the tiles x segments x chunks, so that blocks of later
@@ -3557,17 +3619,50 @@ static int launch_robot_clearance(const pvb_sdf_desc *descs, int n_sdf, const fl
     const long long n_work = n_seg * chunks_per_seg;
     const unsigned gx = (unsigned)(n_work < INT32_MAX ? n_work : INT32_MAX);
     dim3 grid(gx, (unsigned)gy);
+    auto k = ext ? robot_clearance_kernel<true> : robot_clearance_kernel<false>;
     timing_mark(0, stream);
-    if (ext)
-        robot_clearance_kernel<true><<<grid, kRbCfg * kRsWarps, 0, stream>>>(
-            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, (int)seg_len, (int)chunk,
-            (int)chunks_per_seg, keys);
-    else
-        robot_clearance_kernel<false><<<grid, kRbCfg * kRsWarps, 0, stream>>>(
-            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, (int)seg_len, (int)chunk,
-            (int)chunks_per_seg, keys);
+    k<<<grid, kRbCfg * kRsWarps, 0, stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg,
+                                              (int)seg_len, (int)chunk, (int)chunks_per_seg, keys);
     timing_mark(1, stream);
     PVB_CHECK_LAUNCH("pvb_composed_query_clearance(robot)");
+    return PVB_OK;
+}
+
+// The warp units of robot_paired_clearance_kernel and robot_self_clearance_kernel: `rows` rows of `len` points (a
+// segment or a link's K points), each cut into chunks of whole warp steps.  The longest chunk (at least 64 points, at
+// most kRsMaxChunk, or the whole row) that still gives >= 4 waves of resident units, so that the later chunks of a row
+// start from the keys of its earlier ones.
+struct WarpPlan {
+    long long chunk, n_units;
+    unsigned blocks;
+};
+
+static WarpPlan warp_plan(long long rows, long long len) {
+    const long long want = 4ll * sm_count() * PVB_RS_MINB * kRsWarps;    // warp units for 4 waves
+    long long per_row = (want + rows - 1) / rows;
+    if (per_row > (len + 63) / 64) per_row = (len + 63) / 64;
+    if (per_row < (len + kRsMaxChunk - 1) / kRsMaxChunk) per_row = (len + kRsMaxChunk - 1) / kRsMaxChunk;
+    if (per_row < 1) per_row = 1;
+    long long chunk = (len + per_row - 1) / per_row;
+    chunk = (chunk + 31) / 32 * 32;                                      // whole steps of the warp
+    if (chunk > len) chunk = len;
+    const long long n_units = rows * ((len + chunk - 1) / chunk);
+    const long long blocks = (n_units + kRsWarps - 1) / kRsWarps;
+    return {chunk, n_units, (unsigned)(blocks < INT32_MAX ? blocks : INT32_MAX)};
+}
+
+// Launch robot_paired_clearance_kernel over the warp units of warp_plan.
+static int launch_robot_paired_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg,
+                                         int cfg_begin, int cfg_count, const float *pts, long long n_seg,
+                                         long long seg_len, unsigned long long *keys, bool ext, cudaStream_t stream) {
+    const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
+    const WarpPlan p = warp_plan((long long)cfg_count * n_seg, seg_len);
+    auto k = ext ? robot_paired_clearance_kernel<true> : robot_paired_clearance_kernel<false>;
+    timing_mark(0, stream);
+    k<<<p.blocks, kRbCfg * kRsWarps, 0, stream>>>(pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg,
+                                                  (int)seg_len, (int)p.chunk, p.n_units, keys);
+    timing_mark(1, stream);
+    PVB_CHECK_LAUNCH("pvb_composed_query_paired_clearance(robot)");
     return PVB_OK;
 }
 
@@ -3579,131 +3674,32 @@ static int launch_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *x
                             int cfg_count, const float *pts, long long n_seg, long long seg_len, uint32_t mesh_mode,
                             unsigned long long *keys, bool fused, float *out_val, float *out_grad, int *out_point,
                             int *out_which, cudaStream_t stream) {
-    DescPack<MAXS> pack;
-    memcpy(pack.d, descs, sizeof(pvb_sdf_desc) * (size_t)n_sdf);
-    fill_order(pack, n_sdf);
-    // the same switch as launch_composed: nearest-bound-first evaluation of mesh sub-SDFs
-    static const int nearest_first = [] { const char *e = getenv("PVB_COMP_NEAREST_FIRST"); return e ? atoi(e) : 1; }();
-    float margin_max = 0.f;
-    for (int i = 0; i < n_sdf; ++i) margin_max = descs[i].prune_margin > margin_max ? descs[i].prune_margin : margin_max;
+    const DescPack<MAXS> pack = desc_pack<MAXS>(descs, n_sdf);
+    const CompConsts c = comp_consts(descs, n_sdf);
     if (!fused) {
         (kPaired ? composed_paired_clearance_kernel<kMesh, kExt, MAXS> : composed_clearance_kernel<kMesh, kExt, MAXS>)
             <<<grid_for((long long)cfg_count * n_seg * seg_len, kCompThreads, 8), kCompThreads, 0, stream>>>(
-                pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, mesh_mode, keys, nearest_first,
-                margin_max);
+                pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, mesh_mode, keys,
+                c.nearest_first, c.margin_max);
         PVB_CHECK_LAUNCH("pvb_composed_query_clearance");
     }
     (kPaired ? paired_clearance_finish_kernel<kMesh, kExt, MAXS> : clearance_finish_kernel<kMesh, kExt, MAXS>)
         <<<grid_for((long long)cfg_count * n_seg, kCompThreads, 8), kCompThreads, 0, stream>>>(
             pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, mesh_mode, keys, out_val, out_grad,
-            out_point, out_which, nearest_first, margin_max);
+            out_point, out_which, c.nearest_first, c.margin_max);
     PVB_CHECK_LAUNCH("pvb_composed_query_clearance(finish)");
     return PVB_OK;
 }
 
-extern "C" int pvb_composed_query_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,
-                                            const float *xforms, int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
-                                            const float *pts, int64_t n_seg, int64_t seg_len, uint32_t mesh_mode,
-                                            uint64_t *keys, float *out_val, float *out_grad, int32_t *out_point,
-                                            int32_t *out_which, void *stream) {
-    const char *fn = "pvb_composed_query_clearance";
-    if (n_seg < 0 || seg_len < 0 || seg_len >= (1ll << 31) || (seg_len > 0 && n_seg > INT64_MAX / seg_len) ||
-        (cfg_count > 0 && n_seg > INT64_MAX / cfg_count)) {
-        pvb_set_error("%s: invalid argument (n_seg=%lld seg_len=%lld cfg_count=%d; seg_len < 2^31)", fn,
-                      (long long)n_seg, (long long)seg_len, cfg_count);
-        return PVB_ERR_INVALID;
-    }
-    const long long n_pts = n_seg * seg_len;
-    bool any_ext;
-    const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_val,
-                                        out_grad, any_ext);
-    if (bad) return bad;
-    if (n_seg == 0) return PVB_OK;
-    if (cfg_count < 1) {
-        if (n_pts == 0) return PVB_OK;
-        pvb_set_error("%s: no minimum over an empty configuration slab (cfg_count=%d)", fn, cfg_count);
-        return PVB_ERR_INVALID;
-    }
-    if (seg_len == 0) {
-        pvb_set_error("%s: no minimum over an empty segment (seg_len=0, n_seg=%lld)", fn, (long long)n_seg);
-        return PVB_ERR_INVALID;
-    }
-    if (!keys) {
-        pvb_set_error("%s: invalid argument (keys is null)", fn);
-        return PVB_ERR_INVALID;
-    }
-    cudaStream_t s = (cudaStream_t)stream;
-    unsigned long long *k = reinterpret_cast<unsigned long long *>(keys);
-    if (cudaMemsetAsync(k, 0xff, sizeof(uint64_t) * (size_t)cfg_count * (size_t)n_seg, s) != cudaSuccess) {
-        pvb_set_error("%s: cudaMemsetAsync(keys) failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
-        return PVB_ERR_CUDA;
-    }
-    // robot_serial_kernel's sets take the fused kernel: <= 8 GRID links with the bounding-box rule or primitives, and
-    // one grid row per configuration tile
-    const bool fused = !needs_mesh && n_sdf <= kRsMaxS && rs_tile_count(cfg_count) <= kRsMaxGridRows &&
-                       rs_links_ok(descs, n_sdf);
-    if (fused) {
-        const int rc = launch_robot_clearance(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
-                                              k, any_ext, s);
-        if (rc) return rc;
-    }
-#define PVB_CLEARANCE(MESH, TRI)                                                                                   \
-    (n_sdf <= 16 ? launch_clearance<MESH, TRI, 16>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg,   \
-                                                    seg_len, mesh_mode, k, fused, out_val, out_grad, out_point,     \
-                                                    out_which, s)                                                   \
-                 : launch_clearance<MESH, TRI, 128>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg,  \
-                                                     seg_len, mesh_mode, k, fused, out_val, out_grad, out_point,    \
-                                                     out_which, s))
-    const int rc = needs_mesh ? (any_ext ? PVB_CLEARANCE(true, true) : PVB_CLEARANCE(true, false))
-                              : (any_ext ? PVB_CLEARANCE(false, true) : PVB_CLEARANCE(false, false));
-#undef PVB_CLEARANCE
-    return rc;
-}
-
-// Launch robot_paired_clearance_kernel.  Chunk size from the sizes alone: the longest chunk (whole steps of a warp,
-// at least 64 points, or the whole segment) that still gives >= 4 waves of resident units, so that the later chunks of
-// a segment start from the keys of its earlier ones.
-static int launch_robot_paired_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg,
-                                         int cfg_begin, int cfg_count, const float *pts, long long n_seg,
-                                         long long seg_len, unsigned long long *keys, bool ext, cudaStream_t stream) {
-    const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
-    const long long pairs = (long long)cfg_count * n_seg;
-    const long long want = 4ll * sm_count() * PVB_RS_MINB * kRsWarps;    // warp units for 4 waves
-    long long per_seg = (want + pairs - 1) / pairs;
-    if (per_seg > (seg_len + 63) / 64) per_seg = (seg_len + 63) / 64;
-    if (per_seg < (seg_len + kRsMaxChunk - 1) / kRsMaxChunk) per_seg = (seg_len + kRsMaxChunk - 1) / kRsMaxChunk;
-    if (per_seg < 1) per_seg = 1;
-    long long chunk = (seg_len + per_seg - 1) / per_seg;
-    chunk = (chunk + 31) / 32 * 32;                                      // whole steps of the warp
-    if (chunk > seg_len) chunk = seg_len;
-    const long long n_units = pairs * ((seg_len + chunk - 1) / chunk);
-    const long long blocks = (n_units + kRsWarps - 1) / kRsWarps;
-    const unsigned gx = (unsigned)(blocks < INT32_MAX ? blocks : INT32_MAX);
-    timing_mark(0, stream);
-    if (ext)
-        robot_paired_clearance_kernel<true><<<gx, kRbCfg * kRsWarps, 0, stream>>>(
-            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, (int)seg_len, (int)chunk, n_units, keys);
-    else
-        robot_paired_clearance_kernel<false><<<gx, kRbCfg * kRsWarps, 0, stream>>>(
-            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, (int)seg_len, (int)chunk, n_units, keys);
-    timing_mark(1, stream);
-    PVB_CHECK_LAUNCH("pvb_composed_query_paired_clearance(robot)");
-    return PVB_OK;
-}
-
-extern "C" int pvb_composed_query_paired_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,
-                                                   const float *xforms, int32_t n_cfg, int32_t cfg_begin,
-                                                   int32_t cfg_count, const float *pts, int64_t n_seg, int64_t seg_len,
-                                                   uint32_t mesh_mode, uint64_t *keys, float *out_val, float *out_grad,
-                                                   int32_t *out_point, int32_t *out_which, void *stream) {
-    const char *fn = "pvb_composed_query_paired_clearance";
-    if (n_seg < 0 || seg_len < 0 || seg_len >= (1ll << 31) || (seg_len > 0 && n_seg > INT64_MAX / seg_len) ||
-        (cfg_count > 0 && n_seg > INT64_MAX / cfg_count) ||
-        (cfg_count > 0 && n_seg * seg_len > INT64_MAX / cfg_count)) {
-        pvb_set_error("%s: invalid argument (n_seg=%lld seg_len=%lld cfg_count=%d; seg_len < 2^31, "
-                      "cfg_count * n_seg * seg_len < 2^63)", fn, (long long)n_seg, (long long)seg_len, cfg_count);
-        return PVB_ERR_INVALID;
-    }
+// pvb_composed_query_clearance, and pvb_composed_query_paired_clearance (kPaired: configuration c's points are its
+// own n_seg * seg_len); they differ in the point count they bound and in their fused kernel.
+template <bool kPaired>
+static int clearance_query(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh, const float *xforms,
+                           int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count, const float *pts, int64_t n_seg,
+                           int64_t seg_len, uint32_t mesh_mode, uint64_t *keys, float *out_val, float *out_grad,
+                           int32_t *out_point, int32_t *out_which, void *stream) {
+    const char *fn = kPaired ? "pvb_composed_query_paired_clearance" : "pvb_composed_query_clearance";
+    if (int rc = check_segments(fn, n_seg, seg_len, cfg_count, kPaired)) return rc;
     const long long n_pts = n_seg * seg_len;                 // points per configuration
     bool any_ext;
     const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_val,
@@ -3719,40 +3715,45 @@ extern "C" int pvb_composed_query_paired_clearance(const pvb_sdf_desc *descs, in
         pvb_set_error("%s: no minimum over an empty segment (seg_len=0, n_seg=%lld)", fn, (long long)n_seg);
         return PVB_ERR_INVALID;
     }
-    if (!keys) {
-        pvb_set_error("%s: invalid argument (keys is null)", fn);
-        return PVB_ERR_INVALID;
-    }
     cudaStream_t s = (cudaStream_t)stream;
+    if (int rc = reset_keys(fn, keys, (size_t)cfg_count * (size_t)n_seg, s)) return rc;
     unsigned long long *k = reinterpret_cast<unsigned long long *>(keys);
-    if (cudaMemsetAsync(k, 0xff, sizeof(uint64_t) * (size_t)cfg_count * (size_t)n_seg, s) != cudaSuccess) {
-        pvb_set_error("%s: cudaMemsetAsync(keys) failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
-        return PVB_ERR_CUDA;
-    }
-    // robot_serial_kernel's sets take the fused kernel: <= 8 GRID links with the bounding-box rule or primitives (its
-    // 1-D grid has no limit on cfg_count)
-    const bool fused = !needs_mesh && n_sdf <= kRsMaxS && rs_links_ok(descs, n_sdf);
+    // robot_serial_kernel's sets take the fused kernel: <= 8 GRID links with the bounding-box rule or primitives.  The
+    // clearance kernel runs one grid row per configuration tile; the paired kernel's 1-D grid has no limit on cfg_count.
+    const bool fused = !needs_mesh && n_sdf <= kRsMaxS && (kPaired || rs_tile_count(cfg_count) <= kRsMaxGridRows) &&
+                       rs_links_ok(descs, n_sdf);
     if (fused) {
-        const int rc = launch_robot_paired_clearance(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg,
-                                                     seg_len, k, any_ext, s);
+        const int rc = (kPaired ? launch_robot_paired_clearance : launch_robot_clearance)(
+            descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, k, any_ext, s);
         if (rc) return rc;
     }
-#define PVB_PCLEARANCE(MESH, TRI)                                                                                  \
-    (n_sdf <= 16 ? launch_clearance<MESH, TRI, 16, true>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,   \
-                                                          n_seg, seg_len, mesh_mode, k, fused, out_val, out_grad,   \
-                                                          out_point, out_which, s)                                  \
-                 : launch_clearance<MESH, TRI, 128, true>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,  \
-                                                           n_seg, seg_len, mesh_mode, k, fused, out_val, out_grad,  \
-                                                           out_point, out_which, s))
-    const int rc = needs_mesh ? (any_ext ? PVB_PCLEARANCE(true, true) : PVB_PCLEARANCE(true, false))
-                              : (any_ext ? PVB_PCLEARANCE(false, true) : PVB_PCLEARANCE(false, false));
-#undef PVB_PCLEARANCE
-    return rc;
+    return comp_variant(needs_mesh, any_ext, n_sdf, [&](auto kMesh, auto kExt, auto kMaxS) {
+        return launch_clearance<kMesh, kExt, kMaxS, kPaired>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,
+                                                             n_seg, seg_len, mesh_mode, k, fused, out_val, out_grad,
+                                                             out_point, out_which, s);
+    });
 }
 
-// Launch robot_self_clearance_kernel (when some row is not empty), then self_clearance_finish_kernel.  Chunk size as
-// in launch_robot_paired_clearance: the longest chunk (whole steps of a warp, at least 64 points, or all K) that still
-// gives >= 4 waves of resident units.
+extern "C" int pvb_composed_query_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,
+                                            const float *xforms, int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                                            const float *pts, int64_t n_seg, int64_t seg_len, uint32_t mesh_mode,
+                                            uint64_t *keys, float *out_val, float *out_grad, int32_t *out_point,
+                                            int32_t *out_which, void *stream) {
+    return clearance_query<false>(descs, n_sdf, needs_mesh, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
+                                  mesh_mode, keys, out_val, out_grad, out_point, out_which, stream);
+}
+
+extern "C" int pvb_composed_query_paired_clearance(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,
+                                                   const float *xforms, int32_t n_cfg, int32_t cfg_begin,
+                                                   int32_t cfg_count, const float *pts, int64_t n_seg, int64_t seg_len,
+                                                   uint32_t mesh_mode, uint64_t *keys, float *out_val, float *out_grad,
+                                                   int32_t *out_point, int32_t *out_which, void *stream) {
+    return clearance_query<true>(descs, n_sdf, needs_mesh, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
+                                 mesh_mode, keys, out_val, out_grad, out_point, out_which, stream);
+}
+
+// Launch robot_self_clearance_kernel (when some row is not empty) over the warp units of warp_plan, then
+// self_clearance_finish_kernel.
 static int launch_self_clearance(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, const float *inv_xforms,
                                  int n_cfg, int cfg_begin, int cfg_count, const float *link_pts, int K,
                                  const SclRows &rows, int n_src, unsigned long long *keys, float *out_val,
@@ -3760,38 +3761,18 @@ static int launch_self_clearance(const pvb_sdf_desc *descs, int n_sdf, const flo
                                  cudaStream_t stream) {
     const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
     if (n_src > 0) {
-        const long long pairs = (long long)cfg_count * n_src;
-        const long long want = 4ll * sm_count() * PVB_RS_MINB * kRsWarps;    // warp units for 4 waves
-        long long per_src = (want + pairs - 1) / pairs;
-        if (per_src > (K + 63) / 64) per_src = (K + 63) / 64;
-        if (per_src < 1) per_src = 1;
-        long long chunk = (K + per_src - 1) / per_src;
-        chunk = (chunk + 31) / 32 * 32;                                      // whole steps of the warp
-        if (chunk > K) chunk = K;
-        const long long n_units = pairs * ((K + chunk - 1) / chunk);
-        const long long blocks = (n_units + kRsWarps - 1) / kRsWarps;
-        const unsigned gx = (unsigned)(blocks < INT32_MAX ? blocks : INT32_MAX);
+        const WarpPlan p = warp_plan((long long)cfg_count * n_src, K);
+        auto k = ext ? robot_self_clearance_kernel<true> : robot_self_clearance_kernel<false>;
         timing_mark(0, stream);
-        if (ext)
-            robot_self_clearance_kernel<true><<<gx, kRbCfg * kRsWarps, 0, stream>>>(
-                pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, K, rows, n_src, (int)chunk,
-                n_units, keys);
-        else
-            robot_self_clearance_kernel<false><<<gx, kRbCfg * kRsWarps, 0, stream>>>(
-                pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, K, rows, n_src, (int)chunk,
-                n_units, keys);
+        k<<<p.blocks, kRbCfg * kRsWarps, 0, stream>>>(pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count,
+                                                      link_pts, K, rows, n_src, (int)p.chunk, p.n_units, keys);
         timing_mark(1, stream);
         PVB_CHECK_LAUNCH("pvb_composed_query_self_clearance");
     }
-    const unsigned gf = (unsigned)grid_for(cfg_count, kCompThreads, 8);
-    if (ext)
-        self_clearance_finish_kernel<true><<<gf, kCompThreads, 0, stream>>>(
-            pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, K, rows, keys, out_val, out_grad,
-            out_src, out_point, out_which);
-    else
-        self_clearance_finish_kernel<false><<<gf, kCompThreads, 0, stream>>>(
-            pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, K, rows, keys, out_val, out_grad,
-            out_src, out_point, out_which);
+    auto kf = ext ? self_clearance_finish_kernel<true> : self_clearance_finish_kernel<false>;
+    kf<<<(unsigned)grid_for(cfg_count, kCompThreads, 8), kCompThreads, 0, stream>>>(
+        pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, K, rows, keys, out_val, out_grad,
+        out_src, out_point, out_which);
     PVB_CHECK_LAUNCH("pvb_composed_query_self_clearance(finish)");
     return PVB_OK;
 }
@@ -3803,11 +3784,7 @@ extern "C" int pvb_composed_query_self_clearance(const pvb_sdf_desc *descs, int3
                                                  float *out_grad, int32_t *out_src, int32_t *out_point,
                                                  int32_t *out_which, void *stream) {
     const char *fn = "pvb_composed_query_self_clearance";
-    if (K < 1 || K >= (1ll << 24) || !inv_xforms || !allowed) {
-        pvb_set_error("%s: invalid argument (K=%lld; 1 <= K < 2^24, inv_xforms and allowed not null)", fn,
-                      (long long)K);
-        return PVB_ERR_INVALID;
-    }
+    if (int rc = check_link_points(fn, K, inv_xforms, allowed)) return rc;
     bool any_ext;
     const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, link_pts,
                                         (int64_t)n_sdf * K, out_val, out_grad, any_ext);
@@ -3816,37 +3793,15 @@ extern "C" int pvb_composed_query_self_clearance(const pvb_sdf_desc *descs, int3
         pvb_set_error("%s: no minimum over an empty configuration slab (cfg_count=%d)", fn, cfg_count);
         return PVB_ERR_INVALID;
     }
-    // the sets robot_paired_clearance_kernel takes: <= 8 GRID links with the bounding-box rule, or primitives
-    const bool fused = n_sdf <= kRsMaxS && rs_links_ok(descs, n_sdf);
-    if (!fused) {
-        pvb_set_error("%s: the fused query takes at most %d grid (bounding-box rule) or primitive sub-SDFs, no mesh or "
-                      "LOOKUP_GT_SDF grid (n_sdf=%d); compose the per-source paired clearance queries instead", fn,
-                      kRsMaxS, n_sdf);
-        return PVB_ERR_INVALID;
-    }
+    if (int rc = check_fused_only(fn, descs, n_sdf, "compose the per-source paired clearance queries")) return rc;
     SclRows rows;
-    memset(&rows, 0, sizeof(rows));
-    int n_src = 0;
-    for (int i = 0; i < n_sdf; ++i) {
-        if (allowed[i] >> n_sdf) {
-            pvb_set_error("%s: allowed row %d has bits beyond n_sdf=%d (0x%02x)", fn, i, n_sdf, allowed[i]);
-            return PVB_ERR_INVALID;
-        }
-        rows.mask[i] = (unsigned char)(allowed[i] & ~(1u << i));
-        if (rows.mask[i]) rows.src[n_src++] = (unsigned char)i;
-    }
-    if (!keys) {
-        pvb_set_error("%s: invalid argument (keys is null)", fn);
-        return PVB_ERR_INVALID;
-    }
+    int n_src;
+    if (int rc = scl_rows(fn, allowed, n_sdf, rows, n_src)) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    unsigned long long *k = reinterpret_cast<unsigned long long *>(keys);
-    if (cudaMemsetAsync(k, 0xff, sizeof(uint64_t) * (size_t)cfg_count, s) != cudaSuccess) {
-        pvb_set_error("%s: cudaMemsetAsync(keys) failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
-        return PVB_ERR_CUDA;
-    }
+    if (int rc = reset_keys(fn, keys, (size_t)cfg_count, s)) return rc;
     return launch_self_clearance(descs, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, (int)K, rows,
-                                 n_src, k, out_val, out_grad, out_src, out_point, out_which, any_ext, s);
+                                 n_src, reinterpret_cast<unsigned long long *>(keys), out_val, out_grad, out_src,
+                                 out_point, out_which, any_ext, s);
 }
 
 // Bytes of partial sums a collision-cost query needs: one fp32 row of 1 + 6 n_sdf per (configuration, segment, chunk);
@@ -3903,16 +3858,8 @@ extern "C" int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int3
                                                  void *workspace, int64_t workspace_bytes, float *out_cost,
                                                  float *out_twist, void *stream) {
     const char *fn = "pvb_composed_query_collision_cost";
-    if (n_seg < 0 || seg_len < 0 || seg_len >= (1ll << 31) || (seg_len > 0 && n_seg > INT64_MAX / seg_len) ||
-        (cfg_count > 0 && n_seg > INT64_MAX / cfg_count)) {
-        pvb_set_error("%s: invalid argument (n_seg=%lld seg_len=%lld cfg_count=%d; seg_len < 2^31)", fn,
-                      (long long)n_seg, (long long)seg_len, cfg_count);
-        return PVB_ERR_INVALID;
-    }
-    if (!(margin - margin == 0.f)) {                 // NaN or +-inf
-        pvb_set_error("%s: the margin must be finite (margin=%g)", fn, (double)margin);
-        return PVB_ERR_INVALID;
-    }
+    if (int rc = check_segments(fn, n_seg, seg_len, cfg_count, false)) return rc;
+    if (int rc = check_margin(fn, margin)) return rc;
     const long long n_pts = n_seg * seg_len;
     bool any_ext;
     const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_cost,
@@ -3928,13 +3875,7 @@ extern "C" int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int3
         pvb_set_error("%s: invalid argument (out_cost or out_twist is null)", fn);
         return PVB_ERR_INVALID;
     }
-    // the sets robot_serial_kernel takes: <= 8 GRID links with the bounding-box rule, or primitives
-    const bool fused = n_sdf <= kRsMaxS && rs_links_ok(descs, n_sdf);
-    if (!fused) {
-        pvb_set_error("%s: the fused query takes at most %d grid (bounding-box rule) or primitive sub-SDFs, no mesh or "
-                      "LOOKUP_GT_SDF grid (n_sdf=%d); compose it from pvb_composed_query instead", fn, kRsMaxS, n_sdf);
-        return PVB_ERR_INVALID;
-    }
+    if (int rc = check_fused_only(fn, descs, n_sdf, "compose it from pvb_composed_query")) return rc;
     const long long need = collision_cost_bytes(n_sdf, cfg_count, n_seg, seg_len);
     if (need < 0 || (need > 0 && (!workspace || workspace_bytes < need || ((uintptr_t)workspace & 3)))) {
         pvb_set_error("%s: the workspace must hold pvb_collision_cost_workspace() = %lld bytes, 4-byte aligned "
@@ -3952,15 +3893,8 @@ extern "C" int pvb_composed_query_self_collision_cost(const pvb_sdf_desc *descs,
                                                       const uint8_t *allowed, float margin, float *out_cost,
                                                       float *out_twist, void *stream) {
     const char *fn = "pvb_composed_query_self_collision_cost";
-    if (K < 1 || K >= (1ll << 24) || !inv_xforms || !allowed) {
-        pvb_set_error("%s: invalid argument (K=%lld; 1 <= K < 2^24, inv_xforms and allowed not null)", fn,
-                      (long long)K);
-        return PVB_ERR_INVALID;
-    }
-    if (!(margin - margin == 0.f)) {                 // NaN or +-inf
-        pvb_set_error("%s: the margin must be finite (margin=%g)", fn, (double)margin);
-        return PVB_ERR_INVALID;
-    }
+    if (int rc = check_link_points(fn, K, inv_xforms, allowed)) return rc;
+    if (int rc = check_margin(fn, margin)) return rc;
     bool any_ext;
     const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, link_pts,
                                         (int64_t)n_sdf * K, out_cost, out_twist, any_ext);
@@ -3969,37 +3903,17 @@ extern "C" int pvb_composed_query_self_collision_cost(const pvb_sdf_desc *descs,
         pvb_set_error("%s: no cost over an empty configuration slab (cfg_count=%d)", fn, cfg_count);
         return PVB_ERR_INVALID;
     }
-    // the sets robot_self_clearance_kernel takes: <= 8 GRID links with the bounding-box rule, or primitives
-    const bool fused = n_sdf <= kRsMaxS && rs_links_ok(descs, n_sdf);
-    if (!fused) {
-        pvb_set_error("%s: the fused query takes at most %d grid (bounding-box rule) or primitive sub-SDFs, no mesh or "
-                      "LOOKUP_GT_SDF grid (n_sdf=%d); compose the per-source paired queries instead", fn, kRsMaxS,
-                      n_sdf);
-        return PVB_ERR_INVALID;
-    }
+    if (int rc = check_fused_only(fn, descs, n_sdf, "compose the per-source paired queries")) return rc;
     SclRows rows;
-    memset(&rows, 0, sizeof(rows));
-    int n_src = 0;
-    for (int i = 0; i < n_sdf; ++i) {
-        if (allowed[i] >> n_sdf) {
-            pvb_set_error("%s: allowed row %d has bits beyond n_sdf=%d (0x%02x)", fn, i, n_sdf, allowed[i]);
-            return PVB_ERR_INVALID;
-        }
-        rows.mask[i] = (unsigned char)(allowed[i] & ~(1u << i));
-        if (rows.mask[i]) rows.src[n_src++] = (unsigned char)i;
-    }
+    int n_src;
+    if (int rc = scl_rows(fn, allowed, n_sdf, rows, n_src)) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
     const long long blocks = ((long long)cfg_count + kSccWarps - 1) / kSccWarps;
+    auto k = any_ext ? robot_self_collision_cost_kernel<true> : robot_self_collision_cost_kernel<false>;
     timing_mark(0, s);
-    if (any_ext)
-        robot_self_collision_cost_kernel<true><<<(unsigned)blocks, kSccLanes * kSccWarps, 0, s>>>(
-            pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, (int)K, rows, n_src, margin,
-            out_cost, out_twist);
-    else
-        robot_self_collision_cost_kernel<false><<<(unsigned)blocks, kSccLanes * kSccWarps, 0, s>>>(
-            pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count, link_pts, (int)K, rows, n_src, margin,
-            out_cost, out_twist);
+    k<<<(unsigned)blocks, kSccLanes * kSccWarps, 0, s>>>(pack, n_sdf, xforms, inv_xforms, n_cfg, cfg_begin, cfg_count,
+                                                         link_pts, (int)K, rows, n_src, margin, out_cost, out_twist);
     timing_mark(1, s);
     PVB_CHECK_LAUNCH("pvb_composed_query_self_collision_cost");
     return PVB_OK;
