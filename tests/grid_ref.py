@@ -318,3 +318,32 @@ def point_sets(lo, hi, n, seed=0, n_uniform=20000, ulps=4):
 
 def all_points(sets):
     return np.concatenate([sets[k] for k in sorted(sets)])
+
+
+def exact_nodes(g, p):
+    """(mask, ravelled node) of the in-range points whose fp32 cell coordinate (p - min32) * inv_res32 is an integer
+    below n - 1 on every axis: the interpolant there is the table entry, bit for bit."""
+    from pytorch_volumetric_b200.sdf import fast_index_band
+    p32 = np.asarray(p, np.float32)
+    ok = g.in_range(p32.astype(np.float64))
+    k = np.zeros((len(p32), 3), np.int64)
+    for a in range(3):
+        inv = np.float32(fast_index_band(g.lo64[a], g.hi64[a], g.shape[a])[0])
+        with np.errstate(invalid="ignore"):
+            u = ((p32[:, a] - np.float32(g.lo64[a])).astype(np.float32) * inv).astype(np.float32)
+            ok &= (u == np.floor(u)) & (u >= 0) & (u <= g.shape[a] - 2)
+        k[:, a] = np.where(ok, u, 0)
+    return ok, (k[:, 0] * g.shape[1] + k[:, 1]) * g.shape[2] + k[:, 2]
+
+
+def voxel_case(vg, box):
+    """(boundary-dense points [m, d] fp32, reference flat index [m]) of a VoxelGrid over `box` (as it was given)."""
+    import pytorch_volumetric_b200 as pv
+    ranges = pv.get_divisible_range_by_resolution(vg.resolution, box)
+    shape = tuple(vg.get_voxel_values().shape)
+    d = len(shape)
+    lo = np.array([float(min(r)) for r in ranges]); hi = np.array([float(max(r)) for r in ranges])
+    sets = point_sets(np.pad(lo, (0, 3 - d), constant_values=0), np.pad(hi, (0, 3 - d), constant_values=1),
+                      np.pad(np.array(shape), (0, 3 - d), constant_values=2))
+    p = np.ascontiguousarray(all_points(sets)[:, :d])
+    return p, voxel_index(ranges, shape, p)

@@ -1,4 +1,5 @@
 """Shared helpers for the parity tests (test infrastructure; may use oracle/)."""
+import math
 import os
 
 import numpy as np
@@ -251,3 +252,192 @@ def classify_composed(v_gpu, g_gpu, v_ref, g_ref, specs, mats, pts, tol=1e-5):
             unexplained.append((int(a), int(i), float(v_gpu[a, i]), float(v_ref[a, i])))
     rep = {"n": int(bad.size), "exceed": int(len(idx)), "unexplained": len(unexplained), "first": unexplained[:5]}
     return len(idx), len(unexplained), rep
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# GPU-tier compositions the query-form tests share: CachedSDF links from the golden tables, the golden and arm sets,
+# route guards and the per-configuration reductions the fused queries are checked against.
+def cached_from_golden(z, name, tmp_path, table_key="table_val", grad_key="table_grad", range_in=None, **kw):
+    """Write the reference-built tables into a reference-format cache file and let CachedSDF load them
+    (sdf.py:487-495): exercises on-disk cache compatibility and isolates the lookup from the table build."""
+    import pytorch_volumetric_b200 as pv
+    res = float(z["resolution"])
+    range_in = z["range_in"] if range_in is None else range_in
+    ranges = pv.get_divisible_range_by_resolution(res, range_in)
+    key = f"{name} {res} {tuple(ranges)}"
+    shape = [int(s) for s in z["table_shape"]]
+    cache = {key: (torch.from_numpy(z[table_key]).reshape(shape), torch.from_numpy(z[grad_key]))}
+    path = str(tmp_path / f"sdf_cache_{name}.pkl")
+    torch.save(cache, path)
+    gt = pv.MeshSDF(pv_factory(name.rstrip("32")))
+    return pv.CachedSDF(name, res, range_in, gt, device="cuda", cache_path=path, **kw)
+
+
+def golden_sets(tmp_path):
+    import pytorch_volumetric_b200 as pv
+    zc = golden("ref_cachedsdf_probe")
+    near = cached_from_golden(zc, "probe", tmp_path)
+    tri = cached_from_golden(zc, "probe", tmp_path, interpolation="trilinear")
+    z = golden("ref_composed")
+    sph = pv.SphereSDF(float(z["sphere_radius"]))
+    return z, {"nearest": [near, near, near, near], "trilinear": [tri, tri, tri], "mixed": [near, tri, near],
+               "nearest+sphere": [near, near, sph, near], "mixed+sphere": [tri, near, sph, tri]}
+
+
+def no_generic(monkeypatch, comp):
+    def boom(*a, **k):
+        raise AssertionError("generic path taken")
+    monkeypatch.setattr(comp, "_generic_query", boom)
+
+
+def opaque_sdfs(pv, sdfs):
+    class Opaque(pv.ObjectFrameSDF):          # no native descriptor -> generic path
+        def __init__(self, inner):
+            self.inner = inner
+
+        def __call__(self, p):
+            return self.inner(p)
+
+        def surface_bounding_box(self, **kw):
+            return self.inner.surface_bounding_box(**kw)
+
+    return [Opaque(s) for s in sdfs]
+
+
+def cached_arm(tmp_path, interpolation):
+    """The arm of workloads.write_arm with CachedSDF links of the given interpolation."""
+    import pytorch_volumetric_b200 as pv
+    urdf, end = workloads.write_arm(str(tmp_path))
+    chain = pv.build_serial_chain_from_urdf(open(urdf).read(), end).to(device="cuda")
+    return pv.RobotSDF(chain, path_prefix=str(tmp_path),
+                       link_sdf_cls=pv.cache_link_sdf_factory(resolution=0.02, padding=1.0, device="cuda",
+                                                              cache_path=str(tmp_path / "arm.pkl"),
+                                                              interpolation=interpolation))
+
+
+def arm_robot(tmp_path, kind):
+    """cached_arm for kind "nearest" / "trilinear", the primitive arm of workloads.write_primitive_arm otherwise."""
+    import pytorch_volumetric_b200 as pv
+    if kind == "primitive":
+        urdf, end = workloads.write_primitive_arm(str(tmp_path / "prim"))
+        return pv.RobotSDF(pv.build_serial_chain_from_urdf(open(urdf).read(), end).to(device="cuda"),
+                           primitive_visuals=True)
+    return cached_arm(tmp_path, kind)
+
+
+def arm_points(n, seed):
+    lo = [r[0] for r in workloads.ARM_QUERY_RANGE]; hi = [r[1] for r in workloads.ARM_QUERY_RANGE]
+    return workloads.uniform_points(n, lo, hi, seed=seed).cuda()
+
+
+def own_points(q, A, seed):
+    """[A, P, 3] on the GPU: the points q, shuffled and shifted differently for every configuration."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    q = q.cpu()
+    return torch.stack([q[torch.randperm(len(q), generator=g)] + 0.01 * torch.randn(3, generator=g)
+                        for _ in range(A)]).cuda()
+
+
+def swept_reduce(v, g, w, cfg_count, cfg_begin=0):
+    """Lexicographic (value, configuration, sub-SDF) minimum of flat per-configuration results [cfg_count * P]."""
+    P = v.numel() // cfg_count
+    v, g, w = v.reshape(cfg_count, P), g.reshape(cfg_count, P, 3), w.reshape(cfg_count, P)
+    c = (v == v.amin(dim=0)).int().argmax(dim=0)          # the first configuration attaining the minimum
+    return (v.gather(0, c[None])[0], g.gather(0, c[None, :, None].expand(1, P, 3))[0],
+            (c + cfg_begin).to(torch.int32), w.gather(0, c[None])[0])
+
+
+def clearance_reduce(v, g, w, cfg_count, n_seg):
+    """First point attaining the minimum of every (configuration, segment) of flat results [cfg_count * n_seg * N]."""
+    v = v.reshape(cfg_count, n_seg, -1)
+    N = v.shape[-1]
+    g, w = g.reshape(cfg_count, n_seg, N, 3), w.reshape(cfg_count, n_seg, N)
+    i = (v == v.amin(-1, keepdim=True)).int().argmax(-1, keepdim=True)
+    return (v.gather(-1, i).reshape(-1), g.gather(-2, i[..., None].expand(-1, -1, 1, 3)).reshape(-1, 3),
+            i.reshape(-1).to(torch.int32), w.gather(-1, i).reshape(-1))
+
+
+def _which_values(specs, tm, pts, w):
+    """fp64 value of the reported sub-SDF w (A, P) at every pair."""
+    import composed_ref as cr
+    out = np.full(w.shape, np.nan)
+    for s, spec in enumerate(specs):
+        a, i = np.nonzero(w == s)
+        if len(a):
+            q = np.einsum("nij,nj->ni", tm[s, a, :3, :3], pts[i].astype(np.float64)) + tm[s, a, :3, 3]
+            out[a, i] = cr.evaluate(spec, q)[0]
+    return out
+
+
+def assert_fp64(members, tm, pts, v, g, w, what, tol=1e-5):
+    """query(..., return_which=True) against the fp64 composition: grids and primitives through
+    classify_composed (every exceedance a classified flip or tie), meshes through composed_ref.mesh_mismatch;
+    `which` names a sub-SDF whose fp64 value is the result's within the tolerance.  Returns the exceedance mask."""
+    import composed_ref as cr
+    S, A = tm.shape[:2]
+    P = len(pts)
+    v, g, w = (t.cpu().numpy() for t in (v, g, w))
+    v, g, w = v.reshape(A, P), g.reshape(A, P, 3), w.reshape(A, P)
+    specs = [m[1] for m in members]
+    assert ((w >= 0) & (w < S)).all(), what
+    if specs[0]["kind"] == "mesh":
+        ref = cr.compose(specs, tm, pts, per_sub=True)
+        bad_v, bad_g, bad_w, rep = cr.mesh_mismatch(v, g, w, ref, tol, coord_scale=0.2)
+        assert bad_v == 0 and bad_g == 0 and bad_w == 0, (what, rep)
+        return np.zeros((A, P), bool)
+    rv, rg, _rw = cr.compose(specs, tm, pts)
+    n_ex, n_un, rep = classify_composed(v, g, rv, rg, specs, tm, pts, tol)
+    assert n_un == 0, (what, rep)
+    assert n_ex <= 2e-3 * A * P, (what, rep)
+    exceed = (np.abs(v - rv) > tol) | (np.abs(g - rg).max(-1) > tol)
+    assert ((np.abs(_which_values(specs, tm, pts, w) - rv) <= tol) | exceed).all(), what
+    return exceed
+
+
+# ---- self-clearance inputs
+def wide_configurations(A, seed, dtype=torch.float32):
+    """Joint values uniform in +-pi: wide enough that the arm's links pass through one another."""
+    g = torch.Generator().manual_seed(seed)
+    return ((torch.rand(A, 7, generator=g, dtype=torch.float64) * 2 - 1) * math.pi).to(dtype)
+
+
+def allowed_matrix(S, kind):
+    """[S, S] bool: links at least two apart ("default"), an asymmetric pattern, or nothing."""
+    i = torch.arange(S)
+    if kind == "default":
+        return (i[:, None] - i[None, :]).abs() >= 2
+    if kind == "asymmetric":
+        return (i[None, :] - i[:, None] >= 3) | ((i[:, None] == S - 1) & (i[None, :] == 0))
+    return torch.zeros(S, S, dtype=torch.bool)
+
+
+def surface_points(link_sdf, n, seed):
+    from pytorch_volumetric_b200.model_to_sdf import _primitive_surface
+    return _primitive_surface(link_sdf, n, np.random.default_rng(seed))
+
+
+# ---- the reference project's offset wrench robot
+WRENCH_URDF = """<robot name="wrench">
+{links}
+  <link name="offset_wrench"><visual><geometry><mesh filename="wrench.obj"/></geometry></visual></link>
+{joints}
+</robot>"""
+
+
+def write_wrench_urdf(dirname):
+    """Procedural equivalent of the reference's tests/offset_wrench.urdf: 3 prismatic + 3 revolute joints
+    (x, y, z each) in front of one mesh link."""
+    from pytorch_volumetric_b200.meshio import write_obj
+    v, f = workloads.fixture_mesh("wrench")
+    write_obj(os.path.join(dirname, "wrench.obj"), v, f)
+    names = ["link_x_trans", "link_y_trans", "link_z_trans", "link_x_rot", "link_y_rot", "link_z_rot", "offset_wrench"]
+    links = "\n".join(f'  <link name="{n}"/>' for n in names[:-1])
+    axes = ["1 0 0", "0 1 0", "0 0 1"] * 2
+    jn = ["x_trans", "y_trans", "z_trans", "x_rot", "y_rot", "z_rot"]
+    joints = "\n".join(
+        f'  <joint name="{jn[i]}" type="{"prismatic" if i < 3 else "revolute"}"><origin rpy="0 0 0" xyz="0 0 0"/>'
+        f'<parent link="{names[i]}"/><child link="{names[i + 1]}"/><axis xyz="{axes[i]}"/></joint>' for i in range(6))
+    path = os.path.join(dirname, "offset_wrench.urdf")
+    with open(path, "w") as fh:
+        fh.write(WRENCH_URDF.format(links=links, joints=joints))
+    return path

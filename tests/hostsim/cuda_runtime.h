@@ -16,8 +16,10 @@
 #define __device__
 #define __host__
 #define __global__
-#define __forceinline__ inline
-#define __noinline__ __attribute__((noinline))
+// Every translation unit of tests/hostsim is linked into one library: the header's functions get internal linkage, so
+// each unit keeps its own copy (hostsim.cpp's PVB_STAT hook included) instead of the linker picking one of them.
+#define __forceinline__ static inline
+#define __noinline__ static __attribute__((noinline))
 
 struct float2 { float x, y; };
 struct alignas(16) float4 { float x, y, z, w; };

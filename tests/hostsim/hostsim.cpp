@@ -79,10 +79,12 @@ extern "C" void sim_winding(const pvb_sdf_desc *m, const float *pts, long long n
 
 // ComposedSDF / RobotSDF for every (configuration, point) pair: the loop of the composed kernels (visit the
 // sub-SDFs in `order`, composed_xform -> composed_consider, rotate the winning gradient back) around the header's
-// primitives.  xforms: [n_sdf * n_cfg][16] row-major, sub-SDF-major like pvb_composed_query; idx as in the kernels.
-extern "C" void sim_composed(const pvb_sdf_desc *descs, int n_sdf, const unsigned char *order, const float *xforms,
-                             int n_cfg, const float *pts, long long n_pts, uint32_t mesh_mode, float *out_val,
-                             float *out_grad, int *out_which) {
+// primitives, through the composed_consider<kMesh, kExt> instantiation that `mesh` and `ext` pick.
+// xforms: [n_sdf * n_cfg][16] row-major, sub-SDF-major like pvb_composed_query; idx as in the kernels.
+template <bool kMesh, bool kExt>
+static void composed_loop(const pvb_sdf_desc *descs, int n_sdf, const unsigned char *order, const float *xforms,
+                          int n_cfg, const float *pts, long long n_pts, uint32_t mesh_mode, float *out_val,
+                          float *out_grad, int *out_which) {
     NodeStage st; st.smem = nullptr; st.n = 0;
 #pragma omp parallel for schedule(dynamic, 64) collapse(2)
     for (int c = 0; c < n_cfg; ++c) {
@@ -93,8 +95,8 @@ extern "C" void sim_composed(const pvb_sdf_desc *descs, int n_sdf, const unsigne
                 const int s = order ? order[si] : si;
                 const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + c) * 16);
                 const uint64_t idx = ((uint64_t)c * (uint64_t)n_pts + (uint64_t)i) * (uint64_t)n_sdf + (uint64_t)s;
-                composed_consider<true>(descs[s], st, s, composed_xform(row[0], row[1], row[2], p), mesh_mode, idx, best,
-                                        bg, bs);
+                composed_consider<kMesh, kExt>(descs[s], st, s, composed_xform(row[0], row[1], row[2], p), mesh_mode,
+                                               idx, best, bg, bs);
             }
             const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)max(bs, 0) * n_cfg + c) * 16);
             const f3 go = composed_rotate_back(row[0], row[1], row[2], bg);
@@ -103,6 +105,15 @@ extern "C" void sim_composed(const pvb_sdf_desc *descs, int n_sdf, const unsigne
             if (out_which) out_which[o] = bs;
         }
     }
+}
+
+extern "C" void sim_composed(const pvb_sdf_desc *descs, int n_sdf, const unsigned char *order, const float *xforms,
+                             int n_cfg, const float *pts, long long n_pts, uint32_t mesh_mode, int mesh, int ext,
+                             float *out_val, float *out_grad, int *out_which) {
+    using Loop = decltype(&composed_loop<true, true>);
+    static const Loop loops[2][2] = {{composed_loop<false, false>, composed_loop<false, true>},
+                                     {composed_loop<true, false>, composed_loop<true, true>}};
+    loops[mesh != 0][ext != 0](descs, n_sdf, order, xforms, n_cfg, pts, n_pts, mesh_mode, out_val, out_grad, out_which);
 }
 
 extern "C" void sim_sphere(float radius, const float *pts, long long n, float *val, float *grad) {

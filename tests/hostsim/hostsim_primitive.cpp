@@ -23,33 +23,6 @@ extern "C" void simprim_aabb_lb2(const pvb_sdf_desc *d, const float *pts, long l
     for (long long i = 0; i < n; ++i) lb2[i] = composed_aabb_lb2(*d, point(pts, i));
 }
 
-// ComposedSDF for every (configuration, point) pair through composed_consider<kMesh = false, kExt = true>: the loop of
-// the non-mesh extension instantiations (visit the sub-SDFs in `order`, composed_xform -> composed_consider, rotate the
-// winning gradient back).  xforms: [n_sdf * n_cfg][16] row-major, sub-SDF-major like pvb_composed_query.
-extern "C" void simprim_composed(const pvb_sdf_desc *descs, int n_sdf, const unsigned char *order, const float *xforms,
-                                 int n_cfg, const float *pts, long long n_pts, float *out_val, float *out_grad,
-                                 int *out_which) {
-    NodeStage st; st.smem = nullptr; st.n = 0;
-#pragma omp parallel for schedule(dynamic, 64) collapse(2)
-    for (int c = 0; c < n_cfg; ++c) {
-        for (long long i = 0; i < n_pts; ++i) {
-            const f3 p = point(pts, i);
-            float best = PVB_INF; f3 bg = mk3(0.f, 0.f, 0.f); int bs = -1;
-            for (int si = 0; si < n_sdf; ++si) {
-                const int s = order[si];
-                const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + c) * 16);
-                composed_consider<false, true>(descs[s], st, s, composed_xform(row[0], row[1], row[2], p), 0u, 0ull,
-                                               best, bg, bs);
-            }
-            const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)max(bs, 0) * n_cfg + c) * 16);
-            const f3 go = composed_rotate_back(row[0], row[1], row[2], bg);
-            const long long o = (long long)c * n_pts + i;
-            out_val[o] = best; out_grad[3 * o] = go.x; out_grad[3 * o + 1] = go.y; out_grad[3 * o + 2] = go.z;
-            out_which[o] = bs;
-        }
-    }
-}
-
 // robot_serial_kernel's bounding-sphere bound of one link (rs_link_consts, rs_sphere_centre, rs_sphere_lb) under one
 // object->link transform (16 floats, row-major) at every point: lb[i] <= value of the link at point i.
 extern "C" void simprim_sphere_lb(const pvb_sdf_desc *d, const float *xform, const float *pts, long long n, float *lb,

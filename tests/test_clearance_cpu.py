@@ -13,52 +13,21 @@ configuration and every segment of points, the per-configuration result at the f
    step re-evaluates the winner with composed_point).
 4. The C ABI refusals and the Python shape rules, without a GPU."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 import hostsim_lib as hs
+from hostsim_lib import PVB_ERR_INVALID, _p
 from pytorch_volumetric_b200 import _native as nat
-from test_paired_cpu import _table_descs
-from test_swept_cpu import _all_sets, _trajectory
-from test_trilinear_composed_cpu import _sim_composed, _unpruned
-
-PVB_ERR_INVALID = -1        # include/pvb.h pvb_status
-
-_SIM_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-_SIM_LIB = os.path.join(_SIM_DIR, "_build", "libpvb_hostsim_clearance.so")
-_sim = None
-
-
-def _simlib():
-    """tests/hostsim/hostsim_clearance.cpp built like tests/hostsim (g++, -ffp-contract=off), rebuilt when stale."""
-    global _sim
-    if _sim is None:
-        root = os.path.dirname(os.path.dirname(_SIM_DIR))
-        sources = [os.path.join(_SIM_DIR, "hostsim_clearance.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
-                   os.path.join(_SIM_DIR, "hostsim_robot.h"),
-                   os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
-                   os.path.join(root, "include", "pvb.h")]
-        if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
-            os.makedirs(os.path.dirname(_SIM_LIB), exist_ok=True)
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                            "-I", _SIM_DIR, sources[0], "-o", _SIM_LIB], check=True)
-        _sim = ctypes.CDLL(_SIM_LIB)
-    return _sim
-
-
-def _p(a):
-    return ctypes.c_void_p(a.ctypes.data)
 
 
 def _keys(v, idx):
     v = np.ascontiguousarray(v, dtype=np.float32)
     idx = np.ascontiguousarray(idx, dtype=np.uint32)
     out, dec = np.empty(len(v), np.uint64), np.empty(len(v), np.float32)
-    _simlib().simclear_keys(_p(v), _p(idx), ctypes.c_longlong(len(v)), _p(out), _p(dec))
+    hs.lib().simclear_keys(_p(v), _p(idx), ctypes.c_longlong(len(v)), _p(out), _p(dec))
     return out, dec
 
 
@@ -74,16 +43,12 @@ def _fused_keys(descs, xforms, n_cfg, points, n_seg, cfg_begin=0, cfg_count=None
     assert xf.shape == (S * n_cfg, 4, 4) and S <= 8
     keys = np.empty(cfg_count * n_seg, np.uint64)
     evals = ctypes.c_longlong(0)
-    _simlib().simclear_fused(arr, ctypes.c_int(S), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
-                             ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(seg_len),
-                             ctypes.c_int(chunk or seg_len), ctypes.c_int(unit_order), ctypes.c_int(shuffle_seed),
-                             ctypes.c_int(seeded), ctypes.c_int(first), ctypes.c_int(lanes_reversed), _p(keys),
-                             ctypes.byref(evals))
+    hs.lib().simclear_fused(arr, ctypes.c_int(S), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
+                            ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(seg_len),
+                            ctypes.c_int(chunk or seg_len), ctypes.c_int(unit_order), ctypes.c_int(shuffle_seed),
+                            ctypes.c_int(seeded), ctypes.c_int(first), ctypes.c_int(lanes_reversed), _p(keys),
+                            ctypes.byref(evals))
     return keys, evals.value
-
-
-def _margin_max(descs):
-    return max([0.0] + [float(d.prune_margin) for d in descs])
 
 
 def _generic_keys(descs, xforms, n_cfg, points, n_seg, cfg_begin=0, cfg_count=None):
@@ -94,9 +59,9 @@ def _generic_keys(descs, xforms, n_cfg, points, n_seg, cfg_begin=0, cfg_count=No
     xf = np.ascontiguousarray(xforms, dtype=np.float32)
     od = np.asarray(hs.bit_reversed_order(S), dtype=np.uint8)
     keys = np.empty(cfg_count * n_seg, np.uint64)
-    _simlib().simclear_generic(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
-                               ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(len(p) // n_seg),
-                               ctypes.c_float(_margin_max(descs)), _p(keys))
+    hs.lib().simclear_generic(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
+                              ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(len(p) // n_seg),
+                              ctypes.c_float(hs.margin_max(descs)), _p(keys))
     return keys
 
 
@@ -108,10 +73,10 @@ def _finish(descs, xforms, n_cfg, points, n_seg, keys, cfg_begin=0, mesh=0):
     od = np.asarray(hs.bit_reversed_order(S), dtype=np.uint8)
     R = len(keys)
     out = np.empty(R, np.float32), np.empty((R, 3), np.float32), np.empty(R, np.int32), np.empty(R, np.int32)
-    _simlib().simclear_finish(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
-                              ctypes.c_int(R // n_seg), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(len(p) // n_seg),
-                              ctypes.c_int(mesh), ctypes.c_float(_margin_max(descs)), _p(np.ascontiguousarray(keys)),
-                              *[_p(a) for a in out])
+    hs.lib().simclear_finish(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
+                             ctypes.c_int(R // n_seg), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(len(p) // n_seg),
+                             ctypes.c_int(mesh), ctypes.c_float(hs.margin_max(descs)), _p(np.ascontiguousarray(keys)),
+                             *[_p(a) for a in out])
     return out
 
 
@@ -121,7 +86,7 @@ def _reference(descs, xforms, n_cfg, points, n_seg, cfg_begin=0, cfg_count=None)
     cfg_count = n_cfg - cfg_begin if cfg_count is None else cfg_count
     P = len(points)
     L = P // n_seg
-    v, g, w = _sim_composed(descs, xforms, n_cfg, points)
+    v, g, w = hs.composed(descs, xforms, n_cfg, points, ext=True)
     v = v.reshape(n_cfg, n_seg, L)[cfg_begin:cfg_begin + cfg_count]
     g = g.reshape(n_cfg, n_seg, L, 3)[cfg_begin:cfg_begin + cfg_count]
     w = w.reshape(n_cfg, n_seg, L)[cfg_begin:cfg_begin + cfg_count]
@@ -170,7 +135,7 @@ def test_key_order_on_special_values():
 
 def test_key_order_over_all_patterns():
     bad = np.zeros(3, np.int64)
-    _simlib().simclear_check_all_patterns(_p(bad))
+    hs.lib().simclear_check_all_patterns(_p(bad))
     assert bad.tolist() == [0, 0, 0]
 
 
@@ -195,9 +160,9 @@ def _segments(q, n_seg):
 
 @pytest.mark.parametrize("A", [3, 40])
 def test_fused_clearance_equals_the_reduction(built_lib, A):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = zc["tmat"] if A == A0 else _trajectory(zc["tmat"], S, A0, A, seed=A)
+    tm = zc["tmat"] if A == A0 else hs.trajectory(zc["tmat"], S, A0, A, seed=A)
     for n_seg in (6, 1):
         q = _segments(zc["q"], n_seg)
         L = len(q) // n_seg
@@ -209,7 +174,7 @@ def test_fused_clearance_equals_the_reduction(built_lib, A):
             _decoded_equals_finish(keys, fin, (name, n_seg))
             assert len(set(ref[2].tolist())) > 1, name                # the argmin point differs between pairs
             # pruning off (no PVB_GRID_PRUNE_OK: every bound is -inf)
-            unpruned_keys, unpruned = _fused_keys(_unpruned(descs), tm, A, q, n_seg)
+            unpruned_keys, unpruned = _fused_keys(hs.unpruned(descs), tm, A, q, n_seg)
             assert np.array_equal(unpruned_keys, keys), (name, "unpruned")
             assert evals < unpruned, name                            # pruning skips lookups
             # chunk sizes, unit orders, seeding, first visits and lane orders: the same keys
@@ -230,9 +195,9 @@ def test_fused_clearance_equals_the_reduction(built_lib, A):
 
 def test_seeding_prunes_across_blocks(built_lib):
     """Chunks that start from the keys of earlier chunks skip lookups that unseeded chunks make."""
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = _trajectory(zc["tmat"], S, A0, 40, seed=5)
+    tm = hs.trajectory(zc["tmat"], S, A0, 40, seed=5)
     q = _segments(zc["q"], 1)
     descs = sets[0][1]
     seeded = _fused_keys(descs, tm, 40, q, 1, chunk=64, seeded=1)[1]
@@ -241,9 +206,9 @@ def test_seeding_prunes_across_blocks(built_lib):
 
 
 def test_generic_clearance_equals_the_reduction(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = _trajectory(zc["tmat"], S, A0, 20, seed=3)
+    tm = hs.trajectory(zc["tmat"], S, A0, 20, seed=3)
     q = _segments(zc["q"], 6)
     for name, descs in sets:
         keys = _generic_keys(descs, tm, 20, q, 6)
@@ -257,9 +222,9 @@ def test_generic_clearance_equals_the_reduction(built_lib):
 
 
 def test_ties_report_the_first_point(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    base = _trajectory(zc["tmat"], S, A0, 6, seed=7).reshape(S, 6, 4, 4)
+    base = hs.trajectory(zc["tmat"], S, A0, 6, seed=7).reshape(S, 6, 4, 4)
     # configurations 6..11 repeat 0..5, and 12..44 repeat configuration 2
     tm = np.concatenate([base, base, np.repeat(base[:, 2:3], 33, axis=1)], axis=1)
     A = tm.shape[1]
@@ -294,28 +259,28 @@ def test_serial_visit_equals_composed_point_for_every_link_kind(built_lib):
     """robot_serial_kernel's visit sequence (nearest, trilinear, box, cylinder and sphere links, every first visit)
     gives composed_point's bits: value, gradient and link.  The finish step relies on it."""
     import pytorch_volumetric_b200 as pv
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = _trajectory(zc["tmat"], S, A0, 10, seed=9)
+    tm = hs.trajectory(zc["tmat"], S, A0, 10, seed=9)
     q = np.asarray(zc["q"], dtype=np.float32)
     box, cyl = pv.BoxSDF([0.03, 0.05, 0.02]).native_desc("cpu"), pv.CylinderSDF(0.02, 0.07).native_desc("cpu")
     extra = [("box+cylinder", [box, cyl, box, cyl])]
     for name, descs in sets + extra:
-        ref = _sim_composed(descs, tm, 10, q)
+        ref = hs.composed(descs, tm, 10, q, ext=True)
         for first in [-1] + list(range(S)):
             arr = (nat.SdfDesc * S)(*descs)
             xf = np.ascontiguousarray(tm, dtype=np.float32)
             out = (np.empty(10 * len(q), np.float32), np.empty((10 * len(q), 3), np.float32),
                    np.empty(10 * len(q), np.int32))
-            _simlib().simclear_serial_pairs(arr, ctypes.c_int(S), _p(xf), ctypes.c_int(10), _p(q),
-                                            ctypes.c_longlong(len(q)), ctypes.c_int(first), *[_p(a) for a in out])
+            hs.lib().simclear_serial_pairs(arr, ctypes.c_int(S), _p(xf), ctypes.c_int(10), _p(q),
+                                           ctypes.c_longlong(len(q)), ctypes.c_int(first), *[_p(a) for a in out])
             for a, b, what in zip(out, ref, ("val", "grad", "which")):
                 assert np.array_equal(a, b), (name, first, what, int(np.sum(a != b)))
 
 
 # ---------------------------------------------------------------- 4. C ABI refusals (no kernel launch involved)
 def test_abi_refuses_invalid_clearance_queries(built_lib):
-    near, tri, keep = _table_descs("probe")
+    near, tri, keep = hs.table_descs("probe")
     fake = ctypes.c_void_p(1 << 12)           # never dereferenced: every call below fails its argument checks
     L = built_lib
     arr = nat.desc_array([near, near])

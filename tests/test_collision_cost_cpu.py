@@ -17,49 +17,15 @@ sum_p max(0, m - d)^2 and its twist gradient per sub-SDF, and for a robot its jo
 3. The C ABI refusals and the Python shape and margin rules, without a GPU."""
 import ctypes
 import math
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+import hostsim_lib as hs
+from hostsim_lib import PVB_ERR_INVALID, _p
 from pytorch_volumetric_b200 import _native as nat
-from test_paired_cpu import _table_descs
-from test_swept_cpu import _all_sets, _trajectory
-from test_trilinear_composed_cpu import _sim_composed
-
-PVB_ERR_INVALID = -1        # include/pvb.h pvb_status
-
-_SIM_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-_SIM_LIB = os.path.join(_SIM_DIR, "_build", "libpvb_hostsim_collision_cost.so")
-_sim = None
-
-
-def _simlib():
-    """tests/hostsim/hostsim_collision_cost.cpp built like tests/hostsim (g++, -ffp-contract=off), rebuilt when
-    stale."""
-    global _sim
-    if _sim is None:
-        root = os.path.dirname(os.path.dirname(_SIM_DIR))
-        sources = [os.path.join(_SIM_DIR, "hostsim_collision_cost.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
-                   os.path.join(_SIM_DIR, "hostsim_robot.h"),
-                   os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
-                   os.path.join(root, "include", "pvb.h")]
-        if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
-            os.makedirs(os.path.dirname(_SIM_LIB), exist_ok=True)
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                            "-I", _SIM_DIR, sources[0], "-o", _SIM_LIB], check=True)
-        _sim = ctypes.CDLL(_SIM_LIB)
-        _sim.simcc_chunk.restype = ctypes.c_longlong
-        _sim.simcc_chunk.argtypes = [ctypes.c_longlong]
-        _sim.simcc_chunks.restype = ctypes.c_longlong
-        _sim.simcc_chunks.argtypes = [ctypes.c_longlong]
-    return _sim
-
-
-def _p(a):
-    return ctypes.c_void_p(a.ctypes.data)
+from robot_ref import build_robot, joint_values
 
 
 def _fused(descs, xforms, n_cfg, points, n_seg, margin, cfg_begin=0, cfg_count=None, chunk=0, n_acc=8, lanes=32,
@@ -78,11 +44,11 @@ def _fused(descs, xforms, n_cfg, points, n_seg, margin, cfg_begin=0, cfg_count=N
     visited, pv, pg, pw = np.empty(NP, np.uint8), np.empty(NP, np.float32), np.empty((NP, 3), np.float32), \
         np.empty(NP, np.int32)
     evals = ctypes.c_longlong(0)
-    _simlib().simcc_fused(arr, ctypes.c_int(S), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
-                          ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(seg_len),
-                          ctypes.c_float(margin), ctypes.c_int(chunk), ctypes.c_int(n_acc), ctypes.c_int(lanes),
-                          ctypes.c_int(unit_order), ctypes.c_int(shuffle_seed), ctypes.c_int(first), _p(cost),
-                          _p(twist), _p(visited), _p(pv), _p(pg), _p(pw), ctypes.byref(evals))
+    hs.lib().simcc_fused(arr, ctypes.c_int(S), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
+                         ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(seg_len),
+                         ctypes.c_float(margin), ctypes.c_int(chunk), ctypes.c_int(n_acc), ctypes.c_int(lanes),
+                         ctypes.c_int(unit_order), ctypes.c_int(shuffle_seed), ctypes.c_int(first), _p(cost),
+                         _p(twist), _p(visited), _p(pv), _p(pg), _p(pw), ctypes.byref(evals))
     return cost, twist, visited.astype(bool), pv, pg, pw, evals.value
 
 
@@ -113,7 +79,7 @@ def _margins(v):
 
 # ---------------------------------------------------------------- 1. the kernels' sequence
 def test_chunk_rule_depends_on_seg_len_alone():
-    L = _simlib()
+    L = hs.lib()
     for n in (1, 7, 511, 512, 513, 1000, 4096, 131072, 131073, 10 ** 5, 10 ** 6, (1 << 31) - 1):
         c, k = L.simcc_chunk(n), L.simcc_chunks(n)
         assert 1 <= c <= n and k == -(-n // c) and k <= 256, n
@@ -123,15 +89,15 @@ def test_chunk_rule_depends_on_seg_len_alone():
 
 @pytest.mark.parametrize("A", [7, 40])
 def test_fused_cost_equals_the_fp64_composition(built_lib, A):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = zc["tmat"] if A == A0 else _trajectory(zc["tmat"], S, A0, A, seed=A)
+    tm = zc["tmat"] if A == A0 else hs.trajectory(zc["tmat"], S, A0, A, seed=A)
     for n_seg in (1, 4):
         q = np.asarray(zc["q"], dtype=np.float32)[: (len(zc["q"]) // n_seg) * n_seg]
         L = len(q) // n_seg
         pts = q.reshape(n_seg, L, 3)
         for name, descs in sets:
-            v, g, w = _sim_composed(descs, tm, A, q)
+            v, g, w = hs.composed(descs, tm, A, q, ext=True)
             v, g, w = v.reshape(A, n_seg, L), g.reshape(A, n_seg, L, 3), w.reshape(A, n_seg, L)
             for m in _margins(v):
                 what = (name, A, n_seg, m)
@@ -162,13 +128,13 @@ def test_fused_cost_equals_the_fp64_composition(built_lib, A):
 
 
 def test_slabs_reproduce_the_rows_of_the_full_call(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
     A = 70
-    tm = _trajectory(zc["tmat"], S, A0, A, seed=11)
+    tm = hs.trajectory(zc["tmat"], S, A0, A, seed=11)
     q = np.asarray(zc["q"], dtype=np.float32)[:3000]
     for name, descs in sets:
-        v = _sim_composed(descs, tm, A, q)[0]
+        v = hs.composed(descs, tm, A, q, ext=True)[0]
         m = float(np.float32(np.quantile(v, 0.2)))
         cost, twist = _fused(descs, tm, A, q, 3, m)[:2]
         for begin, count in ((0, 1), (5, 32), (31, 2), (33, 37), (69, 1), (1, 69)):
@@ -178,7 +144,7 @@ def test_slabs_reproduce_the_rows_of_the_full_call(built_lib):
 
 
 def test_far_clouds_cost_exactly_zero(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A = int(zc["S"]), int(zc["A"])
     q = np.asarray(zc["q"], dtype=np.float32)[:500] + np.float32(50.0)
     for name, descs in sets:
@@ -189,15 +155,15 @@ def test_far_clouds_cost_exactly_zero(built_lib):
 
 def test_unit_orders_and_duplicates_give_identical_rows(built_lib):
     """Duplicated configurations get identical rows whatever lane and tile they land in."""
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    base = _trajectory(zc["tmat"], S, A0, 5, seed=2).reshape(S, 5, 4, 4)
+    base = hs.trajectory(zc["tmat"], S, A0, 5, seed=2).reshape(S, 5, 4, 4)
     tm = np.concatenate([base] * 9, axis=1)                       # 45 configurations: 5 repeated 9 times
     A = tm.shape[1]
     tm = tm.reshape(S * A, 4, 4)
     q = np.asarray(zc["q"], dtype=np.float32)[:1200]
     for name, descs in sets:
-        v = _sim_composed(descs, tm, A, q)[0]
+        v = hs.composed(descs, tm, A, q, ext=True)[0]
         m = float(np.float32(np.quantile(v, 0.25)))
         cost, twist = _fused(descs, tm, A, q, 2, m, unit_order=2, shuffle_seed=5)[:2]
         cost, twist = cost.reshape(A, 2), twist.reshape(A, 2, S, 6)
@@ -207,7 +173,6 @@ def test_unit_orders_and_duplicates_give_identical_rows(built_lib):
 
 # ---------------------------------------------------------------- 2. the joint gradient of a serial chain
 def _mixed(tmp_path):
-    from test_gpu_robot_fp64 import build_robot
     robot, ref, text = build_robot("mixed", tmp_path, dtype=torch.float64, device="cpu")
     return robot, ref, text
 
@@ -223,7 +188,6 @@ def _ref_cost_terms(ref, q, pts, m):
 
 
 def test_joint_gradient_equals_finite_differences(tmp_path):
-    from test_gpu_robot_fp64 import joint_values
     robot, ref, text = _mixed(tmp_path)
     J, S = len(robot.joint_names), len(robot.sdf_to_link_name)
     assert J == ref.n_joints and S == len(ref.links)
@@ -293,7 +257,7 @@ def test_joint_twists_follow_the_configuration(tmp_path):
 
 # ---------------------------------------------------------------- 3. C ABI refusals and Python rules (no device)
 def test_abi_refuses_invalid_collision_cost_queries(built_lib):
-    near, tri, keep = _table_descs("probe")
+    near, tri, keep = hs.table_descs("probe")
     fake = ctypes.c_void_p(1 << 12)           # never dereferenced: every call below fails its argument checks
     L = built_lib
     arr = nat.desc_array([near, near])
@@ -328,7 +292,7 @@ def test_abi_refuses_invalid_collision_cost_queries(built_lib):
     # the workspace size: one fp32 row of 1 + 6 n_sdf per (configuration, segment, chunk)
     W = L.pvb_collision_cost_workspace
     assert W(2, 4, 10, 100) == 4 * 4 * 10 * 1 * 13
-    assert W(8, 200, 1, 10 ** 5) == 4 * 200 * 1 * _simlib().simcc_chunks(10 ** 5) * 49
+    assert W(8, 200, 1, 10 ** 5) == 4 * 200 * 1 * hs.lib().simcc_chunks(10 ** 5) * 49
     assert W(3, 5, 7, 0) == 0 and W(0, 1, 1, 1) == -1 and W(1, -1, 1, 1) == -1 and W(8, 1 << 30, 1 << 40, 1 << 30) == -1
 
 

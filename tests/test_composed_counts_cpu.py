@@ -22,8 +22,6 @@ import workloads
 from helpers import classify_composed, golden, grid_spec
 from oracle import port
 from pytorch_volumetric_b200 import _native as nat
-from test_paired_cpu import _sim_paired
-from test_trilinear_composed_cpu import _grid_desc, _sim_composed
 
 COUNTS = [17, 32, 33, 64, 65, 127, 128]
 TOL = 1e-5
@@ -58,8 +56,8 @@ def _parts():
     import pytorch_volumetric_b200 as pv
     z = golden("ref_cachedsdf_probe")
     shape = tuple(int(s) for s in z["table_shape"])
-    grid, cached = _grid_desc(torch.from_numpy(z["table_val"]).reshape(shape), torch.from_numpy(z["table_grad"]),
-                              [tuple(r) for r in z["ranges"]], z["bb"], interpolation="nearest")
+    grid, (cached,) = hs.grid_desc(torch.from_numpy(z["table_val"]).reshape(shape), torch.from_numpy(z["table_grad"]),
+                                   [tuple(r) for r in z["ranges"]], z["bb"])
     gs = grid_spec(cached)
     k = np.unravel_index(np.argmin(gs["val"]), gs["val"].shape)
     g_inside = gs["lo"] + np.array(k) * (gs["hi"] - gs["lo"]) / (np.array(gs["val"].shape) - 1)
@@ -147,18 +145,18 @@ def test_host_composition_equals_fp64_in_any_order(S, kind, oracle_lib):
     assert {hs.bit_reversed_order(S)[-1], S - 1, min(31, S - 1)} <= won, (kind, won)
 
     # composed_consider in the visiting loop of the composed kernels (kMesh, kExt instantiation), bit-reversed order
-    got = _sim_composed(descs, xf, A, pts)
+    got = hs.composed(descs, xf, A, pts, ext=True)
     _assert_matches_fp64(*got, members, tm, pts, ref, (S, kind, "composed"))
-    runs = {"index order": _sim_composed(descs, xf, A, pts, order=range(S))}
-    if kind != "mixed":        # hostsim.cpp's loop (the kMesh, non-kExt instantiation) takes grids and meshes only
+    runs = {"index order": hs.composed(descs, xf, A, pts, order=range(S), ext=True)}
+    if kind != "mixed":        # the kMesh, non-kExt instantiation takes grids and meshes only
         runs["hostsim"] = hs.composed(descs, xf, A, pts)
     # composed_point (paired host build) on the same points for every configuration: the fixed order, and the
     # nearest-bound-first loop where it applies (n_sdf <= 32; past that the fixed order runs)
     shared = np.broadcast_to(pts, (A, P, 3))
     for nearest_first in (1, 0):
         for name, order in (("bit-reversed", None), ("index order", range(S))):
-            runs[f"composed_point {name} nf={nearest_first}"] = _sim_paired(descs, xf, A, shared, order=order,
-                                                                            nearest_first=nearest_first)
+            runs[f"composed_point {name} nf={nearest_first}"] = hs.sim_paired(descs, xf, A, shared, order=order,
+                                                                              nearest_first=nearest_first)
     for name, r in runs.items():
         for a, b, part in zip(r, got, ("val", "grad", "which")):
             assert np.array_equal(a, b), (S, kind, name, part, int((a != b).reshape(len(a), -1).any(-1).sum()))
@@ -172,12 +170,12 @@ def test_identical_copies_report_the_first(S, kind):
     descs = [d for d, _s, _c in members]
     tm = np.repeat(workloads.random_rigid(1, seed=5, t_range=0.06).numpy()[:, None], S, axis=0)
     pts = _points(members[:1], tm[:1], 200, seed=1)
-    one = _sim_composed(descs[:1], tm[0], 1, pts)
+    one = hs.composed(descs[:1], tm[0], 1, pts, ext=True)
     for nearest_first in (1, 0):
         for order in (None, range(S)[::-1]):
-            for got in (_sim_composed(descs, tm.reshape(S, 4, 4), 1, pts, order=order),
-                        _sim_paired(descs, tm.reshape(S, 4, 4), 1, pts[None], order=order,
-                                    nearest_first=nearest_first)):
+            for got in (hs.composed(descs, tm.reshape(S, 4, 4), 1, pts, order=order, ext=True),
+                        hs.sim_paired(descs, tm.reshape(S, 4, 4), 1, pts[None], order=order,
+                                      nearest_first=nearest_first)):
                 assert (got[2] == 0).all(), (S, kind, nearest_first)
                 assert np.array_equal(got[0], one[0]) and np.array_equal(got[1], one[1]), (S, kind, nearest_first)
 

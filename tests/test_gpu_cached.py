@@ -5,31 +5,15 @@ import pytest
 import torch
 
 import workloads
-from helpers import golden, pv_factory
+from helpers import cached_from_golden, golden, pv_factory
 
 pytestmark = pytest.mark.gpu
-
-
-def _cached_from_golden(z, name, tmp_path, table_key="table_val", grad_key="table_grad", range_in=None, **kw):
-    """Write the reference-built tables into a reference-format cache file and let CachedSDF load them
-    (sdf.py:487-495): exercises on-disk cache compatibility and isolates the lookup from the table build."""
-    import pytorch_volumetric_b200 as pv
-    res = float(z["resolution"])
-    range_in = z["range_in"] if range_in is None else range_in
-    ranges = pv.get_divisible_range_by_resolution(res, range_in)
-    key = f"{name} {res} {tuple(ranges)}"
-    shape = [int(s) for s in z["table_shape"]]
-    cache = {key: (torch.from_numpy(z[table_key]).reshape(shape), torch.from_numpy(z[grad_key]))}
-    path = str(tmp_path / f"sdf_cache_{name}.pkl")
-    torch.save(cache, path)
-    gt = pv.MeshSDF(pv_factory(name.rstrip("32")))
-    return pv.CachedSDF(name, res, range_in, gt, device="cuda", cache_path=path, **kw)
 
 
 @pytest.mark.parametrize("name", ["probe", "drill"])
 def test_cached_lookup_vs_reference_golden(name, tmp_path):
     z = golden(f"ref_cachedsdf_{name}")
-    c = _cached_from_golden(z, name, tmp_path)
+    c = cached_from_golden(z, name, tmp_path)
     assert tuple(c.voxels.shape) == tuple(int(s) for s in z["table_shape"])
     q = torch.from_numpy(z["q"]).cuda()
     inb = z["inbound"]
@@ -57,7 +41,7 @@ def test_cached_lookup_fp32_range_mode(tmp_path):
     """Range given as Python floats: the reference's view does its index arithmetic in fp32."""
     z = golden("ref_cachedsdf_probe")
     rng32 = [(float(a), float(b)) for a, b in z["range_in"]]
-    c = _cached_from_golden(z, "probe32", tmp_path, "table_val_f32range", "table_grad_f32range", range_in=rng32)
+    c = cached_from_golden(z, "probe32", tmp_path, "table_val_f32range", "table_grad_f32range", range_in=rng32)
     q = torch.from_numpy(z["q"]).cuda()
     inb = z["inbound_f32range"]
     keys = c.voxel_keys(q).cpu().numpy()
@@ -73,7 +57,7 @@ def test_cached_lookup_gt_strategy(tmp_path):
     same kernel."""
     import pytorch_volumetric_b200 as pv
     z = golden("ref_cachedsdf_probe")
-    c = _cached_from_golden(z, "probe", tmp_path, out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
+    c = cached_from_golden(z, "probe", tmp_path, out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
     n = len(z["val_gt"])
     q = torch.from_numpy(z["q"][:n]).cuda()
     val, grad = c(q)
@@ -175,7 +159,7 @@ def test_trilinear_extension_vs_its_cpu_restatement(tmp_path):
     import pytorch_volumetric_b200 as pv
     from oracle import port
     z = golden("ref_cachedsdf_probe")
-    c = _cached_from_golden(z, "probe", tmp_path, interpolation="trilinear")
+    c = cached_from_golden(z, "probe", tmp_path, interpolation="trilinear")
     q = torch.from_numpy(z["q"]).cuda()
     v, g = c(q)
     shape = tuple(int(s) for s in z["table_shape"])
@@ -196,7 +180,7 @@ def test_trilinear_extension_vs_its_cpu_restatement(tmp_path):
     vc, _ = c(centres.cuda())
     inside = c.voxel_keys(centres.cuda()) >= 0
     assert (vc.cpu() - torch.from_numpy(z["table_val"]))[inside.cpu()].abs().max() < 1e-6
-    near = _cached_from_golden(z, "probe", tmp_path)
+    near = cached_from_golden(z, "probe", tmp_path)
     vn, _ = near(q)
     assert (v - vn)[torch.from_numpy(z["inbound"]).cuda()].abs().max() < 2 * float(z["resolution"])
     # the fused composition kernels keep the reference rule: a trilinear CachedSDF composes through the generic path
@@ -204,4 +188,4 @@ def test_trilinear_extension_vs_its_cpu_restatement(tmp_path):
     vcmp, _ = comp(q)
     assert torch.equal(vcmp, v)
     with pytest.raises(ValueError):
-        _cached_from_golden(z, "probe", tmp_path, interpolation="cubic")
+        cached_from_golden(z, "probe", tmp_path, interpolation="cubic")

@@ -7,23 +7,10 @@ import pytest
 import torch
 
 import workloads
-from helpers import golden, pv_factory
-from test_gpu_cached import _cached_from_golden
-from test_gpu_paired import _golden_sets, _no_generic
-from test_gpu_swept import _arm_robot
-from test_gpu_trilinear_composed import _arm, _arm_points, _opaque
+from helpers import (arm_points, arm_robot, cached_arm, cached_from_golden, clearance_reduce, golden, golden_sets,
+                     no_generic, opaque_sdfs, pv_factory)
 
 pytestmark = pytest.mark.gpu
-
-
-def _reduce(v, g, w, cfg_count, n_seg):
-    """First point attaining the minimum of every (configuration, segment) of flat results [cfg_count * n_seg * N]."""
-    v = v.reshape(cfg_count, n_seg, -1)
-    N = v.shape[-1]
-    g, w = g.reshape(cfg_count, n_seg, N, 3), w.reshape(cfg_count, n_seg, N)
-    i = (v == v.amin(-1, keepdim=True)).int().argmax(-1, keepdim=True)
-    return (v.gather(-1, i).reshape(-1), g.gather(-2, i[..., None].expand(-1, -1, 1, 3)).reshape(-1, 3),
-            i.reshape(-1).to(torch.int32), w.gather(-1, i).reshape(-1))
 
 
 def _reference(comp, pts, cfg_begin=0, cfg_count=None):
@@ -31,7 +18,7 @@ def _reference(comp, pts, cfg_begin=0, cfg_count=None):
     cfg_count = n_cfg - cfg_begin if cfg_count is None else cfg_count
     n_seg = pts.reshape(-1, pts.shape[-2], 3).shape[0]
     v, g, w = comp.query(pts.reshape(-1, 3), cfg_begin, cfg_count, return_which=True)
-    return _reduce(v, g, w, cfg_count, n_seg)
+    return clearance_reduce(v, g, w, cfg_count, n_seg)
 
 
 def _assert_clearance(comp, pts, cfg_begin=0, cfg_count=None, what=""):
@@ -44,14 +31,14 @@ def _assert_clearance(comp, pts, cfg_begin=0, cfg_count=None, what=""):
 
 def test_golden_sets_fused(tmp_path, monkeypatch):
     import pytorch_volumetric_b200 as pv
-    z, sets = _golden_sets(tmp_path)
+    z, sets = golden_sets(tmp_path)
     S0, A = int(z["S"]), int(z["A"])
     tm = torch.from_numpy(z["tmat"]).cuda().reshape(S0, A, 4, 4)
     q = torch.from_numpy(z["q"]).cuda()
     for name, sdfs in sets.items():
         S = len(sdfs)
         comp = pv.ComposedSDF(sdfs, pv.Transform3d(matrix=tm[[s % S0 for s in range(S)]].reshape(S * A, 4, 4)))
-        _no_generic(monkeypatch, comp)
+        no_generic(monkeypatch, comp)
         _assert_clearance(comp, q, what=name)
         _assert_clearance(comp, q.reshape(6, 500, 3), cfg_begin=1, cfg_count=2, what=name)
         v, g = comp.clearance(q.reshape(2, 3, 500, 3))
@@ -61,10 +48,10 @@ def test_golden_sets_fused(tmp_path, monkeypatch):
 
 @pytest.mark.parametrize("kind", ["nearest", "trilinear", "primitive"])
 def test_arm_fused(tmp_path, monkeypatch, kind):
-    s = _arm_robot(tmp_path, kind)
+    s = arm_robot(tmp_path, kind)
     s.set_joint_configuration(workloads.arm_configurations(1000).cuda())
-    _no_generic(monkeypatch, s.sdf)
-    pts = _arm_points(6000, seed=21)
+    no_generic(monkeypatch, s.sdf)
+    pts = arm_points(6000, seed=21)
     for count in (1, 7, 31, 32, 33, 200, 1000):
         _assert_clearance(s.sdf, pts, 0, count, what=(kind, count))
     for begin, count in ((3, 200), (500, 33), (999, 1)):
@@ -99,34 +86,34 @@ def test_generic_route(tmp_path, monkeypatch):
         tm[:, :3, 3] = 0.05 * torch.randn(2 * A, 3, generator=torch.Generator().manual_seed(2))
         comp = pv.ComposedSDF([pv.MeshSDF(obj), pv.MeshSDF(obj)], pv.Transform3d(matrix=tm.cuda()))
         comp.set_transforms(comp.obj_frame_to_link_frame, batch_dim=(A,))
-        _no_generic(monkeypatch, comp)
+        no_generic(monkeypatch, comp)
         _assert_clearance(comp, pts, what=obj.name)
         _assert_clearance(comp, pts.reshape(6, 500, 3), 7, 20, what=obj.name)
-    z, sets = _golden_sets(tmp_path)
+    z, sets = golden_sets(tmp_path)
     near = sets["nearest"][0]
     zc = golden("ref_cachedsdf_probe")
-    gt = _cached_from_golden(zc, "probe", tmp_path, out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
+    gt = cached_from_golden(zc, "probe", tmp_path, out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
     q = torch.from_numpy(z["q"]).cuda()
     for name, sdfs in (("12 links", [near] * 12), ("lookup-gt", [near, gt, near])):
         tm = workloads.random_rigid(len(sdfs) * A, seed=4, t_range=0.03).cuda()
         comp = pv.ComposedSDF(sdfs, pv.Transform3d(matrix=tm))
         comp.set_transforms(comp.obj_frame_to_link_frame, batch_dim=(A,))
-        _no_generic(monkeypatch, comp)
+        no_generic(monkeypatch, comp)
         _assert_clearance(comp, q, what=name)
         _assert_clearance(comp, q.reshape(10, 300, 3), 5, 33, what=name)
     # opaque sub-SDFs: the Python reduction over _generic_query chunks
-    s = _arm(tmp_path, "trilinear")
+    s = cached_arm(tmp_path, "trilinear")
     s.set_joint_configuration(workloads.arm_configurations(150).cuda())
-    opaque = pv.ComposedSDF(_opaque(pv, s.sdf.sdfs), s.sdf.obj_frame_to_link_frame)
-    apts = _arm_points(2000, seed=23)
+    opaque = pv.ComposedSDF(opaque_sdfs(pv, s.sdf.sdfs), s.sdf.obj_frame_to_link_frame)
+    apts = arm_points(2000, seed=23)
     _assert_clearance(opaque, apts, what="opaque")
     _assert_clearance(opaque, apts.reshape(4, 500, 3), 10, 100, what="opaque slab")
 
 
 def test_semantics(tmp_path):
     from pytorch_volumetric_b200 import distributed as pd
-    s = _arm(tmp_path, "nearest")
-    pts = _arm_points(3000, seed=24)
+    s = cached_arm(tmp_path, "nearest")
+    pts = arm_points(3000, seed=24)
     # no configuration batch: [*B]
     s.set_joint_configuration(workloads.arm_configurations(1)[0].cuda())
     assert s.sdf.tsf_batch is None
@@ -162,10 +149,10 @@ def test_capability_4096_by_a_million(tmp_path):
     """A = 4096, N = 10^6 on the 8-link arm: the cross product (65.5 GB) does not fit beside anything else; the
     clearance query needs the points, the |A|-sized outputs and keys only.  Compared with the reduction of
     256-configuration query slabs."""
-    s = _arm(tmp_path, "nearest")
+    s = cached_arm(tmp_path, "nearest")
     A, N = 4096, 1_000_000
     s.set_joint_configuration(workloads.arm_configurations(A).cuda())
-    pts = _arm_points(N, seed=25)
+    pts = arm_points(N, seed=25)
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
     base = torch.cuda.memory_allocated()
@@ -177,7 +164,7 @@ def test_capability_4096_by_a_million(tmp_path):
     ref = [[] for _ in range(4)]
     for b in range(0, A, 256):
         v, g, w = s.sdf.query(pts, b, 256, return_which=True)
-        for k, t in enumerate(_reduce(v, g, w, 256, 1)):
+        for k, t in enumerate(clearance_reduce(v, g, w, 256, 1)):
             ref[k].append(t)
         del v, g, w
     for a, b, name in zip(got, [torch.cat(r) for r in ref], ("val", "grad", "point", "which")):

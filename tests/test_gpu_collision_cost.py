@@ -12,11 +12,8 @@ import pytest
 import torch
 
 import workloads
-from helpers import golden, pv_factory
-from test_gpu_cached import _cached_from_golden
-from test_gpu_paired import _golden_sets
-from test_gpu_swept import _arm_robot
-from test_gpu_trilinear_composed import _arm, _arm_points, _opaque
+from helpers import arm_points, arm_robot, cached_arm, cached_from_golden, golden, golden_sets, opaque_sdfs, pv_factory
+from robot_ref import build_robot, joint_values
 
 pytestmark = pytest.mark.gpu
 
@@ -79,7 +76,7 @@ def _margins(comp, pts):
 
 def test_golden_sets_fused(tmp_path, monkeypatch):
     import pytorch_volumetric_b200 as pv
-    z, sets = _golden_sets(tmp_path)
+    z, sets = golden_sets(tmp_path)
     S0, A = int(z["S"]), int(z["A"])
     tm = torch.from_numpy(z["tmat"]).cuda().reshape(S0, A, 4, 4)
     q = torch.from_numpy(z["q"]).cuda()
@@ -95,10 +92,10 @@ def test_golden_sets_fused(tmp_path, monkeypatch):
 
 @pytest.mark.parametrize("kind", ["nearest", "trilinear", "primitive"])
 def test_arm_fused(tmp_path, monkeypatch, kind):
-    s = _arm_robot(tmp_path, kind)
+    s = arm_robot(tmp_path, kind)
     s.set_joint_configuration(workloads.arm_configurations(300).cuda())
     _no_composition(monkeypatch, s.sdf)
-    pts = _arm_points(8000, seed=41)
+    pts = arm_points(8000, seed=41)
     for m in (0.02, 0.1):
         full = _check(s.sdf, pts, m, what=(kind, m))
         assert float(full[0].sum()) > 0 and bool(full[1].any()), (kind, m)
@@ -135,10 +132,10 @@ def test_composition_route(tmp_path):
     for m in _margins(comp, pts):
         _check(comp, pts, m, what=("mesh", m))
         _check(comp, pts.reshape(6, 500, 3), m, 7, 20, what=("mesh slab", m))
-    z, sets = _golden_sets(tmp_path)
+    z, sets = golden_sets(tmp_path)
     near = sets["nearest"][0]
     zc = golden("ref_cachedsdf_probe")
-    gt = _cached_from_golden(zc, "probe", tmp_path, out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
+    gt = cached_from_golden(zc, "probe", tmp_path, out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
     q = torch.from_numpy(z["q"]).cuda()
     for name, sdfs in (("12 links", [near] * 12), ("lookup-gt", [near, gt, near])):
         tm = workloads.random_rigid(len(sdfs) * A, seed=4, t_range=0.03).cuda()
@@ -147,17 +144,17 @@ def test_composition_route(tmp_path):
         for m in _margins(comp, q):
             _check(comp, q, m, what=(name, m))
             _check(comp, q.reshape(10, 300, 3), m, 5, 33, what=(name, m, "slab"))
-    s = _arm(tmp_path, "trilinear")
+    s = cached_arm(tmp_path, "trilinear")
     s.set_joint_configuration(workloads.arm_configurations(150).cuda())
-    opaque = pv.ComposedSDF(_opaque(pv, s.sdf.sdfs), s.sdf.obj_frame_to_link_frame)
-    apts = _arm_points(2000, seed=23)
+    opaque = pv.ComposedSDF(opaque_sdfs(pv, s.sdf.sdfs), s.sdf.obj_frame_to_link_frame)
+    apts = arm_points(2000, seed=23)
     _check(opaque, apts, 0.05, what="opaque")
     _check(opaque, apts.reshape(4, 500, 3), 0.05, 10, 100, what="opaque slab")
 
 
 def test_shapes(tmp_path):
-    s = _arm(tmp_path, "nearest")
-    pts = _arm_points(3000, seed=24)
+    s = cached_arm(tmp_path, "nearest")
+    pts = arm_points(3000, seed=24)
     S, J = len(s.sdf_to_link_name), len(s.joint_names)
     # no configuration batch: [*B]
     s.set_joint_configuration(workloads.arm_configurations(1)[0].cuda())
@@ -188,7 +185,6 @@ def test_shapes(tmp_path):
 def test_joint_gradient_on_a_general_chain_vs_fp64_finite_differences(tmp_path):
     """The mixed primitive chain of test_gpu_robot_fp64.py: over points whose argmin link and shape rule stay put,
     RobotSDF.collision_cost's joint gradient against central differences of the fp64 cost."""
-    from test_gpu_robot_fp64 import build_robot, joint_values
     robot, ref, text = build_robot("mixed", tmp_path)
     J, S = len(robot.joint_names), len(ref.links)
     A = 6
@@ -226,10 +222,10 @@ def test_joint_gradient_on_a_general_chain_vs_fp64_finite_differences(tmp_path):
 def test_joint_gradient_on_the_cached_arm_vs_fp64_jacobian(tmp_path):
     """The cached 8-link arm: the joint gradient against the fp64 Jacobian transpose of the fp32 per-pair outputs,
     through the fp64 joint twists of the same configurations."""
-    s = _arm(tmp_path, "nearest")
+    s = cached_arm(tmp_path, "nearest")
     A = 100
     s.set_joint_configuration(workloads.arm_configurations(A).cuda())
-    pts = _arm_points(20000, seed=42).reshape(2, 10000, 3)
+    pts = arm_points(20000, seed=42).reshape(2, 10000, 3)
     m = 0.05
     cost, grad = s.collision_cost(pts, m)
     rc, rt, ac, at = _reference(s.sdf, pts, m)

@@ -1,42 +1,14 @@
 """GPU parity: ComposedSDF (reference sdf.py:332-433) and RobotSDF (model_to_sdf.py:12-125)."""
 import math
-import os
 
 import numpy as np
 import pytest
 import torch
 
 import workloads
-from helpers import classify_composed, golden, grid_spec, pv_factory, sphere_spec
-from test_gpu_cached import _cached_from_golden
+from helpers import cached_from_golden, classify_composed, golden, grid_spec, pv_factory, sphere_spec, write_wrench_urdf
 
 pytestmark = pytest.mark.gpu
-
-WRENCH_URDF = """<robot name="wrench">
-{links}
-  <link name="offset_wrench"><visual><geometry><mesh filename="wrench.obj"/></geometry></visual></link>
-{joints}
-</robot>"""
-
-
-def write_wrench_urdf(dirname):
-    """Procedural equivalent of the reference's tests/offset_wrench.urdf: 3 prismatic + 3 revolute joints
-    (x, y, z each) in front of one mesh link."""
-    from pytorch_volumetric_b200.meshio import write_obj
-    v, f = workloads.fixture_mesh("wrench")
-    write_obj(os.path.join(dirname, "wrench.obj"), v, f)
-    names = ["link_x_trans", "link_y_trans", "link_z_trans", "link_x_rot", "link_y_rot", "link_z_rot", "offset_wrench"]
-    links = "\n".join(f'  <link name="{n}"/>' for n in names[:-1])
-    axes = ["1 0 0", "0 1 0", "0 0 1"] * 2
-    jn = ["x_trans", "y_trans", "z_trans", "x_rot", "y_rot", "z_rot"]
-    joints = "\n".join(
-        f'  <joint name="{jn[i]}" type="{"prismatic" if i < 3 else "revolute"}"><origin rpy="0 0 0" xyz="0 0 0"/>'
-        f'<parent link="{names[i]}"/><child link="{names[i + 1]}"/><axis xyz="{axes[i]}"/></joint>' for i in range(6))
-    path = os.path.join(dirname, "offset_wrench.urdf")
-    with open(path, "w") as fh:
-        fh.write(WRENCH_URDF.format(links=links, joints=joints))
-    return path
-
 
 def _close(a, b, tol=1e-5):
     return np.abs(a - b) <= tol
@@ -45,7 +17,7 @@ def _close(a, b, tol=1e-5):
 def _composed_from_golden(tmp_path):
     import pytorch_volumetric_b200 as pv
     zc = golden("ref_cachedsdf_probe")
-    cs = _cached_from_golden(zc, "probe", tmp_path)
+    cs = cached_from_golden(zc, "probe", tmp_path)
     z = golden("ref_composed")
     S, A = int(z["S"]), int(z["A"])
     sdfs = [cs, cs, pv.SphereSDF(float(z["sphere_radius"])), cs]

@@ -17,11 +17,9 @@ import torch
 
 import composed_ref as cr
 import workloads
-from helpers import classify_composed, golden, grid_spec
+from helpers import (assert_fp64, cached_from_golden, classify_composed, clearance_reduce, golden, grid_spec,
+                     swept_reduce)
 from oracle import port
-from test_gpu_cached import _cached_from_golden
-from test_gpu_clearance import _reduce as _clearance_reduce
-from test_gpu_swept import _reduce as _swept_reduce
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5
@@ -57,7 +55,7 @@ def parts(tmp_path_factory):
     """(sdf, fp64 spec, interior point in its frame) of every sub-SDF kind."""
     import pytorch_volumetric_b200 as pv
     z = golden("ref_cachedsdf_probe")
-    cached = _cached_from_golden(z, "probe", tmp_path_factory.mktemp("counts"))
+    cached = cached_from_golden(z, "probe", tmp_path_factory.mktemp("counts"))
     gs = grid_spec(cached)
     k = np.unravel_index(np.argmin(gs["val"]), gs["val"].shape)
     g_inside = gs["lo"] + np.array(k) * (gs["hi"] - gs["lo"]) / (np.array(gs["val"].shape) - 1)
@@ -101,41 +99,6 @@ def _setup(parts, kind, S, A, P, seed=0):
     return members, tm, pts
 
 
-def _which_values(specs, tm, pts, w):
-    """fp64 value of the reported sub-SDF w (A, P) at every pair."""
-    out = np.full(w.shape, np.nan)
-    for s, spec in enumerate(specs):
-        a, i = np.nonzero(w == s)
-        if len(a):
-            q = np.einsum("nij,nj->ni", tm[s, a, :3, :3], pts[i].astype(np.float64)) + tm[s, a, :3, 3]
-            out[a, i] = cr.evaluate(spec, q)[0]
-    return out
-
-
-def _assert_fp64(members, tm, pts, v, g, w, what):
-    """query(..., return_which=True) against the fp64 composition: grids and primitives through
-    helpers.classify_composed (every exceedance a classified flip or tie), meshes through composed_ref.mesh_mismatch;
-    `which` names a sub-SDF whose fp64 value is the result's within the tolerance.  Returns the exceedance mask."""
-    S, A = tm.shape[:2]
-    P = len(pts)
-    v, g, w = (t.cpu().numpy() for t in (v, g, w))
-    v, g, w = v.reshape(A, P), g.reshape(A, P, 3), w.reshape(A, P)
-    specs = [m[1] for m in members]
-    assert ((w >= 0) & (w < S)).all(), what
-    if specs[0]["kind"] == "mesh":
-        ref = cr.compose(specs, tm, pts, per_sub=True)
-        bad_v, bad_g, bad_w, rep = cr.mesh_mismatch(v, g, w, ref, TOL, coord_scale=0.2)
-        assert bad_v == 0 and bad_g == 0 and bad_w == 0, (what, rep)
-        return np.zeros((A, P), bool)
-    rv, rg, _rw = cr.compose(specs, tm, pts)
-    n_ex, n_un, rep = classify_composed(v, g, rv, rg, specs, tm, pts, TOL)
-    assert n_un == 0, (what, rep)
-    assert n_ex <= 2e-3 * A * P, (what, rep)
-    exceed = (np.abs(v - rv) > TOL) | (np.abs(g - rg).max(-1) > TOL)
-    assert ((np.abs(_which_values(specs, tm, pts, w) - rv) <= TOL) | exceed).all(), what
-    return exceed
-
-
 def _same(got, ref, what):
     for k, (a, b) in enumerate(zip(got, ref)):
         assert torch.equal(a, b), (what, k, int((a != b).reshape(len(a), -1).any(-1).sum()))
@@ -156,19 +119,19 @@ def _case(kernels, parts, kind, S, A, P):
 
     v, g, w = comp.query(pts, return_which=True)
     kernels.add(_k("composed_query_kernel", *_query_args(kind, S, P)))
-    _assert_fp64(members, tm, pts_np, v, g, w, what)
+    assert_fp64(members, tm, pts_np, v, g, w, what)
 
     # the paired kernel on the same points for every configuration is the cross product itself
     kernels.add(_k("composed_paired_kernel", kmesh, kext, maxs))
     _same(comp.query_paired(pts.expand(A, P, 3).contiguous(), return_which=True), (v, g, w), what + ("paired",))
 
     kernels.add(_k("composed_swept_kernel", kmesh, kext, maxs))
-    _same(comp.query_swept(pts, return_which=True), _swept_reduce(v, g, w, A), what + ("swept",))
+    _same(comp.query_swept(pts, return_which=True), swept_reduce(v, g, w, A), what + ("swept",))
 
     n_seg = 4 if P % 4 == 0 else 1
     kernels |= {_k("composed_clearance_kernel", kmesh, kext, maxs), _k("clearance_finish_kernel", kmesh, kext, maxs)}
     _same(comp.query_clearance(pts.reshape(n_seg, P // n_seg, 3), return_which=True),
-          _clearance_reduce(v, g, w, A, n_seg), what + ("clearance",))
+          clearance_reduce(v, g, w, A, n_seg), what + ("clearance",))
 
     targets = [(torch.full((A * P,), float("nan"), device="cuda"), torch.full((A * P, 3), float("nan"), device="cuda"))
                for _ in range(2)]
@@ -265,7 +228,7 @@ def _robot_case(kernels, comp, members, tm, P, aligned):
     what = (S, A, P, aligned)
     v, g, w = comp.query(pts, return_which=True)
     kernels.add(_k("robot_query_kernel", 16, False, 0))
-    _assert_fp64(members, tm, pts_np, v, g, w, what)
+    assert_fp64(members, tm, pts_np, v, g, w, what)
     # per-configuration slabs take the point-major kernel
     slabs = [comp.query(pts, cfg_begin=a, cfg_count=1, return_which=True) for a in range(A)]
     kernels.add(_k("composed_query_kernel", False, 2 if aligned and P % 4 == 0 else 1, 16, False, False))
@@ -293,11 +256,11 @@ def test_more_than_128_sub_sdfs(kernels, parts, S):
     assert v.shape == (A, P) and g.shape == (A, P, 3)
     vw, gw, w = comp.query(pts, return_which=True)
     _same((vw, gw), (v.reshape(-1), g.reshape(-1, 3)), S)
-    exceed = _assert_fp64(members, tm, pts_np, v, g, w, (S, "call"))
+    exceed = assert_fp64(members, tm, pts_np, v, g, w, (S, "call"))
     rv = cr.compose(specs, tm, pts_np)[0]
 
     sv, sg, sc, sw = comp.swept(pts, return_argmin=True)
-    _same(comp.query_swept(pts, return_which=True), _swept_reduce(vw, gw, w, A), (S, "swept"))
+    _same(comp.query_swept(pts, return_which=True), swept_reduce(vw, gw, w, A), (S, "swept"))
     clean = ~exceed.any(0)
     assert clean.mean() > 0.99
     assert (np.abs(sv.cpu().numpy() - rv.min(0))[clean] <= TOL).all(), S
@@ -305,7 +268,7 @@ def test_more_than_128_sub_sdfs(kernels, parts, S):
     seg = pts.reshape(4, P // 4, 3)
     cv, cg, ci, cw = comp.clearance(seg, return_argmin=True)
     assert cv.shape == (A, 4)
-    _same(comp.query_clearance(seg, return_which=True), _clearance_reduce(vw, gw, w, A, 4), (S, "clearance"))
+    _same(comp.query_clearance(seg, return_which=True), clearance_reduce(vw, gw, w, A, 4), (S, "clearance"))
     clean = ~exceed.reshape(A, 4, P // 4).any(-1)
     assert (np.abs(cv.cpu().numpy() - rv.reshape(A, 4, P // 4).min(-1))[clean] <= TOL).all(), S
 

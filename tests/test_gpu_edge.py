@@ -4,9 +4,7 @@ import pytest
 import torch
 
 import workloads
-from helpers import golden, pv_factory
-from test_gpu_cached import _cached_from_golden
-from test_gpu_composed import write_wrench_urdf
+from helpers import cached_from_golden, golden, pv_factory, write_wrench_urdf
 
 pytestmark = pytest.mark.gpu
 
@@ -14,7 +12,7 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope="module")
 def probe_cached(tmp_path_factory):
     z = golden("ref_cachedsdf_probe")
-    return _cached_from_golden(z, "probe", tmp_path_factory.mktemp("edge")), z
+    return cached_from_golden(z, "probe", tmp_path_factory.mktemp("edge")), z
 
 
 def test_ragged_sizes_match_pointwise(probe_cached):
@@ -69,7 +67,7 @@ def test_gt_strategy_with_non_native_ground_truth(tmp_path):
             return self.inner.surface_bounding_box(**kw)
 
     gt = Wrapped(pv.MeshSDF(obj))
-    native = _cached_from_golden(z, "probe", tmp_path, out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
+    native = cached_from_golden(z, "probe", tmp_path, out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
     ranges_in = z["range_in"]
     opaque = pv.CachedSDF("probe", float(z["resolution"]), ranges_in, gt, device="cuda",
                           out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF,

@@ -25,12 +25,7 @@ import composed_ref as cr
 import grid_ref as gr
 import mesh_ref as mr
 import workloads
-from helpers import golden
-from test_gpu_cached import _cached_from_golden
-from test_gpu_clearance import _reduce as _clearance_reduce
-from test_gpu_composed_counts import _assert_fp64
-from test_gpu_swept import _reduce as _swept_reduce
-from test_gpu_trilinear_composed import _arm, _arm_points
+from helpers import arm_points, assert_fp64, cached_arm, cached_from_golden, clearance_reduce, golden, swept_reduce
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -63,9 +58,9 @@ def make_cached(name, fp32_range, tmp, **kw):
         z = golden(f"ref_cachedsdf_{name}")
         if fp32_range:
             rng32 = [(float(a), float(b)) for a, b in z["range_in"]]
-            return _cached_from_golden(z, name + "32", tmp, "table_val_f32range", "table_grad_f32range",
-                                       range_in=rng32, **kw)
-        return _cached_from_golden(z, name, tmp, **kw)
+            return cached_from_golden(z, name + "32", tmp, "table_val_f32range", "table_grad_f32range",
+                                      range_in=rng32, **kw)
+        return cached_from_golden(z, name, tmp, **kw)
     val, grad = gr.dyadic_table()
     rin = gr.dyadic_ranges(fp32_range)
     ranges = pv.get_divisible_range_by_resolution(gr.DYADIC_RES, rin)
@@ -184,14 +179,13 @@ def test_tma_equals_vec4_bit_for_bit(tmp_path):
 # ---------------------------------------------------------------- standalone trilinear
 @pytest.mark.parametrize("name,fp32_range", TABLES)
 def test_trilinear_kernel_vs_fp64(name, fp32_range, tmp_path):
-    from test_grid_ref_cpu import exact_nodes
     c = make_cached(name, fp32_range, tmp_path, interpolation="trilinear")
     ref = gr.Grid.of(c)
     p = table_points(ref)
     v, g = (t.cpu().numpy() for t in c(torch.from_numpy(p).cuda()))
     rep, bad = gr.compare_trilinear(ref.trilinear(p), v, g)
     assert all(len(b) == 0 for b in bad.values()), (rep, {k: p[x[:5]] for k, x in bad.items()})
-    node, key = exact_nodes(ref, p)
+    node, key = gr.exact_nodes(ref, p)
     assert np.array_equal(v[node], ref.val32.reshape(-1)[key[node]])
     print(name, fp32_range, "trilinear err/bound", rep, "exact nodes", int(node.sum()))
 
@@ -199,7 +193,7 @@ def test_trilinear_kernel_vs_fp64(name, fp32_range, tmp_path):
 # ---------------------------------------------------------------- fused kernels, trilinear links
 def _arm_case(tmp_path, n_cfg, S=8):
     from pytorch_volumetric_b200.transforms import matrix_of
-    s = _arm(tmp_path, "trilinear")
+    s = cached_arm(tmp_path, "trilinear")
     s.set_joint_configuration(workloads.arm_configurations(n_cfg).cuda())
     M = matrix_of(s.sdf.obj_frame_to_link_frame).detach().reshape(8, n_cfg, 4, 4)
     links = list(s.sdf.sdfs)
@@ -218,19 +212,19 @@ def test_trilinear_links_vs_fp64_composition(tmp_path, n_cfg, S, n_pts, offset):
     exceedance a classified cell-face flip, boundary flip or tie; swept and clearance forms equal the reductions."""
     import pytorch_volumetric_b200 as pv
     s, members, M = _arm_case(tmp_path, n_cfg, S)
-    base = _arm_points(n_pts + 1, seed=31)
+    base = arm_points(n_pts + 1, seed=31)
     pts = base.reshape(-1)[3 * offset:3 * (offset + n_pts)].view(n_pts, 3)
     comp = s.sdf if S == 8 else pv.ComposedSDF([m[0] for m in members],
                                                pv.Transform3d(matrix=M.reshape(S * n_cfg, 4, 4)))
     v, g, w = comp.query(pts, return_which=True)
-    _assert_fp64(members, M.cpu().numpy(), pts.cpu().numpy(), v, g, w, (n_cfg, S, n_pts))
+    assert_fp64(members, M.cpu().numpy(), pts.cpu().numpy(), v, g, w, (n_cfg, S, n_pts))
     sw = comp.query_swept(pts, return_which=True)
-    for a, b in zip(sw, _swept_reduce(v, g, w, n_cfg)):
+    for a, b in zip(sw, swept_reduce(v, g, w, n_cfg)):
         assert torch.equal(a, b)
     seg = pts[:n_pts - n_pts % 7].reshape(7, -1, 3)
     cl = comp.query_clearance(seg, return_which=True)
     vs, gs, ws = comp.query(seg.reshape(-1, 3), return_which=True)
-    for a, b in zip(cl, _clearance_reduce(vs, gs, ws, n_cfg, 7)):
+    for a, b in zip(cl, clearance_reduce(vs, gs, ws, n_cfg, 7)):
         assert torch.equal(a, b)
 
 
@@ -253,7 +247,7 @@ def test_lookup_gt_grids_in_composed_kernels_vs_fp64(tmp_path):
     inb = np.stack([spec["ref"].in_range(np.einsum("aij,pj->api", tm[s, :, :3, :3], pts.astype(np.float64)).reshape(-1, 3)
                                          + np.repeat(tm[s, :, :3, 3], P, axis=0)) for s in range(S)])
     assert 0.1 < inb.mean() < 0.9 and (inb.sum(0) >= 2).any() and (inb.sum(0) == 0).any()
-    _assert_fp64(members, tm, pts, v, g, w, "gt grids")
+    assert_fp64(members, tm, pts, v, g, w, "gt grids")
     own = q[None].expand(A, P, 3).contiguous()
     vp, gp, wp = comp.query_paired(own, return_which=True)
     assert torch.equal(vp, v) and torch.equal(gp, g) and torch.equal(wp, w)
@@ -280,11 +274,10 @@ def test_voxel_grid_reads_and_writes_vs_index_rule(d, fp32_range):
     """VoxelGrid on the GPU at boundary-dense points: a write of each point's id lands in the reference's cell
     (one writer per cell kept), and a read returns that cell's content, 0 outside."""
     import pytorch_volumetric_b200 as pv
-    from test_grid_ref_cpu import voxel_case
     box = [(-0.37, 0.41), (0.1, 0.9), (-2.0, -1.3)][:d]
     box = [(float(a), float(b)) for a, b in box] if fp32_range else np.array(box)
     vg = pv.VoxelGrid(0.02, box, device="cuda")
-    p, want = voxel_case(vg, box)
+    p, want = gr.voxel_case(vg, box)
     ncell = vg.get_voxel_values().numel()
     vg.get_voxel_values().reshape(-1).copy_(torch.arange(1, ncell + 1, dtype=torch.float32, device="cuda"))
     got = vg[torch.from_numpy(p).cuda()].cpu().numpy()

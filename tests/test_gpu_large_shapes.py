@@ -40,9 +40,8 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_robot_fp64 import analyse, build_robot, check, joint_values, sample_points
-from test_gpu_swept import _arm_robot
-
+from helpers import arm_robot
+from robot_ref import analyse, build_robot, check, joint_values, sample_points
 pytestmark = pytest.mark.gpu
 
 LIMIT = 65535 * 32              # configurations of 65535 full tiles
@@ -139,7 +138,7 @@ def _robot(kind, tmp_path, C, seed):
     """(RobotSDF with C configurations installed, fp64 RefRobot or None, fp32 joint values)."""
     if kind == "nearest_arm":
         import workloads
-        robot = _arm_robot(tmp_path, "nearest")
+        robot = arm_robot(tmp_path, "nearest")
         q = workloads.arm_configurations(C, seed=seed)
         robot.set_joint_configuration(q.cuda())
         return robot, None, q.numpy()

@@ -13,7 +13,7 @@ import torch
 
 import mesh_ref as mr
 import workloads
-from helpers import golden, pv_factory
+from helpers import cached_from_golden, golden, pv_factory
 
 pytestmark = pytest.mark.gpu
 
@@ -228,10 +228,9 @@ def test_host_pipeline_equals_device_call_and_fp64(name, monkeypatch):
 # ------------------------------------------------------------------ LOOKUP_GT_SDF grids
 def _gt_grid(name, tmp_path):
     import pytorch_volumetric_b200 as pv
-    from test_gpu_cached import _cached_from_golden
     if name == "probe":
-        c = _cached_from_golden(golden("ref_cachedsdf_probe"), "probe", tmp_path,
-                                out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
+        c = cached_from_golden(golden("ref_cachedsdf_probe"), "probe", tmp_path,
+                               out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
     else:
         obj = mesh_obj(name)
         c = pv.CachedSDF(name, 0.002, obj.bounding_box(padding=0.006), pv.MeshSDF(obj), device="cuda",

@@ -7,17 +7,10 @@ import pytest
 import torch
 
 import workloads
-from helpers import golden, pv_factory
-from test_gpu_cached import _cached_from_golden
-from test_gpu_trilinear_composed import _arm, _arm_points, _opaque
+from helpers import (arm_points, cached_arm, cached_from_golden, golden, golden_sets, no_generic, opaque_sdfs,
+                     own_points, pv_factory)
 
 pytestmark = pytest.mark.gpu
-
-
-def _no_generic(monkeypatch, comp):
-    def boom(*a, **k):
-        raise AssertionError("generic path taken")
-    monkeypatch.setattr(comp, "_generic_query", boom)
 
 
 def _assert_equals_slab_queries(comp, own, which=True):
@@ -33,35 +26,17 @@ def _assert_equals_slab_queries(comp, own, which=True):
     return v, g, w
 
 
-def _own_points(q, A, seed):
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    q = q.cpu()
-    return torch.stack([q[torch.randperm(len(q), generator=g)] + 0.01 * torch.randn(3, generator=g)
-                        for _ in range(A)]).cuda()
-
-
-def _golden_sets(tmp_path):
-    import pytorch_volumetric_b200 as pv
-    zc = golden("ref_cachedsdf_probe")
-    near = _cached_from_golden(zc, "probe", tmp_path)
-    tri = _cached_from_golden(zc, "probe", tmp_path, interpolation="trilinear")
-    z = golden("ref_composed")
-    sph = pv.SphereSDF(float(z["sphere_radius"]))
-    return z, {"nearest": [near, near, near, near], "trilinear": [tri, tri, tri], "mixed": [near, tri, near],
-               "nearest+sphere": [near, near, sph, near], "mixed+sphere": [tri, near, sph, tri]}
-
-
 def test_golden_paired_equals_the_call_diagonal(tmp_path, monkeypatch):
     import pytorch_volumetric_b200 as pv
-    z, sets = _golden_sets(tmp_path)
+    z, sets = golden_sets(tmp_path)
     S0, A = int(z["S"]), int(z["A"])
     tm = torch.from_numpy(z["tmat"]).cuda().reshape(S0, A, 4, 4)
-    own = _own_points(torch.from_numpy(z["q"]), A, 0)
+    own = own_points(torch.from_numpy(z["q"]), A, 0)
     P = own.shape[1]
     for name, sdfs in sets.items():
         S = len(sdfs)
         comp = pv.ComposedSDF(sdfs, pv.Transform3d(matrix=tm[[s % S0 for s in range(S)]].reshape(S * A, 4, 4)))
-        _no_generic(monkeypatch, comp)
+        no_generic(monkeypatch, comp)
         v, g = comp.paired(own)
         assert v.shape == (A, P) and g.shape == (A, P, 3)
         cv, cg = comp(own)                                     # [A, A, P]: every configuration at every block
@@ -86,7 +61,7 @@ def test_mesh_paired_equals_slab_queries(monkeypatch):
         tm = torch.eye(4).repeat(2 * A, 1, 1)
         tm[:, :3, 3] = 0.3 * span * torch.randn(2 * A, 3, generator=torch.Generator().manual_seed(2))
         comp = pv.ComposedSDF([pv.MeshSDF(obj), pv.MeshSDF(obj)], pv.Transform3d(matrix=tm.cuda()))
-        _no_generic(monkeypatch, comp)
+        no_generic(monkeypatch, comp)
         own = (torch.rand(A, P, 3, generator=torch.Generator().manual_seed(3)) * 2 - 1).cuda() * span
         _assert_equals_slab_queries(comp, own)
         # a slab of configurations keeps the absolute jitter index
@@ -101,7 +76,7 @@ def test_arm_paired_equals_slab_queries(tmp_path, monkeypatch, scaled):
     point-major kernel the single-configuration ones), and with non-rigid (scaled) transforms."""
     import pytorch_volumetric_b200 as pv
     from pytorch_volumetric_b200.transforms import matrix_of
-    s = _arm(tmp_path, "nearest")
+    s = cached_arm(tmp_path, "nearest")
     A, P = 200, 4096
     s.set_joint_configuration(workloads.arm_configurations(A).cuda())
     comp = s.sdf
@@ -112,8 +87,8 @@ def test_arm_paired_equals_slab_queries(tmp_path, monkeypatch, scaled):
         M[3, 20:26, :3, :3] *= 0.97
         M[0, 150:, :3, :3] *= 1.02
         comp = pv.ComposedSDF(comp.sdfs, pv.Transform3d(matrix=M.reshape(S * A, 4, 4)))
-    _no_generic(monkeypatch, comp)
-    own = torch.stack([_arm_points(P, seed=100 + a) for a in range(A)])
+    no_generic(monkeypatch, comp)
+    own = torch.stack([arm_points(P, seed=100 + a) for a in range(A)])
     _assert_equals_slab_queries(comp, own)
     if not scaled:
         v, g = s.paired(own)                                   # RobotSDF delegates to its ComposedSDF
@@ -123,10 +98,10 @@ def test_arm_paired_equals_slab_queries(tmp_path, monkeypatch, scaled):
 
 def test_edge_shapes(tmp_path, monkeypatch):
     import pytorch_volumetric_b200 as pv
-    s = _arm(tmp_path, "nearest")
-    _no_generic(monkeypatch, s.sdf)
+    s = cached_arm(tmp_path, "nearest")
+    no_generic(monkeypatch, s.sdf)
     s.set_joint_configuration(workloads.arm_configurations(7).cuda())
-    base = _arm_points(7 * 3 * 5 + 1, seed=5)
+    base = arm_points(7 * 3 * 5 + 1, seed=5)
     for P in (1, 3):
         _assert_equals_slab_queries(s.sdf, base[:7 * P].reshape(7, P, 3))
     # a misaligned view: points start 4 bytes into the buffer
@@ -148,7 +123,7 @@ def test_edge_shapes(tmp_path, monkeypatch):
     assert vh64.dtype == torch.float64 and torch.equal(vh64, vd.cpu().double())
     # a 2-D configuration batch [2, 3] with extra *B dimensions: points [2, 3, 4, 5, 3] -> [2, 3, 4, 5]
     s.set_joint_configuration(workloads.arm_configurations(6).cuda().reshape(2, 3, -1))
-    pts = _arm_points(6 * 20, seed=6).reshape(2, 3, 4, 5, 3)
+    pts = arm_points(6 * 20, seed=6).reshape(2, 3, 4, 5, 3)
     v, g = s.paired(pts)
     assert v.shape == (2, 3, 4, 5) and g.shape == (2, 3, 4, 5, 3)
     flat_v, flat_g = s.sdf.query_paired(pts.reshape(6, 20, 3))
@@ -157,13 +132,13 @@ def test_edge_shapes(tmp_path, monkeypatch):
         s.paired(pts.reshape(3, 2, 4, 5, 3))
     # A = 1, and no configuration batch at all: paired == __call__
     s.set_joint_configuration(workloads.arm_configurations(1).cuda())
-    pts = _arm_points(300, seed=7).reshape(1, 300, 3)
+    pts = arm_points(300, seed=7).reshape(1, 300, 3)
     v, g = s.paired(pts)
     cv, cg = s(pts)
     assert torch.equal(v, cv[0]) and torch.equal(g, cg[0])
     s.set_joint_configuration(workloads.arm_configurations(1)[0].cuda())
     assert s.sdf.tsf_batch is None
-    pts = _arm_points(300, seed=8)
+    pts = arm_points(300, seed=8)
     v, g = s.paired(pts)
     cv, cg = s(pts)
     assert torch.equal(v, cv) and torch.equal(g, cg)
@@ -173,23 +148,23 @@ def test_generic_route_equals_fused(tmp_path):
     """Opaque sub-SDFs (no native descriptor) take the unfused paired path: values and argmin equal the fused path
     exactly, gradients within 1e-6 (torch matmul instead of FMAs for the rotation back)."""
     import pytorch_volumetric_b200 as pv
-    z, sets = _golden_sets(tmp_path)
+    z, sets = golden_sets(tmp_path)
     S0, A = int(z["S"]), int(z["A"])
     tm = torch.from_numpy(z["tmat"]).cuda().reshape(S0, A, 4, 4)
-    own = _own_points(torch.from_numpy(z["q"]), A, 1)
+    own = own_points(torch.from_numpy(z["q"]), A, 1)
     for name in ("nearest+sphere", "mixed+sphere"):
         sdfs = sets[name]
         tsf = pv.Transform3d(matrix=tm.reshape(S0 * A, 4, 4))
         vf, gf, wf = pv.ComposedSDF(sdfs, tsf).query_paired(own, return_which=True)
-        vg, gg, wg = pv.ComposedSDF(_opaque(pv, sdfs), tsf).query_paired(own, return_which=True)
+        vg, gg, wg = pv.ComposedSDF(opaque_sdfs(pv, sdfs), tsf).query_paired(own, return_which=True)
         assert torch.equal(vf, vg) and torch.equal(wf, wg), name
         assert float((gf - gg).abs().max()) < 1e-6, name
-    s = _arm(tmp_path, "trilinear")
+    s = cached_arm(tmp_path, "trilinear")
     s.set_joint_configuration(workloads.arm_configurations(40).cuda())
-    own = torch.stack([_arm_points(1000, seed=200 + a) for a in range(40)])
+    own = torch.stack([arm_points(1000, seed=200 + a) for a in range(40)])
     tsf = s.sdf.obj_frame_to_link_frame
     vf, gf, wf = pv.ComposedSDF(s.sdf.sdfs, tsf).query_paired(own, return_which=True)
-    vg, gg, wg = pv.ComposedSDF(_opaque(pv, s.sdf.sdfs), tsf).query_paired(own, return_which=True)
+    vg, gg, wg = pv.ComposedSDF(opaque_sdfs(pv, s.sdf.sdfs), tsf).query_paired(own, return_which=True)
     assert torch.equal(vf, vg) and torch.equal(wf, wg)
     assert float((gf - gg).abs().max()) < 1e-6
 
@@ -200,7 +175,7 @@ def test_trilinear_with_lookup_gt_is_refused(tmp_path):
     import pytorch_volumetric_b200 as pv
     from pytorch_volumetric_b200 import _native as nat
     zc = golden("ref_cachedsdf_probe")
-    tri = _cached_from_golden(zc, "probe", tmp_path, interpolation="trilinear")
+    tri = cached_from_golden(zc, "probe", tmp_path, interpolation="trilinear")
 
     class TriGt(pv.ObjectFrameSDF):
         def __call__(self, p):
@@ -225,9 +200,9 @@ def test_trilinear_with_lookup_gt_is_refused(tmp_path):
 
 def test_sharded_paired_single_rank(tmp_path):
     from pytorch_volumetric_b200 import distributed as pd
-    s = _arm(tmp_path, "nearest")
+    s = cached_arm(tmp_path, "nearest")
     s.set_joint_configuration(workloads.arm_configurations(12).cuda().reshape(3, 4, -1))
-    pts = _arm_points(12 * 50, seed=9).reshape(3, 4, 5, 10, 3)
+    pts = arm_points(12 * 50, seed=9).reshape(3, 4, 5, 10, 3)
     v_ref, g_ref = s.paired(pts)
     v, g = pd.sharded_robot_query(s, pts, gather=True, paired=True)
     assert torch.equal(v, v_ref) and torch.equal(g, g_ref)

@@ -9,12 +9,8 @@ import pytest
 import torch
 
 import workloads
-from helpers import golden, pv_factory
-from test_gpu_cached import _cached_from_golden
-from test_gpu_clearance import _reduce
-from test_gpu_paired import _golden_sets, _no_generic, _own_points
-from test_gpu_swept import _arm_robot
-from test_gpu_trilinear_composed import _arm, _arm_points, _opaque
+from helpers import (arm_points, arm_robot, cached_arm, cached_from_golden, clearance_reduce, golden, golden_sets,
+                     no_generic, opaque_sdfs, own_points, pv_factory)
 
 pytestmark = pytest.mark.gpu
 
@@ -25,7 +21,7 @@ def _reference(comp, own, cfg_begin=0, cfg_count=None):
     N = own.shape[-2]
     n_seg = own.numel() // (3 * N * cfg_count)
     v, g, w = comp.query_paired(own, cfg_begin, cfg_count, return_which=True)
-    return _reduce(v, g, w, cfg_count, n_seg)
+    return clearance_reduce(v, g, w, cfg_count, n_seg)
 
 
 def _assert_pc(comp, own, cfg_begin=0, cfg_count=None, what=""):
@@ -47,15 +43,15 @@ def _assert_equals_per_configuration(comp, own, cfg_begin, configs, got, what=""
 
 def test_golden_sets_fused(tmp_path, monkeypatch):
     import pytorch_volumetric_b200 as pv
-    z, sets = _golden_sets(tmp_path)
+    z, sets = golden_sets(tmp_path)
     S0, A = int(z["S"]), int(z["A"])
     tm = torch.from_numpy(z["tmat"]).cuda().reshape(S0, A, 4, 4)
-    own = _own_points(torch.from_numpy(z["q"]), A, 0)
+    own = own_points(torch.from_numpy(z["q"]), A, 0)
     own = own[:, :(own.shape[1] // 6) * 6]
     for name, sdfs in sets.items():
         S = len(sdfs)
         comp = pv.ComposedSDF(sdfs, pv.Transform3d(matrix=tm[[s % S0 for s in range(S)]].reshape(S * A, 4, 4)))
-        _no_generic(monkeypatch, comp)
+        no_generic(monkeypatch, comp)
         got = _assert_pc(comp, own, what=name)
         _assert_equals_per_configuration(comp, own, 0, range(A), got, what=name)
         seg = own.reshape(A, 6, -1, 3)
@@ -67,10 +63,10 @@ def test_golden_sets_fused(tmp_path, monkeypatch):
 
 @pytest.mark.parametrize("kind", ["nearest", "trilinear", "primitive"])
 def test_arm_fused(tmp_path, monkeypatch, kind):
-    s = _arm_robot(tmp_path, kind)
+    s = arm_robot(tmp_path, kind)
     s.set_joint_configuration(workloads.arm_configurations(1000).cuda())
-    _no_generic(monkeypatch, s.sdf)
-    pts = _arm_points(1000 * 600, seed=31).reshape(1000, 600, 3)
+    no_generic(monkeypatch, s.sdf)
+    pts = arm_points(1000 * 600, seed=31).reshape(1000, 600, 3)
     for count in (1, 7, 31, 32, 33, 200, 1000):
         _assert_pc(s.sdf, pts[:count], 0, count, what=(kind, count))
     for begin, count in ((3, 200), (500, 33), (999, 1)):
@@ -79,7 +75,7 @@ def test_arm_fused(tmp_path, monkeypatch, kind):
         _assert_equals_per_configuration(s.sdf, pts[begin:begin + count].reshape(count, 3, 200, 3), begin,
                                          (0, count - 1), got, what=(kind, begin))
     # segment shapes: N = 6000, B = (2, 3), N = 5 and N = 1
-    big = _arm_points(20 * 6000, seed=32).reshape(20, 6000, 3)
+    big = arm_points(20 * 6000, seed=32).reshape(20, 6000, 3)
     _assert_pc(s.sdf, big, 0, 20, what=(kind, "N=6000"))
     _assert_pc(s.sdf, pts[:200].reshape(200, 2, 3, 100, 3), 0, 200, what=(kind, "B=(2,3)"))
     _assert_pc(s.sdf, pts[:33].reshape(33, 120, 5, 3), 0, 33, what=(kind, "N=5"))
@@ -94,11 +90,11 @@ def test_arm_fused(tmp_path, monkeypatch, kind):
 
 def test_seventy_thousand_configurations(tmp_path, monkeypatch):
     """70 000 configurations x 16 points: more configuration tiles than a grid row can hold, on the fused route."""
-    s = _arm(tmp_path, "nearest")
+    s = cached_arm(tmp_path, "nearest")
     A = 70_000
     s.set_joint_configuration(workloads.arm_configurations(A).cuda())
-    _no_generic(monkeypatch, s.sdf)
-    pts = _arm_points(A * 16, seed=33).reshape(A, 16, 3)
+    no_generic(monkeypatch, s.sdf)
+    pts = arm_points(A * 16, seed=33).reshape(A, 16, 3)
     got = _assert_pc(s.sdf, pts, what="70000")
     _assert_equals_per_configuration(s.sdf, pts, 0, (0, 65_535, 65_536, A - 1), got, what="70000")
 
@@ -117,23 +113,23 @@ def test_generic_route(tmp_path, monkeypatch):
         tm[:, :3, 3] = 0.05 * torch.randn(2 * A, 3, generator=torch.Generator().manual_seed(2))
         comp = pv.ComposedSDF([pv.MeshSDF(obj), pv.MeshSDF(obj)], pv.Transform3d(matrix=tm.cuda()))
         comp.set_transforms(comp.obj_frame_to_link_frame, batch_dim=(A,))
-        _no_generic(monkeypatch, comp)
+        no_generic(monkeypatch, comp)
         got = _assert_pc(comp, own, what=obj.name)
         _assert_equals_per_configuration(comp, own, 0, range(A), got, what=obj.name)
         sub = own[7:27].reshape(20, 6, 100, 3)
         got = _assert_pc(comp, sub, 7, 20, what=obj.name)
         _assert_equals_per_configuration(comp, sub, 7, (0, 19), got, what=obj.name)
-    z, sets = _golden_sets(tmp_path)
+    z, sets = golden_sets(tmp_path)
     near = sets["nearest"][0]
     zc = golden("ref_cachedsdf_probe")
-    gt = _cached_from_golden(zc, "probe", tmp_path, out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
-    gown = _own_points(torch.from_numpy(z["q"]), A, 1)
+    gt = cached_from_golden(zc, "probe", tmp_path, out_of_bounds_strategy=pv.OutOfBoundsStrategy.LOOKUP_GT_SDF)
+    gown = own_points(torch.from_numpy(z["q"]), A, 1)
     gown = gown[:, :(gown.shape[1] // 10) * 10]
     for name, sdfs in (("12 links", [near] * 12), ("lookup-gt", [near, gt, near])):
         tm = workloads.random_rigid(len(sdfs) * A, seed=4, t_range=0.03).cuda()
         comp = pv.ComposedSDF(sdfs, pv.Transform3d(matrix=tm))
         comp.set_transforms(comp.obj_frame_to_link_frame, batch_dim=(A,))
-        _no_generic(monkeypatch, comp)
+        no_generic(monkeypatch, comp)
         _assert_pc(comp, gown, what=name)
         _assert_pc(comp, gown[5:38].reshape(33, 10, -1, 3), 5, 33, what=name)
     # more than 128 sub-SDFs and opaque sub-SDFs: the Python reduction over _generic_query chunks
@@ -141,10 +137,10 @@ def test_generic_route(tmp_path, monkeypatch):
     many = pv.ComposedSDF([near] * 129, pv.Transform3d(matrix=tm))
     many.set_transforms(many.obj_frame_to_link_frame, batch_dim=(4,))
     _assert_pc(many, gown[:4].reshape(4, 2, -1, 3), what="129")
-    s = _arm(tmp_path, "trilinear")
+    s = cached_arm(tmp_path, "trilinear")
     s.set_joint_configuration(workloads.arm_configurations(150).cuda())
-    opaque = pv.ComposedSDF(_opaque(pv, s.sdf.sdfs), s.sdf.obj_frame_to_link_frame)
-    apts = _arm_points(150 * 400, seed=34).reshape(150, 400, 3)
+    opaque = pv.ComposedSDF(opaque_sdfs(pv, s.sdf.sdfs), s.sdf.obj_frame_to_link_frame)
+    apts = arm_points(150 * 400, seed=34).reshape(150, 400, 3)
     got = _assert_pc(opaque, apts, what="opaque")
     _assert_pc(opaque, apts[10:110].reshape(100, 4, 100, 3), 10, 100, what="opaque slab")
     # the opaque path names the fused route's points, values and links (its gradient is rotated back by a torch
@@ -155,8 +151,8 @@ def test_generic_route(tmp_path, monkeypatch):
 
 
 def test_semantics(tmp_path):
-    s = _arm(tmp_path, "nearest")
-    pts = _arm_points(200 * 3 * 500, seed=35)
+    s = cached_arm(tmp_path, "nearest")
+    pts = arm_points(200 * 3 * 500, seed=35)
     # no configuration batch: clearance()
     s.set_joint_configuration(workloads.arm_configurations(1)[0].cuda())
     assert s.sdf.tsf_batch is None

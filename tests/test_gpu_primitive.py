@@ -11,14 +11,9 @@ import torch
 
 import primitive_ref as pr
 import workloads
+from helpers import arm_points, no_generic
 
 pytestmark = pytest.mark.gpu
-
-
-def _no_generic(monkeypatch, comp):
-    def boom(*a, **k):
-        raise AssertionError("generic path taken")
-    monkeypatch.setattr(comp, "_generic_query", boom)
 
 
 def _tolerance(rv, q):
@@ -96,11 +91,6 @@ def _arm(tmp_path, mixed):
                                                               cache_path=str(d / "cache.pkl")))
 
 
-def _arm_points(n, seed):
-    lo = [r[0] for r in workloads.ARM_QUERY_RANGE]; hi = [r[1] for r in workloads.ARM_QUERY_RANGE]
-    return workloads.uniform_points(n, lo, hi, seed=seed).cuda()
-
-
 def _fp64_values(robot, pts):
     """Values [S, A, P] (fp64) of every link at every point: primitives restated in fp64 under the fp32 link
     transforms carried out in fp64; cached mesh links through their own CachedSDF (the voxel rule)."""
@@ -139,8 +129,8 @@ def test_arm_fused_vs_fp64_composition(tmp_path, monkeypatch, mixed):
     assert len(robot.sdf.sdfs) == 8
     A, P = 200, 100_000
     robot.set_joint_configuration(workloads.arm_configurations(A).cuda())
-    pts = _arm_points(P, seed=31)
-    _no_generic(monkeypatch, robot.sdf)
+    pts = arm_points(P, seed=31)
+    no_generic(monkeypatch, robot.sdf)
     v, g, w = robot.sdf.query(pts, return_which=True)
     ref = _fp64_values(robot, pts)
     rv, rw = ref.min(0)
@@ -166,7 +156,7 @@ def test_arm_serial_kernel_equals_slab_queries(tmp_path, mixed):
     """robot_serial_kernel (>= 8 configurations) == the point-major kernel (one configuration per launch), bit for bit
     with the argmin index, at full and ragged shapes."""
     robot = _arm(tmp_path, mixed)
-    base = _arm_points(100_004, seed=9)
+    base = arm_points(100_004, seed=9)
     for n_cfg, n_pts, shift in ((200, 100_000, 0), (40, 4100, 0), (33, 1001, 1), (8, 2048, 0)):
         robot.set_joint_configuration(workloads.arm_configurations(n_cfg).cuda())
         pts = base.reshape(-1)[3 * shift:3 * (shift + n_pts)].view(n_pts, 3)
@@ -183,7 +173,7 @@ def test_sphere_sets_unchanged_by_the_extension_route(tmp_path, monkeypatch):
     import pytorch_volumetric_b200 as pv
     robot = _arm(tmp_path, False)
     robot.set_joint_configuration(workloads.arm_configurations(40).cuda())
-    pts = _arm_points(4096, seed=5)
+    pts = arm_points(4096, seed=5)
 
     class Opaque(pv.ObjectFrameSDF):
         def __init__(self, inner):
@@ -198,7 +188,7 @@ def test_sphere_sets_unchanged_by_the_extension_route(tmp_path, monkeypatch):
     tsf = robot.sdf.obj_frame_to_link_frame
     sph = [pv.SphereSDF(r) for r in (0.05, 0.08, 0.11, 0.06, 0.09, 0.07, 0.05, 0.1)]
     fused = pv.ComposedSDF(sph, tsf)
-    _no_generic(monkeypatch, fused)
+    no_generic(monkeypatch, fused)
     vf, gf, wf = fused.query(pts, return_which=True)
     vg, gg, wg = pv.ComposedSDF([Opaque(s) for s in sph], tsf).query(pts, return_which=True)
     assert torch.equal(vf, vg) and torch.equal(wf, wg) and float((gf - gg).abs().max()) < 1e-6
@@ -210,14 +200,14 @@ def test_arm_paired_and_multi_destination(tmp_path, mixed):
     robot = _arm(tmp_path, mixed)
     A, N = 24, 1000
     robot.set_joint_configuration(workloads.arm_configurations(A).cuda())
-    per = _arm_points(A * N, seed=41).reshape(A, N, 3)
+    per = arm_points(A * N, seed=41).reshape(A, N, 3)
     pv_, pg = robot.paired(per)
     assert pv_.shape == (A, N) and pg.shape == (A, N, 3)
     for a in (0, 7, A - 1):
         v1, g1 = robot.sdf.query(per[a], cfg_begin=a, cfg_count=1)
         assert torch.equal(pv_[a], v1) and torch.equal(pg[a], g1.reshape(N, 3)), a
     # query_into with 3 destinations, in two slabs
-    pts = _arm_points(4096, seed=42)
+    pts = arm_points(4096, seed=42)
     v_ref, g_ref = robot.sdf.query(pts)
     bufs = [(torch.full((A * 4096,), -7.0, device="cuda"), torch.full((A * 4096 * 3,), -7.0, device="cuda"))
             for _ in range(3)]

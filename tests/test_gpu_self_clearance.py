@@ -15,17 +15,10 @@ import torch
 
 import robot_ref as rr
 import workloads
-from test_gpu_robot_fp64 import build_robot, joint_values, link_tolerances, point_bound
-from test_gpu_swept import _arm_robot
-from test_gpu_trilinear_composed import _opaque
+from helpers import allowed_matrix, arm_robot, opaque_sdfs, surface_points, wide_configurations
+from robot_ref import build_robot, joint_values, link_tolerances, point_bound
 
 pytestmark = pytest.mark.gpu
-
-
-def _wide_configurations(A, seed, dtype=torch.float32):
-    """Joint values uniform in +-pi: wide enough that the arm's links pass through one another."""
-    g = torch.Generator().manual_seed(seed)
-    return ((torch.rand(A, 7, generator=g, dtype=torch.float64) * 2 - 1) * math.pi).to(dtype)
 
 
 def _routes(monkeypatch, comp, lp, allowed, cfg_begin=0, cfg_count=None):
@@ -54,30 +47,21 @@ def _assert_same(got, ref, what):
         assert torch.equal(a, b), (what, name, int((a != b).sum()))
 
 
-def _allowed(S, kind):
-    i = torch.arange(S)
-    if kind == "default":
-        return (i[:, None] - i[None, :]).abs() >= 2
-    if kind == "asymmetric":
-        return (i[None, :] - i[:, None] >= 3) | ((i[:, None] == S - 1) & (i[None, :] == 0))
-    return torch.zeros(S, S, dtype=torch.bool)
-
-
 # ---------------------------------------------------------------- 1. fused == composition
 @pytest.mark.parametrize("kind", ["nearest", "trilinear", "primitive"])
 def test_fused_equals_composition_on_the_arm(tmp_path, monkeypatch, kind):
-    robot = _arm_robot(tmp_path, kind)
+    robot = arm_robot(tmp_path, kind)
     S = len(robot.sdf.sdfs)
     cases = [(A, 33) for A in (1, 7, 31, 32, 33, 200, 1000)] + [(200, K) for K in (1, 31, 32, 256, 1000)]
     signs = set()
     for A, K in cases:
-        robot.set_joint_configuration(_wide_configurations(A, seed=A + K).cuda())
+        robot.set_joint_configuration(wide_configurations(A, seed=A + K).cuda())
         lp = robot.link_surface_points(num_points=K, seed=K)
         assert lp.shape == (S, K, 3)
         for which in ("default", "asymmetric", "empty"):
             if which != "default" and (A, K) not in ((33, 33), (200, 256)):
                 continue
-            allowed = _allowed(S, which)
+            allowed = allowed_matrix(S, which)
             fused, ref = _routes(monkeypatch, robot.sdf, lp, allowed)
             _assert_same(fused, ref, (kind, A, K, which))
             if which == "empty":
@@ -88,14 +72,14 @@ def test_fused_equals_composition_on_the_arm(tmp_path, monkeypatch, kind):
                 assert m.all() and (fused[2] != fused[4]).all()
         if A == 200 and K == 256:
             for begin, count in ((0, 1), (17, 100), (199, 1), (50, 150)):
-                fused, ref = _routes(monkeypatch, robot.sdf, lp, _allowed(S, "default"), begin, count)
+                fused, ref = _routes(monkeypatch, robot.sdf, lp, allowed_matrix(S, "default"), begin, count)
                 _assert_same(fused, ref, (kind, begin, count))
     assert {-1.0, 1.0} <= signs, (kind, signs)               # links really intersect, and really clear one another
 
 
 def test_fused_equals_composition_at_70000_configurations(tmp_path, monkeypatch):
-    robot = _arm_robot(tmp_path, "primitive")
-    robot.set_joint_configuration(_wide_configurations(70_000, seed=5).cuda())
+    robot = arm_robot(tmp_path, "primitive")
+    robot.set_joint_configuration(wide_configurations(70_000, seed=5).cuda())
     lp = robot.link_surface_points(num_points=32, seed=1)
     fused, ref = _routes(monkeypatch, robot.sdf, lp, robot.self_collision_pairs())
     _assert_same(fused, ref, "70000")
@@ -135,12 +119,13 @@ def test_composition_route_on_meshes_12_links_and_opaque(tmp_path):
     tsf = pv.Transform3d(matrix=workloads.random_rigid(12 * A, seed=4, t_range=0.12).cuda())
     comp = pv.ComposedSDF(prim, tsf)
     comp.set_transforms(tsf, batch_dim=(A,))
-    lp12 = torch.cat([torch.from_numpy(_surface(s, 24, k)) for k, s in enumerate(prim)]).reshape(12, 24, 3).float()
+    lp12 = torch.cat([torch.from_numpy(surface_points(s, 24, k)) for k, s in enumerate(prim)])
+    lp12 = lp12.reshape(12, 24, 3).float()
     lp12 = lp12.cuda()
     allowed12 = torch.ones(12, 12, dtype=torch.bool)
     out12 = comp.self_clearance(lp12, allowed12, return_argmin=True)
     assert out12[0].shape == (A,) and (out12[2] != out12[4]).all()
-    opaque = pv.ComposedSDF(_opaque(pv, prim[:8]), None)
+    opaque = pv.ComposedSDF(opaque_sdfs(pv, prim[:8]), None)
     native = pv.ComposedSDF(prim[:8], None)
     m8 = pv.Transform3d(matrix=tsf.get_matrix().reshape(12, A, 4, 4)[:8].reshape(-1, 4, 4))
     for c in (opaque, native):
@@ -153,11 +138,6 @@ def test_composition_route_on_meshes_12_links_and_opaque(tmp_path):
     # back with a torch matmul: equal values and indices, gradients to rounding
     for t, u, name in zip(a, b, ("val", "grad", "src", "point", "which")):
         assert torch.equal(t, u) if name != "grad" else torch.allclose(t, u, atol=1e-6), name
-
-
-def _surface(link_sdf, n, seed):
-    from pytorch_volumetric_b200.model_to_sdf import _primitive_surface
-    return _primitive_surface(link_sdf, n, np.random.default_rng(seed))
 
 
 # ---------------------------------------------------------------- 3. against fp64
@@ -230,8 +210,8 @@ def test_self_clearance_against_fp64(tmp_path, kind):
 
 # ---------------------------------------------------------------- 4. shapes, dtypes, repeatability
 def test_batch_float64_and_repeat(tmp_path):
-    robot = _arm_robot(tmp_path, "primitive")
-    q = _wide_configurations(60, seed=9)
+    robot = arm_robot(tmp_path, "primitive")
+    q = wide_configurations(60, seed=9)
     robot.set_joint_configuration(q.cuda().reshape(3, 20, 7))
     v, g, src, pt, which = robot.self_clearance(return_argmin=True)
     assert v.shape == (3, 20) and g.shape == (3, 20, 3) and src.dtype == torch.int64 and pt.shape == (3, 20)

@@ -21,10 +21,8 @@ import torch
 
 import robot_ref as rr
 import workloads
-from test_gpu_robot_fp64 import build_robot, joint_values
-from test_gpu_self_clearance import _allowed, _surface, _wide_configurations
-from test_gpu_swept import _arm_robot
-from test_gpu_trilinear_composed import _opaque
+from helpers import allowed_matrix, arm_robot, opaque_sdfs, surface_points, wide_configurations
+from robot_ref import build_robot, joint_values
 
 pytestmark = pytest.mark.gpu
 
@@ -139,17 +137,17 @@ def _check_arm(monkeypatch, robot, lp, allowed, m, what):
 # ---------------------------------------------------------------- 1-3. the arm
 @pytest.mark.parametrize("kind", ["nearest", "trilinear", "primitive"])
 def test_fused_equals_composition_on_the_arm(tmp_path, monkeypatch, kind):
-    robot = _arm_robot(tmp_path, kind)
+    robot = arm_robot(tmp_path, kind)
     S = len(robot.sdf.sdfs)
     A, K = 200, 1024
     # half the configurations wide (links pass through one another), half about the nominal pose (most clear)
-    q = torch.cat([_wide_configurations(A // 2, seed=3), workloads.arm_configurations(A // 2, seed=4)])
+    q = torch.cat([wide_configurations(A // 2, seed=3), workloads.arm_configurations(A // 2, seed=4)])
     robot.set_joint_configuration(q.cuda())
     lp = robot.link_surface_points(num_points=K, seed=1)
     seen_zero = False
     for m in (0.02, 0.1):
         for which in ("default", "asymmetric"):
-            allowed = _allowed(S, which)
+            allowed = allowed_matrix(S, which)
             fused, ref = _check_arm(monkeypatch, robot, lp, allowed, m, (kind, m, which))
             assert (fused[0] > 0).any(), (kind, m, which)
             seen_zero |= bool((fused[0] == 0).any())
@@ -163,7 +161,7 @@ def test_fused_equals_composition_on_the_arm(tmp_path, monkeypatch, kind):
         moves = robot.joint_moves_link()
         moved = moves[0]
         assert not moved.all() and moved.sum() >= 3
-        allowed = _allowed(S, "default") & moved[:, None] & moved[None, :]
+        allowed = allowed_matrix(S, "default") & moved[:, None] & moved[None, :]
         fused, ref = _check_arm(monkeypatch, robot, lp, allowed, m, (kind, m, "rigid"))
         assert (fused[0] > 0).any()
         seen_zero |= bool((fused[0] == 0).any())
@@ -176,9 +174,9 @@ def test_fused_equals_composition_on_the_arm(tmp_path, monkeypatch, kind):
 
 def test_fused_equals_composition_at_70000_configurations(tmp_path, monkeypatch):
     for kind in ("nearest", "primitive"):
-        robot = _arm_robot(tmp_path / kind, kind)
+        robot = arm_robot(tmp_path / kind, kind)
         robot.sdf.clearance_generic_chunk = 8192                  # fewer launches for the composition route
-        robot.set_joint_configuration(_wide_configurations(70_000, seed=5).cuda())
+        robot.set_joint_configuration(wide_configurations(70_000, seed=5).cuda())
         lp = robot.link_surface_points(num_points=32, seed=1)
         allowed = robot.self_collision_pairs()
         for m in (0.02, 0.1):
@@ -284,14 +282,15 @@ def test_composition_route_on_meshes_12_links_and_opaque(tmp_path):
     tsf = pv.Transform3d(matrix=workloads.random_rigid(12 * A, seed=4, t_range=0.12).cuda())
     comp = pv.ComposedSDF(prim, tsf)
     comp.set_transforms(tsf, batch_dim=(A,))
-    lp12 = torch.cat([torch.from_numpy(_surface(s, 24, k)) for k, s in enumerate(prim)]).reshape(12, 24, 3).float()
+    lp12 = torch.cat([torch.from_numpy(surface_points(s, 24, k)) for k, s in enumerate(prim)])
+    lp12 = lp12.reshape(12, 24, 3).float()
     lp12 = lp12.cuda()
     allowed12 = torch.ones(12, 12, dtype=torch.bool)
     got = comp.query_self_collision_cost(lp12, allowed12, 0.05)
     _assert_close(got, _reference(comp, lp12, allowed12, 0.05), "12 links")
     assert bool((got[0] > 0).any())
     # an opaque 8-link prefix (composition route) against the same links made native (fused route)
-    opaque = pv.ComposedSDF(_opaque(pv, prim[:8]), None)
+    opaque = pv.ComposedSDF(opaque_sdfs(pv, prim[:8]), None)
     native = pv.ComposedSDF(prim[:8], None)
     m8 = pv.Transform3d(matrix=tsf.get_matrix().reshape(12, A, 4, 4)[:8].reshape(-1, 4, 4))
     for c in (opaque, native):
@@ -308,9 +307,9 @@ def test_composition_route_on_meshes_12_links_and_opaque(tmp_path):
 # ---------------------------------------------------------------- 6. shapes
 def test_shapes_float64_and_empty_rows(tmp_path):
     import pytorch_volumetric_b200 as pv
-    robot = _arm_robot(tmp_path, "primitive")
+    robot = arm_robot(tmp_path, "primitive")
     S, J = len(robot.sdf.sdfs), len(robot.joint_names)
-    q = _wide_configurations(60, seed=9)
+    q = wide_configurations(60, seed=9)
     robot.set_joint_configuration(q.cuda().reshape(3, 20, 7))
     c, g = robot.self_collision_cost(0.05)
     assert c.shape == (3, 20) and g.shape == (3, 20, J)

@@ -8,7 +8,6 @@ import torch
 import grid_ref as gr
 import hostsim_lib as hs
 from helpers import golden
-from test_trilinear_composed_cpu import _grid_desc, _sim_trilinear
 
 
 def golden_grid(name, fp32_range=False):
@@ -43,9 +42,7 @@ def points(g, seed=0):
 def host_desc(g, interpolation="nearest"):
     tv = torch.from_numpy(g.val32)
     tg = torch.from_numpy(g.grad.astype(np.float32))
-    if interpolation == "nearest":
-        return hs.grid_desc(tv, tg, g.ranges, g.bb32)
-    return _grid_desc(tv, tg, g.ranges, g.bb32, interpolation)
+    return hs.grid_desc(tv, tg, g.ranges, g.bb32, interpolation=interpolation)
 
 
 @pytest.mark.parametrize("name,fp32_range", [("probe", False), ("probe", True), ("drill", False)])
@@ -84,29 +81,13 @@ def test_trilinear_within_bounds_on_host_build(name, fp32_range):
     sets = gr.point_sets(g.lo64, g.hi64, g.shape)
     p = gr.all_points(sets)
     d, _keep = host_desc(g, "trilinear")
-    val, grad = _sim_trilinear(d, p)
+    val, grad = hs.grid_trilinear(d, p)
     rep, bad = gr.compare_trilinear(g.trilinear(p), val, grad)
     assert all(len(b) == 0 for b in bad.values()), (rep, {k: p[v[:5]] for k, v in bad.items()})
-    node, key = exact_nodes(g, p)
+    node, key = gr.exact_nodes(g, p)
     assert np.array_equal(val[node], g.val32.reshape(-1)[key[node]])
     if name == "dyadic":
         assert node.sum() > 2000                  # every lattice node off the upper faces is exact in fp32 here
-
-
-def exact_nodes(g, p):
-    """(mask, ravelled node) of the in-range points whose fp32 cell coordinate (p - min32) * inv_res32 is an integer
-    below n - 1 on every axis: the interpolant there is the table entry, bit for bit."""
-    from pytorch_volumetric_b200.sdf import fast_index_band
-    p32 = np.asarray(p, np.float32)
-    ok = g.in_range(p32.astype(np.float64))
-    k = np.zeros((len(p32), 3), np.int64)
-    for a in range(3):
-        inv = np.float32(fast_index_band(g.lo64[a], g.hi64[a], g.shape[a])[0])
-        with np.errstate(invalid="ignore"):
-            u = ((p32[:, a] - np.float32(g.lo64[a])).astype(np.float32) * inv).astype(np.float32)
-            ok &= (u == np.floor(u)) & (u >= 0) & (u <= g.shape[a] - 2)
-        k[:, a] = np.where(ok, u, 0)
-    return ok, (k[:, 0] * g.shape[1] + k[:, 1]) * g.shape[2] + k[:, 2]
 
 
 def test_bounds_are_tight():
@@ -122,7 +103,7 @@ def test_bounds_are_tight():
         worst["box value"] = max(worst["box value"], rep["value"])
         worst["box grad"] = max(worst["box grad"], rep["grad"])
         d, _keep = host_desc(g, "trilinear")
-        val, grad = _sim_trilinear(d, p)
+        val, grad = hs.grid_trilinear(d, p)
         ref = g.trilinear(p)
         inb = ref["inb"]
         rep, _ = gr.compare_trilinear({k: (v[inb] if k != "alt" else v[:, inb]) for k, v in ref.items()},
@@ -144,19 +125,6 @@ def test_voxel_index_rule_equals_host_gridview(d, fp32_range):
     box = [(float(a), float(b)) for a, b in box] if fp32_range else np.array(box)
     vg = pv.VoxelGrid(0.02, box)
     vg.get_voxel_values().reshape(-1).copy_(torch.arange(1, vg.get_voxel_values().numel() + 1, dtype=torch.float32))
-    p, want = voxel_case(vg, box)
+    p, want = gr.voxel_case(vg, box)
     got = vg[torch.from_numpy(p)].numpy()
     assert np.array_equal(got, np.where(want >= 0, want + 1, 0).astype(np.float32))
-
-
-def voxel_case(vg, box):
-    """(boundary-dense points [m, d] fp32, reference flat index [m]) of a VoxelGrid over `box` (as it was given)."""
-    import pytorch_volumetric_b200 as pv
-    ranges = pv.get_divisible_range_by_resolution(vg.resolution, box)
-    shape = tuple(vg.get_voxel_values().shape)
-    d = len(shape)
-    lo = np.array([float(min(r)) for r in ranges]); hi = np.array([float(max(r)) for r in ranges])
-    sets = gr.point_sets(np.pad(lo, (0, 3 - d), constant_values=0), np.pad(hi, (0, 3 - d), constant_values=1),
-                         np.pad(np.array(shape), (0, 3 - d), constant_values=2))
-    p = np.ascontiguousarray(gr.all_points(sets)[:, :d])
-    return p, gr.voxel_index(ranges, shape, p)

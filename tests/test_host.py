@@ -8,6 +8,7 @@ import pytest
 import torch
 
 import workloads
+from robot_ref import MIXED_URDF
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -336,23 +337,6 @@ def test_mesh_readers_edge_cases(tmp_path):
     meshio.write_obj(str(tmp_path / "rt.obj"), vv, ff)
     v2, f2 = meshio.read_obj(str(tmp_path / "rt.obj"))
     assert np.array_equal(v2, vv) and np.array_equal(f2, ff)
-
-
-MIXED_URDF = """<robot name="mixed">
-  <link name="base"><visual><origin xyz="0 0 0.1" rpy="0.1 -0.2 0.3"/><geometry><mesh filename="a.obj" scale="2 2 2"/></geometry></visual>
-                    <visual><geometry><box size="0.1 0.1 0.1"/></geometry></visual></link>
-  <link name="l1"/>
-  <link name="l2"><visual><origin xyz="0.01 0 0" rpy="0 0 1.5"/><geometry><mesh filename="package://b.obj"/></geometry></visual></link>
-  <link name="l3"><visual><geometry><mesh filename="c.obj"/></geometry></visual></link>
-  <link name="tool"><visual><geometry><mesh filename="d.obj"/></geometry></visual></link>
-  <link name="side"><visual><geometry><mesh filename="e.obj"/></geometry></visual></link>
-  <joint name="j_fixed" type="fixed"><parent link="base"/><child link="l1"/><origin xyz="0 0 0.3" rpy="0 0.5 0"/></joint>
-  <joint name="j_rev" type="revolute"><parent link="l1"/><child link="l2"/><origin xyz="0.1 0.2 0" rpy="0.3 0 -0.4"/>
-         <axis xyz="1 1 0"/><limit lower="-3" upper="3"/></joint>
-  <joint name="j_pris" type="prismatic"><parent link="l2"/><child link="l3"/><origin xyz="0 0 0.2"/><axis xyz="0 -1 0.5"/></joint>
-  <joint name="j_cont" type="continuous"><parent link="l3"/><child link="tool"/><origin xyz="0.05 0 0" rpy="1.0 0 0"/><axis xyz="0 0 -1"/></joint>
-  <joint name="j_side" type="revolute"><parent link="l1"/><child link="side"/><axis xyz="0 0 1"/></joint>
-</robot>"""
 
 
 def test_urdf_chain_mixed_joint_types_match_oracle_restatement():

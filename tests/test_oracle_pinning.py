@@ -6,7 +6,7 @@ import pytest
 import torch
 
 import workloads
-from helpers import golden, port_mesh
+from helpers import golden, port_mesh, write_wrench_urdf
 from oracle import port, tp_pytorch_kinematics as opk
 
 
@@ -114,7 +114,6 @@ def test_port_robot_table_build_equals_reference_run(tmp_path, oracle_lib):
     (resolution 0.008, padding 0.05, same numpy seed for the ray draws) on the procedural twin of
     tests/offset_wrench.urdf, reproduces bit for bit what the unmodified reference computed for the same joint values
     and points (oracle/make_golden.py: ref_robot_wrench_r008)."""
-    from test_gpu_composed import write_wrench_urdf
     z = golden("ref_robot_wrench_r008")
     urdf = write_wrench_urdf(str(tmp_path))
     chain = opk.build_serial_chain_from_urdf(open(urdf).read(), "offset_wrench")
@@ -132,7 +131,6 @@ def test_port_robot_equals_reference_golden(tmp_path, oracle_lib):
     unmodified reference produced (oracle/make_golden.py: ref_robot_wrench) -- FK + offset composition bit-exact,
     values / gradients bit-exact on the reference-built link table.  Needs no copy of the reference."""
     from oracle import tp_pytorch_kinematics as opk
-    from test_gpu_composed import write_wrench_urdf
     z = golden("ref_robot_wrench")
     urdf = write_wrench_urdf(str(tmp_path))
     chain = opk.build_serial_chain_from_urdf(open(urdf).read(), "offset_wrench")

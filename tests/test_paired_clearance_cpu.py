@@ -13,69 +13,14 @@ per-configuration result at the first point attaining the minimum.
 3. The general route (composed_paired_clearance_kernel and its finish) gives the fused route's keys and results.
 4. The C ABI refusals and the Python shape rules, without a GPU."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 import hostsim_lib as hs
+from hostsim_lib import PVB_ERR_INVALID, _p
 from pytorch_volumetric_b200 import _native as nat
-from test_paired_cpu import _own_points, _table_descs
-from test_swept_cpu import _all_sets, _trajectory
-from test_trilinear_composed_cpu import _sim_composed, _unpruned
-
-PVB_ERR_INVALID = -1        # include/pvb.h pvb_status
-
-_SIM_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-_SIM_LIB = os.path.join(_SIM_DIR, "_build", "libpvb_hostsim_paired_clearance.so")
-_sim = None
-
-
-def _simlib():
-    """tests/hostsim/hostsim_paired_clearance.cpp built like tests/hostsim (g++, -ffp-contract=off), rebuilt when
-    stale."""
-    global _sim
-    if _sim is None:
-        root = os.path.dirname(os.path.dirname(_SIM_DIR))
-        sources = [os.path.join(_SIM_DIR, "hostsim_paired_clearance.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
-                   os.path.join(_SIM_DIR, "hostsim_robot.h"),
-                   os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
-                   os.path.join(root, "include", "pvb.h")]
-        if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
-            os.makedirs(os.path.dirname(_SIM_LIB), exist_ok=True)
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                            "-I", _SIM_DIR, sources[0], "-o", _SIM_LIB], check=True)
-        _sim = ctypes.CDLL(_SIM_LIB)
-    return _sim
-
-
-def _p(a):
-    return ctypes.c_void_p(a.ctypes.data)
-
-
-def _margin_max(descs):
-    return max([0.0] + [float(d.prune_margin) for d in descs])
-
-
-def _fused_keys(descs, xforms, n_cfg, own, cfg_begin=0, chunk=None, lanes=32, share=1, unit_order=0, shuffle_seed=0,
-                seeded=1, first=-1, steps_reversed=0):
-    """(keys [cfg_count * n_seg], lookups) of robot_paired_clearance_kernel's sequence; own [cfg_count, n_seg, L, 3]."""
-    cfg_count, n_seg, L = own.shape[:3]
-    p = np.ascontiguousarray(own, dtype=np.float32)
-    S = len(descs)
-    arr = (nat.SdfDesc * S)(*descs)
-    xf = np.ascontiguousarray(xforms, dtype=np.float32)
-    assert xf.shape == (S * n_cfg, 4, 4) and S <= 8
-    keys = np.empty(cfg_count * n_seg, np.uint64)
-    evals = ctypes.c_longlong(0)
-    _simlib().simpcl_fused(arr, ctypes.c_int(S), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
-                           ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(L),
-                           ctypes.c_int(chunk or L), ctypes.c_int(lanes), ctypes.c_int(share),
-                           ctypes.c_int(unit_order), ctypes.c_int(shuffle_seed), ctypes.c_int(seeded),
-                           ctypes.c_int(first), ctypes.c_int(steps_reversed), _p(keys), ctypes.byref(evals))
-    return keys, evals.value
 
 
 def _generic_keys(descs, xforms, n_cfg, own, cfg_begin=0):
@@ -86,26 +31,10 @@ def _generic_keys(descs, xforms, n_cfg, own, cfg_begin=0):
     xf = np.ascontiguousarray(xforms, dtype=np.float32)
     od = np.asarray(hs.bit_reversed_order(S), dtype=np.uint8)
     keys = np.empty(cfg_count * n_seg, np.uint64)
-    _simlib().simpcl_generic(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
-                             ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(L),
-                             ctypes.c_float(_margin_max(descs)), _p(keys))
-    return keys
-
-
-def _finish(descs, xforms, n_cfg, own, keys, cfg_begin=0, mesh=0):
-    cfg_count, n_seg, L = own.shape[:3]
-    p = np.ascontiguousarray(own, dtype=np.float32)
-    S = len(descs)
-    arr = (nat.SdfDesc * S)(*descs)
-    xf = np.ascontiguousarray(xforms, dtype=np.float32)
-    od = np.asarray(hs.bit_reversed_order(S), dtype=np.uint8)
-    R = len(keys)
-    out = np.empty(R, np.float32), np.empty((R, 3), np.float32), np.empty(R, np.int32), np.empty(R, np.int32)
-    _simlib().simpcl_finish(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
+    hs.lib().simpcl_generic(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
                             ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(n_seg), ctypes.c_int(L),
-                            ctypes.c_int(mesh), ctypes.c_float(_margin_max(descs)), _p(np.ascontiguousarray(keys)),
-                            *[_p(a) for a in out])
-    return out
+                            ctypes.c_float(hs.margin_max(descs)), _p(keys))
+    return keys
 
 
 def _reference(descs, xforms, n_cfg, own, cfg_begin=0):
@@ -116,7 +45,7 @@ def _reference(descs, xforms, n_cfg, own, cfg_begin=0):
     tm = np.asarray(xforms, dtype=np.float32).reshape(S, n_cfg, 4, 4)
     out = [[] for _ in range(4)]
     for c in range(cfg_count):
-        v, g, w = _sim_composed(descs, tm[:, cfg_begin + c], 1, own[c].reshape(-1, 3))
+        v, g, w = hs.composed(descs, tm[:, cfg_begin + c], 1, own[c].reshape(-1, 3), ext=True)
         v, g, w = v.reshape(n_seg, L), g.reshape(n_seg, L, 3), w.reshape(n_seg, L)
         i = np.argmax(v == v.min(axis=-1, keepdims=True), axis=-1)[..., None]
         for k, t in enumerate((np.take_along_axis(v, i, -1).reshape(-1),
@@ -133,49 +62,50 @@ def _assert_same(got, ref, what):
 
 def _clouds(zc, A, n_seg, L, seed):
     """[A, n_seg, L, 3]: every configuration its own shuffled, shifted copy of the golden points."""
-    return _own_points(zc["q"], A, seed)[:, :n_seg * L].reshape(A, n_seg, L, 3)
+    return hs.own_points(zc["q"], A, seed)[:, :n_seg * L].reshape(A, n_seg, L, 3)
 
 
 # ---------------------------------------------------------------- 1. the fused sequence
 @pytest.mark.parametrize("A", [3, 40])
 def test_fused_paired_clearance_equals_the_reduction(built_lib, A):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = zc["tmat"] if A == A0 else _trajectory(zc["tmat"], S, A0, A, seed=A)
+    tm = zc["tmat"] if A == A0 else hs.trajectory(zc["tmat"], S, A0, A, seed=A)
     for n_seg, L in ((3, 300), (1, 700)):
         own = _clouds(zc, A, n_seg, L, seed=A + n_seg)
         for name, descs in sets:
             ref = _reference(descs, tm, A, own)
-            keys, evals = _fused_keys(descs, tm, A, own)
-            _assert_same(_finish(descs, tm, A, own, keys), ref, (name, n_seg))
+            keys, evals = hs.pcl_keys(descs, tm, A, own)
+            _assert_same(hs.pcl_finish(descs, tm, A, own, keys), ref, (name, n_seg))
             assert len(set(ref[2].tolist())) > 1, name                # the argmin point differs between pairs
             # pruning off (no PVB_GRID_PRUNE_OK: every bound is -inf)
-            unpruned_keys, unpruned = _fused_keys(_unpruned(descs), tm, A, own)
+            unpruned_keys, unpruned = hs.pcl_keys(hs.unpruned(descs), tm, A, own)
             assert np.array_equal(unpruned_keys, keys), (name, "unpruned")
             assert evals < unpruned, name
             # chunk sizes, unit widths, sharing, unit orders, seeding and step orders: the same keys
             for chunk in (7, 32, 64, L):
                 for lanes in (32, 256):
                     for order, seed in ((0, 0), (1, 0), (2, chunk + lanes)):
-                        got = _fused_keys(descs, tm, A, own, chunk=chunk, lanes=lanes, share=(order + 1) & 1,
+                        got = hs.pcl_keys(descs, tm, A, own, chunk=chunk, lanes=lanes, share=(order + 1) & 1,
                                           unit_order=order, shuffle_seed=seed, seeded=(chunk + order) & 1,
                                           steps_reversed=order & 1)[0]
                         assert np.array_equal(got, keys), (name, n_seg, chunk, lanes, order)
             for first in range(S):
-                got = _fused_keys(descs, tm, A, own, chunk=64, first=first, steps_reversed=first & 1)[0]
+                got = hs.pcl_keys(descs, tm, A, own, chunk=64, first=first, steps_reversed=first & 1)[0]
                 assert np.array_equal(got, keys), (name, n_seg, first)
             # slabs: the absolute configuration picks the transforms
             for begin, count in ((1, A - 1), (A // 2, 1), (A - 2, 2)):
                 sub = own[begin:begin + count]
-                ks = _fused_keys(descs, tm, A, sub, cfg_begin=begin, chunk=64)[0]
-                _assert_same(_finish(descs, tm, A, sub, ks, cfg_begin=begin), _reference(descs, tm, A, sub, begin),
+                ks = hs.pcl_keys(descs, tm, A, sub, cfg_begin=begin, chunk=64)[0]
+                _assert_same(hs.pcl_finish(descs, tm, A, sub, ks, cfg_begin=begin),
+                             _reference(descs, tm, A, sub, begin),
                              (name, begin, count))
 
 
 def test_ties_report_the_first_point(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    base = _trajectory(zc["tmat"], S, A0, 6, seed=7).reshape(S, 6, 4, 4)
+    base = hs.trajectory(zc["tmat"], S, A0, 6, seed=7).reshape(S, 6, 4, 4)
     # configurations 6..11 repeat 0..5 with the same clouds, and 12..44 repeat configuration 2 and its cloud
     tm = np.concatenate([base, base, np.repeat(base[:, 2:3], 33, axis=1)], axis=1)
     A = tm.shape[1]
@@ -186,12 +116,12 @@ def test_ties_report_the_first_point(built_lib):
     for name, descs in sets:
         ref = _reference(descs, tm, A, own)
         assert (ref[2] < 75).all()
-        for keys in (_fused_keys(descs, tm, A, own)[0],
-                     _fused_keys(descs, tm, A, own, chunk=7, unit_order=1, share=0)[0],
-                     _fused_keys(descs, tm, A, own, chunk=32, lanes=256, unit_order=2, shuffle_seed=3,
+        for keys in (hs.pcl_keys(descs, tm, A, own)[0],
+                     hs.pcl_keys(descs, tm, A, own, chunk=7, unit_order=1, share=0)[0],
+                     hs.pcl_keys(descs, tm, A, own, chunk=32, lanes=256, unit_order=2, shuffle_seed=3,
                                  steps_reversed=1)[0],
                      _generic_keys(descs, tm, A, own)):
-            _assert_same(_finish(descs, tm, A, own, keys), ref, name)
+            _assert_same(hs.pcl_finish(descs, tm, A, own, keys), ref, name)
         v = ref[0].reshape(A, 4)
         assert np.array_equal(v[0:6], v[6:12]) and (v[12:] == v[2]).all()
     # a sub-SDF listed twice under the same transforms: the first of the two wins its ties
@@ -200,18 +130,18 @@ def test_ties_report_the_first_point(built_lib):
     tm5 = np.concatenate([base[0:1], base[1:2], base[0:1], base[2:3], base[3:4]], axis=0).reshape(5 * 6, 4, 4)
     ref = _reference(dup, tm5, 6, c6)
     assert (ref[3] != 2).all() and (ref[3] == 0).any()
-    _assert_same(_finish(dup, tm5, 6, c6, _fused_keys(dup, tm5, 6, c6, chunk=32)[0]), ref, "dup")
-    _assert_same(_finish(dup, tm5, 6, c6, _generic_keys(dup, tm5, 6, c6), mesh=1), ref, "dup generic")
+    _assert_same(hs.pcl_finish(dup, tm5, 6, c6, hs.pcl_keys(dup, tm5, 6, c6, chunk=32)[0]), ref, "dup")
+    _assert_same(hs.pcl_finish(dup, tm5, 6, c6, _generic_keys(dup, tm5, 6, c6), mesh=1), ref, "dup generic")
 
 
 # ---------------------------------------------------------------- 2. pruning
 def test_pruning_on_a_scene_cloud(built_lib):
     """A cloud of a few flat patches around the object, shifted per configuration (an environment per configuration):
     the bounds skip most links, seeding skips more, and so does the warp's shared running value."""
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
     A, N = 24, 2048
-    tm = _trajectory(zc["tmat"], S, A0, A, seed=13)
+    tm = hs.trajectory(zc["tmat"], S, A0, A, seed=13)
     q = np.asarray(zc["q"], dtype=np.float64)
     lo, hi = q.min(0), q.max(0)
     g = np.random.default_rng(14)
@@ -225,38 +155,38 @@ def test_pruning_on_a_scene_cloud(built_lib):
             patches.append(pts)
         own[a, 0] = np.concatenate(patches) + g.normal(0.0, 0.01, 3)
     for name, descs in sets:
-        keys, evals = _fused_keys(descs, tm, A, own, chunk=256)
-        _assert_same(_finish(descs, tm, A, own, keys), _reference(descs, tm, A, own), name)
+        keys, evals = hs.pcl_keys(descs, tm, A, own, chunk=256)
+        _assert_same(hs.pcl_finish(descs, tm, A, own, keys), _reference(descs, tm, A, own), name)
         assert evals < A * N * S, (name, evals)
-        unseeded = _fused_keys(descs, tm, A, own, chunk=256, seeded=0)[1]
-        unshared = _fused_keys(descs, tm, A, own, chunk=256, share=0)[1]
+        unseeded = hs.pcl_keys(descs, tm, A, own, chunk=256, seeded=0)[1]
+        unshared = hs.pcl_keys(descs, tm, A, own, chunk=256, share=0)[1]
         assert evals <= unseeded and evals <= unshared, (name, evals, unseeded, unshared)
     descs = sets[0][1]
-    assert _fused_keys(descs, tm, A, own, chunk=256)[1] < _fused_keys(descs, tm, A, own, chunk=256, share=0)[1]
+    assert hs.pcl_keys(descs, tm, A, own, chunk=256)[1] < hs.pcl_keys(descs, tm, A, own, chunk=256, share=0)[1]
 
 
 # ---------------------------------------------------------------- 3. the general route
 def test_generic_paired_clearance_equals_the_fused_route(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = _trajectory(zc["tmat"], S, A0, 20, seed=3)
+    tm = hs.trajectory(zc["tmat"], S, A0, 20, seed=3)
     own = _clouds(zc, 20, 6, 100, seed=4)
     for name, descs in sets:
         keys = _generic_keys(descs, tm, 20, own)
-        fused = _fused_keys(descs, tm, 20, own, chunk=32)[0]
+        fused = hs.pcl_keys(descs, tm, 20, own, chunk=32)[0]
         assert np.array_equal(keys, fused), name
-        fin = _finish(descs, tm, 20, own, keys, mesh=1)
-        assert all(np.array_equal(a, b) for a, b in zip(fin, _finish(descs, tm, 20, own, fused))), name
+        fin = hs.pcl_finish(descs, tm, 20, own, keys, mesh=1)
+        assert all(np.array_equal(a, b) for a, b in zip(fin, hs.pcl_finish(descs, tm, 20, own, fused))), name
         _assert_same(fin, _reference(descs, tm, 20, own), name)
         sub = own[5:14]
         ks = _generic_keys(descs, tm, 20, sub, cfg_begin=5)
-        _assert_same(_finish(descs, tm, 20, sub, ks, cfg_begin=5, mesh=1), _reference(descs, tm, 20, sub, 5),
+        _assert_same(hs.pcl_finish(descs, tm, 20, sub, ks, cfg_begin=5, mesh=1), _reference(descs, tm, 20, sub, 5),
                      (name, "slab"))
 
 
 # ---------------------------------------------------------------- 4. C ABI refusals (no kernel launch involved)
 def test_abi_refuses_invalid_paired_clearance_queries(built_lib):
-    near, tri, keep = _table_descs("probe")
+    near, tri, keep = hs.table_descs("probe")
     fake = ctypes.c_void_p(1 << 12)           # never dereferenced: every call below fails its argument checks
     L = built_lib
     arr = nat.desc_array([near, near])

@@ -8,8 +8,6 @@ configuration evaluated at its own points.
 2. The 64-bit pair index arithmetic near and above 2^31 pairs.
 3. The C ABI refusals, and the shape rules of the Python layer, without a GPU."""
 import ctypes
-import os
-import subprocess
 import types
 
 import numpy as np
@@ -17,115 +15,43 @@ import pytest
 import torch
 
 import hostsim_lib as hs
-from helpers import golden
+from hostsim_lib import PVB_ERR_INVALID, _p
 from pytorch_volumetric_b200 import _native as nat
-from test_trilinear_composed_cpu import _grid_desc, _sim_composed, _unpruned
-
-PVB_ERR_INVALID = -1        # include/pvb.h pvb_status
-
-_SIM_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-_SIM_LIB = os.path.join(_SIM_DIR, "_build", "libpvb_hostsim_paired.so")
-_sim = None
-
-
-def _simlib():
-    """tests/hostsim/hostsim_paired.cpp built like tests/hostsim (g++, -ffp-contract=off), rebuilt when stale."""
-    global _sim
-    if _sim is None:
-        root = os.path.dirname(os.path.dirname(_SIM_DIR))
-        sources = [os.path.join(_SIM_DIR, "hostsim_paired.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
-                   os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
-                   os.path.join(root, "include", "pvb.h")]
-        if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
-            os.makedirs(os.path.dirname(_SIM_LIB), exist_ok=True)
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                            "-I", _SIM_DIR, sources[0], "-o", _SIM_LIB], check=True)
-        _sim = ctypes.CDLL(_SIM_LIB)
-    return _sim
-
-
-def _p(a):
-    return ctypes.c_void_p(a.ctypes.data)
-
-
-def _sim_paired(descs, xforms, n_cfg, points, cfg_begin=0, order=None, nearest_first=1):
-    """(val, grad, which) of configurations cfg_begin.. at their own points [cfg_count, P, 3]."""
-    p = np.ascontiguousarray(points, dtype=np.float32)
-    cfg_count, P = p.shape[0], p.shape[1]
-    S = len(descs)
-    arr = (nat.SdfDesc * S)(*descs)
-    xf = np.ascontiguousarray(xforms, dtype=np.float32)
-    assert xf.shape == (S * n_cfg, 4, 4)
-    order = hs.bit_reversed_order(S) if order is None else list(order)
-    od = np.asarray(order, dtype=np.uint8)
-    margin_max = max([0.0] + [float(d.prune_margin) for d in descs])
-    n = cfg_count * P
-    val, grad, which = np.empty(n, np.float32), np.empty((n, 3), np.float32), np.empty(n, np.int32)
-    _simlib().simpair_composed(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
-                               ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(P), ctypes.c_int(nearest_first),
-                               ctypes.c_float(margin_max), _p(val), _p(grad), _p(which))
-    return val, grad, which
-
-
-def _table_descs(name):
-    z = golden(f"ref_cachedsdf_{name}")
-    shape = tuple(int(s) for s in z["table_shape"])
-    args = (torch.from_numpy(z["table_val"]).reshape(shape), torch.from_numpy(z["table_grad"]),
-            [tuple(r) for r in z["ranges"]], z["bb"])
-    near, k1 = _grid_desc(*args, interpolation="nearest")
-    tri, k2 = _grid_desc(*args, interpolation="trilinear")
-    return near, tri, (k1, k2)
-
-
-def _sets():
-    zc = golden("ref_composed")
-    sph = hs.sphere_desc(float(zc["sphere_radius"]))
-    pn, pt, k1 = _table_descs("probe")
-    dn, dt, k2 = _table_descs("drill")
-    return zc, [("nearest", [pn, pn, sph, pn]), ("trilinear", [pt, pt, sph, pt]), ("mixed", [pn, pt, sph, dt]),
-                ("drill", [dn, dt, dn, sph])], (k1, k2)
-
-
-def _own_points(q, A, seed):
-    """[A, P, 3]: the golden points, shuffled and shifted differently for every configuration."""
-    g = np.random.default_rng(seed)
-    q = np.asarray(q, dtype=np.float32)
-    return np.stack([q[g.permutation(len(q))] + g.normal(0.0, 0.01, 3).astype(np.float32) for _ in range(A)])
 
 
 def test_paired_equals_the_cross_product_diagonal(built_lib):
-    zc, sets, keep = _sets()
+    zc, sets, keep = hs.sets()
     S, A = int(zc["S"]), int(zc["A"])
-    own = _own_points(zc["q"], A, 0)
+    own = hs.own_points(zc["q"], A, 0)
     P = own.shape[1]
     for name, descs in sets:
         # the cross product over all A * P points, then configuration a's own block on its diagonal
-        cv, cg, cw = _sim_composed(descs, zc["tmat"], A, own.reshape(-1, 3))
+        cv, cg, cw = hs.composed(descs, zc["tmat"], A, own.reshape(-1, 3), ext=True)
         cv, cg, cw = cv.reshape(A, A, P), cg.reshape(A, A, P, 3), cw.reshape(A, A, P)
         dv = np.stack([cv[a, a] for a in range(A)]).reshape(-1)
         dg = np.stack([cg[a, a] for a in range(A)]).reshape(-1, 3)
         dw = np.stack([cw[a, a] for a in range(A)]).reshape(-1)
         for nearest_first in (1, 0):
-            v, g, w = _sim_paired(descs, zc["tmat"], A, own, nearest_first=nearest_first)
+            v, g, w = hs.sim_paired(descs, zc["tmat"], A, own, nearest_first=nearest_first)
             assert np.array_equal(v, dv) and np.array_equal(g, dg) and np.array_equal(w, dw), (name, nearest_first)
         # pruning off, other visiting orders
         for order in (range(S), list(range(S))[::-1], [2, 0, 3, 1]):
-            for d in (descs, _unpruned(descs)):
-                v, g, w = _sim_paired(d, zc["tmat"], A, own, order=order, nearest_first=0)
+            for d in (descs, hs.unpruned(descs)):
+                v, g, w = hs.sim_paired(d, zc["tmat"], A, own, order=order, nearest_first=0)
                 assert np.array_equal(v, dv) and np.array_equal(g, dg) and np.array_equal(w, dw), (name, order)
         # a slab of the configurations, indexed by the absolute configuration
-        v, g, w = _sim_paired(descs, zc["tmat"], A, own[1:3], cfg_begin=1)
+        v, g, w = hs.sim_paired(descs, zc["tmat"], A, own[1:3], cfg_begin=1)
         assert np.array_equal(v, dv[P:3 * P]) and np.array_equal(w, dw[P:3 * P]), name
 
 
 def test_paired_on_shared_points_equals_the_cross_product(built_lib):
     """The same points for every configuration: the paired query is the cross product itself."""
-    zc, sets, keep = _sets()
+    zc, sets, keep = hs.sets()
     A = int(zc["A"])
     q = np.asarray(zc["q"], dtype=np.float32)
     for name, descs in sets:
-        ref = _sim_composed(descs, zc["tmat"], A, q)
-        got = _sim_paired(descs, zc["tmat"], A, np.broadcast_to(q, (A,) + q.shape))
+        ref = hs.composed(descs, zc["tmat"], A, q, ext=True)
+        got = hs.sim_paired(descs, zc["tmat"], A, np.broadcast_to(q, (A,) + q.shape))
         assert all(np.array_equal(a, b) for a, b in zip(ref, got)), name
 
 
@@ -141,8 +67,8 @@ def test_pair_index_arithmetic_is_64_bit(built_lib, P):
     t = np.array(sorted({x for x in cand if 0 <= x < n_pairs}), dtype=np.int64)
     c, i = np.empty_like(t), np.empty_like(t)
     jit = np.empty(len(t), dtype=np.uint64)
-    _simlib().simpair_index(_p(t), ctypes.c_longlong(len(t)), ctypes.c_longlong(P), ctypes.c_int(cfg_begin),
-                            ctypes.c_int(S), ctypes.c_int(s), _p(c), _p(i), _p(jit))
+    hs.lib().simpair_index(_p(t), ctypes.c_longlong(len(t)), ctypes.c_longlong(P), ctypes.c_int(cfg_begin),
+                           ctypes.c_int(S), ctypes.c_int(s), _p(c), _p(i), _p(jit))
     for k, tk in enumerate(t.tolist()):
         assert (int(c[k]), int(i[k])) == divmod(tk, P), tk
         cfg = cfg_begin + tk // P
@@ -151,7 +77,7 @@ def test_pair_index_arithmetic_is_64_bit(built_lib, P):
 
 # ---------------------------------------------------------------- C ABI refusals (no kernel launch involved)
 def test_abi_refuses_invalid_paired_queries(built_lib):
-    near, tri, keep = _table_descs("probe")
+    near, tri, keep = hs.table_descs("probe")
     fake = ctypes.c_void_p(1 << 12)           # never dereferenced: every call below fails its argument checks
     L = built_lib
     arr = nat.desc_array([near, near])

@@ -1,7 +1,7 @@
 """CPU tier for analytic URDF primitives (BoxSDF, CylinderSDF, SphereSDF links) in the fused composed kernels.
 
-1. The device arithmetic (pvb_device.cuh compiled for the host by tests/hostsim/hostsim_primitive.cpp): box_eval,
-   cylinder_eval and primitive_eval against the fp64 restatements of tests/primitive_ref.py, with the tie rules.
+1. The device arithmetic (pvb_device.cuh compiled for the host, tests/hostsim_lib.py): box_eval, cylinder_eval and
+   primitive_eval against the fp64 restatements of tests/primitive_ref.py, with the tie rules.
 2. The bound contract the kernels' pruning relies on: value >= dist(q, bb) - prune_margin, with dist(q, bb) as the
    kernels compute it, and the serial robot kernel's sphere bound with primitive descriptors.
 3. composed_consider with the extension flag over a mixed set (golden probe table, nearest and trilinear, with box,
@@ -9,73 +9,31 @@
 4. The C ABI refusals of unknown kinds, and the Python construction of primitive links from a URDF."""
 import ctypes
 import logging
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 import hostsim_lib as hs
+from hostsim_lib import PVB_ERR_INVALID, _p
 import primitive_ref as pr
 from helpers import golden
 from oracle import port
 from pytorch_volumetric_b200 import _native as nat
 
-PVB_ERR_INVALID = -1        # include/pvb.h pvb_status
-
-_SIM_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-_SIM_LIB = os.path.join(_SIM_DIR, "_build", "libpvb_hostsim_primitive.so")
-_sim = None
-
-
-def _simlib():
-    """tests/hostsim/hostsim_primitive.cpp built like tests/hostsim (g++, -ffp-contract=off), rebuilt when stale."""
-    global _sim
-    if _sim is None:
-        root = os.path.dirname(os.path.dirname(_SIM_DIR))
-        sources = [os.path.join(_SIM_DIR, "hostsim_primitive.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
-                   os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
-                   os.path.join(root, "include", "pvb.h")]
-        if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
-            os.makedirs(os.path.dirname(_SIM_LIB), exist_ok=True)
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                            "-I", _SIM_DIR, sources[0], "-o", _SIM_LIB], check=True)
-        _sim = ctypes.CDLL(_SIM_LIB)
-    return _sim
-
-
-def _p(a):
-    return ctypes.c_void_p(a.ctypes.data)
-
 
 def _sim_eval(desc, points, fn=2):
     p = np.ascontiguousarray(points, dtype=np.float32); n = len(p)
     val, grad = np.empty(n, np.float32), np.empty((n, 3), np.float32)
-    _simlib().simprim_eval(ctypes.byref(desc), ctypes.c_int(fn), _p(p), ctypes.c_longlong(n), _p(val), _p(grad))
+    hs.lib().simprim_eval(ctypes.byref(desc), ctypes.c_int(fn), _p(p), ctypes.c_longlong(n), _p(val), _p(grad))
     return val, grad
 
 
 def _sim_lb2(desc, points):
     p = np.ascontiguousarray(points, dtype=np.float32); n = len(p)
     lb2 = np.empty(n, np.float32)
-    _simlib().simprim_aabb_lb2(ctypes.byref(desc), _p(p), ctypes.c_longlong(n), _p(lb2))
+    hs.lib().simprim_aabb_lb2(ctypes.byref(desc), _p(p), ctypes.c_longlong(n), _p(lb2))
     return lb2
-
-
-def _sim_composed(descs, xforms, n_cfg, points, order=None):
-    p = np.ascontiguousarray(points, dtype=np.float32); n = len(p); S = len(descs)
-    arr = (nat.SdfDesc * S)(*descs)
-    xf = np.ascontiguousarray(xforms, dtype=np.float32)
-    assert xf.shape == (S * n_cfg, 4, 4)
-    order = hs.bit_reversed_order(S) if order is None else list(order)
-    assert sorted(order) == list(range(S))
-    od = np.asarray(order, dtype=np.uint8)
-    val, grad = np.empty(n_cfg * n, np.float32), np.empty((n_cfg * n, 3), np.float32)
-    which = np.empty(n_cfg * n, np.int32)
-    _simlib().simprim_composed(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), _p(p), ctypes.c_longlong(n),
-                               _p(val), _p(grad), _p(which))
-    return val, grad, which
 
 
 def _prims():
@@ -227,8 +185,8 @@ def test_serial_sphere_bound_with_primitive_links():
             xf = np.ascontiguousarray(m, dtype=np.float32)
             lb = np.empty(len(pts), np.float32)
             vm = ctypes.c_float()
-            _simlib().simprim_sphere_lb(ctypes.byref(desc), _p(xf), _p(pts), ctypes.c_longlong(len(pts)), _p(lb),
-                                        ctypes.byref(vm))
+            hs.lib().simprim_sphere_lb(ctypes.byref(desc), _p(xf), _p(pts), ctypes.c_longlong(len(pts)), _p(lb),
+                                       ctypes.byref(vm))
             local = (pts.astype(np.float64) @ m[:3, :3].T.astype(np.float64) + m[:3, 3]).astype(np.float32)
             v, _ = _sim_eval(desc, local, fn)
             assert (lb <= v).all(), (name, float((lb - v).max()))
@@ -268,15 +226,6 @@ def _set(kind):
     return z, [grids["trilinear"], p["box"], p["cylinder"], p["sphere"], p["cube"]], keep
 
 
-def _unpruned(descs):
-    out = []
-    for d in descs:
-        c = d.copy()
-        c.flags &= ~nat.PVB_GRID_PRUNE_OK
-        out.append(c)
-    return out
-
-
 def _xforms(S, A, seed):
     import workloads
     return workloads.random_rigid(S * A, seed=seed, t_range=0.08).numpy()
@@ -294,16 +243,16 @@ def test_composed_extension_independent_of_pruning_and_order(kind):
     S, A = len(descs), 6
     xf = _xforms(S, A, 21)
     q = _points(z, 4000, 22)
-    ref = _sim_composed(descs, xf, A, q, order=range(S))
+    ref = hs.composed(descs, xf, A, q, order=range(S), mesh=False, ext=True)
     rng = np.random.default_rng(3)
     for order in (list(range(S))[::-1], hs.bit_reversed_order(S), list(rng.permutation(S))):
-        got = _sim_composed(descs, xf, A, q, order=order)
+        got = hs.composed(descs, xf, A, q, order=order, mesh=False, ext=True)
         assert all(np.array_equal(a, b) for a, b in zip(ref, got)), (kind, order)
     for order in (range(S), list(rng.permutation(S))):
-        got = _sim_composed(_unpruned(descs), xf, A, q, order=order)
+        got = hs.composed(hs.unpruned(descs), xf, A, q, order=order, mesh=False, ext=True)
         assert all(np.array_equal(a, b) for a, b in zip(ref, got)), (kind, "unpruned", order)
     # every sub-SDF alone (nothing to prune), argmin in numpy: first index on ties, like torch
-    per = [_sim_composed([descs[s]], xf[s * A:(s + 1) * A], A, q) for s in range(S)]
+    per = [hs.composed([descs[s]], xf[s * A:(s + 1) * A], A, q, mesh=False, ext=True) for s in range(S)]
     vals = np.stack([p[0] for p in per])
     assert np.array_equal(ref[2], vals.argmin(0).astype(np.int32)) and np.array_equal(ref[0], vals.min(0))
     assert len(set(ref[2].tolist())) == S            # every sub-SDF wins somewhere
@@ -329,7 +278,7 @@ def test_composed_extension_vs_fp64_composition():
                 vals[s, a], grads[s, a] = rv.numpy(), rg.numpy()
             else:
                 vals[s, a], grads[s, a] = pr.primitive_ref(descs[s], local)
-    v, gr, w = _sim_composed(descs, xf, A, q)
+    v, gr, w = hs.composed(descs, xf, A, q, mesh=False, ext=True)
     v, gr, w = v.reshape(A, P), gr.reshape(A, P, 3), w.reshape(A, P)
     which = vals.argmin(0)
     assert np.abs(v - vals.min(0)).max() < 5e-6
@@ -481,6 +430,6 @@ def test_sphere_sets_bit_identical_on_the_extension_path():
     sph = hs.sphere_desc(float(zc["sphere_radius"]))
     near = grids["nearest"]
     for descs in ([near, near, sph, near], [sph, near, near, sph], [p["sphere"], sph, near, near]):
-        old = hs.composed(descs, zc["tmat"], A, zc["q"])               # composed_consider<kMesh, kExt = false>
-        new = _sim_composed(descs, zc["tmat"], A, zc["q"])             # composed_consider<false, kExt = true>
+        old = hs.composed(descs, zc["tmat"], A, zc["q"])                            # composed_consider<true, false>
+        new = hs.composed(descs, zc["tmat"], A, zc["q"], mesh=False, ext=True)      # composed_consider<false, true>
         assert all(np.array_equal(a, b) for a, b in zip(old, new))

@@ -9,9 +9,8 @@ import torch
 
 import primitive_ref as pr
 import robot_ref as rr
-from test_gpu_robot_fp64 import (CHAINS, build_robot, fk_bound, joint_values, point_bound, tessellated_box,
-                                 write_chain)
-from test_host import MIXED_URDF
+from robot_ref import (CHAINS, MIXED_URDF, build_robot, fk_bound, joint_values, point_bound, tessellated_box,
+                       write_chain)
 
 
 def _oracle_chain_fp64(text, end):

@@ -5,39 +5,13 @@ the true point-to-AABB distance minus the prune margin -- the kernel's pruning i
 reject a link whose transform is not an isometry or whose descriptor lacks PVB_GRID_PRUNE_OK; slots beyond n_sdf are
 +inf.  The nearest-link selection over such bounds always names a real link."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
 import hostsim_lib as hs
+from hostsim_lib import _p
 import workloads
 from pytorch_volumetric_b200 import _native as nat
-
-_SIM_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-_SIM_LIB = os.path.join(_SIM_DIR, "_build", "libpvb_hostsim_rsbound.so")
-_sim = None
-
-
-def _simlib():
-    """tests/hostsim/hostsim_rsbound.cpp built like tests/hostsim (g++, -ffp-contract=off), rebuilt when stale."""
-    global _sim
-    if _sim is None:
-        root = os.path.dirname(os.path.dirname(_SIM_DIR))
-        sources = [os.path.join(_SIM_DIR, "hostsim_rsbound.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
-                   os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
-                   os.path.join(root, "include", "pvb.h")]
-        if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
-            os.makedirs(os.path.dirname(_SIM_LIB), exist_ok=True)
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                            "-I", _SIM_DIR, sources[0], "-o", _SIM_LIB], check=True)
-        _sim = ctypes.CDLL(_SIM_LIB)
-        _sim.simrs_visit_margin.restype = ctypes.c_float
-    return _sim
-
-
-def _p(a):
-    return ctypes.c_void_p(a.ctypes.data)
 
 
 def _box_desc(rng, prune_ok=True):
@@ -57,7 +31,7 @@ def _sphere_lb(descs, xforms, n_cfg, pts):
     arr = (nat.SdfDesc * len(descs))(*descs)
     xf = np.ascontiguousarray(xforms, dtype=np.float32)
     p = np.ascontiguousarray(pts, dtype=np.float32)
-    _simlib().simrs_sphere_lb(arr, len(descs), _p(xf), n_cfg, _p(p), ctypes.c_longlong(len(p)), _p(lb))
+    hs.lib().simrs_sphere_lb(arr, len(descs), _p(xf), n_cfg, _p(p), ctypes.c_longlong(len(p)), _p(lb))
     return lb
 
 
@@ -102,8 +76,8 @@ def test_non_isometric_and_unprunable_links_are_never_rejected():
     assert never(lb[:, :, 1]).all()
     assert never(lb[0::2, :, 2]).all() and np.isfinite(lb[1::2, :, 2]).all()
     assert np.isfinite(lb[:, :, [0, 3]]).all()
-    assert _simlib().simrs_visit_margin(ctypes.byref(descs[0])) == np.float32(descs[0].prune_margin)
-    assert np.isposinf(_simlib().simrs_visit_margin(ctypes.byref(descs[1])))
+    assert hs.lib().simrs_visit_margin(ctypes.byref(descs[0])) == np.float32(descs[0].prune_margin)
+    assert np.isposinf(hs.lib().simrs_visit_margin(ctypes.byref(descs[1])))
     # the first link to visit is always a real one, whatever mix of finite, -inf, NaN and +inf bounds comes in
     rows = lb.reshape(-1, 8)
     pred = np.empty(len(rows), np.int32)

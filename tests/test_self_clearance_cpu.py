@@ -14,57 +14,14 @@ points of every source sub-SDF against the sub-SDFs its row of `allowed` names.
 4. The C ABI refusals and the Python shape rules, without a GPU."""
 import ctypes
 import math
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+import hostsim_lib as hs
+from hostsim_lib import PVB_ERR_INVALID, _p
 from pytorch_volumetric_b200 import _native as nat
-from test_paired_clearance_cpu import _finish as _pcl_finish, _fused_keys as _pcl_keys
-from test_paired_cpu import _table_descs
-from test_swept_cpu import _all_sets, _trajectory
-
-PVB_ERR_INVALID = -1        # include/pvb.h pvb_status
-
-_SIM_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-_SIM_LIB = os.path.join(_SIM_DIR, "_build", "libpvb_hostsim_self_clearance.so")
-_sim = None
-
-
-def _simlib():
-    """tests/hostsim/hostsim_self_clearance.cpp built like tests/hostsim (g++, -ffp-contract=off), rebuilt when
-    stale."""
-    global _sim
-    if _sim is None:
-        root = os.path.dirname(os.path.dirname(_SIM_DIR))
-        sources = [os.path.join(_SIM_DIR, "hostsim_self_clearance.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
-                   os.path.join(_SIM_DIR, "hostsim_robot.h"),
-                   os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
-                   os.path.join(root, "include", "pvb.h")]
-        if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
-            os.makedirs(os.path.dirname(_SIM_LIB), exist_ok=True)
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                            "-I", _SIM_DIR, sources[0], "-o", _SIM_LIB], check=True)
-        _sim = ctypes.CDLL(_SIM_LIB)
-        _sim.simscl_key.restype = ctypes.c_uint64
-        _sim.simscl_key.argtypes = [ctypes.c_float, ctypes.c_int, ctypes.c_int]
-    return _sim
-
-
-def _p(a):
-    return ctypes.c_void_p(a.ctypes.data)
-
-
-def _masks(allowed):
-    S = len(allowed)
-    return np.array([sum(1 << j for j in range(S) if allowed[i][j] and j != i) for i in range(S)], dtype=np.uint8)
-
-
-def _inverse(xforms):
-    """W = M^-1 in fp64, rounded to fp32 (any fp32 matrix serves: both routes read the same W)."""
-    return np.linalg.inv(np.asarray(xforms, dtype=np.float64)).astype(np.float32)
 
 
 def _fused(descs, xf, inv, n_cfg, lp, allowed, cfg_begin=0, cfg_count=None, chunk=None, lanes=32, share=1,
@@ -74,11 +31,11 @@ def _fused(descs, xf, inv, n_cfg, lp, allowed, cfg_begin=0, cfg_count=None, chun
     cfg_count = n_cfg - cfg_begin if cfg_count is None else cfg_count
     keys = np.empty(cfg_count, np.uint64)
     visits = np.zeros(64, np.int64)
-    _simlib().simscl_fused((nat.SdfDesc * S)(*descs), ctypes.c_int(S), _p(xf), _p(inv), ctypes.c_int(n_cfg),
-                           ctypes.c_int(cfg_begin), ctypes.c_int(cfg_count), _p(lp), ctypes.c_int(K),
-                           _p(_masks(allowed)), ctypes.c_int(chunk or K), ctypes.c_int(lanes), ctypes.c_int(share),
-                           ctypes.c_int(unit_order), ctypes.c_int(shuffle_seed), ctypes.c_int(seeded),
-                           ctypes.c_int(first), _p(keys), _p(visits))
+    hs.lib().simscl_fused((nat.SdfDesc * S)(*descs), ctypes.c_int(S), _p(xf), _p(inv), ctypes.c_int(n_cfg),
+                          ctypes.c_int(cfg_begin), ctypes.c_int(cfg_count), _p(lp), ctypes.c_int(K),
+                          _p(hs.masks(allowed)), ctypes.c_int(chunk or K), ctypes.c_int(lanes), ctypes.c_int(share),
+                          ctypes.c_int(unit_order), ctypes.c_int(shuffle_seed), ctypes.c_int(seeded),
+                          ctypes.c_int(first), _p(keys), _p(visits))
     return keys, visits.reshape(8, 8)
 
 
@@ -87,9 +44,9 @@ def _finish(descs, xf, inv, n_cfg, lp, allowed, keys, cfg_begin=0):
     R = len(keys)
     out = (np.empty(R, np.float32), np.empty((R, 3), np.float32), np.empty(R, np.int32), np.empty(R, np.int32),
            np.empty(R, np.int32))
-    _simlib().simscl_finish((nat.SdfDesc * S)(*descs), ctypes.c_int(S), _p(xf), _p(inv), ctypes.c_int(n_cfg),
-                            ctypes.c_int(cfg_begin), ctypes.c_int(R), _p(lp), ctypes.c_int(K), _p(_masks(allowed)),
-                            _p(np.ascontiguousarray(keys)), *[_p(a) for a in out])
+    hs.lib().simscl_finish((nat.SdfDesc * S)(*descs), ctypes.c_int(S), _p(xf), _p(inv), ctypes.c_int(n_cfg),
+                           ctypes.c_int(cfg_begin), ctypes.c_int(R), _p(lp), ctypes.c_int(K), _p(hs.masks(allowed)),
+                           _p(np.ascontiguousarray(keys)), *[_p(a) for a in out])
     return out
 
 
@@ -101,7 +58,7 @@ def _pose(inv, n_cfg, i, lp_i, cfg_begin, cfg_count):
     w = np.ascontiguousarray(w)
     p = np.ascontiguousarray(lp_i, dtype=np.float32)
     out = np.empty((cfg_count, len(p), 3), np.float32)
-    _simlib().simscl_pose(_p(w), ctypes.c_int(cfg_count), _p(p), ctypes.c_int(len(p)), _p(out))
+    hs.lib().simscl_pose(_p(w), ctypes.c_int(cfg_count), _p(p), ctypes.c_int(len(p)), _p(out))
     return out
 
 
@@ -120,8 +77,8 @@ def _composition_route(descs, xf, inv, n_cfg, lp, allowed, cfg_begin=0, cfg_coun
         x = _pose(inv, n_cfg, i, lp[i], cfg_begin, cfg_count)[:, None]              # [cfg_count, 1, K, 3]
         sub = [descs[j] for j in js]
         sub_xf = np.ascontiguousarray(tm[js].reshape(len(js) * n_cfg, 4, 4))
-        keys = _pcl_keys(sub, sub_xf, n_cfg, x, cfg_begin=cfg_begin)[0]
-        v, g, pt, w = _pcl_finish(sub, sub_xf, n_cfg, x, keys, cfg_begin=cfg_begin)
+        keys = hs.pcl_keys(sub, sub_xf, n_cfg, x, cfg_begin=cfg_begin)[0]
+        v, g, pt, w = hs.pcl_finish(sub, sub_xf, n_cfg, x, keys, cfg_begin=cfg_begin)
         per.append((i, v, g, pt, np.asarray(js, np.int32)[w]))
     if not per:
         return (np.full(cfg_count, np.inf, np.float32), np.zeros((cfg_count, 3), np.float32),
@@ -142,31 +99,8 @@ def _assert_same(got, ref, what):
 
 
 def _key_of(ref):
-    return np.array([_simlib().simscl_key(float(v), int(i), int(k)) for v, i, k in zip(ref[0], ref[2], ref[3])],
+    return np.array([hs.lib().simscl_key(float(v), int(i), int(k)) for v, i, k in zip(ref[0], ref[2], ref[3])],
                     np.uint64)
-
-
-def _link_points(zc, tm, S, n_cfg, K, seed):
-    """[S, K, 3] fp32: golden query points near the object, carried into every sub-SDF's frame by configuration 0's
-    transform -- posed by another configuration they land near the other sub-SDFs."""
-    g = np.random.default_rng(seed)
-    q = np.asarray(zc["q"], dtype=np.float64)
-    m = np.asarray(tm, dtype=np.float64).reshape(S, n_cfg, 4, 4)[:, 0]
-    out = np.empty((S, K, 3))
-    for i in range(S):
-        pts = q[g.choice(len(q), K, replace=K > len(q))] + g.normal(0.0, 0.01, 3)
-        out[i] = pts @ m[i, :3, :3].T + m[i, :3, 3]
-    return out.astype(np.float32)
-
-
-def _allowed_cases(S):
-    full = [[i != j for j in range(S)] for i in range(S)]
-    asym = [[j > i for j in range(S)] for i in range(S)]                        # upper triangle only
-    row0 = [[i != j and i != 1 for j in range(S)] for i in range(S)]            # row 1 empty
-    sparse = [[False] * S for _ in range(S)]
-    sparse[S - 1][0] = True
-    return {"full": full, "asymmetric": asym, "empty row": row0, "one pair": sparse,
-            "empty": [[False] * S for _ in range(S)]}
 
 
 # ---------------------------------------------------------------- 1. key packing
@@ -174,7 +108,7 @@ def test_self_clearance_key_orders_value_then_source_then_point():
     values = [-np.inf, -1.5, -1e-30, -0.0, 0.0, 1e-30, 0.25, 0.25000003, np.inf, np.nan]
     ks = [0, 1, 2, (1 << 24) - 2, (1 << 24) - 1]
     cands = [(v, i, k) for v in values for i in range(8) for k in ks]
-    keys = [_simlib().simscl_key(v, i, k) for v, i, k in cands]
+    keys = [hs.lib().simscl_key(v, i, k) for v, i, k in cands]
 
     def rank(c):
         v, i, k = c
@@ -191,16 +125,16 @@ def test_self_clearance_key_orders_value_then_source_then_point():
 # ---------------------------------------------------------------- 2. the fused sequence against the composition
 @pytest.mark.parametrize("A", [3, 37])
 def test_fused_self_clearance_equals_the_composition_route(built_lib, A):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = zc["tmat"] if A == A0 else _trajectory(zc["tmat"], S, A0, A, seed=A)
+    tm = zc["tmat"] if A == A0 else hs.trajectory(zc["tmat"], S, A0, A, seed=A)
     tm = np.ascontiguousarray(tm, dtype=np.float32)
-    inv = _inverse(tm)
+    inv = hs.inverse(tm)
     for name, descs in sets:
         S = len(descs)
         for K in (1, 45, 130):
-            lp = _link_points(zc, tm, S, A, K, seed=K + A)
-            for case, allowed in _allowed_cases(S).items():
+            lp = hs.link_points(zc, tm, S, A, K, seed=K + A)
+            for case, allowed in hs.allowed_cases(S).items():
                 ref = _composition_route(descs, tm, inv, A, lp, allowed)
                 keys, visits = _fused(descs, tm, inv, A, lp, allowed)
                 _assert_same(_finish(descs, tm, inv, A, lp, allowed, keys), ref, (name, K, case))
@@ -209,7 +143,7 @@ def test_fused_self_clearance_equals_the_composition_route(built_lib, A):
                     continue
                 assert np.array_equal(keys, _key_of(ref)), (name, K, case)
                 # a masked link is never visited
-                m = _masks(allowed)
+                m = hs.masks(allowed)
                 for i in range(S):
                     for j in range(8):
                         if not (int(m[i]) >> j) & 1:
@@ -224,7 +158,7 @@ def test_fused_self_clearance_equals_the_composition_route(built_lib, A):
                     got = _fused(descs, tm, inv, A, lp, allowed, chunk=32, first=first, lanes=64)[0]
                     assert np.array_equal(got, keys), (name, K, case, first)
             # slabs: the absolute configuration picks the transforms
-            allowed = _allowed_cases(S)["full"]
+            allowed = hs.allowed_cases(S)["full"]
             for begin, count in ((1, A - 1), (A // 2, 1), (A - 2, 2)):
                 ks = _fused(descs, tm, inv, A, lp, allowed, cfg_begin=begin, cfg_count=count, chunk=32)[0]
                 _assert_same(_finish(descs, tm, inv, A, lp, allowed, ks, cfg_begin=begin),
@@ -233,30 +167,30 @@ def test_fused_self_clearance_equals_the_composition_route(built_lib, A):
 
 def test_self_clearance_argmins_vary(built_lib):
     """The golden sub-SDFs overlap: configurations in collision, values that differ, and an argmin that moves."""
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = np.ascontiguousarray(_trajectory(zc["tmat"], S, A0, 40, seed=5), dtype=np.float32)
-    inv = _inverse(tm)
+    tm = np.ascontiguousarray(hs.trajectory(zc["tmat"], S, A0, 40, seed=5), dtype=np.float32)
+    inv = hs.inverse(tm)
     for name, descs in sets:
         S = len(descs)
-        lp = _link_points(zc, tm, S, 40, 64, seed=9)
-        ref = _composition_route(descs, tm, inv, 40, lp, _allowed_cases(S)["full"])
+        lp = hs.link_points(zc, tm, S, 40, 64, seed=9)
+        ref = _composition_route(descs, tm, inv, 40, lp, hs.allowed_cases(S)["full"])
         assert (ref[0] < 0).any() and len(set(ref[0].tolist())) > 1, name
         assert len(set(zip(ref[2].tolist(), ref[3].tolist()))) > 1, name
 
 
 def test_ties_report_the_first_source_and_point(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    base = _trajectory(zc["tmat"], S, A0, 6, seed=7).reshape(S, 6, 4, 4)
+    base = hs.trajectory(zc["tmat"], S, A0, 6, seed=7).reshape(S, 6, 4, 4)
     descs = sets[0][1]
     # sub-SDF 0 listed twice (positions 0 and 2) under the same transforms, with the same link points; every link's
     # points twice in a row
     dup = [descs[0], descs[1], descs[0], descs[2]]
     tm = np.ascontiguousarray(np.concatenate([base[0:1], base[1:2], base[0:1], base[2:3]]).reshape(24, 4, 4),
                               dtype=np.float32)
-    inv = _inverse(tm)
-    lp = _link_points(zc, tm, 4, 6, 50, seed=3)
+    inv = hs.inverse(tm)
+    lp = hs.link_points(zc, tm, 4, 6, 50, seed=3)
     lp[2] = lp[0]
     lp = np.ascontiguousarray(np.concatenate([lp, lp], axis=1))
     allowed = [[i != j and {i, j} != {0, 2} for j in range(4)] for i in range(4)]
@@ -347,7 +281,7 @@ def test_link_surface_points_of_primitives_lie_on_the_surface(tmp_path):
 
 # ---------------------------------------------------------------- 4. C ABI refusals (no kernel launch involved)
 def test_abi_refuses_invalid_self_clearance_queries(built_lib):
-    near, tri, keep = _table_descs("probe")
+    near, tri, keep = hs.table_descs("probe")
     fake = ctypes.c_void_p(1 << 12)           # never dereferenced: every call below fails its argument checks
     L = built_lib
     arr = nat.desc_array([near, near, tri])

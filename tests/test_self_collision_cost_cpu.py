@@ -16,46 +16,15 @@ the target, -tau to the source), and for a robot its joint gradient.
 4. The C ABI refusals and the Python shape rules, without a GPU."""
 import ctypes
 import math
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 import hostsim_lib as hs
+from hostsim_lib import PVB_ERR_INVALID, _p
 from pytorch_volumetric_b200 import _native as nat
-from test_paired_cpu import _sim_paired, _table_descs
-from test_self_clearance_cpu import _allowed_cases, _inverse, _link_points, _masks
-from test_swept_cpu import _all_sets, _trajectory
-
-PVB_ERR_INVALID = -1        # include/pvb.h pvb_status
-
-_SIM_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-_SIM_LIB = os.path.join(_SIM_DIR, "_build", "libpvb_hostsim_self_collision_cost.so")
-_sim = None
-
-
-def _simlib():
-    """tests/hostsim/hostsim_self_collision_cost.cpp built like tests/hostsim (g++, -ffp-contract=off), rebuilt when
-    stale."""
-    global _sim
-    if _sim is None:
-        root = os.path.dirname(os.path.dirname(_SIM_DIR))
-        sources = [os.path.join(_SIM_DIR, "hostsim_self_collision_cost.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
-                   os.path.join(_SIM_DIR, "hostsim_robot.h"),
-                   os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
-                   os.path.join(root, "include", "pvb.h")]
-        if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
-            os.makedirs(os.path.dirname(_SIM_LIB), exist_ok=True)
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                            "-I", _SIM_DIR, sources[0], "-o", _SIM_LIB], check=True)
-        _sim = ctypes.CDLL(_SIM_LIB)
-    return _sim
-
-
-def _p(a):
-    return ctypes.c_void_p(a.ctypes.data)
+from robot_ref import build_robot, joint_values
 
 
 def _fused(descs, xf, inv, n_cfg, lp, allowed, margin, cfg_begin=0, cfg_count=None, lanes=32, cfg_order=0,
@@ -70,11 +39,11 @@ def _fused(descs, xf, inv, n_cfg, lp, allowed, margin, cfg_begin=0, cfg_count=No
     vis, pv, pg, pw, px = np.empty(NP, np.uint8), np.empty(NP, np.float32), np.empty((NP, 3), np.float32), \
         np.empty(NP, np.int32), np.empty((NP, 3), np.float32)
     evals = ctypes.c_longlong(0)
-    _simlib().simscc_fused((nat.SdfDesc * S)(*descs), ctypes.c_int(S), _p(xf), _p(inv), ctypes.c_int(n_cfg),
-                           ctypes.c_int(cfg_begin), ctypes.c_int(cfg_count), _p(lp), ctypes.c_int(K),
-                           _p(_masks(allowed)), ctypes.c_float(margin), ctypes.c_int(lanes), ctypes.c_int(cfg_order),
-                           ctypes.c_int(shuffle_seed), ctypes.c_int(first), _p(cost), _p(twist), _p(vis), _p(pv),
-                           _p(pg), _p(pw), _p(px), ctypes.byref(evals))
+    hs.lib().simscc_fused((nat.SdfDesc * S)(*descs), ctypes.c_int(S), _p(xf), _p(inv), ctypes.c_int(n_cfg),
+                          ctypes.c_int(cfg_begin), ctypes.c_int(cfg_count), _p(lp), ctypes.c_int(K),
+                          _p(hs.masks(allowed)), ctypes.c_float(margin), ctypes.c_int(lanes), ctypes.c_int(cfg_order),
+                          ctypes.c_int(shuffle_seed), ctypes.c_int(first), _p(cost), _p(twist), _p(vis), _p(pv),
+                          _p(pg), _p(pw), _p(px), ctypes.byref(evals))
     sh = (cfg_count, S, K)
     return (cost, twist, vis.astype(bool).reshape(sh), pv.reshape(sh), pg.reshape(*sh, 3), pw.reshape(sh),
             px.reshape(*sh, 3), evals.value)
@@ -86,7 +55,7 @@ def _pose(inv, n_cfg, i, lp_i):
     w = np.ascontiguousarray(np.asarray(inv, dtype=np.float32).reshape(S, n_cfg, 4, 4)[i])
     p = np.ascontiguousarray(lp_i, dtype=np.float32)
     out = np.empty((n_cfg, len(p), 3), np.float32)
-    _simlib().simscc_pose(_p(w), ctypes.c_int(n_cfg), _p(p), ctypes.c_int(len(p)), _p(out))
+    hs.lib().simscc_pose(_p(w), ctypes.c_int(n_cfg), _p(p), ctypes.c_int(len(p)), _p(out))
     return out
 
 
@@ -106,7 +75,7 @@ def _per_point(descs, xf, inv, n_cfg, lp, allowed):
         if not js:
             continue
         sub_xf = np.ascontiguousarray(tm[js].reshape(len(js) * n_cfg, 4, 4))
-        vi, gi, wi = _sim_paired([descs[j] for j in js], sub_xf, n_cfg, x[:, i])
+        vi, gi, wi = hs.sim_paired([descs[j] for j in js], sub_xf, n_cfg, x[:, i])
         v[:, i], g[:, i] = vi.reshape(n_cfg, K), gi.reshape(n_cfg, K, 3)
         w[:, i] = np.asarray(js, np.int32)[wi.reshape(n_cfg, K)]
     return v, g, w, x
@@ -148,17 +117,17 @@ def _margin(v, allowed_pairs, q):
 # ---------------------------------------------------------------- 1. the kernel's sequence
 @pytest.mark.parametrize("A", [3, 37])
 def test_fused_self_collision_cost_equals_the_fp64_sum(built_lib, A):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S0, A0 = int(zc["S"]), int(zc["A"])
-    tm = zc["tmat"] if A == A0 else _trajectory(zc["tmat"], S0, A0, A, seed=A)
+    tm = zc["tmat"] if A == A0 else hs.trajectory(zc["tmat"], S0, A0, A, seed=A)
     tm = np.ascontiguousarray(tm, dtype=np.float32)
-    inv = _inverse(tm)
+    inv = hs.inverse(tm)
     contributed = 0
     for name, descs in sets:
         S = len(descs)
         for K in (1, 45, 130):
-            lp = _link_points(zc, tm, S, A, K, seed=K + A)
-            for case, allowed in _allowed_cases(S).items():
+            lp = hs.link_points(zc, tm, S, A, K, seed=K + A)
+            for case, allowed in hs.allowed_cases(S).items():
                 v, g, w, x = _per_point(descs, tm, inv, A, lp, allowed)
                 if case == "empty":
                     cost, twist = _fused(descs, tm, inv, A, lp, allowed, 0.05)[:2]
@@ -193,15 +162,15 @@ def test_fused_self_collision_cost_equals_the_fp64_sum(built_lib, A):
 
 
 def test_slabs_reproduce_the_rows_of_the_full_call(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S0, A0 = int(zc["S"]), int(zc["A"])
     A = 40
-    tm = np.ascontiguousarray(_trajectory(zc["tmat"], S0, A0, A, seed=11), dtype=np.float32)
-    inv = _inverse(tm)
+    tm = np.ascontiguousarray(hs.trajectory(zc["tmat"], S0, A0, A, seed=11), dtype=np.float32)
+    inv = hs.inverse(tm)
     for name, descs in sets:
         S = len(descs)
-        lp = _link_points(zc, tm, S, A, 70, seed=4)
-        allowed = _allowed_cases(S)["full"]
+        lp = hs.link_points(zc, tm, S, A, 70, seed=4)
+        allowed = hs.allowed_cases(S)["full"]
         v, _, w, _ = _per_point(descs, tm, inv, A, lp, allowed)
         m = _margin(v, w >= 0, 0.2)
         cost, twist = _fused(descs, tm, inv, A, lp, allowed, m)[:2]
@@ -216,15 +185,15 @@ def test_slabs_reproduce_the_rows_of_the_full_call(built_lib):
 def test_ties_and_duplicated_points(built_lib):
     """A sub-SDF listed twice under the same transforms (ties between targets: the first wins) and every link's
     points twice in a row (identical terms from two lanes)."""
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S0, A0 = int(zc["S"]), int(zc["A"])
-    base = _trajectory(zc["tmat"], S0, A0, 6, seed=7).reshape(S0, 6, 4, 4)
+    base = hs.trajectory(zc["tmat"], S0, A0, 6, seed=7).reshape(S0, 6, 4, 4)
     for name, descs in sets[:3]:
         dup = [descs[0], descs[1], descs[0], descs[2]]
         tm = np.ascontiguousarray(np.concatenate([base[0:1], base[1:2], base[0:1], base[2:3]]).reshape(24, 4, 4),
                                   dtype=np.float32)
-        inv = _inverse(tm)
-        lp = _link_points(zc, tm, 4, 6, 50, seed=3)
+        inv = hs.inverse(tm)
+        lp = hs.link_points(zc, tm, 4, 6, 50, seed=3)
         lp[2] = lp[0]
         lp = np.ascontiguousarray(np.concatenate([lp, lp], axis=1))
         allowed = [[i != j and {i, j} != {0, 2} for j in range(4)] for i in range(4)]
@@ -292,26 +261,25 @@ def test_sign_convention_on_two_spheres(built_lib):
 
 
 def test_far_apart_links_and_empty_rows_cost_exactly_zero(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S0, A = int(zc["S"]), int(zc["A"])
     tm = np.ascontiguousarray(zc["tmat"], dtype=np.float32)
-    inv = _inverse(tm)
+    inv = hs.inverse(tm)
     for name, descs in sets:
         S = len(descs)
-        lp = _link_points(zc, tm, S, A, 40, seed=2)
+        lp = hs.link_points(zc, tm, S, A, 40, seed=2)
         # every source's points far from every link: each step is skipped by its bounds
         far = np.ascontiguousarray(lp + np.float32(50.0))
         inv_far = inv.copy()
-        cost, twist, vis, pv, pg, pw, px, evals = _fused(descs, tm, inv_far, A, far, _allowed_cases(S)["full"], 0.05)
+        cost, twist, vis, pv, pg, pw, px, evals = _fused(descs, tm, inv_far, A, far, hs.allowed_cases(S)["full"], 0.05)
         assert not cost.any() and not twist.any() and not vis.any() and evals == 0, name
         # no allowed pair at all
-        cost, twist, vis, pv, pg, pw, px, evals = _fused(descs, tm, inv, A, lp, _allowed_cases(S)["empty"], 1e3)
+        cost, twist, vis, pv, pg, pw, px, evals = _fused(descs, tm, inv, A, lp, hs.allowed_cases(S)["empty"], 1e3)
         assert not cost.any() and not twist.any() and not vis.any() and evals == 0, name
 
 
 # ---------------------------------------------------------------- 3. the joint gradient of a serial chain
 def test_joint_gradient_equals_finite_differences(tmp_path):
-    from test_gpu_robot_fp64 import build_robot, joint_values
     from robot_ref import rigid_inverse
     robot, ref, text = build_robot("mixed", tmp_path, dtype=torch.float64, device="cpu")
     J, S = len(robot.joint_names), len(robot.sdf_to_link_name)
@@ -382,7 +350,7 @@ def test_joint_gradient_equals_finite_differences(tmp_path):
 
 # ---------------------------------------------------------------- 4. C ABI refusals and Python rules (no device)
 def test_abi_refuses_invalid_self_collision_cost_queries(built_lib):
-    near, tri, keep = _table_descs("probe")
+    near, tri, keep = hs.table_descs("probe")
     fake = ctypes.c_void_p(1 << 12)           # never dereferenced: every call below fails its argument checks
     L = built_lib
     arr = nat.desc_array([near, near, tri])

@@ -9,44 +9,14 @@ the minimum over the configurations.
 2. Ties on purpose: duplicated configurations and duplicated sub-SDFs report the first of each.
 3. The C ABI refusals and the Python shape rules, without a GPU."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 import hostsim_lib as hs
+from hostsim_lib import PVB_ERR_INVALID, _p
 from pytorch_volumetric_b200 import _native as nat
-from test_paired_cpu import _sets, _table_descs
-from test_trilinear_composed_cpu import _sim_composed, _unpruned
-
-PVB_ERR_INVALID = -1        # include/pvb.h pvb_status
-
-_SIM_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-_SIM_LIB = os.path.join(_SIM_DIR, "_build", "libpvb_hostsim_swept.so")
-_sim = None
-
-
-def _simlib():
-    """tests/hostsim/hostsim_swept.cpp built like tests/hostsim (g++, -ffp-contract=off), rebuilt when stale."""
-    global _sim
-    if _sim is None:
-        root = os.path.dirname(os.path.dirname(_SIM_DIR))
-        sources = [os.path.join(_SIM_DIR, "hostsim_swept.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
-                   os.path.join(_SIM_DIR, "hostsim_robot.h"),
-                   os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
-                   os.path.join(root, "include", "pvb.h")]
-        if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
-            os.makedirs(os.path.dirname(_SIM_LIB), exist_ok=True)
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                            "-I", _SIM_DIR, sources[0], "-o", _SIM_LIB], check=True)
-        _sim = ctypes.CDLL(_SIM_LIB)
-    return _sim
-
-
-def _p(a):
-    return ctypes.c_void_p(a.ctypes.data)
 
 
 def _outs(n):
@@ -63,9 +33,9 @@ def _sim_fused(descs, xforms, n_cfg, points, cfg_begin=0, cfg_count=None, first=
     assert xf.shape == (S * n_cfg, 4, 4) and S <= 8
     out = _outs(len(p))
     evals = ctypes.c_longlong(0)
-    _simlib().simswept_fused(arr, ctypes.c_int(S), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
-                             ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(len(p)), ctypes.c_int(first),
-                             ctypes.c_int(lanes_reversed), *[_p(a) for a in out], ctypes.byref(evals))
+    hs.lib().simswept_fused(arr, ctypes.c_int(S), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
+                            ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(len(p)), ctypes.c_int(first),
+                            ctypes.c_int(lanes_reversed), *[_p(a) for a in out], ctypes.byref(evals))
     return out + (evals.value,)
 
 
@@ -79,9 +49,9 @@ def _sim_generic(descs, xforms, n_cfg, points, cfg_begin=0, cfg_count=None):
     od = np.asarray(hs.bit_reversed_order(S), dtype=np.uint8)
     margin_max = max([0.0] + [float(d.prune_margin) for d in descs])
     out = _outs(len(p))
-    _simlib().simswept_generic(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
-                               ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(len(p)), ctypes.c_float(margin_max),
-                               *[_p(a) for a in out])
+    hs.lib().simswept_generic(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), ctypes.c_int(cfg_begin),
+                              ctypes.c_int(cfg_count), _p(p), ctypes.c_longlong(len(p)), ctypes.c_float(margin_max),
+                              *[_p(a) for a in out])
     return out
 
 
@@ -89,44 +59,13 @@ def _reference(descs, xforms, n_cfg, points, cfg_begin=0, cfg_count=None):
     """The lexicographic (value, configuration, sub-SDF) reduction of the per-configuration results."""
     cfg_count = n_cfg - cfg_begin if cfg_count is None else cfg_count
     P = len(points)
-    v, g, w = _sim_composed(descs, xforms, n_cfg, points)
+    v, g, w = hs.composed(descs, xforms, n_cfg, points, ext=True)
     v = v.reshape(n_cfg, P)[cfg_begin:cfg_begin + cfg_count]
     g = g.reshape(n_cfg, P, 3)[cfg_begin:cfg_begin + cfg_count]
     w = w.reshape(n_cfg, P)[cfg_begin:cfg_begin + cfg_count]
     c = np.argmax(v == v.min(axis=0), axis=0)                 # first configuration attaining the minimum
     i = np.arange(P)
     return v[c, i], g[c, i], (c + cfg_begin).astype(np.int32), w[c, i]
-
-
-def _trajectory(tmat, S, A0, A, seed):
-    """[S * A, 4, 4]: A configurations, configuration a the golden configuration a % A0 moved by a small rigid motion
-    of the object frame (a robot-like sweep: the same motion for every sub-SDF of a configuration)."""
-    g = np.random.default_rng(seed)
-    m = np.asarray(tmat, dtype=np.float64).reshape(S, A0, 4, 4)
-    out = np.empty((S, A, 4, 4))
-    for a in range(A):
-        w = g.normal(0.0, 0.15, 3)
-        th = np.linalg.norm(w)
-        k = np.array([[0, -w[2], w[1]], [w[2], 0, -w[0]], [-w[1], w[0], 0]]) / max(th, 1e-12)
-        T = np.eye(4)
-        T[:3, :3] = np.eye(3) + np.sin(th) * k + (1 - np.cos(th)) * (k @ k)
-        T[:3, 3] = g.normal(0.0, 0.01, 3)
-        out[:, a] = m[:, a % A0] @ T
-    return out.reshape(S * A, 4, 4).astype(np.float32)
-
-
-def _primitive_set():
-    import pytorch_volumetric_b200 as pv
-    return [pv.BoxSDF([0.05, 0.03, 0.04]).native_desc("cpu"), pv.CylinderSDF(0.015, 0.06).native_desc("cpu"),
-            pv.SphereSDF(0.02).native_desc("cpu"), pv.BoxSDF([0.02, 0.02, 0.08]).native_desc("cpu")]
-
-
-def _all_sets():
-    zc, sets, keep = _sets()
-    _, tri_probe, keep2 = _table_descs("probe")
-    prim = _primitive_set()
-    return zc, sets + [("primitive", prim), ("primitive+grid", [prim[0], sets[0][1][0], prim[1], tri_probe])], \
-        (keep, keep2)
 
 
 def _assert_same(got, ref, what):
@@ -136,9 +75,9 @@ def _assert_same(got, ref, what):
 
 @pytest.mark.parametrize("A", [3, 40])
 def test_fused_swept_equals_the_reduction(built_lib, A):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = zc["tmat"] if A == A0 else _trajectory(zc["tmat"], S, A0, A, seed=A)
+    tm = zc["tmat"] if A == A0 else hs.trajectory(zc["tmat"], S, A0, A, seed=A)
     q = np.asarray(zc["q"], dtype=np.float32)
     for name, descs in sets:
         ref = _reference(descs, tm, A, q)
@@ -146,7 +85,7 @@ def test_fused_swept_equals_the_reduction(built_lib, A):
         _assert_same(got[:4], ref, name)
         assert len(set(got[2].tolist())) > 1, name                  # the minimum moves between configurations
         # pruning off (no PVB_GRID_PRUNE_OK: every bound is -inf), then every first visit and the other lane order
-        unpruned = _sim_fused(_unpruned(descs), tm, A, q)
+        unpruned = _sim_fused(hs.unpruned(descs), tm, A, q)
         _assert_same(unpruned[:4], ref, (name, "unpruned"))
         assert got[4] < unpruned[4], name                          # pruning skips lookups
         for first in range(S):
@@ -160,9 +99,9 @@ def test_fused_swept_equals_the_reduction(built_lib, A):
 def test_fused_swept_prunes_across_tiles(built_lib):
     """With 40 configurations (a 32-configuration tile, then 8), the second tile's lanes prune against the point's
     best from the first: fewer lookups than the two tiles run as separate slabs."""
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = _trajectory(zc["tmat"], S, A0, 40, seed=5)
+    tm = hs.trajectory(zc["tmat"], S, A0, 40, seed=5)
     q = np.asarray(zc["q"], dtype=np.float32)
     descs = sets[0][1]
     swept = _sim_fused(descs, tm, 40, q)[4]
@@ -172,9 +111,9 @@ def test_fused_swept_prunes_across_tiles(built_lib):
 
 
 def test_generic_swept_equals_the_reduction(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    tm = _trajectory(zc["tmat"], S, A0, 20, seed=3)
+    tm = hs.trajectory(zc["tmat"], S, A0, 20, seed=3)
     q = np.asarray(zc["q"], dtype=np.float32)
     for name, descs in sets:
         _assert_same(_sim_generic(descs, tm, 20, q), _reference(descs, tm, 20, q), name)
@@ -183,9 +122,9 @@ def test_generic_swept_equals_the_reduction(built_lib):
 
 
 def test_ties_report_the_first_configuration_and_sub_sdf(built_lib):
-    zc, sets, keep = _all_sets()
+    zc, sets, keep = hs.all_sets()
     S, A0 = int(zc["S"]), int(zc["A"])
-    base = _trajectory(zc["tmat"], S, A0, 6, seed=7).reshape(S, 6, 4, 4)
+    base = hs.trajectory(zc["tmat"], S, A0, 6, seed=7).reshape(S, 6, 4, 4)
     # configurations 6..11 repeat 0..5, and 12..44 all repeat configuration 2: every minimum is attained at least twice
     tm = np.concatenate([base, base, np.repeat(base[:, 2:3], 33, axis=1)], axis=1)
     A = tm.shape[1]
@@ -210,7 +149,7 @@ def test_ties_report_the_first_configuration_and_sub_sdf(built_lib):
 
 # ---------------------------------------------------------------- C ABI refusals (no kernel launch involved)
 def test_abi_refuses_invalid_swept_queries(built_lib):
-    near, tri, keep = _table_descs("probe")
+    near, tri, keep = hs.table_descs("probe")
     fake = ctypes.c_void_p(1 << 12)           # never dereferenced: every call below fails its argument checks
     L = built_lib
     arr = nat.desc_array([near, near])

@@ -5,91 +5,22 @@ ComposedSDF / RobotSDF).
    exceeds the running minimum -- holds for the trilinear interpolant with the margin `grid_prune_margin` measures
    for the nearest-voxel rule (the interpolant is a convex combination of 8 corner values; the weighted mean
    distance of q to the corners is at most half a cell diagonal).
-2. The device arithmetic (pvb_device.cuh compiled for the host by tests/hostsim/hostsim_trilinear.cpp):
-   grid_trilinear_eval against the fp64 restatement oracle.port.trilinear_lookup_port, and composed_consider over
-   trilinear and mixed compositions -- independent of pruning and visiting order, and equal to an fp64 restatement
+2. The device arithmetic (pvb_device.cuh compiled for the host, tests/hostsim_lib.py):
+   grid_trilinear_eval against the fp64 restatement oracle.port.trilinear_lookup_port, and composed_consider<true, true>
+   over trilinear and mixed compositions -- independent of pruning and visiting order, and equal to an fp64 restatement
    of the composition."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 import hostsim_lib as hs
+from hostsim_lib import PVB_ERR_INVALID
 from helpers import golden
 from oracle import port
 from pytorch_volumetric_b200 import _native as nat
 from pytorch_volumetric_b200.sdf import grid_prune_margin
-
-PVB_ERR_INVALID = -1        # include/pvb.h pvb_status
-
-_SIM_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
-_SIM_LIB = os.path.join(_SIM_DIR, "_build", "libpvb_hostsim_trilinear.so")
-_sim = None
-
-
-def _simlib():
-    """tests/hostsim/hostsim_trilinear.cpp built like tests/hostsim (g++, -ffp-contract=off), rebuilt when stale."""
-    global _sim
-    if _sim is None:
-        root = os.path.dirname(os.path.dirname(_SIM_DIR))
-        sources = [os.path.join(_SIM_DIR, "hostsim_trilinear.cpp"), os.path.join(_SIM_DIR, "cuda_runtime.h"),
-                   os.path.join(root, "pytorch_volumetric_b200", "csrc", "pvb_device.cuh"),
-                   os.path.join(root, "include", "pvb.h")]
-        if not os.path.exists(_SIM_LIB) or any(os.path.getmtime(f) > os.path.getmtime(_SIM_LIB) for f in sources):
-            os.makedirs(os.path.dirname(_SIM_LIB), exist_ok=True)
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                            "-I", _SIM_DIR, sources[0], "-o", _SIM_LIB], check=True)
-        _sim = ctypes.CDLL(_SIM_LIB)
-    return _sim
-
-
-def _p(a):
-    return ctypes.c_void_p(a.ctypes.data)
-
-
-def _grid_desc(table_val, table_grad, ranges, bb, interpolation):
-    """pvb_sdf_desc (GRID, bounding-box rule) built by the product's CachedSDF._make_desc over CPU tensors, as
-    tests/hostsim_lib.grid_desc does, with the given interpolation.  Returns (desc, keepalive)."""
-    from pytorch_volumetric_b200 import sdf as S
-    from pytorch_volumetric_b200.voxel import GridView
-    c = object.__new__(S.CachedSDF)
-    c.ranges = ranges
-    c.voxels = GridView(table_val, ranges, invalid_value=None)
-    c.voxels_grad = table_grad
-    c._table = torch.cat([table_val.reshape(-1, 1), table_grad], 1).contiguous()
-    c.bb = torch.as_tensor(np.asarray(bb))
-    c._cdev = torch.device("cpu")
-    c.out_of_bounds_strategy = S.OutOfBoundsStrategy.BOUNDING_BOX
-    c.interpolation = interpolation
-    return c._make_desc(), c
-
-
-def _sim_trilinear(desc, points):
-    p = np.ascontiguousarray(points, dtype=np.float32); n = len(p)
-    val, grad = np.empty(n, np.float32), np.empty((n, 3), np.float32)
-    _simlib().simtri_grid_trilinear(ctypes.byref(desc), _p(p), ctypes.c_longlong(n), _p(val), _p(grad))
-    return val, grad
-
-
-def _sim_composed(descs, xforms, n_cfg, points, order=None):
-    """(val [n_cfg*P], grad [n_cfg*P,3], which [n_cfg*P]) through composed_consider<true, true>; `order` as in
-    hostsim_lib.composed (default: the kernels' bit-reversed order)."""
-    p = np.ascontiguousarray(points, dtype=np.float32); n = len(p); S = len(descs)
-    arr = (nat.SdfDesc * S)(*descs)
-    xf = np.ascontiguousarray(xforms, dtype=np.float32)
-    assert xf.shape == (S * n_cfg, 4, 4)
-    order = hs.bit_reversed_order(S) if order is None else list(order)
-    assert sorted(order) == list(range(S))
-    od = np.asarray(order, dtype=np.uint8)
-    val, grad = np.empty(n_cfg * n, np.float32), np.empty((n_cfg * n, 3), np.float32)
-    which = np.empty(n_cfg * n, np.int32)
-    _simlib().simtri_composed(arr, ctypes.c_int(S), _p(od), _p(xf), ctypes.c_int(n_cfg), _p(p), ctypes.c_longlong(n),
-                              _p(val), _p(grad), _p(which))
-    return val, grad, which
-
 
 def _aabb_distance(q, bb):
     q = np.asarray(q, dtype=np.float64)
@@ -159,8 +90,8 @@ def _probe_descs():
     shape = tuple(int(s) for s in z["table_shape"])
     args = (torch.from_numpy(z["table_val"]).reshape(shape), torch.from_numpy(z["table_grad"]),
             [tuple(r) for r in z["ranges"]], z["bb"])
-    tri, k1 = _grid_desc(*args, interpolation="trilinear")
-    near, k2 = _grid_desc(*args, interpolation="nearest")
+    tri, k1 = hs.grid_desc(*args, interpolation="trilinear")
+    near, k2 = hs.grid_desc(*args, interpolation="nearest")
     return z, tri, near, (k1, k2)
 
 
@@ -176,7 +107,7 @@ def test_grid_trilinear_eval_vs_its_cpu_restatement(built_lib):
     shape = tuple(int(s) for s in z["table_shape"])
     lo = np.array([r[0] for r in ranges]); hi = np.array([r[1] for r in ranges])
     q = np.concatenate([z["q"].astype(np.float32), _in_and_out(lo, hi, 100_000, 3)])
-    v, g = _sim_trilinear(tri, q)
+    v, g = hs.grid_trilinear(tri, q)
     rv, rg, inb = port.trilinear_lookup_port(torch.from_numpy(z["table_val"]).reshape(shape), ranges, z["bb"],
                                              torch.from_numpy(q))
     rv, rg, inb = rv.numpy(), rg.numpy(), inb.numpy()
@@ -198,28 +129,19 @@ def _compositions():
                    ("mixed2", [tri, near, near, sph])], keep
 
 
-def _unpruned(descs):
-    out = []
-    for d in descs:
-        c = d.copy()
-        c.flags &= ~nat.PVB_GRID_PRUNE_OK
-        out.append(c)
-    return out
-
-
 def test_composed_trilinear_independent_of_pruning_and_order(built_lib):
     z, zc, sets, keep = _compositions()
     S, A = int(zc["S"]), int(zc["A"])
     for name, descs in sets:
-        ref = _sim_composed(descs, zc["tmat"], A, zc["q"], order=range(S))
+        ref = hs.composed(descs, zc["tmat"], A, zc["q"], order=range(S), ext=True)
         for order in (list(range(S))[::-1], hs.bit_reversed_order(S), [2, 0, 3, 1]):
-            got = _sim_composed(descs, zc["tmat"], A, zc["q"], order=order)
+            got = hs.composed(descs, zc["tmat"], A, zc["q"], order=order, ext=True)
             assert all(np.array_equal(a, b) for a, b in zip(ref, got)), (name, order)
         for order in (range(S), [3, 1, 2, 0]):
-            got = _sim_composed(_unpruned(descs), zc["tmat"], A, zc["q"], order=order)
+            got = hs.composed(hs.unpruned(descs), zc["tmat"], A, zc["q"], order=order, ext=True)
             assert all(np.array_equal(a, b) for a, b in zip(ref, got)), (name, "unpruned", order)
         # every sub-SDF alone (nothing to prune), argmin in numpy: first index on ties, like torch
-        per = [_sim_composed([descs[s]], zc["tmat"][s * A:(s + 1) * A], A, zc["q"]) for s in range(S)]
+        per = [hs.composed([descs[s]], zc["tmat"][s * A:(s + 1) * A], A, zc["q"], ext=True) for s in range(S)]
         vals = np.stack([p[0] for p in per])
         which = vals.argmin(0)
         assert np.array_equal(ref[2], which.astype(np.int32)) and np.array_equal(ref[0], vals.min(0)), name
@@ -234,7 +156,7 @@ def test_composed_trilinear_vs_fp64_restatement(built_lib):
     q = np.asarray(zc["q"], dtype=np.float64)
     P = len(q)
     mats = np.asarray(zc["tmat"], dtype=np.float64).reshape(S, A, 4, 4)
-    v, _, w = _sim_composed(sets[0][1], zc["tmat"], A, zc["q"])
+    v, _, w = hs.composed(sets[0][1], zc["tmat"], A, zc["q"], ext=True)
     v, w = v.reshape(A, P), w.reshape(A, P)
     vals = np.empty((S, A, P))
     for s in range(S):
