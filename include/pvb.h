@@ -313,6 +313,26 @@ int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf, 
                                       int64_t seg_len, float margin, void *workspace, int64_t workspace_bytes,
                                       float *out_cost, float *out_twist, void *stream);
 
+/* ---- EXTENSION: paired collision-cost query, each configuration's hinge cost over its OWN cloud ----
+ * The reference has no such operator.  pts DEVICE [cfg_count][n_seg][seg_len][3] (object frame): configuration
+ * cfg_begin + c is evaluated at pts[c] only.  Row c * n_seg + b of out_cost and out_twist (layouts of
+ * pvb_composed_query_collision_cost) is pvb_composed_query_collision_cost of configuration cfg_begin + c alone
+ * (cfg_count = 1) over pts[c], segment b, bit for bit: the same (d, g, s) per point -- pvb_composed_query_paired's --,
+ * the same terms and the same summation order, which depends on seg_len alone (pvb_device.cuh collision_cost_chunk).
+ * So the sums are deterministic, repeated calls give identical bits and a slab reproduces the rows of a larger call.
+ * workspace DEVICE, at least pvb_collision_cost_workspace(n_sdf, cfg_count, n_seg, seg_len) bytes, 4-byte aligned
+ * (may be NULL when that is 0).  Serves the sets pvb_composed_query_collision_cost serves: at most 8 GRID sub-SDFs with
+ * the bounding-box rule (nearest or trilinear) or primitives.  PVB_ERR_INVALID for every other set (mesh, LOOKUP_GT_SDF
+ * grids, more than 8 sub-SDFs: callers compose pvb_composed_query_paired), for a margin that is not finite,
+ * cfg_count < 1 with points, seg_len >= 2^31, cfg_count * n_seg * seg_len overflowing int64, a workspace that is too
+ * small, null outputs with segments and configurations, and the argument checks of pvb_composed_query.  n_seg == 0
+ * does nothing. */
+int pvb_composed_query_paired_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,
+                                             int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count, const float *pts,
+                                             int64_t n_seg, int64_t seg_len, float margin, void *workspace,
+                                             int64_t workspace_bytes, float *out_cost, float *out_twist,
+                                             void *stream);
+
 /* ---- EXTENSION: self-collision-cost query, a hinge cost between every configuration's own links and its twists ----
  * The reference has no such operator.  xforms, inv_xforms, link_pts and allowed as in
  * pvb_composed_query_self_clearance.  The definition:

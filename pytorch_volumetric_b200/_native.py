@@ -160,7 +160,13 @@ _SIGNATURES = {
                                                          ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64,
                                                          ctypes.c_float, ctypes.c_void_p, ctypes.c_int64,
                                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
-    "pvb_composed_query_self_collision_cost": (ctypes.c_int, [ctypes.POINTER(SdfDesc), ctypes.c_int32,
+    "pvb_composed_query_paired_collision_cost": (ctypes.c_int, [ctypes.POINTER(SdfDesc), ctypes.c_int32,
+                                                                ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                                                ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,
+                                                                ctypes.c_int64, ctypes.c_float, ctypes.c_void_p,
+                                                                ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
+                                                                ctypes.c_void_p]),
+    "pvb_composed_query_self_collision_cost":(ctypes.c_int, [ctypes.POINTER(SdfDesc), ctypes.c_int32,
                                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
                                                               ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p,
                                                               ctypes.c_int64, ctypes.c_void_p, ctypes.c_float,

@@ -2317,6 +2317,122 @@ collision_cost_finish_kernel(const float *__restrict__ partial, long long n_rows
     }
 }
 
+// collision_cost_term added into running sums, every product fused into its sum: cost += h^2 and tw[k] += t x_k as
+// one fmaf each.  That is what robot_collision_cost_kernel's compiled code does with `cost += t.cost` and
+// `a[k] += t.tw[k]` (nvcc contracts each product with its sum; the PTX of both kExt shows the seven fma.rn).  In the
+// sub-step loop of robot_paired_collision_cost_kernel the compiler would otherwise hoist h * h out of the loop and
+// round it twice.  The host build (-ffp-contract=off) of both kernels keeps collision_cost_term and plain sums: it
+// checks the summation order.
+__device__ __forceinline__ void collision_cost_add(float m, float d, f3 g, f3 p, float *cost, float *tw, int stride) {
+    const float h = m - d, t = 2.f * h;
+    const float x[6] = {g.x, g.y, g.z, cc_diff_of_products(p.y, g.z, p.z, g.y),
+                        cc_diff_of_products(p.z, g.x, p.x, g.z), cc_diff_of_products(p.x, g.y, p.y, g.x)};
+    *cost = __fmaf_rn(h, h, *cost);
+#pragma unroll
+    for (int k = 0; k < 6; ++k) tw[k * stride] = __fmaf_rn(t, x[k], tw[k * stride]);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Paired collision-cost query on the sets robot_collision_cost_kernel takes: configuration c against its OWN points,
+// pts [cfg_count][n_seg][seg_len][3].  The same partials as robot_collision_cost_kernel, in the same layout and with
+// the same summation order (pvb_device.cuh: collision_cost_chunk), so that collision_cost_finish_kernel completes them
+// and row c * n_seg + b is the shared-cloud kernel's row of configuration cfg_begin + c over points[c], bit for bit.
+// robot_collision_cost_kernel cannot serve here: its lanes are the configurations of one shared point.
+//   * Work unit: (configuration, segment, chunk), owned by one warp, numbered chunk-major as in
+//     robot_paired_clearance_kernel; the warps of a 1-D grid stride over them, so any cfg_count fits.
+//   * Staging as robot_paired_clearance_kernel: the configuration's transform rows and sphere centres once per unit in
+//     the warp's slot of shared memory, __syncwarp only.
+//   * A 32-point step is skipped by the whole warp when no lane has a link whose sphere bound is below m; otherwise
+//     each lane runs rs_swept_pair on its own point with its own nearest link first and bp = m, so every (d, g, s)
+//     below m is the per-pair query's bit for bit (the visiting order never changes it).
+//   * Accumulators: chunk point j belongs to accumulator j mod 8 = lane & 7 (j0 is a multiple of 32), kept in column
+//     lane & 7 of the warp's acc[e][8].  Accumulator w must take its points in ascending order, i.e. lanes w, w + 8,
+//     w + 16, w + 24 in turn: four ordered sub-steps, lanes 8r .. 8r + 7 adding in sub-step r, __syncwarp between
+//     them.  A lane that does not contribute adds nothing, as in robot_collision_cost_kernel.  The terms go in through
+//     collision_cost_add: the products fused into the sums as that kernel's compiled code fuses them.
+//   * End of unit: lane e adds row e's 8 accumulators in order in fp64 and stores the partial rounded to fp32.  No
+//     atomics anywhere.
+struct __align__(16) PccSmem {
+    float4 xf[kRsWarps][3 * kRsMaxS];
+    float4 sph[kRsWarps][3 * kRsMaxS / 4];
+    float acc[kRsWarps][1 + 6 * kRsMaxS][kCcWarps];
+};
+
+template <bool kExt>
+__global__ void __launch_bounds__(kRbCfg * kRsWarps, 3)
+robot_paired_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf,
+                                   const float *__restrict__ xforms, int n_cfg, int cfg_begin, int cfg_count,
+                                   const float *__restrict__ pts, long long n_seg, int seg_len, int chunk,
+                                   int chunks_per_seg, float margin, long long n_units, float *__restrict__ partial) {
+    __shared__ PccSmem sm;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const int E = 1 + 6 * n_sdf;
+    const float m = margin;
+    const long long pairs = (long long)cfg_count * n_seg;
+    float *const acc_all = &sm.acc[warp][0][0];
+    float *const acc = acc_all + (lane & (kCcWarps - 1));    // this lane's accumulator column
+    // uniform per warp: every lane takes part in the votes and __syncwarp
+    for (long long w = (long long)blockIdx.x * kRsWarps + warp; w < n_units; w += (long long)gridDim.x * kRsWarps) {
+        const long long kc = w / pairs, cb = w - kc * pairs;  // chunk index; c * n_seg + b
+        const int cfg = cfg_begin + (int)(cb / n_seg);
+        const int i0 = (int)kc * chunk;
+        const int len = min(chunk, seg_len - i0);
+        const long long pt0 = cb * seg_len + i0;             // pts[c][b][i0]
+        __syncwarp();                                        // the previous unit is no longer read
+        if (lane < 3 * n_sdf) {
+            const int si = lane / 3;
+            sm.xf[warp][lane] = __ldg(reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg) * 16) +
+                                      (lane - 3 * si));
+        }
+        for (int e = lane; e < E * kCcWarps; e += 32) acc_all[e] = 0.f;
+        __syncwarp();
+        if (lane < kRsMaxS) {
+            const f3 co = lane < n_sdf ? rs_sphere_centre(pk.d[lane], sm.xf[warp][3 * lane], sm.xf[warp][3 * lane + 1],
+                                                          sm.xf[warp][3 * lane + 2])
+                                       : mk3(0.f, 0.f, 0.f);
+            float *c = reinterpret_cast<float *>(&sm.sph[warp][0]) + 3 * lane;
+            c[0] = co.x; c[1] = co.y; c[2] = co.z;
+        }
+        __syncwarp();
+#pragma unroll 1
+        for (int j0 = 0; j0 < len; j0 += 32) {
+            const int j = j0 + lane;
+            const bool on = j < len;
+            const f3 p = on ? load_point(pts, pt0 + j) : mk3(0.f, 0.f, 0.f);
+            float lb[kRsMaxS], key[kRsMaxS];
+            rs_point_bounds(sm.sph[warp], pk.sph_rad, p, low3_off, 0xffu, lb, key);
+            if (!__any_sync(0xffffffffu, on && collision_cost_near(lb, m))) continue;
+            auto link = [&](const int si, const float thr, float4 &o) -> bool {
+                const pvb_sdf_desc &d = pk.d[si];
+                const float4 r0 = sm.xf[warp][3 * si], r1 = sm.xf[warp][3 * si + 1], r2 = sm.xf[warp][3 * si + 2];
+                return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
+            };
+            float best;
+            f3 bg;
+            int bs;
+            // lanes past the end prune everything that has a bound (bp = -inf); their result is not used
+            rs_swept_pair(lb, rs_nearest(key, n_sdf), on ? m : -PVB_INF, link, best, bg, bs);
+            const bool add = on && bs >= 0 && best < m;
+#pragma unroll 1
+            for (int r = 0; r < kRbCfg / kCcWarps; ++r) {
+                if (lane / kCcWarps == r && add) {
+                    const f3 g = composed_rotate_back(sm.xf[warp][3 * bs], sm.xf[warp][3 * bs + 1],
+                                                      sm.xf[warp][3 * bs + 2], bg);
+                    collision_cost_add(m, best, g, p, acc, acc + (1 + 6 * bs) * kCcWarps, kCcWarps);
+                }
+                __syncwarp();
+            }
+        }
+        __syncwarp();
+        for (int e = lane; e < E; e += 32) {
+            double s = 0.0;
+            for (int v = 0; v < kCcWarps; ++v) s += (double)acc_all[e * kCcWarps + v];
+            partial[((size_t)cb * chunks_per_seg + kc) * E + e] = (float)s;
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // Self-collision-cost query on the sets robot_self_clearance_kernel takes (pvb_device.cuh: the definition and the
 // summation order): for every configuration of the slab, cost and the 6 n_sdf twist components, stored once each.
@@ -3822,15 +3938,27 @@ extern "C" int64_t pvb_collision_cost_workspace(int32_t n_sdf, int32_t cfg_count
     return collision_cost_bytes(n_sdf, cfg_count, n_seg, seg_len);
 }
 
-// robot_collision_cost_kernel over every (tile, segment, chunk) unit, then collision_cost_finish_kernel.
+// robot_collision_cost_kernel over every (tile, segment, chunk) unit, then collision_cost_finish_kernel.  kPaired:
+// robot_paired_collision_cost_kernel over every (configuration, segment, chunk) warp unit instead.
+template <bool kPaired>
 static int launch_collision_cost(const pvb_sdf_desc *descs, int n_sdf, const float *xforms, int n_cfg, int cfg_begin,
                                  int cfg_count, const float *pts, long long n_seg, long long seg_len, float margin,
                                  float *partial, float *out_cost, float *out_twist, bool ext, cudaStream_t stream) {
-    const char *fn = "pvb_composed_query_collision_cost";
+    const char *fn = kPaired ? "pvb_composed_query_paired_collision_cost" : "pvb_composed_query_collision_cost";
     const RobotPack<kRsMaxS> pack = rs_pack(descs, n_sdf);
     const int E = 1 + 6 * n_sdf;
     const long long chunk = collision_cost_chunk(seg_len), cps = collision_cost_chunks(seg_len);
-    if (cps > 0) {
+    if (cps > 0 && kPaired) {
+        auto k = ext ? robot_paired_collision_cost_kernel<true> : robot_paired_collision_cost_kernel<false>;
+        const long long n_units = (long long)cfg_count * n_seg * cps;
+        const long long blocks = (n_units + kRsWarps - 1) / kRsWarps;
+        timing_mark(0, stream);
+        k<<<(unsigned)(blocks < INT32_MAX ? blocks : INT32_MAX), kRbCfg * kRsWarps, 0, stream>>>(
+            pack, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, (int)seg_len, (int)chunk, (int)cps, margin,
+            n_units, partial);
+        timing_mark(1, stream);
+        PVB_CHECK_LAUNCH("pvb_composed_query_paired_collision_cost");
+    } else if (cps > 0) {
         auto k = ext ? robot_collision_cost_kernel<true> : robot_collision_cost_kernel<false>;
         if (!ensure_smem(k, ext ? kSlotCollisionCostExt : kSlotCollisionCost, cc_smem_bytes(kRsMaxS))) {
             pvb_set_error("%s: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed", fn);
@@ -3848,21 +3976,25 @@ static int launch_collision_cost(const pvb_sdf_desc *descs, int n_sdf, const flo
     const long long rows = (long long)cfg_count * n_seg;
     collision_cost_finish_kernel<<<grid_for(rows * E, kCompThreads, 8), kCompThreads, 0, stream>>>(
         partial, rows, (int)cps, E, out_cost, out_twist);
-    PVB_CHECK_LAUNCH("pvb_composed_query_collision_cost(finish)");
+    PVB_CHECK_LAUNCH(kPaired ? "pvb_composed_query_paired_collision_cost(finish)"
+                             : "pvb_composed_query_collision_cost(finish)");
     return PVB_OK;
 }
 
-extern "C" int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,
-                                                 int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
-                                                 const float *pts, int64_t n_seg, int64_t seg_len, float margin,
-                                                 void *workspace, int64_t workspace_bytes, float *out_cost,
-                                                 float *out_twist, void *stream) {
-    const char *fn = "pvb_composed_query_collision_cost";
-    if (int rc = check_segments(fn, n_seg, seg_len, cfg_count, false)) return rc;
+// pvb_composed_query_collision_cost, and pvb_composed_query_paired_collision_cost (kPaired: configuration c's points
+// are its own n_seg * seg_len); they differ in the point count they bound and in their kernel, not in the workspace.
+template <bool kPaired>
+static int collision_cost_query(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms, int32_t n_cfg,
+                                int32_t cfg_begin, int32_t cfg_count, const float *pts, int64_t n_seg, int64_t seg_len,
+                                float margin, void *workspace, int64_t workspace_bytes, float *out_cost,
+                                float *out_twist, void *stream) {
+    const char *fn = kPaired ? "pvb_composed_query_paired_collision_cost" : "pvb_composed_query_collision_cost";
+    if (int rc = check_segments(fn, n_seg, seg_len, cfg_count, kPaired)) return rc;
     if (int rc = check_margin(fn, margin)) return rc;
-    const long long n_pts = n_seg * seg_len;
+    const long long n_pts = n_seg * seg_len;                 // points per configuration
     bool any_ext;
-    const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_pts, out_cost,
+    const int bad = composed_check_args(fn, descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts,
+                                        kPaired ? (cfg_count > 0 ? cfg_count * n_pts : 0) : n_pts, out_cost,
                                         out_twist, any_ext);
     if (bad) return bad;
     if (n_seg == 0) return PVB_OK;
@@ -3875,16 +4007,37 @@ extern "C" int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int3
         pvb_set_error("%s: invalid argument (out_cost or out_twist is null)", fn);
         return PVB_ERR_INVALID;
     }
-    if (int rc = check_fused_only(fn, descs, n_sdf, "compose it from pvb_composed_query")) return rc;
+    if (int rc = check_fused_only(fn, descs, n_sdf, kPaired ? "compose it from pvb_composed_query_paired"
+                                                             : "compose it from pvb_composed_query"))
+        return rc;
     const long long need = collision_cost_bytes(n_sdf, cfg_count, n_seg, seg_len);
     if (need < 0 || (need > 0 && (!workspace || workspace_bytes < need || ((uintptr_t)workspace & 3)))) {
         pvb_set_error("%s: the workspace must hold pvb_collision_cost_workspace() = %lld bytes, 4-byte aligned "
                       "(got %lld bytes)", fn, need, (long long)workspace_bytes);
         return PVB_ERR_INVALID;
     }
-    return launch_collision_cost(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, margin,
-                                 reinterpret_cast<float *>(workspace), out_cost, out_twist, any_ext,
-                                 (cudaStream_t)stream);
+    return launch_collision_cost<kPaired>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len,
+                                          margin, reinterpret_cast<float *>(workspace), out_cost, out_twist, any_ext,
+                                          (cudaStream_t)stream);
+}
+
+extern "C" int pvb_composed_query_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,
+                                                 int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                                                 const float *pts, int64_t n_seg, int64_t seg_len, float margin,
+                                                 void *workspace, int64_t workspace_bytes, float *out_cost,
+                                                 float *out_twist, void *stream) {
+    return collision_cost_query<false>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, margin,
+                                       workspace, workspace_bytes, out_cost, out_twist, stream);
+}
+
+extern "C" int pvb_composed_query_paired_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf,
+                                                        const float *xforms, int32_t n_cfg, int32_t cfg_begin,
+                                                        int32_t cfg_count, const float *pts, int64_t n_seg,
+                                                        int64_t seg_len, float margin, void *workspace,
+                                                        int64_t workspace_bytes, float *out_cost, float *out_twist,
+                                                        void *stream) {
+    return collision_cost_query<true>(descs, n_sdf, xforms, n_cfg, cfg_begin, cfg_count, pts, n_seg, seg_len, margin,
+                                      workspace, workspace_bytes, out_cost, out_twist, stream);
 }
 
 extern "C" int pvb_composed_query_self_collision_cost(const pvb_sdf_desc *descs, int32_t n_sdf, const float *xforms,

@@ -314,6 +314,16 @@ class RobotSDF(sdf.ObjectFrameSDF):
         grad = self.joint_gradient(twist, self.joint_twists(), self.joint_moves_link())
         return cost, grad.to(cost.dtype)
 
+    def paired_collision_cost(self, points_in_object_frame, margin):
+        """Every installed joint configuration against its own cloud: points [*A, *B, N, 3] in the robot frame ->
+        (cost [*A, *B], joint_grad [*A, *B, J]) in the points' dtype and on their device, J in `joint_names` order.
+        Entry [a, b] is collision_cost of configuration a alone over points[a, b]: ComposedSDF.paired_collision_cost's
+        twist gradient through joint_gradient(twist, joint_twists(), joint_moves_link()).  Not autograd: the gradient
+        is an output of the query."""
+        cost, twist = self.sdf.paired_collision_cost(points_in_object_frame, margin)
+        grad = self.joint_gradient(twist, self.joint_twists(), self.joint_moves_link())
+        return cost, grad.to(cost.dtype)
+
     def self_collision_cost(self, margin, link_points=None, allowed=None):
         """For every installed joint configuration, the soft self-collision cost between the robot's own links and its
         derivative with respect to the joint values: link_points [S, K, 3] (default: link_surface_points()) are posed

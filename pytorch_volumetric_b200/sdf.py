@@ -1244,7 +1244,6 @@ class ComposedSDF(ObjectFrameSDF):
         (cfg_count * n_seg,) / (cfg_count * n_seg, S, 6) fp32 tensors on the GPU, configuration-major.  Raises
         ValueError before any device work on malformed points, a margin that is not finite, or a slab without
         configurations when there are points."""
-        S = len(self.sdfs)
         n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
         m = self._collision_cost_margin(margin)
         shape = tuple(points_in_object_frame.shape)
@@ -1253,10 +1252,16 @@ class ComposedSDF(ObjectFrameSDF):
         n_seg, seg_len = math.prod(shape[:-2]), shape[-2]
         if cfg_begin < 0 or cfg_count < 0 or cfg_begin + cfg_count > n_cfg or (cfg_count < 1 and n_seg * seg_len > 0):
             raise ValueError(f"collision-cost query: invalid configuration slab [{cfg_begin}, +{cfg_count}) of {n_cfg}")
-        with _query_points(points_in_object_frame) as (device, p):
+        return self._collision_cost_query(points_in_object_frame, m, cfg_begin, cfg_count, n_seg, seg_len)
+
+    def _collision_cost_query(self, points, m, cfg_begin, cfg_count, n_seg, seg_len, paired=False):
+        """query_collision_cost (paired=False) or query_paired_collision_cost (paired=True) once their checks have
+        passed: the form's fused entry point, or `_composed_collision_cost` for the sets the fused kernels refuse."""
+        S, n_cfg = len(self.sdfs), _config_count(self.tsf_batch)
+        with _query_points(points) as (device, p):
             R = cfg_count * n_seg
             if not self._self_clearance_fused(device):
-                return self._composed_collision_cost(p, m, cfg_begin, cfg_count, n_seg, seg_len)
+                return self._composed_collision_cost(p, m, cfg_begin, cfg_count, n_seg, seg_len, paired=paired)
             descs_arr, _ = self._native_descs(device)
             xf = self._xforms_on(device)
             cost = torch.empty(R, dtype=torch.float32, device=device)
@@ -1264,27 +1269,35 @@ class ComposedSDF(ObjectFrameSDF):
             lib = nat.lib()
             need = lib.pvb_collision_cost_workspace(S, cfg_count, n_seg, seg_len)
             ws = torch.empty(max(need, 0) // 4, dtype=torch.float32, device=device)
-            nat.check(lib.pvb_composed_query_collision_cost(descs_arr, S, nat.ptr(xf), n_cfg, cfg_begin, cfg_count,
-                                                            nat.ptr(p), n_seg, seg_len, m,
-                                                            nat.ptr(ws) if need > 0 else None, need, nat.ptr(cost),
-                                                            nat.ptr(twist), nat.stream_ptr(device)),
-                      "pvb_composed_query_collision_cost")
+            entry = lib.pvb_composed_query_paired_collision_cost if paired else lib.pvb_composed_query_collision_cost
+            nat.check(entry(descs_arr, S, nat.ptr(xf), n_cfg, cfg_begin, cfg_count, nat.ptr(p), n_seg, seg_len, m,
+                            nat.ptr(ws) if need > 0 else None, need, nat.ptr(cost), nat.ptr(twist),
+                            nat.stream_ptr(device)), entry.__name__)
         return cost, twist
 
-    def _composed_collision_cost(self, p, m, cfg_begin, cfg_count, n_seg, seg_len):
+    def _composed_collision_cost(self, p, m, cfg_begin, cfg_count, n_seg, seg_len, paired=False):
         """query_collision_cost by composition, for the sets the fused kernel refuses: query(..., return_which=True)
         on chunks of `clearance_generic_chunk` configurations, the terms in fp64, grouped by sub-SDF with one mask and
-        one sum per sub-SDF (torch's sums are deterministic; scatter_add / index_add on CUDA are not)."""
+        one sum per sub-SDF (torch's sums are deterministic; scatter_add / index_add on CUDA are not).  paired: p holds
+        cfg_count blocks of n_seg * seg_len points, block c for configuration cfg_begin + c only, evaluated with
+        query_paired (query_paired_collision_cost)."""
         S = len(self.sdfs)
         R = cfg_count * n_seg
         cost = torch.zeros(R, dtype=torch.float32, device=p.device)
         twist = torch.zeros(R, S, 6, dtype=torch.float32, device=p.device)
         if R == 0 or seg_len == 0:
             return cost, twist
-        pts = p.double().reshape(n_seg, seg_len, 3)
+        n_pts = n_seg * seg_len
+        shared = None if paired else p.double().reshape(n_seg, seg_len, 3)
         for c0 in range(cfg_begin, cfg_begin + cfg_count, self.clearance_generic_chunk):
             cc = min(self.clearance_generic_chunk, cfg_begin + cfg_count - c0)
-            v, g, w = self.query(p, cfg_begin=c0, cfg_count=cc, return_which=True)
+            if paired:
+                own = p[(c0 - cfg_begin) * n_pts:(c0 - cfg_begin + cc) * n_pts]
+                v, g, w = self.query_paired(own, cfg_begin=c0, cfg_count=cc, return_which=True)
+                pts = own.double().reshape(cc, n_seg, seg_len, 3)
+            else:
+                v, g, w = self.query(p, cfg_begin=c0, cfg_count=cc, return_which=True)
+                pts = shared
             v, g, w = v.reshape(cc, n_seg, seg_len), g.reshape(cc, n_seg, seg_len, 3), w.reshape(cc, n_seg, seg_len)
             h = (m - v.double()).clamp_min(0.0)                     # 0 exactly where d >= m
             g = g.double()
@@ -1311,6 +1324,52 @@ class ComposedSDF(ObjectFrameSDF):
         m = self._collision_cost_margin(margin)
         out = self.query_collision_cost(points_in_object_frame, m)
         return self._deliver(points_in_object_frame, out, (*(self.tsf_batch or ()), *pts_shape[:-2]))
+
+    def query_paired_collision_cost(self, points_in_object_frame, margin, cfg_begin=0, cfg_count=None):
+        """Paired form of `query_collision_cost`: configuration cfg_begin + c against its own points only.  The points
+        reshape to [cfg_count, n_seg, N, 3], N = points.shape[-2]; entry c * n_seg + b of the result, cost and twist,
+        is query_collision_cost(points[c], margin, cfg_begin=cfg_begin + c, cfg_count=1)[b] -- the margin rounded to
+        fp32, the terms of the (d, g, s) query_paired(..., return_which=True) gives at each point, object-frame twists
+        about the origin, and 0 with all-zero twists for N = 0.
+
+        Sets of at most 8 grid (bounding-box rule) or primitive sub-SDFs run in one fused kernel
+        (pvb_composed_query_paired_collision_cost), bit-identical to that definition; every other set is composed from
+        `query_paired` in chunks of `clearance_generic_chunk` configurations and reduced in torch, equal to it within
+        fp32 rounding.  Returns flat (cfg_count * n_seg,) / (cfg_count * n_seg, S, 6) fp32 tensors on the GPU,
+        configuration-major.  Raises ValueError before any device work on malformed points, points that do not split
+        into cfg_count blocks, an invalid slab or a margin that is not finite."""
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
+        m = self._collision_cost_margin(margin)
+        shape = tuple(points_in_object_frame.shape)
+        if len(shape) < 2 or shape[-1] != 3:
+            raise ValueError(f"paired collision-cost query: points {shape} must be [..., N, 3]")
+        lead, seg_len = math.prod(shape[:-2]), shape[-2]
+        if cfg_begin < 0 or cfg_count < 0 or cfg_begin + cfg_count > n_cfg:
+            raise ValueError(f"paired collision-cost query: invalid configuration slab [{cfg_begin}, +{cfg_count}) of "
+                             f"{n_cfg}")
+        if (lead % cfg_count) if cfg_count > 0 else lead:
+            raise ValueError(f"paired collision-cost query: points {shape} do not split into {cfg_count} blocks of "
+                             f"[n_seg, N, 3]")
+        n_seg = lead // cfg_count if cfg_count > 0 else 0
+        return self._collision_cost_query(points_in_object_frame, m, cfg_begin, cfg_count, n_seg, seg_len,
+                                          paired=True)
+
+    def paired_collision_cost(self, points_in_object_frame, margin):
+        """Every installed configuration against its own cloud: points [*A, *B, N, 3], A the configuration batch, give
+        (cost [*A, *B], twist_grad [*A, *B, S, 6]) in the points' dtype and on their device.  Entry [a, b] is
+        configuration a's collision cost over points[a, b] and its twist gradient per sub-SDF: what collision_cost of
+        configuration a alone gives over points[a] (bit for bit on the fused sets), without |A| times the work of
+        collision_cost over every cloud.  Without a configuration batch it is collision_cost.  Semantics and routes are
+        those of `query_paired_collision_cost`.  Not a reference operator (an extension), and not autograd: the
+        gradient is an output of the query.  Raises ValueError before any device work when the leading dimensions of
+        the points are not A, when they are not [..., N, 3], or when the margin is not finite."""
+        if self.tsf_batch is None:
+            return self.collision_cost(points_in_object_frame, margin)
+        pts_shape = tuple(points_in_object_frame.shape)
+        self._check_leading_batch(pts_shape, "paired collision-cost query", "..., N, 3", 2, separate_mismatch=True)
+        m = self._collision_cost_margin(margin)
+        out = self.query_paired_collision_cost(points_in_object_frame, m)
+        return self._deliver(points_in_object_frame, out, pts_shape[:-2])
 
     def query_self_collision_cost(self, link_points, allowed, margin, cfg_begin=0, cfg_count=None):
         """Self-collision cost of configurations [cfg_begin, cfg_begin + cfg_count) and its twist gradient per
