@@ -680,6 +680,15 @@ __device__ __forceinline__ SdfOut primitive_eval(const pvb_sdf_desc &d, f3 q) {
 // sdf.py:392-433): the rigid transform into a sub-frame, the exact rejection bound, one "consider this sub-SDF"
 // step of the running argmin, and the gradient rotation back to the object frame.
 
+// The transforms of every query take the layout [S][n_cfg][4][4], row-major: the rows [R | t] of sub-SDF s in
+// configuration cfg are the first three float4 of its matrix.
+__host__ __device__ inline const float4 *xf_rows(const float *m, int n_cfg, int s, size_t cfg) {
+    return reinterpret_cast<const float4 *>(m + ((size_t)s * n_cfg + cfg) * 16);
+}
+__host__ __device__ inline float4 *xf_rows(float *m, int n_cfg, int s, size_t cfg) {
+    return reinterpret_cast<float4 *>(m + ((size_t)s * n_cfg + cfg) * 16);
+}
+
 // Transform3d.transform_points: R p + t (sdf.py:399); rows r0..r2 of the 4x4 object->sub-frame matrix
 __device__ __forceinline__ f3 composed_xform(const float4 &r0, const float4 &r1, const float4 &r2, f3 v) {
     return mk3(fmaf(r0.x, v.x, fmaf(r0.y, v.y, fmaf(r0.z, v.z, r0.w))),
@@ -919,6 +928,9 @@ __device__ __forceinline__ float rs_bound_key(float lb, int low3_off, int si) {
     return __int_as_float(rs_and_or(__float_as_int(lb), low3_off, si));
 }
 
+// low3_off of the kernels: ~7 in a register the compiler cannot fold (n_sdf <= 8, so n_sdf >> 30 is 0)
+__device__ __forceinline__ int rs_low3_off(int n_sdf) { return ~7 | (n_sdf >> 30); }
+
 __device__ __forceinline__ float rs_min(float a, float b) {
 #ifdef __CUDA_ARCH__
     return fminf(a, b);             // FMNMX: a NaN operand loses, signalling or not
@@ -965,6 +977,18 @@ __device__ __forceinline__ f3 rs_sphere_centre(const pvb_sdf_desc &d, float4 r0,
     const float dev = fmaxf(fmaxf(fmaxf(fabsf(e00), fabsf(e11)), fmaxf(fabsf(e22), fabsf(e01))),
                             fmaxf(fabsf(e02), fabsf(e12)));
     return dev < 1e-5f ? co : mk3(__int_as_float(0x7fffffff), 0.f, 0.f);
+}
+
+// Slot si of a configuration's staged row of sphere centres ({x, y, z} of the 8 links back to back: 6 float4), from
+// the link descriptors descs and its staged transform rows xf (link si at xf[3 si .. 3 si + 2]), both read only for
+// si < n_sdf.  Slots beyond n_sdf get centre 0: with the radius -inf that rs_pack gives them, their bound is +inf --
+// never the nearest, never visited.
+__device__ __forceinline__ void rs_centre_slot(const pvb_sdf_desc *descs, int si, int n_sdf, const float4 *xf,
+                                               float4 *sph) {
+    const f3 co =
+        si < n_sdf ? rs_sphere_centre(descs[si], xf[3 * si], xf[3 * si + 1], xf[3 * si + 2]) : mk3(0.f, 0.f, 0.f);
+    float *c = reinterpret_cast<float *>(sph) + 3 * si;
+    c[0] = co.x; c[1] = co.y; c[2] = co.z;
 }
 
 __device__ __forceinline__ float rsqrt_approx(float x) {      // one MUFU.RSQ, no denormal fix-up (callers keep x >= 1e-20)

@@ -729,7 +729,7 @@ composed_query_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
                     const float4 *row = reinterpret_cast<const float4 *>(s_xf[s]);      // 3 x LDS.128 broadcast
                     r0 = row[0]; r1 = row[1]; r2 = row[2];
                 } else {
-                    const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
+                    const float4 *row = xf_rows(xforms, n_cfg, s, cfg);
                     r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
                 }
             };
@@ -860,7 +860,7 @@ composed_paired_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, 
         paired_index(t, n_pts, c, i);
         const int cfg = cfg_begin + (int)c;
         auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) {
-            const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
+            const float4 *row = xf_rows(xforms, n_cfg, s, cfg);
             r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
         };
         const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st, load_point(pts, t),
@@ -893,7 +893,7 @@ composed_swept_kernel(const __grid_constant__ DescPack<MAXS> descs, int n_sdf, c
         for (int c = 0; c < cfg_count; ++c) {
             const int cfg = cfg_begin + c;
             auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) {
-                const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
+                const float4 *row = xf_rows(xforms, n_cfg, s, cfg);
                 r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
             };
             const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st, p, mesh_mode,
@@ -940,7 +940,7 @@ __device__ __forceinline__ void clearance_pairs(const DescPack<MAXS> &descs, int
             const long long b = i / seg_len;
             const int cfg = cfg_begin + (int)c;
             auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) {
-                const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
+                const float4 *row = xf_rows(xforms, n_cfg, s, cfg);
                 r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
             };
             const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st,
@@ -1006,7 +1006,7 @@ __device__ __forceinline__ void clearance_finish(const DescPack<MAXS> &descs, in
         const long long i = b * seg_len + ip;
         const int cfg = cfg_begin + (int)c;
         auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) {
-            const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
+            const float4 *row = xf_rows(xforms, n_cfg, s, cfg);
             r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
         };
         const ComposedOut o = composed_point<kMesh, kExt>(descs.d, descs.order, n_sdf, load_xf, st,
@@ -1574,6 +1574,30 @@ struct __align__(16) RsTile {
     float4 sph[kRbCfg][3 * kRsMaxS / 4 + 1];
 };
 
+// The `link` of rs_swept_pair on staged rows xf (link si at xf[3 si .. 3 si + 2]): rs_link_visit.
+template <bool kExt>
+__device__ __forceinline__ auto rs_staged_link(const RobotPack<kRsMaxS> &pk, const float4 *xf, const f3 &p) {
+    return [&pk, xf, &p](const int si, const float thr, float4 &o) -> bool {
+        return rs_link_visit<kExt>(pk.d[si], pk.visit_margin[si], xf[3 * si], xf[3 * si + 1], xf[3 * si + 2], p, thr,
+                                   o);
+    };
+}
+
+// the smallest clearance key over the lanes that differ from this one in lane bits off .. 16 (off a power of two)
+__device__ __forceinline__ unsigned long long warp_min_key(unsigned long long k, int off) {
+    for (int o = 16; o >= off; o >>= 1) {
+        const unsigned long long v = __shfl_xor_sync(0xffffffffu, k, o);
+        k = v < k ? v : k;
+    }
+    return k;
+}
+
+// the minimum of v over the warp
+__device__ __forceinline__ float warp_min(float v) {
+    for (int off = 16; off > 0; off >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, off));
+    return v;
+}
+
 struct __align__(16) RsSmem : RsTile {
     // per-warp staging, LC rows x (8 * 32/LC values + 1) resp. (24 * 32/LC gradient floats + 1): at most 32 x 9 / 32 x 25
     float sv[kRsWarps][kRbCfg][kRsValStride];
@@ -1644,8 +1668,7 @@ robot_serial_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, co
     const int row_pts = pts_per_step << w_log2;                             // points per row of the tile
     const int vstride = row_pts + 1, gstride = 3 * row_pts + 1;             // odd: conflict-free STS.32 across lanes
     const int col0 = (kCoop ? warp * pts_per_step : 0) + sub * npt;         // this lane's first column
-    // ~7 in a register the compiler cannot fold (n_sdf <= 8): (bits & ~7) | si is then ONE LOP3 with the immediate si
-    const int low3_off = ~7 | (n_sdf >> 30);
+    const int low3_off = rs_low3_off(n_sdf);   // (bits & ~7) | si is then ONE LOP3 with the immediate si
     float *const sv_lane = sv + cl * vstride + col0, *const sg_lane = sg + cl * gstride + 3 * col0;
     const int n_super = (n_chunks + kRsWarps - 1) / kRsWarps;
     for (int sup = blockIdx.x; sup < n_super; sup += gx_tile) {
@@ -1796,7 +1819,7 @@ robot_swept_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, con
     for (int j = threadIdx.x; j < npb; j += blockDim.x) {
         sm.best[j].val = PVB_INF; sm.best[j].cfg = -1;
     }
-    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const int low3_off = rs_low3_off(n_sdf);
     const int n_tiles = (cfg_count >> 5) + __popc((unsigned)(cfg_count & 31));
     for (int t = 0; t < n_tiles; ++t) {
         int c0, lc_log2;
@@ -1855,7 +1878,7 @@ robot_swept_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf, con
     for (int j = threadIdx.x; j < npb; j += blockDim.x) {
         const SweptBest b = sm.best[j];
         const int cfg = cfg_begin + b.cfg;
-        const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)max(b.which, 0) * n_cfg + cfg) * 16);
+        const float4 *row = xf_rows(xforms, n_cfg, max(b.which, 0), cfg);
         const f3 go = composed_rotate_back(__ldg(row), __ldg(row + 1), __ldg(row + 2), b.grad);
         const long long i = base + j;
         out_val[i] = b.val;
@@ -1913,7 +1936,7 @@ robot_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf,
         c[0] = co.x; c[1] = co.y; c[2] = co.z;
     }
     __syncthreads();
-    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const int low3_off = rs_low3_off(n_sdf);
     const int groups = kRsWarps << sub_log2;                 // point groups of the block
     const int gid = (warp << sub_log2) + sub;
     const long long n_work = n_seg * chunks_per_seg;
@@ -1936,11 +1959,7 @@ robot_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n_sdf,
             float lb[kRsMaxS], key[kRsMaxS];
             rs_point_bounds(sm.sph[cl], pk.sph_rad, p, low3_off, 0xffu, lb, key);
             const int pred = __shfl_sync(0xffffffffu, rs_nearest(key, n_sdf), sub << lc_log2);
-            auto link = [&](const int si, const float thr, float4 &o) -> bool {
-                const pvb_sdf_desc &d = pk.d[si];
-                const float4 r0 = sm.xf[cl][3 * si], r1 = sm.xf[cl][3 * si + 1], r2 = sm.xf[cl][3 * si + 2];
-                return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
-            };
+            const auto link = rs_staged_link<kExt>(pk, sm.xf[cl], p);
             float best;
             f3 bg;
             int bs;
@@ -1998,7 +2017,7 @@ robot_paired_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int
                               unsigned long long *__restrict__ keys) {
     __shared__ PclSmem sm;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const int low3_off = rs_low3_off(n_sdf);
     const long long pairs = (long long)cfg_count * n_seg;
     // uniform per warp: every lane takes part in the shuffles
     for (long long w = (long long)blockIdx.x * kRsWarps + warp; w < n_units; w += (long long)gridDim.x * kRsWarps) {
@@ -2010,17 +2029,10 @@ robot_paired_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int
         __syncwarp();                                        // the previous unit's staging is no longer read
         if (lane < 3 * n_sdf) {
             const int si = lane / 3;
-            sm.xf[warp][lane] = __ldg(reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg) * 16) +
-                                      (lane - 3 * si));
+            sm.xf[warp][lane] = __ldg(xf_rows(xforms, n_cfg, si, cfg) + (lane - 3 * si));
         }
         __syncwarp();
-        if (lane < kRsMaxS) {
-            const f3 co = lane < n_sdf ? rs_sphere_centre(pk.d[lane], sm.xf[warp][3 * lane], sm.xf[warp][3 * lane + 1],
-                                                          sm.xf[warp][3 * lane + 2])
-                                       : mk3(0.f, 0.f, 0.f);
-            float *c = reinterpret_cast<float *>(&sm.sph[warp][0]) + 3 * lane;
-            c[0] = co.x; c[1] = co.y; c[2] = co.z;
-        }
+        if (lane < kRsMaxS) rs_centre_slot(pk.d, lane, n_sdf, sm.xf[warp], sm.sph[warp]);
         __syncwarp();
         unsigned long long *const kp = keys + cb;
         const unsigned long long seed_key = __ldcg(kp);
@@ -2034,26 +2046,19 @@ robot_paired_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int
             const f3 p = on ? load_point(pts, pt0 + j) : mk3(0.f, 0.f, 0.f);
             float lb[kRsMaxS], key[kRsMaxS];
             rs_point_bounds(sm.sph[warp], pk.sph_rad, p, low3_off, 0xffu, lb, key);
-            auto link = [&](const int si, const float thr, float4 &o) -> bool {
-                const pvb_sdf_desc &d = pk.d[si];
-                const float4 r0 = sm.xf[warp][3 * si], r1 = sm.xf[warp][3 * si + 1], r2 = sm.xf[warp][3 * si + 2];
-                return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
-            };
             float best;
             f3 bg;
             int bs;
             // lanes past the end prune everything that has a bound (bp = -inf); their result is not used
-            rs_swept_pair(lb, rs_nearest(key, n_sdf), on ? fminf(rv, seed) : -PVB_INF, link, best, bg, bs);
+            rs_swept_pair(lb, rs_nearest(key, n_sdf), on ? fminf(rv, seed) : -PVB_INF,
+                          rs_staged_link<kExt>(pk, sm.xf[warp], p), best, bg, bs);
             if (on && bs >= 0) {
                 const unsigned long long kk = clearance_key(best, (uint32_t)(i0 + j));
                 if (kk < run) { run = kk; rv = best; }
             }
-            for (int off = 16; off > 0; off >>= 1) rv = fminf(rv, __shfl_xor_sync(0xffffffffu, rv, off));
+            rv = warp_min(rv);
         }
-        for (int off = 16; off > 0; off >>= 1) {
-            const unsigned long long o = __shfl_xor_sync(0xffffffffu, run, off);
-            run = o < run ? o : run;
-        }
+        run = warp_min_key(run, 1);
         if (lane == 0 && run < seed_key) atomicMin(kp, run);
     }
 }
@@ -2093,7 +2098,7 @@ robot_self_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n
                             unsigned long long *__restrict__ keys) {
     __shared__ SclSmem sm;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const int low3_off = rs_low3_off(n_sdf);
     const long long pairs = (long long)cfg_count * n_src;
     // uniform per warp: every lane takes part in the shuffles
     for (long long w = (long long)blockIdx.x * kRsWarps + warp; w < n_units; w += (long long)gridDim.x * kRsWarps) {
@@ -2107,12 +2112,9 @@ robot_self_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n
         __syncwarp();                                        // the previous unit's staging is no longer read
         if (lane < 3 * n_sdf) {
             const int si = lane / 3;
-            sm.xf[warp][lane] = __ldg(reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg) * 16) +
-                                      (lane - 3 * si));
+            sm.xf[warp][lane] = __ldg(xf_rows(xforms, n_cfg, si, cfg) + (lane - 3 * si));
         } else if (lane >= 3 * kRsMaxS && lane < 3 * kRsMaxS + 3) {
-            sm.inv[warp][lane - 3 * kRsMaxS] =
-                __ldg(reinterpret_cast<const float4 *>(inv_xforms + ((size_t)i * n_cfg + cfg) * 16) +
-                      (lane - 3 * kRsMaxS));
+            sm.inv[warp][lane - 3 * kRsMaxS] = __ldg(xf_rows(inv_xforms, n_cfg, i, cfg) + (lane - 3 * kRsMaxS));
         }
         __syncwarp();
         if (lane < kRsMaxS) {
@@ -2152,12 +2154,9 @@ robot_self_clearance_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n
                 const unsigned long long kk = self_clearance_key(best, i, k0 + j);
                 if (kk < run) { run = kk; rv = best; }
             }
-            for (int off = 16; off > 0; off >>= 1) rv = fminf(rv, __shfl_xor_sync(0xffffffffu, rv, off));
+            rv = warp_min(rv);
         }
-        for (int off = 16; off > 0; off >>= 1) {
-            const unsigned long long o = __shfl_xor_sync(0xffffffffu, run, off);
-            run = o < run ? o : run;
-        }
+        run = warp_min_key(run, 1);
         if (lane == 0 && run < seed_key) atomicMin(kp, run);
     }
 }
@@ -2177,7 +2176,7 @@ self_clearance_finish_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int 
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < cfg_count; c += stride) {
         const int cfg = cfg_begin + c;
         auto rows_of = [&](const float *m, int s, float4 &r0, float4 &r1, float4 &r2) {
-            const float4 *row = reinterpret_cast<const float4 *>(m + ((size_t)s * n_cfg + cfg) * 16);
+            const float4 *row = xf_rows(m, n_cfg, s, cfg);
             r0 = __ldg(row); r1 = __ldg(row + 1); r2 = __ldg(row + 2);
         };
         auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) { rows_of(xforms, s, r0, r1, r2); };
@@ -2233,7 +2232,7 @@ robot_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n
     const int E = 1 + 6 * n_sdf;
     float *const acc = acc_all + warp * E * kCcLaneStride + lane;       // this lane's column
     const int n_tiles = (cfg_count + 31) >> 5;
-    const int low3_off = ~7 | (n_sdf >> 30);                           // as in robot_serial_kernel: ~7, not foldable
+    const int low3_off = rs_low3_off(n_sdf);
     const float m = margin;
     for (long long u = blockIdx.x; u < n_units; u += gridDim.x) {
         const long long sc = u / n_tiles;                               // segment * chunks_per_seg + chunk
@@ -2247,7 +2246,7 @@ robot_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n
         for (int item = threadIdx.x; item < kRbCfg * n_sdf; item += blockDim.x) {
             const int ci = item & 31, si = item >> 5;
             const int cfg = cfg_begin + min(c0 + ci, cfg_count - 1);
-            const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg) * 16);
+            const float4 *row = xf_rows(xforms, n_cfg, si, cfg);
             sm.xf[ci][3 * si] = __ldg(row); sm.xf[ci][3 * si + 1] = __ldg(row + 1); sm.xf[ci][3 * si + 2] = __ldg(row + 2);
         }
         for (int e = 0; e < E; ++e) acc[e * kCcLaneStride] = 0.f;
@@ -2269,11 +2268,7 @@ robot_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, int n
             rs_point_bounds(sm.sph[lane], pk.sph_rad, p, low3_off, 0xffu, lb, key);
             if (!__any_sync(0xffffffffu, collision_cost_near(lb, m))) continue;
             const int pred = __shfl_sync(0xffffffffu, rs_nearest(key, n_sdf), 0);
-            auto link = [&](const int si, const float thr, float4 &o) -> bool {
-                const pvb_sdf_desc &d = pk.d[si];
-                const float4 r0 = sm.xf[lane][3 * si], r1 = sm.xf[lane][3 * si + 1], r2 = sm.xf[lane][3 * si + 2];
-                return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
-            };
+            const auto link = rs_staged_link<kExt>(pk, sm.xf[lane], p);
             float best;
             f3 bg;
             int bs;
@@ -2366,7 +2361,7 @@ robot_paired_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk
                                    int chunks_per_seg, float margin, long long n_units, float *__restrict__ partial) {
     __shared__ PccSmem sm;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const int low3_off = rs_low3_off(n_sdf);
     const int E = 1 + 6 * n_sdf;
     const float m = margin;
     const long long pairs = (long long)cfg_count * n_seg;
@@ -2382,8 +2377,7 @@ robot_paired_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk
         __syncwarp();                                        // the previous unit is no longer read
         if (lane < 3 * n_sdf) {
             const int si = lane / 3;
-            sm.xf[warp][lane] = __ldg(reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg) * 16) +
-                                      (lane - 3 * si));
+            sm.xf[warp][lane] = __ldg(xf_rows(xforms, n_cfg, si, cfg) + (lane - 3 * si));
         }
         for (int e = lane; e < E * kCcWarps; e += 32) acc_all[e] = 0.f;
         __syncwarp();
@@ -2403,11 +2397,7 @@ robot_paired_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk
             float lb[kRsMaxS], key[kRsMaxS];
             rs_point_bounds(sm.sph[warp], pk.sph_rad, p, low3_off, 0xffu, lb, key);
             if (!__any_sync(0xffffffffu, on && collision_cost_near(lb, m))) continue;
-            auto link = [&](const int si, const float thr, float4 &o) -> bool {
-                const pvb_sdf_desc &d = pk.d[si];
-                const float4 r0 = sm.xf[warp][3 * si], r1 = sm.xf[warp][3 * si + 1], r2 = sm.xf[warp][3 * si + 2];
-                return rs_link_visit<kExt>(d, pk.visit_margin[si], r0, r1, r2, p, thr, o);
-            };
+            const auto link = rs_staged_link<kExt>(pk, sm.xf[warp], p);
             float best;
             f3 bg;
             int bs;
@@ -2465,7 +2455,7 @@ robot_self_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, 
                                  float *__restrict__ out_cost, float *__restrict__ out_twist) {
     __shared__ SccSmem sm;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int low3_off = ~7 | (n_sdf >> 30);                 // as in robot_serial_kernel: ~7, not foldable
+    const int low3_off = rs_low3_off(n_sdf);
     const int E = 1 + 6 * n_sdf;
     const float m = margin;
     float *const acc = &sm.acc[warp][0][lane];                 // this lane's column
@@ -2475,26 +2465,18 @@ robot_self_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, 
         __syncwarp();                                        // the previous configuration is no longer read
         if (lane < 3 * n_sdf) {
             const int si = lane / 3;
-            sm.xf[warp][lane] = __ldg(reinterpret_cast<const float4 *>(xforms + ((size_t)si * n_cfg + cfg) * 16) +
-                                      (lane - 3 * si));
+            sm.xf[warp][lane] = __ldg(xf_rows(xforms, n_cfg, si, cfg) + (lane - 3 * si));
         }
         for (int e = 0; e < E; ++e) acc[e * kCcLaneStride] = 0.f;
         __syncwarp();
-        if (lane < kRsMaxS) {
-            const f3 co = lane < n_sdf ? rs_sphere_centre(pk.d[lane], sm.xf[warp][3 * lane], sm.xf[warp][3 * lane + 1],
-                                                          sm.xf[warp][3 * lane + 2])
-                                       : mk3(0.f, 0.f, 0.f);
-            float *cc = reinterpret_cast<float *>(&sm.sph[warp][0]) + 3 * lane;
-            cc[0] = co.x; cc[1] = co.y; cc[2] = co.z;
-        }
+        if (lane < kRsMaxS) rs_centre_slot(pk.d, lane, n_sdf, sm.xf[warp], sm.sph[warp]);
 #pragma unroll 1
         for (int t = 0; t < n_src; ++t) {
             const int i = rows.src[t];
             const unsigned mask = rows.mask[i];
             __syncwarp();                                    // the previous source's W_i is no longer read
             if (lane < 3)
-                sm.inv[warp][lane] =
-                    __ldg(reinterpret_cast<const float4 *>(inv_xforms + ((size_t)i * n_cfg + cfg) * 16) + lane);
+                sm.inv[warp][lane] = __ldg(xf_rows(inv_xforms, n_cfg, i, cfg) + lane);
             __syncwarp();
             const float4 w0 = sm.inv[warp][0], w1 = sm.inv[warp][1], w2 = sm.inv[warp][2];
             float *const acc_i = acc + (1 + 6 * i) * kCcLaneStride;
@@ -2764,7 +2746,7 @@ __global__ void fk_serial_kernel(const __grid_constant__ FkPlan plan, const floa
 #pragma unroll
             for (int e = 0; e < 12; ++e) off.m[e] = lk.mesh_from_link[e];
             const Rt34 m = rt_mul(off, inv);
-            float4 *dst = reinterpret_cast<float4 *>(out + ((size_t)lk.slot * n_cfg + a) * 16);
+            float4 *dst = xf_rows(out, n_cfg, lk.slot, a);
             dst[0] = make_float4(m.m[0], m.m[1], m.m[2], m.m[3]);
             dst[1] = make_float4(m.m[4], m.m[5], m.m[6], m.m[7]);
             dst[2] = make_float4(m.m[8], m.m[9], m.m[10], m.m[11]);

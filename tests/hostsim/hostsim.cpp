@@ -93,12 +93,12 @@ static void composed_loop(const pvb_sdf_desc *descs, int n_sdf, const unsigned c
             float best = PVB_INF; f3 bg = mk3(0.f, 0.f, 0.f); int bs = -1;
             for (int si = 0; si < n_sdf; ++si) {
                 const int s = order ? order[si] : si;
-                const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + c) * 16);
+                const float4 *row = xf_rows(xforms, n_cfg, s, c);
                 const uint64_t idx = ((uint64_t)c * (uint64_t)n_pts + (uint64_t)i) * (uint64_t)n_sdf + (uint64_t)s;
                 composed_consider<kMesh, kExt>(descs[s], st, s, composed_xform(row[0], row[1], row[2], p), mesh_mode,
                                                idx, best, bg, bs);
             }
-            const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)max(bs, 0) * n_cfg + c) * 16);
+            const float4 *row = xf_rows(xforms, n_cfg, max(bs, 0), c);
             const f3 go = composed_rotate_back(row[0], row[1], row[2], bg);
             const long long o = (long long)c * n_pts + i;
             out_val[o] = best; out_grad[3 * o] = go.x; out_grad[3 * o + 1] = go.y; out_grad[3 * o + 2] = go.z;

@@ -20,7 +20,7 @@ extern "C" void simpair_composed(const pvb_sdf_desc *descs, int n_sdf, const uns
         paired_index(t, n_pts, c, i);
         const int cfg = cfg_begin + (int)c;
         auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) {
-            const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + cfg) * 16);
+            const float4 *row = xf_rows(xforms, n_cfg, s, cfg);
             r0 = row[0]; r1 = row[1]; r2 = row[2];
         };
         const f3 p = mk3(pts[3 * t], pts[3 * t + 1], pts[3 * t + 2]);

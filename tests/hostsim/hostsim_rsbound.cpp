@@ -16,7 +16,7 @@ extern "C" void simrs_sphere_lb(const pvb_sdf_desc *descs, int n_sdf, const floa
             f3 cen = mk3(0.f, 0.f, 0.f);
             if (s < n_sdf) {
                 rs_link_consts(descs[s], rad, margin);
-                const float4 *row = reinterpret_cast<const float4 *>(xforms + ((size_t)s * n_cfg + c) * 16);
+                const float4 *row = xf_rows(xforms, n_cfg, s, c);
                 cen = rs_sphere_centre(descs[s], row[0], row[1], row[2]);
             }
             for (long long i = 0; i < n_pts; ++i)
