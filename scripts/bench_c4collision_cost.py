@@ -6,29 +6,19 @@ same cost, twist gradient and joint gradient in torch, on the 8-link arm.
     python scripts/bench_c4collision_cost.py [--steps K] [--warmup W] [--rounds R]
 
 Arms: cached nearest, cached trilinear and primitive links.  Clouds: uniform in ARM_QUERY_RANGE and the tabletop scene
-of bench_c4clearance.py.  Margins 0.02 and 0.1 m.  Shapes: 200 x 10^5, 4096 x 10^5 and 200 x (1000 segments x 1000).
+of c4bench.scene_points.  Margins 0.02 and 0.1 m.  Shapes: 200 x 10^5, 4096 x 10^5 and 200 x (1000 segments x 1000).
 Device time per call from CUDA events around K calls after W warm-up calls, the two arms alternating for R rounds;
 pairs/s = |A| * points / time.  For each arm, the largest error of its cost and joint gradient against the fp64 sum
 of the same fp32 per-pair outputs, relative to the sum of |term| of each entry, and the largest difference between the
 two arms on the same scale; the fused arm's error is asserted <= 1e-5.  One JSON line per shape
 with the card's name and power limit.  Meshes and table caches go to a temporary directory that is removed at exit."""
-import argparse
 import json
-import os
-import shutil
-import statistics
-import sys
-import tempfile
+import math
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-import workloads  # noqa: E402
-from bench_c4clearance import scene_points  # noqa: E402
-from bench_c4swept import make_robot  # noqa: E402
-from bench_c4tri import card, timed  # noqa: E402
+import c4bench  # first: puts the repository root on sys.path
+import workloads
 
 
 def per_pair_cost(robot, pts, m, dtype=torch.float32, cfg_chunk=None):
@@ -66,58 +56,38 @@ def per_pair_cost(robot, pts, m, dtype=torch.float32, cfg_chunk=None):
     return [torch.cat(o) if o else None for o in out]
 
 
-def rel_err(got, ref, bound):
-    return float(((got.double() - ref).abs() / bound.clamp_min(1e-30)).max())
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--rounds", type=int, default=2)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_c4collision_cost.py needs a CUDA device")
-    gpu = card()
-    lo = [r[0] for r in workloads.ARM_QUERY_RANGE]; hi = [r[1] for r in workloads.ARM_QUERY_RANGE]
-    uniform = lambda n, s: workloads.uniform_points(n, lo, hi, seed=s)   # noqa: E731
-    tmp = tempfile.mkdtemp(prefix="pvb_c4collision_cost_")
-    try:
-        robots = {k: make_robot(k, tmp) for k in ("nearest", "trilinear", "primitive")}
+    with c4bench.session(10, 2, 2) as (args, tmp):
+        gpu = c4bench.card()
+        robots = {k: c4bench.make_robot(k, tmp) for k in ("nearest", "trilinear", "primitive")}
         for A, seg_shape in ((200, (100_000,)), (4096, (100_000,)), (200, (1000, 1000))):
             for kind, robot in robots.items():
                 robot.set_joint_configuration(workloads.arm_configurations(A).cuda())
-                for cloud in (uniform, scene_points):
-                    n = 1
-                    for s in seg_shape:
-                        n *= s
+                for cloud in (c4bench.uniform, c4bench.scene_points):
+                    n = math.prod(seg_shape)
                     pts = cloud(n, 300).reshape(*seg_shape, 3).cuda()
                     for m in (0.02, 0.1):
                         m = torch.tensor(m, dtype=torch.float32).item()     # the fp32 margin every route uses
-                        arms = {"fused": lambda r=robot, p=pts, m=m: r.collision_cost(p, m),
-                                "per_pair_then_torch": lambda r=robot, p=pts, m=m: per_pair_cost(r, p, m)[:2]}
+                        arms = {"fused": lambda i, r=robot, p=pts, m=m: r.collision_cost(p, m),
+                                "per_pair_then_torch": lambda i, r=robot, p=pts, m=m: per_pair_cost(r, p, m)[:2]}
                         rc, rg, ac, ag = per_pair_cost(robot, pts, m, torch.float64, cfg_chunk=256)
                         err, outs = {}, {}
                         for k, f in arms.items():
-                            c, g = f()
+                            c, g = f(0)
                             outs[k] = (c.reshape(rc.shape).double(), g.reshape(rg.shape).double())
-                            err[k] = {"cost": rel_err(outs[k][0], rc, ac), "joint_grad": rel_err(outs[k][1], rg, ag)}
+                            err[k] = {"cost": c4bench.rel_err(outs[k][0], rc, ac),
+                                      "joint_grad": c4bench.rel_err(outs[k][1], rg, ag)}
                         (fc, fg), (bc, bg) = outs["fused"], outs["per_pair_then_torch"]
-                        agree = {"cost": rel_err(fc, bc, ac), "joint_grad": rel_err(fg, bg, ag)}
+                        agree = {"cost": c4bench.rel_err(fc, bc, ac), "joint_grad": c4bench.rel_err(fg, bg, ag)}
                         # the torch arm's own fp32 cross products cancel where p is nearly parallel to g, so only the
                         # fused arm is held to the bound; the difference between the arms is reported
                         within = err["fused"]["cost"] <= 1e-5 and err["fused"]["joint_grad"] <= 1e-5
                         del outs, fc, fg, bc, bg
                         del rc, rg, ac, ag
                         torch.cuda.empty_cache()
-                        rounds = {k: [] for k in arms}
-                        for _ in range(args.rounds):
-                            for k, step in arms.items():
-                                rounds[k].append(timed(lambda i, f=step: f(), args.steps, args.warmup))
-                                torch.cuda.empty_cache()
-                        ms = {k: statistics.median(v) for k, v in rounds.items()}
+                        rounds, ms = c4bench.alternate(arms, args, empty_cache=True)
                         pairs = A * n
-                        line = {"links": kind, "cloud": "scene" if cloud is scene_points else "uniform",
+                        line = {"links": kind, "cloud": "scene" if cloud is c4bench.scene_points else "uniform",
                                 "n_cfg": A, "points": list(seg_shape), "margin": m,
                                 "fused_ms": ms["fused"], "fused_pairs_per_s": pairs / (ms["fused"] * 1e-3),
                                 "baseline_ms": ms["per_pair_then_torch"],
@@ -130,8 +100,6 @@ def main():
                         assert within, line
                     del pts
                     torch.cuda.empty_cache()
-    finally:
-        shutil.rmtree(tmp, ignore_errors=True)
 
 
 if __name__ == "__main__":

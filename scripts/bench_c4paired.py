@@ -10,51 +10,24 @@ numbers without a paired query, timed in rounds that alternate with it:
 One GPU.  Device time per step from CUDA events around K steps of each arm.  Prints one JSON line per shape
 (A configurations x P points each): pairs per second per arm, whether the arms' outputs are bit-identical, and the
 card's name and power limit.  Table caches go to a temporary directory that is removed at exit."""
-import argparse
 import json
-import os
-import shutil
-import statistics
 import sys
-import tempfile
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import workloads  # noqa: E402
-from bench_c4tri import card, timed  # noqa: E402
+import c4bench  # first: puts the repository root on sys.path
+import workloads
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--shapes", default="200x10000,4096x2048,65536x64")
-    args = ap.parse_args()
-    shapes = [tuple(int(x) for x in s.split("x")) for s in args.shapes.split(",")]
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_c4paired.py measures the GPU path and needs a CUDA device")
-    import pytorch_volumetric_b200 as pv
-    from pytorch_volumetric_b200 import _native
-    if _native.lib_missing():
-        raise SystemExit("libpvb.so is missing: build it first (python -c \"import __graft_entry__ as g; g.build()\")")
-
-    info = card()
-    tmp = tempfile.mkdtemp(prefix="pvb_c4paired_")
-    try:
-        urdf, end = workloads.write_arm(os.path.join(tmp, "arm"))
-        chain = pv.build_serial_chain_from_urdf(open(urdf).read(), end).to(device="cuda")
-        robot = pv.RobotSDF(chain, path_prefix=os.path.dirname(urdf),
-                            link_sdf_cls=pv.cache_link_sdf_factory(resolution=0.02, padding=1.0, device="cuda",
-                                                                   cache_path=os.path.join(tmp, "cache.pkl")))
-        lo = [r[0] for r in workloads.ARM_QUERY_RANGE]; hi = [r[1] for r in workloads.ARM_QUERY_RANGE]
+    with c4bench.session(10, 2, 3, shapes="200x10000,4096x2048,65536x64") as (args, tmp):
+        shapes = [tuple(int(x) for x in s.split("x")) for s in args.shapes.split(",")]
+        info = c4bench.card()
+        robot = c4bench.make_robot("nearest", tmp)
         for A, P in shapes:
             robot.set_joint_configuration(workloads.arm_configurations(A).cuda())
             comp = robot.sdf
-            own = workloads.uniform_points(A * P, lo, hi, seed=4).cuda().reshape(A, P, 3)
+            own = c4bench.uniform(A * P, seed=4).cuda().reshape(A, P, 3)
             val = torch.empty(A * P, device="cuda")
             grad = torch.empty(A * P, 3, device="cuda")
 
@@ -75,17 +48,13 @@ def main():
             arms = {"paired": paired, "loop": loop}
             if (A, P) == (200, 10_000):
                 arms["cross"] = cross
-            ms = {k: [] for k in arms}
-            for _ in range(args.rounds):
-                for k, f in arms.items():
-                    ms[k].append(timed(f, args.steps, args.warmup))
+            ms, med = c4bench.alternate(arms, args)
             outs = {k: f(0) for k, f in arms.items()}
             ref_v, ref_g = outs["paired"]
             ref_v, ref_g = ref_v.reshape(-1), ref_g.reshape(-1, 3)
             equal = all(torch.equal(v.reshape(-1), ref_v) and torch.equal(g.reshape(-1, 3), ref_g)
                         for v, g in outs.values())
             del outs
-            med = {k: statistics.median(v) for k, v in ms.items()}
             print(json.dumps({
                 "workload": f"RobotSDF.paired, synthetic 7-DOF arm (8 links, CachedSDF res=0.02 pad=1.0) x {A} "
                             f"configurations x {P} points each, value+gradient",
@@ -94,8 +63,6 @@ def main():
                 "ms_per_step": med, "rounds_ms": ms, "arms_bit_equal": equal,
                 "steps": args.steps, "warmup": args.warmup, "card": info}), flush=True)
             torch.cuda.empty_cache()
-    finally:
-        shutil.rmtree(tmp, ignore_errors=True)
     return 0
 
 

@@ -6,30 +6,19 @@ of configurations, fp64 terms and one masked sum per link) followed by the same 
     python scripts/bench_c4paired_collision_cost.py [--steps K] [--warmup W] [--rounds R]
 
 Shapes (A configurations x points per configuration): 200 x 10^4, 4096 x 2048, 65 536 x 64 and 1024 x (8 segments x
-256), with nearest, trilinear and primitive links, the two clouds of bench_c4paired_clearance.py (uniform per
+256), with nearest, trilinear and primitive links, the two clouds of c4bench.clouds (uniform per
 configuration, and the tabletop scene shifted per configuration), and margins 0.02 and 0.1 m.  Before timing, both
 arms are compared with the fp64 sum of the same fp32 per-pair outputs (query_paired(..., return_which=True)), and
 asserted to agree with each other within 1e-5 of the sum of |term| of every cost and joint-gradient entry.  Device
 time per call from CUDA events around K calls after W warm-up calls, the two arms alternating for R rounds; pairs/s =
 A * (points per configuration) / time.  Prints one JSON line per shape with the card's name and power limit.  Meshes
 and table caches go to a temporary directory that is removed at exit."""
-import argparse
 import json
-import os
-import shutil
-import statistics
-import sys
-import tempfile
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-import workloads  # noqa: E402
-from bench_c4paired_clearance import clouds  # noqa: E402
-from bench_c4swept import make_robot  # noqa: E402
-from bench_c4tri import card, timed  # noqa: E402
+import c4bench  # first: puts the repository root on sys.path
+import workloads
 
 
 def composition(robot, own, m):
@@ -69,49 +58,32 @@ def fp64_reference(robot, own, m, cfg_chunk=256):
     return [torch.cat(o) for o in out]
 
 
-def rel_err(got, ref, bound):
-    return float(((got.double().reshape(ref.shape) - ref).abs() / bound.clamp_min(1e-30)).max())
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--rounds", type=int, default=3)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_c4paired_collision_cost.py needs a CUDA device")
-    gpu = card()
-    tmp = tempfile.mkdtemp(prefix="pvb_c4pcollision_cost_")
-    try:
-        robots = {k: make_robot(k, tmp) for k in ("nearest", "trilinear", "primitive")}
+    with c4bench.session(10, 2, 3) as (args, tmp):
+        gpu = c4bench.card()
+        robots = {k: c4bench.make_robot(k, tmp) for k in ("nearest", "trilinear", "primitive")}
         shapes = [("a200_n1e4", 200, (10_000,)), ("a4096_n2048", 4096, (2048,)), ("a65536_n64", 65_536, (64,)),
                   ("a1024_seg8_n256", 1024, (8, 256))]
         for name, A, seg_shape in shapes:
             for cloud in ("uniform", "scene"):
-                own = clouds(cloud, A, seg_shape, 300)
+                own = c4bench.clouds(cloud, A, seg_shape, 300).cuda()
                 for kind, robot in robots.items():
                     robot.set_joint_configuration(workloads.arm_configurations(A).cuda())
                     for m in (0.02, 0.1):
                         m = torch.tensor(m, dtype=torch.float32).item()     # the fp32 margin every route uses
-                        arms = {"fused": lambda r=robot, m=m: r.paired_collision_cost(own, m),
-                                "composition": lambda r=robot, m=m: composition(r, own, m)}
+                        arms = {"fused": lambda i, r=robot, m=m: r.paired_collision_cost(own, m),
+                                "composition": lambda i, r=robot, m=m: composition(r, own, m)}
                         rc, rg, ac, ag = fp64_reference(robot, own, m)
-                        outs = {k: f() for k, f in arms.items()}
-                        err = {k: {"cost": rel_err(c, rc, ac), "joint_grad": rel_err(g, rg, ag)}
+                        outs = {k: f(0) for k, f in arms.items()}
+                        err = {k: {"cost": c4bench.rel_err(c, rc, ac), "joint_grad": c4bench.rel_err(g, rg, ag)}
                                for k, (c, g) in outs.items()}
                         (fc, fg), (bc, bg) = outs["fused"], outs["composition"]
-                        agree = {"cost": rel_err(fc, bc.double().reshape(rc.shape), ac),
-                                 "joint_grad": rel_err(fg, bg.double().reshape(rg.shape), ag)}
+                        agree = {"cost": c4bench.rel_err(fc, bc.double().reshape(rc.shape), ac),
+                                 "joint_grad": c4bench.rel_err(fg, bg.double().reshape(rg.shape), ag)}
                         contributing = int((rc > 0).sum())
                         del outs, fc, fg, bc, bg, rc, rg, ac, ag
                         torch.cuda.empty_cache()
-                        rounds = {k: [] for k in arms}
-                        for _ in range(args.rounds):
-                            for k, step in arms.items():
-                                rounds[k].append(timed(lambda i, f=step: f(), args.steps, args.warmup))
-                                torch.cuda.empty_cache()
-                        ms = {k: statistics.median(v) for k, v in rounds.items()}
+                        rounds, ms = c4bench.alternate(arms, args, empty_cache=True)
                         pairs = A * own[0].numel() // 3
                         line = {"shape": name, "links": kind, "cloud": cloud, "n_cfg": A, "points": list(seg_shape),
                                 "margin": m, "fused_ms": ms["fused"], "fused_pairs_per_s": pairs / (ms["fused"] * 1e-3),
@@ -124,8 +96,6 @@ def main():
                         assert agree["cost"] <= 1e-5 and agree["joint_grad"] <= 1e-5, line
                 del own
                 torch.cuda.empty_cache()
-    finally:
-        shutil.rmtree(tmp, ignore_errors=True)
 
 
 if __name__ == "__main__":

@@ -12,22 +12,15 @@ in fp64 under the fp32 link transforms) over all configurations and the first 10
 be within 1e-5; the tessellated arm's error is reported.  Prints one JSON line with ms per step, pairs per second,
 the per-round times, the errors and the card's name and power limit.  Meshes and table caches go to a temporary
 directory that is removed at exit.  The reference project has no primitive links, so there is no reference arm."""
-import argparse
 import json
 import os
-import shutil
-import statistics
-import sys
-import tempfile
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-import workloads  # noqa: E402
-from bench_c4tri import card, timed  # noqa: E402
+import c4bench  # first: puts the repository root on sys.path
+import pytorch_volumetric_b200 as pv
+import workloads
 
 
 def tessellate(geom):
@@ -91,7 +84,6 @@ def write_tessellated_arm(dirname):
 
 def fp64_composition(prim_robot, pts):
     """min over links of the exact primitives in fp64, under prim_robot's fp32 link transforms: [A, P]."""
-    import pytorch_volumetric_b200 as pv
     from pytorch_volumetric_b200.transforms import matrix_of
     S = len(prim_robot.sdf.sdfs)
     M = matrix_of(prim_robot.sdf.obj_frame_to_link_frame).detach().double().reshape(S, -1, 4, 4)
@@ -115,22 +107,9 @@ def fp64_composition(prim_robot, pts):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=50)
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--n-cfg", type=int, default=200)
-    ap.add_argument("--n-pts", type=int, default=100_000)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_c4prim.py needs a CUDA device")
-    import pytorch_volumetric_b200 as pv
-    tmp = tempfile.mkdtemp(prefix="pvb_c4prim_")
-    try:
+    with c4bench.session(50, 5, 3, n_cfg=200, n_pts=100_000) as (args, tmp):
         th = workloads.arm_configurations(args.n_cfg).cuda()
-        urdf, end = workloads.write_primitive_arm(os.path.join(tmp, "prim"))
-        prim = pv.RobotSDF(pv.build_serial_chain_from_urdf(open(urdf).read(), end).to(device="cuda"),
-                           primitive_visuals=True)
+        prim = c4bench.make_robot("primitive", tmp)
         urdf, end = write_tessellated_arm(os.path.join(tmp, "tess"))
         tess = pv.RobotSDF(pv.build_serial_chain_from_urdf(open(urdf).read(), end).to(device="cuda"),
                            path_prefix=os.path.join(tmp, "tess"),
@@ -138,8 +117,7 @@ def main():
                                                                   cache_path=os.path.join(tmp, "tess", "cache.pkl")))
         for r in (prim, tess):
             r.set_joint_configuration(th)
-        lo = [r[0] for r in workloads.ARM_QUERY_RANGE]; hi = [r[1] for r in workloads.ARM_QUERY_RANGE]
-        bufs = [workloads.uniform_points(args.n_pts, lo, hi, seed=100 + i).cuda() for i in range(3)]
+        bufs = [c4bench.uniform(args.n_pts, seed=100 + i).cuda() for i in range(3)]
 
         # accuracy against the fp64 composition of the exact primitives
         sub = bufs[0][:10_000]
@@ -153,20 +131,15 @@ def main():
         assert err["primitive"]["max_abs"] < 1e-5, err
 
         pairs = args.n_cfg * args.n_pts
-        rounds = {"primitive": [], "tessellated": []}
-        for _ in range(args.rounds):
-            for name, robot in (("primitive", prim), ("tessellated", tess)):
-                rounds[name].append(timed(lambda i, r=robot: r(bufs[i % 3]), args.steps, args.warmup))
-        ms = {k: statistics.median(v) for k, v in rounds.items()}
+        rounds, ms = c4bench.alternate({"primitive": lambda i: prim(bufs[i % 3]),
+                                        "tessellated": lambda i: tess(bufs[i % 3])}, args)
         line = {"metric": "c4prim_pairs_per_s", "value": pairs / (ms["primitive"] * 1e-3), "unit": "pairs/s",
                 "ms_per_step": ms["primitive"], "tessellated_ms_per_step": ms["tessellated"],
                 "tessellated_pairs_per_s": pairs / (ms["tessellated"] * 1e-3),
                 "speedup_vs_tessellated": ms["tessellated"] / ms["primitive"], "rounds_ms": rounds,
                 "error_vs_fp64": err, "n_cfg": args.n_cfg, "n_pts": args.n_pts, "steps": args.steps,
-                "warmup": args.warmup, "gpu": card()}
+                "warmup": args.warmup, "gpu": c4bench.card()}
         print(json.dumps(line))
-    finally:
-        shutil.rmtree(tmp, ignore_errors=True)
 
 
 if __name__ == "__main__":

@@ -12,28 +12,17 @@ timing, the two arms are asserted to agree within 1e-5 of the sum of |term| of e
 time per call from CUDA events around K calls after W warm-up calls, the two arms alternating for R rounds, median
 reported; pairs/s = A * S * (points per link) / time.  Prints one JSON line per (shape, links, margin) with the card's
 name and power limit.  Meshes and table caches go to a temporary directory that is removed at exit."""
-import argparse
 import json
-import math
-import os
-import shutil
-import statistics
-import sys
-import tempfile
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-from bench_c4swept import make_robot  # noqa: E402
-from bench_c4tri import card, timed  # noqa: E402
+import c4bench  # first: puts the repository root on sys.path
+import pytorch_volumetric_b200 as pv
+from pytorch_volumetric_b200 import _native as nat
 
 
 def abs_terms(comp, lp, rows, m, A):
     """sum|h^2| [A] and sum|tau| [A, S, 6] of every entry, from the composition route's own per-point values."""
-    import pytorch_volumetric_b200 as pv
-    from pytorch_volumetric_b200 import _native as nat
     S, K = lp.shape[:2]
     dev = lp.device
     xf = comp._xforms_on(dev).reshape(S, A, 4, 4)
@@ -66,20 +55,11 @@ def abs_terms(comp, lp, rows, m, A):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_c4self_collision_cost.py needs a CUDA device")
-    gpu = card()
-    tmp = tempfile.mkdtemp(prefix="pvb_c4selfcost_")
-    try:
-        robots = {k: make_robot(k, tmp) for k in ("nearest", "trilinear", "primitive")}
+    with c4bench.session(20, 3, 3) as (args, tmp):
+        gpu = c4bench.card()
+        robots = {k: c4bench.make_robot(k, tmp) for k in ("nearest", "trilinear", "primitive")}
         for name, A, K in (("a200_k1024", 200, 1024), ("a4096_k256", 4096, 256), ("a65536_k64", 65_536, 64)):
-            g = torch.Generator().manual_seed(A)
-            q = ((torch.rand(A, 7, generator=g, dtype=torch.float64) * 2 - 1) * math.pi).float().cuda()
+            q = c4bench.crossing_configurations(A)
             for kind, robot in robots.items():
                 robot.set_joint_configuration(q)
                 comp = robot.sdf
@@ -99,11 +79,7 @@ def main():
                     assert err_c <= 1e-5 and err_t <= 1e-5, (name, kind, margin, err_c, err_t)
                     contributing = int((got[0] > 0).sum())
                     del got, ref, ac, at
-                    rounds = {k: [] for k in arms}
-                    for _ in range(args.rounds):
-                        for k, step in arms.items():
-                            rounds[k].append(timed(step, args.steps, args.warmup))
-                    ms = {k: statistics.median(v) for k, v in rounds.items()}
+                    rounds, ms = c4bench.alternate(arms, args)
                     pairs = A * S * K
                     line = {"shape": name, "links": kind, "margin": margin, "n_cfg": A, "points_per_link": K,
                             "n_links": S, "fused_ms": ms["fused"], "fused_pairs_per_s": pairs / (ms["fused"] * 1e-3),
@@ -114,8 +90,6 @@ def main():
                             "rounds_ms": rounds, "steps": args.steps, "warmup": args.warmup, "gpu": gpu}
                     print(json.dumps(line), flush=True)
             torch.cuda.empty_cache()
-    finally:
-        shutil.rmtree(tmp, ignore_errors=True)
 
 
 if __name__ == "__main__":

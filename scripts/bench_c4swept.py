@@ -11,21 +11,12 @@ Both arms are asserted to give identical values, gradients and configuration ind
 Device time per step from CUDA events around K steps after W warm-up steps, the two arms alternating for R rounds;
 pairs/s = |A| * N / time.  Prints one JSON line per shape with the card's name and power limit.  Meshes and table
 caches go to a temporary directory that is removed at exit."""
-import argparse
 import json
-import os
-import shutil
-import statistics
-import sys
-import tempfile
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-import workloads  # noqa: E402
-from bench_c4tri import card, timed  # noqa: E402
+import c4bench  # first: puts the repository root on sys.path
+import workloads
 
 
 def reduce_cross_product(robot, pts):
@@ -36,40 +27,17 @@ def reduce_cross_product(robot, pts):
     return v.gather(0, c[None])[0], g.gather(0, c[None, :, None].expand(1, c.numel(), 3))[0], c
 
 
-def make_robot(kind, tmp):
-    import pytorch_volumetric_b200 as pv
-    if kind == "primitive":
-        urdf, end = workloads.write_primitive_arm(os.path.join(tmp, "prim"))
-        return pv.RobotSDF(pv.build_serial_chain_from_urdf(open(urdf).read(), end).to(device="cuda"),
-                           primitive_visuals=True)
-    d = os.path.join(tmp, kind)
-    urdf, end = workloads.write_arm(d)
-    return pv.RobotSDF(pv.build_serial_chain_from_urdf(open(urdf).read(), end).to(device="cuda"), path_prefix=d,
-                       link_sdf_cls=pv.cache_link_sdf_factory(resolution=0.02, padding=1.0, device="cuda",
-                                                              cache_path=os.path.join(d, "cache.pkl"),
-                                                              interpolation=kind))
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_c4swept.py needs a CUDA device")
-    gpu = card()
-    lo = [r[0] for r in workloads.ARM_QUERY_RANGE]; hi = [r[1] for r in workloads.ARM_QUERY_RANGE]
-    tmp = tempfile.mkdtemp(prefix="pvb_c4swept_")
-    try:
-        robots = {k: make_robot(k, tmp) for k in ("nearest", "trilinear", "primitive")}
+    with c4bench.session(20, 3, 3) as (args, tmp):
+        gpu = c4bench.card()
+        robots = {k: c4bench.make_robot(k, tmp) for k in ("nearest", "trilinear", "primitive")}
         shapes = [("c4", "nearest", 200, 100_000, True), ("c4_trilinear", "trilinear", 200, 100_000, True),
                   ("c4_primitive", "primitive", 200, 100_000, True), ("a4096_n1e5", "nearest", 4096, 100_000, True),
                   ("a4096_n1e6", "nearest", 4096, 1_000_000, False)]
         for name, kind, A, N, baseline in shapes:
             robot = robots[kind]
             robot.set_joint_configuration(workloads.arm_configurations(A).cuda())
-            bufs = [workloads.uniform_points(N, lo, hi, seed=100 + i).cuda() for i in range(2)]
+            bufs = [c4bench.uniform(N, seed=100 + i).cuda() for i in range(2)]
             arms = {"swept": lambda i, r=robot: r.swept(bufs[i % 2], return_argmin=True)}
             identical = None
             if baseline:
@@ -79,12 +47,7 @@ def main():
                 identical = bool(torch.equal(sv, rv) and torch.equal(sg, rg) and torch.equal(sc, rc))
                 assert identical, name
                 del sv, sg, sc, rv, rg, rc
-            rounds = {k: [] for k in arms}
-            for _ in range(args.rounds):
-                for k, step in arms.items():
-                    rounds[k].append(timed(step, args.steps, args.warmup))
-                    torch.cuda.empty_cache()
-            ms = {k: statistics.median(v) for k, v in rounds.items()}
+            rounds, ms = c4bench.alternate(arms, args, empty_cache=True)
             line = {"shape": name, "links": kind, "n_cfg": A, "n_pts": N,
                     "swept_ms": ms["swept"], "swept_pairs_per_s": A * N / (ms["swept"] * 1e-3),
                     "baseline_ms": ms.get("cross_product_then_min"),
@@ -96,8 +59,6 @@ def main():
             print(json.dumps(line), flush=True)
             del bufs, arms
             torch.cuda.empty_cache()
-    finally:
-        shutil.rmtree(tmp, ignore_errors=True)
 
 
 if __name__ == "__main__":
