@@ -481,6 +481,8 @@ int pvb_compact_nonempty(const void *data, int64_t n, int32_t elem_bytes, double
                          int64_t capacity, int64_t *out_index, int64_t *out_count, void *stream);
 
 /* ---- rigid transform helpers used by the generic (unfused) composition path ---- */
+/* out[b][i] = xforms[b] applied to pts[i] (pts DEVICE [n_pts][3], out DEVICE [n_tf][n_pts][3]), the FMA chain of the
+ * composed kernels' transform; any n_tf >= 0, PVB_ERR_INVALID when n_tf * n_pts * 3 overflows int64 */
 int pvb_transform_points(const float *xforms, int32_t n_tf, const float *pts, int64_t n_pts,
                          float *out, void *stream);
 /* paired: out[b][i] = xforms[b] applied to pts[b][i] (pts / out DEVICE [n_tf][n_pts][3]), same arithmetic as the

@@ -2900,14 +2900,17 @@ __global__ void mesh_sample_kernel(const double *__restrict__ verts, const int *
 }
 
 // ======================================================== transform points
-__global__ void transform_points_kernel(const float *__restrict__ xforms, int n_tf, const float *__restrict__ pts,
-                                        long long n_pts, float *__restrict__ out) {
-    const int b = blockIdx.y;
-    const float *xf = xforms + (size_t)b * 16;
+// out[t] = M_{t / n_pts} applied to pts[t % n_pts]: every transform to every point (the unfused composition).  One
+// flat 64-bit index over the n_tf x n_pts pairs, so that no grid dimension bounds the transform count.
+__global__ void transform_points_kernel(const float *__restrict__ xforms, const float *__restrict__ pts,
+                                        long long n_pts, long long n, float *__restrict__ out) {
     const long long stride = (long long)gridDim.x * blockDim.x;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_pts; i += stride) {
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
+        long long b, i;
+        paired_index(t, n_pts, b, i);
+        const float *xf = xforms + b * 16;
         const f3 p = load_point(pts, i);
-        float *o = out + ((size_t)b * n_pts + i) * 3;
+        float *o = out + 3 * t;
         o[0] = fmaf(xf[0], p.x, fmaf(xf[1], p.y, fmaf(xf[2], p.z, xf[3])));
         o[1] = fmaf(xf[4], p.x, fmaf(xf[5], p.y, fmaf(xf[6], p.z, xf[7])));
         o[2] = fmaf(xf[8], p.x, fmaf(xf[9], p.y, fmaf(xf[10], p.z, xf[11])));
@@ -4392,13 +4395,14 @@ extern "C" int pvb_transform_points_paired(const float *xforms, int32_t n_tf, co
 
 extern "C" int pvb_transform_points(const float *xforms, int32_t n_tf, const float *pts, int64_t n_pts, float *out,
                                     void *stream) {
-    if (!xforms || n_tf < 0 || n_pts < 0 || (n_tf > 0 && n_pts > 0 && (!pts || !out)) || n_tf > 65535) {
+    if (!xforms || n_tf < 0 || n_pts < 0 || (n_tf > 0 && n_pts > 0 && (!pts || !out)) ||
+        (n_tf > 0 && n_pts > INT64_MAX / 3 / n_tf)) {
         pvb_set_error("pvb_transform_points: invalid argument");
         return PVB_ERR_INVALID;
     }
     if (n_tf == 0 || n_pts == 0) return PVB_OK;
-    dim3 grid((unsigned)grid_for(n_pts, 256, 8), (unsigned)n_tf);
-    transform_points_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(xforms, n_tf, pts, n_pts, out);
+    const long long n = (long long)n_tf * n_pts;
+    transform_points_kernel<<<grid_for(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(xforms, pts, n_pts, n, out);
     PVB_CHECK_LAUNCH("pvb_transform_points");
     return PVB_OK;
 }

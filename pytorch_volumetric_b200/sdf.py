@@ -1533,30 +1533,40 @@ class ComposedSDF(ObjectFrameSDF):
                                                              int(mc_grad) + 12 * cfg_begin * P,
                                                              nat.stream_ptr(device)), "pvb_composed_query_multicast")
 
+    #: (configuration, point) pairs per chunk of `_generic_query` (bounds its per-sub-SDF temporaries)
+    generic_chunk_pairs = 1 << 20
+
     def _generic_query(self, p, cfg_begin, cfg_count, n_cfg, return_which, paired=False):
         """Sub-SDFs without a native descriptor (user subclasses, nested compositions): per-SDF evaluation through
-        their own __call__, with the transform and the running min still on the GPU.  paired: p holds cfg_count
-        blocks of P points, block c for configuration cfg_begin + c only (query_paired)."""
+        their own __call__, with the transform and the running min still on the GPU, over chunks of at most
+        `generic_chunk_pairs` pairs (one configuration at least), each written into its rows of the result.  paired:
+        p holds cfg_count blocks of P points, block c for configuration cfg_begin + c only (query_paired)."""
         S = len(self.sdfs)
         device = p.device
         P = (p.shape[0] // cfg_count if cfg_count else 0) if paired else p.shape[0]
-        M = self._xforms_on(device).reshape(S, n_cfg, 4, 4)[:, cfg_begin:cfg_begin + cfg_count]
+        M = self._xforms_on(device).reshape(S, n_cfg, 4, 4)
         best = torch.full((cfg_count * P,), float("inf"), dtype=torch.float32, device=device)
         bgrad = torch.zeros(cfg_count * P, 3, dtype=torch.float32, device=device)
         bwhich = torch.full((cfg_count * P,), -1, dtype=torch.int32, device=device)
         transform = nat.lib().pvb_transform_points_paired if paired else nat.lib().pvb_transform_points
-        for i, sdf in enumerate(self.sdfs):
-            xf = M[i].contiguous()
-            local = torch.empty(cfg_count, P, 3, dtype=torch.float32, device=device)
-            nat.check(transform(nat.ptr(xf), cfg_count, nat.ptr(p), P, nat.ptr(local), nat.stream_ptr(device)),
-                      "pvb_transform_points")
-            v, g = sdf(local)
-            v = v.to(device=device, dtype=torch.float32).reshape(cfg_count, P)
-            g = g.to(device=device, dtype=torch.float32).reshape(cfg_count, P, 3) @ xf[:, :3, :3]
-            better = (v.reshape(-1) < best) | (bwhich < 0)
-            best = torch.where(better, v.reshape(-1), best)
-            bgrad = torch.where(better.unsqueeze(-1), g.reshape(-1, 3), bgrad)
-            bwhich = torch.where(better, torch.full_like(bwhich, i), bwhich)
+        step = max(1, self.generic_chunk_pairs // max(P, 1))
+        for c0 in range(0, cfg_count if P > 0 else 0, step):
+            cc = min(step, cfg_count - c0)
+            rows = slice(c0 * P, (c0 + cc) * P)
+            pts = p[rows] if paired else p
+            cbest, cgrad, cwhich = best[rows], bgrad[rows], bwhich[rows]        # views: the chunk's result rows
+            for i, sdf in enumerate(self.sdfs):
+                xf = M[i, cfg_begin + c0:cfg_begin + c0 + cc].contiguous()
+                local = torch.empty(cc, P, 3, dtype=torch.float32, device=device)
+                nat.check(transform(nat.ptr(xf), cc, nat.ptr(pts), P, nat.ptr(local), nat.stream_ptr(device)),
+                          transform.__name__)
+                v, g = sdf(local)
+                v = v.to(device=device, dtype=torch.float32).reshape(-1)
+                g = (g.to(device=device, dtype=torch.float32).reshape(cc, P, 3) @ xf[:, :3, :3]).reshape(-1, 3)
+                better = (v < cbest) | (cwhich < 0)
+                cbest.copy_(torch.where(better, v, cbest))
+                cgrad.copy_(torch.where(better.unsqueeze(-1), g, cgrad))
+                cwhich.masked_fill_(better, i)
         return (best, bgrad, bwhich) if return_which else (best, bgrad)
 
     #: host callers with at least this many result bytes get their result streamed out slab by slab

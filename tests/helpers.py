@@ -223,7 +223,8 @@ def _trilinear_alternatives(ref, q, R, s):
 
 
 def classify_composed(v_gpu, g_gpu, v_ref, g_ref, specs, mats, pts, tol=1e-5):
-    """v_*: (A, P) values, g_*: (A, P, 3); mats: (S, A, 4, 4) object->sub-frame; pts (P, 3).
+    """v_*: (A, P) values, g_*: (A, P, 3); mats: (S, A, 4, 4) object->sub-frame; pts (P, 3), or (A, P, 3) with
+    configuration a at its own points (the paired form).
     Returns (n_exceed, n_unexplained, report).  An exceedance is explained when the GPU output equals, within `tol`,
     one of the legitimate alternatives of flip_candidates AND is a possible minimum over the sub-SDFs (between the
     min over sub-SDFs of their smallest and of their largest alternative)."""
@@ -234,7 +235,8 @@ def classify_composed(v_gpu, g_gpu, v_ref, g_ref, specs, mats, pts, tol=1e-5):
     pts = np.asarray(pts, dtype=np.float64)
     unexplained = []
     for a, i in idx:
-        cands = flip_candidates(specs, mats[:, a], pts[i])
+        p = pts[a, i] if pts.ndim == 3 else pts[i]
+        cands = flip_candidates(specs, mats[:, a], p)
         # a valid output is min over sub-SDFs of ONE alternative each: it lies between the two extreme choices
         per_s = {}
         for cv, _cg, s_, _sl in cands:
@@ -358,13 +360,14 @@ def clearance_reduce(v, g, w, cfg_count, n_seg):
 
 
 def _which_values(specs, tm, pts, w):
-    """fp64 value of the reported sub-SDF w (A, P) at every pair."""
+    """fp64 value of the reported sub-SDF w (A, P) at every pair; pts (P, 3) or, paired, (A, P, 3)."""
     import composed_ref as cr
     out = np.full(w.shape, np.nan)
     for s, spec in enumerate(specs):
         a, i = np.nonzero(w == s)
         if len(a):
-            q = np.einsum("nij,nj->ni", tm[s, a, :3, :3], pts[i].astype(np.float64)) + tm[s, a, :3, 3]
+            p = pts[a, i] if pts.ndim == 3 else pts[i]
+            q = np.einsum("nij,nj->ni", tm[s, a, :3, :3], p.astype(np.float64)) + tm[s, a, :3, 3]
             out[a, i] = cr.evaluate(spec, q)[0]
     return out
 
@@ -372,10 +375,11 @@ def _which_values(specs, tm, pts, w):
 def assert_fp64(members, tm, pts, v, g, w, what, tol=1e-5):
     """query(..., return_which=True) against the fp64 composition: grids and primitives through
     classify_composed (every exceedance a classified flip or tie), meshes through composed_ref.mesh_mismatch;
-    `which` names a sub-SDF whose fp64 value is the result's within the tolerance.  Returns the exceedance mask."""
+    `which` names a sub-SDF whose fp64 value is the result's within the tolerance.  pts (P, 3), or (A, P, 3) for
+    query_paired.  Returns the exceedance mask."""
     import composed_ref as cr
     S, A = tm.shape[:2]
-    P = len(pts)
+    P = pts.shape[-2]
     v, g, w = (t.cpu().numpy() for t in (v, g, w))
     v, g, w = v.reshape(A, P), g.reshape(A, P, 3), w.reshape(A, P)
     specs = [m[1] for m in members]
