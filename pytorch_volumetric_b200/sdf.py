@@ -769,6 +769,14 @@ class ComposedSDF(ObjectFrameSDF):
                              f"A = {batch} leading")
 
     @staticmethod
+    def _paired_block(lead, cfg_count):
+        """The size of each of the cfg_count blocks, one per configuration, that a paired form's `lead` leading points
+        split into (0 for an empty slab without points); None when they do not split."""
+        if (lead % cfg_count) if cfg_count > 0 else lead:
+            return None
+        return lead // cfg_count if cfg_count > 0 else 0
+
+    @staticmethod
     def _deliver(points, outs, shape, device=None):
         """Flat query results as a public form returns them: values and gradients in the points' dtype (fp32 for
         non-tensors), index outputs as int64, on `device` -- by default the points' device, CPU for non-tensors --
@@ -853,10 +861,9 @@ class ComposedSDF(ObjectFrameSDF):
         S = len(self.sdfs)
         n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
         shape = tuple(points_in_object_frame.shape)
-        n = math.prod(shape[:-1])
-        if shape[-1:] != (3,) or (n % cfg_count if cfg_count else n):
+        P = self._paired_block(math.prod(shape[:-1]), cfg_count)
+        if shape[-1:] != (3,) or P is None:
             raise ValueError(f"paired query: points {shape} do not split into {cfg_count} blocks of [P, 3]")
-        P = n // cfg_count if cfg_count else 0
         with _query_points(points_in_object_frame) as (device, p):
             descs_arr, needs_mesh = self._native_descs(device)
             if descs_arr is None:
@@ -887,8 +894,19 @@ class ComposedSDF(ObjectFrameSDF):
         self._check_leading_batch(pts_shape, "paired query", "..., 3", 1)
         return self._deliver(points_in_object_frame, self.query_paired(points_in_object_frame), pts_shape[:-1])
 
-    #: configurations per `_generic_query` chunk of the unfused swept fold (bounds its cfg_chunk x P temporaries)
-    swept_generic_chunk = 64
+    #: configurations per chunk of every composition route (bounds its chunk x P temporaries)
+    composition_chunk = 64
+
+    def _composition_chunks(self, p, cfg_begin, cfg_count, paired=False):
+        """The walk of the composition routes: (c0, cc, points, v, g, w) of every chunk of the slab, ascending, with
+        (v, g, w) = query(points, c0, cc, return_which=True) at points = p -- paired (p holds one block of points
+        per configuration), query_paired at the chunk's own blocks.  Nothing when there are no points."""
+        n_pts = p.shape[0] // max(cfg_count, 1) if paired else p.shape[0]
+        for c0 in range(cfg_begin, cfg_begin + (cfg_count if n_pts > 0 else 0), self.composition_chunk):
+            cc = min(self.composition_chunk, cfg_begin + cfg_count - c0)
+            pts = p[(c0 - cfg_begin) * n_pts:(c0 - cfg_begin + cc) * n_pts] if paired else p
+            query = self.query_paired if paired else self.query
+            yield (c0, cc, pts, *query(pts, cfg_begin=c0, cfg_count=cc, return_which=True))
 
     def query_swept(self, points_in_object_frame, cfg_begin=0, cfg_count=None, return_which=False):
         """Swept form of `query`: at every point, the result of the configuration of the slab
@@ -907,7 +925,7 @@ class ComposedSDF(ObjectFrameSDF):
             P = p.shape[0]
             descs_arr, needs_mesh = self._native_descs(device)
             if descs_arr is None:
-                return self._generic_swept(p, cfg_begin, cfg_count, n_cfg, return_which)
+                return self._composed_swept(p, cfg_begin, cfg_count, return_which)
             xf = self._xforms_on(device)
             val = torch.empty(P, dtype=torch.float32, device=device)
             grad = torch.empty(P, 3, dtype=torch.float32, device=device)
@@ -919,18 +937,16 @@ class ComposedSDF(ObjectFrameSDF):
                                                          nat.stream_ptr(device)), "pvb_composed_query_swept")
         return (val, grad, cfg, which) if return_which else (val, grad)
 
-    def _generic_swept(self, p, cfg_begin, cfg_count, n_cfg, return_which):
-        """query_swept for sub-SDFs without native descriptors: configuration chunks through `_generic_query` in
-        ascending order; within a chunk the first configuration attaining the minimum, across chunks a strictly
-        smaller value -- the same (value, configuration, sub-SDF) order as the fused kernels."""
+    def _composed_swept(self, p, cfg_begin, cfg_count, return_which):
+        """query_swept for sub-SDFs without native descriptors, over `_composition_chunks`: within a chunk the first
+        configuration attaining the minimum, across chunks a strictly smaller value -- the same (value, configuration,
+        sub-SDF) order as the fused kernels."""
         P = p.shape[0]
         best = torch.full((P,), float("inf"), dtype=torch.float32, device=p.device)
         bgrad = torch.zeros(P, 3, dtype=torch.float32, device=p.device)
         bcfg = torch.full((P,), -1, dtype=torch.int32, device=p.device)
         bwhich = torch.full((P,), -1, dtype=torch.int32, device=p.device)
-        for c0 in range(cfg_begin, cfg_begin + (cfg_count if P > 0 else 0), self.swept_generic_chunk):
-            cc = min(self.swept_generic_chunk, cfg_begin + cfg_count - c0)
-            v, g, w = self._generic_query(p, c0, cc, n_cfg, True)
+        for c0, cc, _, v, g, w in self._composition_chunks(p, cfg_begin, cfg_count):
             v, g, w = v.reshape(cc, P), g.reshape(cc, P, 3), w.reshape(cc, P)
             first = (v == v.amin(dim=0)).int().argmax(dim=0)          # first configuration attaining the minimum
             cv = v.gather(0, first[None])[0]
@@ -956,9 +972,6 @@ class ComposedSDF(ObjectFrameSDF):
         out = self.query_swept(points_in_object_frame, return_which=return_argmin)
         return self._deliver(points_in_object_frame, out, pts_shape[:-1])
 
-    #: configurations per `_generic_query` chunk of the unfused clearance query (bounds its cfg_chunk x P temporaries)
-    clearance_generic_chunk = 64
-
     @staticmethod
     def _clearance_segments(shape):
         """(n_seg, seg_len) of points [*B, N, 3]; ValueError when they are not [..., N, 3]."""
@@ -983,13 +996,12 @@ class ComposedSDF(ObjectFrameSDF):
 
     def _clearance_query(self, points, cfg_begin, cfg_count, n_seg, seg_len, return_which, paired=False):
         """query_clearance (paired=False) or query_paired_clearance (paired=True) once their checks have passed: the
-        form's fused entry point, or `_generic_clearance` for the sets the fused kernels do not take."""
+        form's fused entry point, or `_composed_clearance` for the sets the fused kernels do not take."""
         S, n_cfg = len(self.sdfs), _config_count(self.tsf_batch)
         with _query_points(points) as (device, p):
             descs_arr, needs_mesh = self._native_descs(device)
             if descs_arr is None:
-                return self._generic_clearance(p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which,
-                                               paired=paired)
+                return self._composed_clearance(p, cfg_begin, cfg_count, n_seg, seg_len, return_which, paired=paired)
             xf = self._xforms_on(device)
             R = max(cfg_count, 0) * n_seg
             keys = torch.empty(R, dtype=torch.int64, device=device)
@@ -1016,25 +1028,22 @@ class ComposedSDF(ObjectFrameSDF):
         i = torch.arange(v.shape[-1], device=v.device, dtype=torch.int64)
         return ((h - (1 << 31)) << 32) | i
 
-    def _generic_clearance(self, p, cfg_begin, cfg_count, n_cfg, n_seg, seg_len, return_which, paired=False):
-        """query_clearance for sub-SDFs without native descriptors: configuration chunks through `_generic_query`,
-        each reduced over the points of every segment by the kernels' key order.  paired: p holds cfg_count blocks of
-        n_seg * seg_len points, block c for configuration cfg_begin + c only (query_paired_clearance)."""
+    @classmethod
+    def _first_minimum(cls, v):
+        """The index (int64) along the last dimension of v of the first minimum in `_clearance_keys` order."""
+        return cls._clearance_keys(v).amin(dim=-1) & 0xFFFFFFFF
+
+    def _composed_clearance(self, p, cfg_begin, cfg_count, n_seg, seg_len, return_which, paired=False):
+        """query_clearance (paired: query_paired_clearance) for sub-SDFs without native descriptors, over
+        `_composition_chunks`: each chunk reduced over the points of every segment by the kernels' key order."""
         R = max(cfg_count, 0) * n_seg
         val = torch.empty(R, dtype=torch.float32, device=p.device)
         grad = torch.empty(R, 3, dtype=torch.float32, device=p.device)
         point = torch.empty(R, dtype=torch.int32, device=p.device)
         which = torch.empty(R, dtype=torch.int32, device=p.device)
-        n_pts = n_seg * seg_len
-        for c0 in range(cfg_begin, cfg_begin + (cfg_count if R > 0 else 0), self.clearance_generic_chunk):
-            cc = min(self.clearance_generic_chunk, cfg_begin + cfg_count - c0)
-            if paired:
-                own = p[(c0 - cfg_begin) * n_pts:(c0 - cfg_begin + cc) * n_pts]
-                v, g, w = self._generic_query(own, c0, cc, n_cfg, True, paired=True)
-            else:
-                v, g, w = self._generic_query(p, c0, cc, n_cfg, True)
+        for c0, cc, _, v, g, w in self._composition_chunks(p, cfg_begin, cfg_count, paired):
             v, g, w = v.reshape(cc, n_seg, seg_len), g.reshape(cc, n_seg, seg_len, 3), w.reshape(cc, n_seg, seg_len)
-            i = (self._clearance_keys(v).amin(dim=-1) & 0xFFFFFFFF)[..., None]
+            i = self._first_minimum(v)[..., None]
             out = slice((c0 - cfg_begin) * n_seg, (c0 - cfg_begin + cc) * n_seg)
             val[out] = v.gather(-1, i).reshape(-1)
             grad[out] = g.gather(-2, i[..., None].expand(cc, n_seg, 1, 3)).reshape(-1, 3)
@@ -1069,10 +1078,10 @@ class ComposedSDF(ObjectFrameSDF):
         _, cfg_count = self._slab(cfg_begin, cfg_count)
         shape = tuple(points_in_object_frame.shape)
         lead, seg_len = self._clearance_segments(shape)
-        if (lead % cfg_count) if cfg_count > 0 else lead:
+        n_seg = self._paired_block(lead, cfg_count)
+        if n_seg is None:
             raise ValueError(f"paired clearance query: points {shape} do not split into {cfg_count} blocks of "
                              f"[n_seg, N, 3]")
-        n_seg = lead // cfg_count if cfg_count > 0 else 0
         if n_seg > 0 and seg_len == 0:
             raise ValueError("paired clearance query: no minimum over an empty segment (N = 0)")
         return self._clearance_query(points_in_object_frame, cfg_begin, cfg_count, n_seg, seg_len, return_which,
@@ -1162,28 +1171,38 @@ class ComposedSDF(ObjectFrameSDF):
                       "pvb_composed_query_self_clearance")
         return (val, grad, src, point, which) if return_which else (val, grad)
 
-    def _composed_self_clearance(self, p, K, rows, cfg_begin, cfg_count, return_which):
-        """query_self_clearance by composition, the definition of its result: for every source i with an allowed
-        row, link_points[i] posed by W_i of the slab (pvb_transform_points_paired), then
-        query_paired_clearance(..., return_which=True) of ComposedSDF([sdfs[j] for allowed j], their transform rows),
-        its sub-SDF index mapped back; then the minimum over i by (value, i)."""
+    def _self_sources(self, rows, device):
+        """The sources of the self routes: (i, js, sub) for every sub-SDF i with an allowed row, js the sub-SDFs
+        rows[i] allows and sub = ComposedSDF([sdfs[j] for j in js]) with their transform rows on `device`."""
         S, n_cfg = len(self.sdfs), _config_count(self.tsf_batch)
-        device = p.device
         xf = self._xforms_on(device).reshape(S, n_cfg, 4, 4)
-        inv = self._inv_xforms_on(device).reshape(S, n_cfg, 4, 4)
-        lp = p.reshape(S, K, 3)
-        per_src = []
         for i in range(S):
             js = [j for j in range(S) if rows[i][j]]
-            if not js:
-                continue
-            w_i = inv[i, cfg_begin:cfg_begin + cfg_count].contiguous()
-            own = lp[i].expand(cfg_count, K, 3).contiguous()
-            x = torch.empty(cfg_count, K, 3, dtype=torch.float32, device=device)
-            nat.check(nat.lib().pvb_transform_points_paired(nat.ptr(w_i), cfg_count, nat.ptr(own), K, nat.ptr(x),
-                                                            nat.stream_ptr(device)), "pvb_transform_points_paired")
-            sub = ComposedSDF([self.sdfs[j] for j in js], None)
-            sub.set_transforms(Transform3d(matrix=xf[js].reshape(len(js) * n_cfg, 4, 4)), batch_dim=(n_cfg,))
+            if js:
+                sub = ComposedSDF([self.sdfs[j] for j in js], None)
+                sub.set_transforms(Transform3d(matrix=xf[js].reshape(len(js) * n_cfg, 4, 4)), batch_dim=(n_cfg,))
+                yield i, js, sub
+
+    def _posed_link_points(self, lp, i, c0, cc):
+        """link_points[i] of lp [S, K, 3] fp32, posed by W_i of configurations [c0, c0 + cc): [cc, K, 3] fp32 from
+        pvb_transform_points_paired."""
+        (S, K, _), device = lp.shape, lp.device
+        w_i = self._inv_xforms_on(device).reshape(S, -1, 4, 4)[i, c0:c0 + cc].contiguous()
+        own = lp[i].expand(cc, K, 3).contiguous()
+        x = torch.empty(cc, K, 3, dtype=torch.float32, device=device)
+        nat.check(nat.lib().pvb_transform_points_paired(nat.ptr(w_i), cc, nat.ptr(own), K, nat.ptr(x),
+                                                        nat.stream_ptr(device)), "pvb_transform_points_paired")
+        return x
+
+    def _composed_self_clearance(self, p, K, rows, cfg_begin, cfg_count, return_which):
+        """query_self_clearance by composition, the definition of its result: for every source, its points posed over
+        the slab and query_paired_clearance(..., return_which=True) of its sub-composition, the sub-SDF index mapped
+        back; then the minimum over the sources by (value, source)."""
+        device = p.device
+        lp = p.reshape(len(self.sdfs), K, 3)
+        per_src = []
+        for i, js, sub in self._self_sources(rows, device):
+            x = self._posed_link_points(lp, i, cfg_begin, cfg_count)
             v, g, pt, w = sub.query_paired_clearance(x, cfg_begin=cfg_begin, cfg_count=cfg_count, return_which=True)
             w = torch.tensor(js, dtype=torch.int32, device=device)[w.long()]
             per_src.append((i, v, g, pt, w))
@@ -1193,7 +1212,7 @@ class ComposedSDF(ObjectFrameSDF):
             idx = [torch.full((cfg_count,), -1, dtype=torch.int32, device=device) for _ in range(3)]
             return (val, grad, *idx) if return_which else (val, grad)
         v = torch.stack([r[1] for r in per_src], dim=1)                                   # [cfg_count, n_src]
-        pos = (self._clearance_keys(v).amin(dim=-1) & 0xFFFFFFFF)[:, None]                 # first source on ties
+        pos = self._first_minimum(v)[:, None]                                              # first source on ties
         val = v.gather(1, pos).reshape(-1)
         grad = torch.stack([r[2] for r in per_src], dim=1).gather(1, pos[..., None].expand(cfg_count, 1, 3))
         grad = grad.reshape(-1, 3)
@@ -1239,7 +1258,7 @@ class ComposedSDF(ObjectFrameSDF):
 
         Sets of at most 8 grid (bounding-box rule) or primitive sub-SDFs run in one fused kernel
         (pvb_composed_query_collision_cost); every other set is composed from `query` in chunks of
-        `clearance_generic_chunk` configurations and reduced in torch.  Both are deterministic, and the fused route's
+        `composition_chunk` configurations and reduced in torch.  Both are deterministic, and the fused route's
         rows do not depend on the slab: a configuration split reproduces the full call bit for bit.  Returns flat
         (cfg_count * n_seg,) / (cfg_count * n_seg, S, 6) fp32 tensors on the GPU, configuration-major.  Raises
         ValueError before any device work on malformed points, a margin that is not finite, or a slab without
@@ -1275,33 +1294,27 @@ class ComposedSDF(ObjectFrameSDF):
                             nat.stream_ptr(device)), entry.__name__)
         return cost, twist
 
+    @staticmethod
+    def _hinge_terms(v, g, x, m):
+        """The terms of a collision cost in fp64 at values v [...], gradients g [..., 3] and points x (broadcast to
+        g) for margin m: (h, tau) with h = max(0, m - v), 0 exactly where v >= m, and tau = 2h (g, x x g) [..., 6]."""
+        h = (m - v.double()).clamp_min(0.0)
+        g = g.double()
+        return h, torch.cat([g, torch.linalg.cross(x.double().expand_as(g), g, dim=-1)], dim=-1) * (2.0 * h)[..., None]
+
     def _composed_collision_cost(self, p, m, cfg_begin, cfg_count, n_seg, seg_len, paired=False):
-        """query_collision_cost by composition, for the sets the fused kernel refuses: query(..., return_which=True)
-        on chunks of `clearance_generic_chunk` configurations, the terms in fp64, grouped by sub-SDF with one mask and
-        one sum per sub-SDF (torch's sums are deterministic; scatter_add / index_add on CUDA are not).  paired: p holds
-        cfg_count blocks of n_seg * seg_len points, block c for configuration cfg_begin + c only, evaluated with
-        query_paired (query_paired_collision_cost)."""
+        """query_collision_cost (paired: query_paired_collision_cost) by composition, for the sets the fused kernel
+        refuses: `_composition_chunks`, the `_hinge_terms` grouped by sub-SDF with one mask and one sum per sub-SDF
+        (torch's sums are deterministic; scatter_add / index_add on CUDA are not)."""
         S = len(self.sdfs)
         R = cfg_count * n_seg
         cost = torch.zeros(R, dtype=torch.float32, device=p.device)
         twist = torch.zeros(R, S, 6, dtype=torch.float32, device=p.device)
-        if R == 0 or seg_len == 0:
-            return cost, twist
-        n_pts = n_seg * seg_len
         shared = None if paired else p.double().reshape(n_seg, seg_len, 3)
-        for c0 in range(cfg_begin, cfg_begin + cfg_count, self.clearance_generic_chunk):
-            cc = min(self.clearance_generic_chunk, cfg_begin + cfg_count - c0)
-            if paired:
-                own = p[(c0 - cfg_begin) * n_pts:(c0 - cfg_begin + cc) * n_pts]
-                v, g, w = self.query_paired(own, cfg_begin=c0, cfg_count=cc, return_which=True)
-                pts = own.double().reshape(cc, n_seg, seg_len, 3)
-            else:
-                v, g, w = self.query(p, cfg_begin=c0, cfg_count=cc, return_which=True)
-                pts = shared
+        for c0, cc, x, v, g, w in self._composition_chunks(p, cfg_begin, cfg_count, paired):
+            pts = x.double().reshape(cc, n_seg, seg_len, 3) if paired else shared
             v, g, w = v.reshape(cc, n_seg, seg_len), g.reshape(cc, n_seg, seg_len, 3), w.reshape(cc, n_seg, seg_len)
-            h = (m - v.double()).clamp_min(0.0)                     # 0 exactly where d >= m
-            g = g.double()
-            terms = torch.cat([g, torch.linalg.cross(pts.expand_as(g), g, dim=-1)], dim=-1) * (2.0 * h)[..., None]
+            h, terms = self._hinge_terms(v, g, pts, m)
             out = slice((c0 - cfg_begin) * n_seg, (c0 - cfg_begin + cc) * n_seg)
             cost[out] = (h * h).sum(dim=-1).reshape(-1).float()
             for s in range(S):
@@ -1334,7 +1347,7 @@ class ComposedSDF(ObjectFrameSDF):
 
         Sets of at most 8 grid (bounding-box rule) or primitive sub-SDFs run in one fused kernel
         (pvb_composed_query_paired_collision_cost), bit-identical to that definition; every other set is composed from
-        `query_paired` in chunks of `clearance_generic_chunk` configurations and reduced in torch, equal to it within
+        `query_paired` in chunks of `composition_chunk` configurations and reduced in torch, equal to it within
         fp32 rounding.  Returns flat (cfg_count * n_seg,) / (cfg_count * n_seg, S, 6) fp32 tensors on the GPU,
         configuration-major.  Raises ValueError before any device work on malformed points, points that do not split
         into cfg_count blocks, an invalid slab or a margin that is not finite."""
@@ -1347,10 +1360,10 @@ class ComposedSDF(ObjectFrameSDF):
         if cfg_begin < 0 or cfg_count < 0 or cfg_begin + cfg_count > n_cfg:
             raise ValueError(f"paired collision-cost query: invalid configuration slab [{cfg_begin}, +{cfg_count}) of "
                              f"{n_cfg}")
-        if (lead % cfg_count) if cfg_count > 0 else lead:
+        n_seg = self._paired_block(lead, cfg_count)
+        if n_seg is None:
             raise ValueError(f"paired collision-cost query: points {shape} do not split into {cfg_count} blocks of "
                              f"[n_seg, N, 3]")
-        n_seg = lead // cfg_count if cfg_count > 0 else 0
         return self._collision_cost_query(points_in_object_frame, m, cfg_begin, cfg_count, n_seg, seg_len,
                                           paired=True)
 
@@ -1422,37 +1435,23 @@ class ComposedSDF(ObjectFrameSDF):
         return cost, twist
 
     def _composed_self_collision_cost(self, p, K, rows, m, cfg_begin, cfg_count):
-        """query_self_collision_cost by composition, the definition of its result: for every source i with an
-        allowed row and every chunk of `clearance_generic_chunk` configurations, link_points[i] posed by W_i
-        (pvb_transform_points_paired), then query_paired(..., return_which=True) of ComposedSDF([sdfs[j] for allowed
-        j], their transform rows), its sub-SDF index mapped back; the terms in fp64, one masked sum per target, and
-        the source's total subtracted (torch's sums are deterministic; scatter_add / index_add on CUDA are not)."""
-        S, n_cfg = len(self.sdfs), _config_count(self.tsf_batch)
+        """query_self_collision_cost by composition, the definition of its result: for every source and chunk, its
+        points posed and query_paired(..., return_which=True) of its sub-composition; the `_hinge_terms`, one masked
+        sum per target, and the source's total subtracted (torch's sums are deterministic; scatter_add / index_add
+        on CUDA are not)."""
+        S = len(self.sdfs)
         device = p.device
-        xf = self._xforms_on(device).reshape(S, n_cfg, 4, 4)
-        inv = self._inv_xforms_on(device).reshape(S, n_cfg, 4, 4)
         lp = p.reshape(S, K, 3)
         cost = torch.zeros(cfg_count, dtype=torch.float64, device=device)
         twist = torch.zeros(cfg_count, S, 6, dtype=torch.float64, device=device)
-        for i in range(S):
-            js = [j for j in range(S) if rows[i][j]]
-            if not js:
-                continue
-            sub = ComposedSDF([self.sdfs[j] for j in js], None)
-            sub.set_transforms(Transform3d(matrix=xf[js].reshape(len(js) * n_cfg, 4, 4)), batch_dim=(n_cfg,))
+        for i, js, sub in self._self_sources(rows, device):
             js_t = torch.tensor(js, dtype=torch.long, device=device)
-            for c0 in range(cfg_begin, cfg_begin + cfg_count, self.clearance_generic_chunk):
-                cc = min(self.clearance_generic_chunk, cfg_begin + cfg_count - c0)
-                w_i = inv[i, c0:c0 + cc].contiguous()
-                own = lp[i].expand(cc, K, 3).contiguous()
-                x = torch.empty(cc, K, 3, dtype=torch.float32, device=device)
-                nat.check(nat.lib().pvb_transform_points_paired(nat.ptr(w_i), cc, nat.ptr(own), K, nat.ptr(x),
-                                                                nat.stream_ptr(device)), "pvb_transform_points_paired")
+            for c0 in range(cfg_begin, cfg_begin + cfg_count, self.composition_chunk):
+                cc = min(self.composition_chunk, cfg_begin + cfg_count - c0)
+                x = self._posed_link_points(lp, i, c0, cc)
                 v, g, w = sub.query_paired(x, cfg_begin=c0, cfg_count=cc, return_which=True)
-                v, g, w = v.reshape(cc, K).double(), g.reshape(cc, K, 3).double(), js_t[w.long()].reshape(cc, K)
-                h = (m - v).clamp_min(0.0)                          # 0 exactly where d >= m
-                xd = x.double()
-                tau = torch.cat([g, torch.linalg.cross(xd, g, dim=-1)], dim=-1) * (2.0 * h)[..., None]
+                h, tau = self._hinge_terms(v.reshape(cc, K), g.reshape(cc, K, 3), x, m)
+                w = js_t[w.long()].reshape(cc, K)
                 rs = slice(c0 - cfg_begin, c0 - cfg_begin + cc)
                 cost[rs] += (h * h).sum(dim=-1)
                 for j in js:

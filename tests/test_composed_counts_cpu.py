@@ -9,7 +9,8 @@ transforms past the 64 the point-major kernel keeps in shared memory, the mesh n
    nearest-bound-first order -- over grid, mixed grid / primitive and closed-mesh sets, against the fp64 composition of
    tests/composed_ref.py up to classified flips and ties, and bit-identical under the bit-reversed and the index
    order.  Every set holds duplicated sub-SDFs, so the first-index tie rule decides some pairs.
-3. ComposedSDF with more than 128 descriptor-bearing sub-SDFs takes the generic path instead of raising."""
+3. ComposedSDF with more than 128 descriptor-bearing sub-SDFs takes the generic path instead of raising, and its
+   composition routes walk the slab in chunks of 64 configurations and reduce them as the fused kernels do."""
 import contextlib
 
 import numpy as np
@@ -19,7 +20,7 @@ import torch
 import composed_ref as cr
 import hostsim_lib as hs
 import workloads
-from helpers import classify_composed, golden, grid_spec
+from helpers import classify_composed, clearance_reduce, golden, grid_spec, swept_reduce
 from oracle import port
 from pytorch_volumetric_b200 import _native as nat
 
@@ -206,6 +207,83 @@ def test_more_than_128_sub_sdfs_take_the_generic_path(monkeypatch):
         assert comp.swept(pts)[0].shape == (2, 5)
         assert comp.clearance(pts)[0].shape == (3, 2)
         assert comp.paired(torch.zeros(3, 5, 3))[0].shape == (3, 5)
-        assert calls == [(0, 3, 3, False), (0, 3, 3, False), (0, 3, 3, False), (0, 3, 3, True)], (S, calls)
+        assert comp.paired_clearance(torch.zeros(3, 2, 5, 3))[0].shape == (3, 2)
+        assert comp.collision_cost(pts, 0.1)[1].shape == (3, 2, S, 6)
+        assert comp.paired_collision_cost(torch.zeros(3, 2, 5, 3), 0.1)[1].shape == (3, 2, S, 6)
+        assert calls == [(0, 3, 3, False)] * 3 + [(0, 3, 3, True)] * 2 + [(0, 3, 3, False), (0, 3, 3, True)], \
+            (S, calls)
         with pytest.raises(NotImplementedError, match="128"):
             comp.query_into(pts, [(torch.zeros(30), torch.zeros(30, 3))])
+
+
+def _quarters(rng, lo, hi, shape):
+    return torch.from_numpy(rng.integers(lo, hi, shape) / 4).float()
+
+
+@pytest.mark.parametrize("n_cfg, slabs", [(1, [(0, 1)]), (63, [(0, 63)]), (64, [(0, 64)]), (65, [(0, 65), (1, 63)]),
+                                          (129, [(0, 129), (30, 70), (64, 65)])])
+def test_generic_composition_chunks_and_reductions(monkeypatch, n_cfg, slabs):
+    """The composition routes of a set the fused kernels do not take, with `_generic_query` faked on the CPU: each
+    form's chunks of 64 configurations of its slab, in ascending order, and its reduction of the chunks' results.
+    The fake's results come from seeded tables, one for the shared cloud and one for the paired blocks: values from
+    nine multiples of 1/4, some zeros negative, so that the minima over configurations and over points meet ties;
+    gradients and points are multiples of 1/4 too, so every fp64 hinge term and sum below is exact."""
+    import pytorch_volumetric_b200 as pv
+    monkeypatch.setattr(nat, "compute_device", lambda *a, **k: None)
+    monkeypatch.setattr(torch.cuda, "device", lambda d: contextlib.nullcontext())
+    S, n_seg, N, m = 129, 3, 4, 1.0
+    comp = pv.ComposedSDF([pv.SphereSDF(0.01) for _ in range(S)], None)
+    comp.set_transforms(pv.Transform3d(matrix=workloads.random_rigid(S * n_cfg, seed=n_cfg)), batch_dim=(n_cfg,))
+    rng = np.random.default_rng(n_cfg)
+    tables = {}
+    for paired in (False, True):
+        v = _quarters(rng, -3, 6, (n_cfg, n_seg * N))
+        v[(v == 0) & torch.from_numpy(rng.random(v.shape) < 0.5)] = -0.0
+        tables[paired] = (v, _quarters(rng, -4, 5, (n_cfg, n_seg * N, 3)),
+                          torch.from_numpy(rng.integers(0, S, (n_cfg, n_seg * N))).int())
+    calls = []
+
+    def fake(p, cfg_begin, cfg_count, n_cfg_, return_which, paired=False):
+        calls.append((cfg_begin, cfg_count, n_cfg_, paired))
+        P = p.shape[0] // cfg_count if paired else p.shape[0]
+        assert return_which
+        return tuple(t[cfg_begin:cfg_begin + cfg_count, :P].flatten(0, 1) for t in tables[paired])
+    monkeypatch.setattr(comp, "_generic_query", fake)
+
+    for begin, count in slabs:
+        rows = slice(begin, begin + count)
+        chunks = [(c0, min(64, begin + count - c0), n_cfg) for c0 in range(begin, begin + count, 64)]
+        cloud = _quarters(rng, -4, 5, (n_seg, N, 3))
+        own = _quarters(rng, -4, 5, (count, n_seg, N, 3))
+        flat = {paired: tuple(t[rows].flatten(0, 1) for t in tables[paired]) for paired in (False, True)}
+
+        def run(fn, *args):
+            calls.clear()
+            out = fn(*args, cfg_begin=begin, cfg_count=count)
+            return out, list(calls)
+
+        out, got = run(lambda p, **kw: comp.query_swept(p, return_which=True, **kw), cloud.reshape(-1, 3))
+        assert got == [(*c, False) for c in chunks], (begin, count, got)
+        for a, b in zip(out, swept_reduce(*flat[False], count, begin)):
+            assert torch.equal(a, b), (begin, count, "swept")
+        for paired, pts in ((False, cloud), (True, own)):
+            fn = comp.query_paired_clearance if paired else comp.query_clearance
+            out, got = run(lambda p, **kw: fn(p, return_which=True, **kw), pts)
+            assert got == [(*c, paired) for c in chunks], (begin, count, paired, got)
+            for a, b in zip(out, clearance_reduce(*flat[paired], count, n_seg)):
+                assert torch.equal(a, b), (begin, count, paired, "clearance")
+
+            fn = comp.query_paired_collision_cost if paired else comp.query_collision_cost
+            (cost, twist), got = run(fn, pts, m)
+            assert got == [(*c, paired) for c in chunks], (begin, count, paired, got)
+            v, g, w = (t.double().numpy().reshape(count, n_seg, N, -1) for t in flat[paired])
+            x = np.broadcast_to(pts.double().numpy(), (count, n_seg, N, 3))
+            ref_cost = np.zeros((count, n_seg))
+            ref_twist = np.zeros((count, n_seg, S, 6))
+            for a, b, k in np.ndindex(count, n_seg, N):
+                h = max(m - v[a, b, k, 0], 0.0)
+                ref_cost[a, b] += h * h
+                ref_twist[a, b, int(w[a, b, k, 0])] += 2 * h * np.concatenate([g[a, b, k], np.cross(x[a, b, k],
+                                                                                                    g[a, b, k])])
+            assert torch.equal(cost, torch.from_numpy(ref_cost).float().reshape(-1)), (begin, count, paired)
+            assert torch.equal(twist, torch.from_numpy(ref_twist).float().reshape(-1, S, 6)), (begin, count, paired)

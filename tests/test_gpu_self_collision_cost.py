@@ -175,7 +175,7 @@ def test_fused_equals_composition_on_the_arm(tmp_path, monkeypatch, kind):
 def test_fused_equals_composition_at_70000_configurations(tmp_path, monkeypatch):
     for kind in ("nearest", "primitive"):
         robot = arm_robot(tmp_path / kind, kind)
-        robot.sdf.clearance_generic_chunk = 8192                  # fewer launches for the composition route
+        robot.sdf.composition_chunk = 8192                        # fewer launches for the composition route
         robot.set_joint_configuration(wide_configurations(70_000, seed=5).cuda())
         lp = robot.link_surface_points(num_points=32, seed=1)
         allowed = robot.self_collision_pairs()
