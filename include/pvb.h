@@ -423,6 +423,16 @@ typedef struct pvb_fk_link {
 int pvb_fk_serial(const pvb_fk_frame *frames, int32_t n_frames, const pvb_fk_link *links, int32_t n_links,
                   const float *q, int32_t n_cfg, int32_t n_joints, float *out_xforms, void *stream);
 
+/* ---- the same for a kinematic tree (kinematics.Chain) ----
+ * T_f = T_{parents[f]} @ origin_f @ motion_f(q[q_index_f]), the root's parent pose the identity; the output layout,
+ * the links and the rest of the arguments are those of pvb_fk_serial.  parents: HOST int32[n_frames] in depth-first
+ * pre-order: parents[0] == -1, and for f > 0 parents[f] is f - 1 or an ancestor of f - 1.  pvb_fk_serial is this
+ * walk with parents[f] = f - 1. */
+#define PVB_FK_TREE_MAX_FRAMES 64
+#define PVB_FK_TREE_MAX_LINKS 64
+int pvb_fk_tree(const pvb_fk_frame *frames, const int32_t *parents, int32_t n_frames, const pvb_fk_link *links,
+                int32_t n_links, const float *q, int32_t n_cfg, int32_t n_joints, float *out_xforms, void *stream);
+
 /* ---- peer-visible device buffers (one process per GPU, same node) ----
  * pvb_ipc_alloc: cudaMalloc on the current device (IPC handles need a whole allocation, not a slice of a caching
  * allocator's segment); pvb_ipc_export fills a 64-byte handle another PROCESS passes to pvb_ipc_open to map the

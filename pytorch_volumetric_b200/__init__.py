@@ -14,7 +14,7 @@ _EXPORTS = {
     _voxel: ("ExpandingVoxelGrid", "VoxelGrid", "VoxelSet", "Voxels", "get_coordinates_and_points_in_grid",
              "get_divisible_range_by_resolution", "voxel_down_sample"),
     _tf: ("Transform3d", "Translate"),
-    _kin: ("SerialChain", "build_serial_chain_from_urdf"),
+    _kin: ("Chain", "SerialChain", "build_chain_from_urdf", "build_serial_chain_from_urdf"),
 }
 for _module, _names in _EXPORTS.items():
     for _name in _names:

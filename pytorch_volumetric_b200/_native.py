@@ -92,6 +92,7 @@ class FkLink(ctypes.Structure):
 
 FK_FIXED, FK_REVOLUTE, FK_PRISMATIC = 0, 1, 2
 FK_MAX_FRAMES, FK_MAX_LINKS = 32, 16
+FK_TREE_MAX_FRAMES, FK_TREE_MAX_LINKS = 64, 64
 
 
 class OutTarget(ctypes.Structure):
@@ -181,6 +182,8 @@ _SIGNATURES = {
                                                     ctypes.c_void_p, ctypes.c_void_p]),
     "pvb_fk_serial": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int32,
                                      ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]),
+    "pvb_fk_tree": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int32,
+                                   ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]),
     "pvb_voxel_index": (ctypes.c_int, [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
                                        ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "pvb_voxel_scatter": (ctypes.c_int, [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,

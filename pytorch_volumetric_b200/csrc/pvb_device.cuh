@@ -5,6 +5,7 @@
 //   bvh_parity     ray/triangle crossing parity              (count_intersections role, sdf.py:152-154)
 //   mesh_eval      ObjectFactory._do_object_frame_closest_point epilogue (sdf.py:139-164)
 //   composed_point ComposedSDF.__call__ for one (configuration, point) pair (sdf.py:392-433)
+//   fk_walk        forward kinematics of one configuration along a chain or a tree (model_to_sdf.py:82-115)
 #pragma once
 #include "../../include/pvb.h"
 #include <cuda_runtime.h>
@@ -1304,5 +1305,150 @@ __device__ __forceinline__ bool collision_cost_near(const float (&lb)[8], float 
 // fp64 and rounded to fp32 once.  The order depends on K, S and allowed alone: not on the slab, the grid or the SM
 // count, so repeated calls give identical bits and a slab reproduces the rows of the full call.
 constexpr int kSccLanes = 32;                     // lanes of a configuration's warp: its accumulators
+
+// ----------------------------------------------------------------------------
+// Forward kinematics (fk_serial_kernel, fk_tree_kernel; RobotSDF.set_joint_configuration, model_to_sdf.py:82-115):
+// for every joint configuration a and every mesh link s, the object->mesh-frame transform
+// (FK_s(q_a) @ visual_offset_s)^-1 = offset_s^-1 @ FK_s(q_a)^-1, written link-major (row s * A + a) as the 4x4
+// row-major matrices the composed kernels read.  One walk, fk_walk, serves chains and trees: one thread per
+// configuration carries the running pose in registers, T <- T_parent @ joint_origin @ motion(q_j) (revolute:
+// Rodrigues rotation about the axis, prismatic: translation along it, fixed: identity), the same fp32 products the
+// eager path takes as dozens of small launches.
+template <int kFrames, int kLinks> struct FkPlan {
+    pvb_fk_frame frame[kFrames];
+    pvb_fk_link link[kLinks];
+    int n_frames, n_links;
+};
+// A tree adds the branch poses: frame f first reloads its parent's pose from save slot load[f] when its parent is not
+// frame f - 1 (-1: it continues from f - 1's pose), and after its joint stores its own pose into slot save[f] when a
+// child other than f + 1 will reload it (-1: none).  fk_tree_slots fills both.
+template <int kFrames, int kLinks> struct FkTreePlan : FkPlan<kFrames, kLinks> {
+    int8_t load[kFrames], save[kFrames];
+    int n_saves;
+};
+
+struct Rt34 { float m[12]; };       // rows of [R | t]
+
+__host__ __device__ __forceinline__ Rt34 rt_mul(const Rt34 &a, const float *b) {  // a @ b, both [R | t] with last row 0 0 0 1
+    Rt34 o;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            float v = a.m[4 * r] * b[c] + a.m[4 * r + 1] * b[4 + c] + a.m[4 * r + 2] * b[8 + c];
+            if (c == 3) v += a.m[4 * r + 3];
+            o.m[4 * r + c] = v;
+        }
+    }
+    return o;
+}
+
+// The check and the save slots of a tree plan.  Returns -1 when `parents` is a depth-first pre-order (parents[0] ==
+// -1; for f > 0, parents[f] is f - 1 or an ancestor of f - 1) and fills load / save / n_saves; otherwise returns the
+// first frame that breaks it.  Frame f saves when some child other than f + 1 reloads it, into the slot numbered by the
+// saving frames strictly above it: the frames that follow f in pre-order until its last child are its descendants,
+// whose slots are larger, so its pose stays in place until that child reloads it, and at most the tree depth is live.
+// n_frames <= PVB_FK_TREE_MAX_FRAMES.
+__host__ __device__ inline int fk_tree_slots(const int32_t *parents, int n_frames, int8_t *load, int8_t *save,
+                                             int *n_saves) {
+    for (int f = 0; f < n_frames; ++f) {
+        const int p = parents[f];
+        if (f == 0) {
+            if (p != -1) return 0;
+            continue;
+        }
+        if (p < 0 || p >= f) return f;
+        int up = f - 1;
+        while (up != p && up >= 0) up = parents[up];
+        if (up != p) return f;
+    }
+    bool saves[PVB_FK_TREE_MAX_FRAMES] = {};
+    int above[PVB_FK_TREE_MAX_FRAMES];
+    for (int f = 1; f < n_frames; ++f)
+        if (parents[f] != f - 1) saves[parents[f]] = true;
+    *n_saves = 0;
+    for (int f = 0; f < n_frames; ++f) {
+        const int p = parents[f];
+        above[f] = p < 0 ? 0 : above[p] + (saves[p] ? 1 : 0);
+        save[f] = (int8_t)(saves[f] ? above[f] : -1);
+        load[f] = (int8_t)(f > 0 && p != f - 1 ? save[p] : -1);
+        if (saves[f] && above[f] + 1 > *n_saves) *n_saves = above[f] + 1;
+    }
+    return -1;
+}
+
+// a read through the read-only data cache on the device; a plain load in a host build
+__host__ __device__ __forceinline__ float fk_ldg(const float *p) {
+#ifdef __CUDA_ARCH__
+    return __ldg(p);
+#else
+    return *p;
+#endif
+}
+
+// Configuration a of the plan: every link's transform into `out`.  kTree: reload and save branch poses through
+// `saves` (slot k's 12 floats at saves[(12 k + e) * save_stride]); a chain touches no save slot and takes exactly
+// the products of the plain walk.
+template <bool kTree, class Plan>
+__host__ __device__ __forceinline__ void fk_walk(const Plan &plan, const float *__restrict__ q, int n_joints, int n_cfg,
+                                                 int a, float *__restrict__ out, float *saves, int save_stride) {
+    Rt34 cur;
+#pragma unroll
+    for (int e = 0; e < 12; ++e) cur.m[e] = (e % 5 == 0) ? 1.f : 0.f;
+    int next_link = 0;
+    for (int f = 0; f < plan.n_frames; ++f) {
+        const pvb_fk_frame &fr = plan.frame[f];
+        if constexpr (kTree) {
+            if (plan.load[f] >= 0) {
+#pragma unroll
+                for (int e = 0; e < 12; ++e) cur.m[e] = saves[(12 * plan.load[f] + e) * save_stride];
+            }
+        }
+        cur = rt_mul(cur, fr.origin);
+        if (fr.joint_type != PVB_FK_FIXED) {
+            const float th = fk_ldg(q + (size_t)a * n_joints + fr.q_index);
+            float mot[12];
+            const float x = fr.axis[0], y = fr.axis[1], z = fr.axis[2];
+            if (fr.joint_type == PVB_FK_REVOLUTE) {
+                const float c = cosf(th), s = sinf(th), t = 1.f - c;
+                mot[0] = c + x * x * t;     mot[1] = x * y * t - z * s; mot[2] = x * z * t + y * s;  mot[3] = 0.f;
+                mot[4] = y * x * t + z * s; mot[5] = c + y * y * t;     mot[6] = y * z * t - x * s;  mot[7] = 0.f;
+                mot[8] = z * x * t - y * s; mot[9] = z * y * t + x * s; mot[10] = c + z * z * t;     mot[11] = 0.f;
+            } else {
+                mot[0] = 1.f; mot[1] = 0.f; mot[2] = 0.f; mot[3] = x * th;
+                mot[4] = 0.f; mot[5] = 1.f; mot[6] = 0.f; mot[7] = y * th;
+                mot[8] = 0.f; mot[9] = 0.f; mot[10] = 1.f; mot[11] = z * th;
+            }
+            cur = rt_mul(cur, mot);
+        }
+        if constexpr (kTree) {
+            if (plan.save[f] >= 0) {
+#pragma unroll
+                for (int e = 0; e < 12; ++e) saves[(12 * plan.save[f] + e) * save_stride] = cur.m[e];
+            }
+        }
+        // mesh links attached to this frame (sorted by frame on the host)
+        while (next_link < plan.n_links && plan.link[next_link].frame == f) {
+            const pvb_fk_link &lk = plan.link[next_link];
+            // rigid inverse of the link pose: [R^T | -R^T t]
+            float inv[12];
+#pragma unroll
+            for (int r = 0; r < 3; ++r) {
+                inv[4 * r] = cur.m[r]; inv[4 * r + 1] = cur.m[4 + r]; inv[4 * r + 2] = cur.m[8 + r];
+                inv[4 * r + 3] = -(cur.m[r] * cur.m[3] + cur.m[4 + r] * cur.m[7] + cur.m[8 + r] * cur.m[11]);
+            }
+            Rt34 off;
+#pragma unroll
+            for (int e = 0; e < 12; ++e) off.m[e] = lk.mesh_from_link[e];
+            const Rt34 m = rt_mul(off, inv);
+            float4 *dst = xf_rows(out, n_cfg, lk.slot, a);
+            dst[0] = make_float4(m.m[0], m.m[1], m.m[2], m.m[3]);
+            dst[1] = make_float4(m.m[4], m.m[5], m.m[6], m.m[7]);
+            dst[2] = make_float4(m.m[8], m.m[9], m.m[10], m.m[11]);
+            dst[3] = make_float4(0.f, 0.f, 0.f, 1.f);
+            ++next_link;
+        }
+    }
+}
 
 }  // namespace pvb

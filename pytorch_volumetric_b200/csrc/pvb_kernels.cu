@@ -2677,83 +2677,29 @@ compact_write_kernel(const T *__restrict__ data, long long n, T empty, const uns
 }
 
 // ======================================================== forward kinematics
-// RobotSDF.set_joint_configuration (model_to_sdf.py:82-115): for every joint configuration a and every mesh link s,
-// the object->mesh-frame transform (FK_s(q_a) @ visual_offset_s)^-1 = offset_s^-1 @ FK_s(q_a)^-1, written link-major
-// (row s * A + a) as the 4x4 row-major matrices the composed kernels read.  One thread per configuration walks the
-// serial chain in registers: T <- T @ joint_origin @ motion(q_j) (revolute: Rodrigues rotation about the axis,
-// prismatic: translation along it, fixed: identity), the same fp32 products the eager path took as dozens of small
-// launches (this kernel: one launch for every configuration).
-struct FkPlan {
-    pvb_fk_frame frame[PVB_FK_MAX_FRAMES];
-    pvb_fk_link link[PVB_FK_MAX_LINKS];
-    int n_frames, n_links;
-};
+// RobotSDF.set_joint_configuration: the walk is pvb_device.cuh's fk_walk.  A chain (pvb_fk_serial) keeps its plan at
+// 32 frames and 16 links; a tree (pvb_fk_tree) takes up to 64 of each and keeps its saved branch poses in shared
+// memory, slot-major with one column per thread, sized by the plan's slot count.
+using FkSerialPlan = FkPlan<PVB_FK_MAX_FRAMES, PVB_FK_MAX_LINKS>;
+using FkTreePlanMax = FkTreePlan<PVB_FK_TREE_MAX_FRAMES, PVB_FK_TREE_MAX_LINKS>;
+constexpr int kFkThreads = 64;
+// a kernel's parameters may take up to 32764 bytes on sm_70+ with CUDA 12.1 or later; the plan travels by value
+static_assert(sizeof(FkTreePlanMax) + 2 * sizeof(void *) + 2 * sizeof(int) <= 32764, "fk_tree_kernel parameters");
 
-struct Rt34 { float m[12]; };       // rows of [R | t]
-
-__device__ __forceinline__ Rt34 rt_mul(const Rt34 &a, const float *b) {       // a @ b, both [R | t] with last row 0 0 0 1
-    Rt34 o;
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            float v = a.m[4 * r] * b[c] + a.m[4 * r + 1] * b[4 + c] + a.m[4 * r + 2] * b[8 + c];
-            if (c == 3) v += a.m[4 * r + 3];
-            o.m[4 * r + c] = v;
-        }
-    }
-    return o;
-}
-
-__global__ void fk_serial_kernel(const __grid_constant__ FkPlan plan, const float *__restrict__ q, int n_cfg,
+__global__ void fk_serial_kernel(const __grid_constant__ FkSerialPlan plan, const float *__restrict__ q, int n_cfg,
                                  int n_joints, float *__restrict__ out) {
     const int a = blockIdx.x * blockDim.x + threadIdx.x;
     if (a >= n_cfg) return;
-    Rt34 cur;
-#pragma unroll
-    for (int e = 0; e < 12; ++e) cur.m[e] = (e % 5 == 0) ? 1.f : 0.f;
-    int next_link = 0;
-    for (int f = 0; f < plan.n_frames; ++f) {
-        const pvb_fk_frame &fr = plan.frame[f];
-        cur = rt_mul(cur, fr.origin);
-        if (fr.joint_type != PVB_FK_FIXED) {
-            const float th = __ldg(q + (size_t)a * n_joints + fr.q_index);
-            float mot[12];
-            const float x = fr.axis[0], y = fr.axis[1], z = fr.axis[2];
-            if (fr.joint_type == PVB_FK_REVOLUTE) {
-                const float c = cosf(th), s = sinf(th), t = 1.f - c;
-                mot[0] = c + x * x * t;     mot[1] = x * y * t - z * s; mot[2] = x * z * t + y * s;  mot[3] = 0.f;
-                mot[4] = y * x * t + z * s; mot[5] = c + y * y * t;     mot[6] = y * z * t - x * s;  mot[7] = 0.f;
-                mot[8] = z * x * t - y * s; mot[9] = z * y * t + x * s; mot[10] = c + z * z * t;     mot[11] = 0.f;
-            } else {
-                mot[0] = 1.f; mot[1] = 0.f; mot[2] = 0.f; mot[3] = x * th;
-                mot[4] = 0.f; mot[5] = 1.f; mot[6] = 0.f; mot[7] = y * th;
-                mot[8] = 0.f; mot[9] = 0.f; mot[10] = 1.f; mot[11] = z * th;
-            }
-            cur = rt_mul(cur, mot);
-        }
-        // mesh links attached to this frame (sorted by frame on the host)
-        while (next_link < plan.n_links && plan.link[next_link].frame == f) {
-            const pvb_fk_link &lk = plan.link[next_link];
-            // rigid inverse of the link pose: [R^T | -R^T t]
-            float inv[12];
-#pragma unroll
-            for (int r = 0; r < 3; ++r) {
-                inv[4 * r] = cur.m[r]; inv[4 * r + 1] = cur.m[4 + r]; inv[4 * r + 2] = cur.m[8 + r];
-                inv[4 * r + 3] = -(cur.m[r] * cur.m[3] + cur.m[4 + r] * cur.m[7] + cur.m[8 + r] * cur.m[11]);
-            }
-            Rt34 off;
-#pragma unroll
-            for (int e = 0; e < 12; ++e) off.m[e] = lk.mesh_from_link[e];
-            const Rt34 m = rt_mul(off, inv);
-            float4 *dst = xf_rows(out, n_cfg, lk.slot, a);
-            dst[0] = make_float4(m.m[0], m.m[1], m.m[2], m.m[3]);
-            dst[1] = make_float4(m.m[4], m.m[5], m.m[6], m.m[7]);
-            dst[2] = make_float4(m.m[8], m.m[9], m.m[10], m.m[11]);
-            dst[3] = make_float4(0.f, 0.f, 0.f, 1.f);
-            ++next_link;
-        }
-    }
+    fk_walk<false>(plan, q, n_joints, n_cfg, a, out, nullptr, 0);
+}
+
+__global__ void __launch_bounds__(kFkThreads) fk_tree_kernel(const __grid_constant__ FkTreePlanMax plan,
+                                                             const float *__restrict__ q, int n_cfg, int n_joints,
+                                                             float *__restrict__ out) {
+    extern __shared__ float fk_saved_poses[];
+    const int a = blockIdx.x * blockDim.x + threadIdx.x;
+    if (a >= n_cfg) return;
+    fk_walk<true>(plan, q, n_joints, n_cfg, a, out, fk_saved_poses + threadIdx.x, kFkThreads);
 }
 
 // =================================================================== chamfer
@@ -4253,6 +4199,35 @@ extern "C" int pvb_compact_nonempty(const void *data, int64_t n, int32_t elem_by
     return PVB_OK;
 }
 
+// The checks both forward-kinematics entry points make on their links and joint columns.  distinct_slots: every
+// output slot written once (pvb_fk_tree; pvb_fk_serial keeps its own rule).
+static int fk_check_links(const char *who, const pvb_fk_frame *frames, int n_frames, const pvb_fk_link *links,
+                          int n_links, int n_joints, bool distinct_slots) {
+    int prev = -1;
+    bool taken[PVB_FK_TREE_MAX_LINKS] = {};
+    for (int s = 0; s < n_links; ++s) {
+        const pvb_fk_link &lk = links[s];
+        if (lk.frame < prev || lk.frame < 0 || lk.frame >= n_frames || lk.slot < 0 || lk.slot >= n_links ||
+            (distinct_slots && taken[lk.slot])) {
+            pvb_set_error(distinct_slots ? "%s: links must be sorted by frame, with frame in [0, n_frames) and distinct "
+                                           "slots in [0, n_links)"
+                                         : "%s: links must be sorted by frame, with frame in [0, n_frames) and slot in "
+                                           "[0, n_links)", who);
+            return PVB_ERR_INVALID;
+        }
+        if (distinct_slots) taken[lk.slot] = true;
+        prev = lk.frame;
+    }
+    for (int f = 0; f < n_frames; ++f) {
+        const pvb_fk_frame &fr = frames[f];
+        if (fr.joint_type != PVB_FK_FIXED && (fr.q_index < 0 || fr.q_index >= n_joints)) {
+            pvb_set_error("%s: frame %d reads joint value %d of %d", who, f, fr.q_index, n_joints);
+            return PVB_ERR_INVALID;
+        }
+    }
+    return PVB_OK;
+}
+
 extern "C" int pvb_fk_serial(const pvb_fk_frame *frames, int32_t n_frames, const pvb_fk_link *links, int32_t n_links,
                              const float *q, int32_t n_cfg, int32_t n_joints, float *out_xforms, void *stream) {
     if (!frames || !links || n_frames < 1 || n_frames > PVB_FK_MAX_FRAMES || n_links < 1 || n_links > PVB_FK_MAX_LINKS ||
@@ -4265,31 +4240,57 @@ extern "C" int pvb_fk_serial(const pvb_fk_frame *frames, int32_t n_frames, const
         pvb_set_error("pvb_fk_serial: out_xforms must be 16-byte aligned");
         return PVB_ERR_INVALID;
     }
-    FkPlan plan;
+    FkSerialPlan plan;
     memset(&plan, 0, sizeof(plan));
     plan.n_frames = n_frames;
     plan.n_links = n_links;
     memcpy(plan.frame, frames, sizeof(pvb_fk_frame) * (size_t)n_frames);
     memcpy(plan.link, links, sizeof(pvb_fk_link) * (size_t)n_links);
-    int prev = -1;
-    for (int s = 0; s < n_links; ++s) {
-        const pvb_fk_link &lk = plan.link[s];
-        if (lk.frame < prev || lk.frame < 0 || lk.frame >= n_frames || lk.slot < 0 || lk.slot >= n_links) {
-            pvb_set_error("pvb_fk_serial: links must be sorted by frame, with frame in [0, n_frames) and slot in [0, n_links)");
-            return PVB_ERR_INVALID;
-        }
-        prev = lk.frame;
-    }
-    for (int f = 0; f < n_frames; ++f) {
-        const pvb_fk_frame &fr = plan.frame[f];
-        if (fr.joint_type != PVB_FK_FIXED && (fr.q_index < 0 || fr.q_index >= n_joints)) {
-            pvb_set_error("pvb_fk_serial: frame %d reads joint value %d of %d", f, fr.q_index, n_joints);
-            return PVB_ERR_INVALID;
-        }
-    }
+    if (fk_check_links("pvb_fk_serial", plan.frame, n_frames, plan.link, n_links, n_joints, false) != PVB_OK)
+        return PVB_ERR_INVALID;
     if (n_cfg == 0) return PVB_OK;
-    fk_serial_kernel<<<(n_cfg + 63) / 64, 64, 0, (cudaStream_t)stream>>>(plan, q, n_cfg, n_joints, out_xforms);
+    fk_serial_kernel<<<(n_cfg + kFkThreads - 1) / kFkThreads, kFkThreads, 0, (cudaStream_t)stream>>>(plan, q, n_cfg,
+                                                                                                     n_joints, out_xforms);
     PVB_CHECK_LAUNCH("pvb_fk_serial");
+    return PVB_OK;
+}
+
+extern "C" int pvb_fk_tree(const pvb_fk_frame *frames, const int32_t *parents, int32_t n_frames,
+                           const pvb_fk_link *links, int32_t n_links, const float *q, int32_t n_cfg, int32_t n_joints,
+                           float *out_xforms, void *stream) {
+    if (!frames || !parents || !links || n_frames < 1 || n_frames > PVB_FK_TREE_MAX_FRAMES || n_links < 1 ||
+        n_links > PVB_FK_TREE_MAX_LINKS || n_cfg < 0 || n_joints < 0 ||
+        (n_cfg > 0 && (!out_xforms || (n_joints > 0 && !q)))) {
+        pvb_set_error("pvb_fk_tree: invalid argument (n_frames=%d n_links=%d n_cfg=%d n_joints=%d)", n_frames, n_links,
+                      n_cfg, n_joints);
+        return PVB_ERR_INVALID;
+    }
+    if ((uintptr_t)out_xforms % 16) {
+        pvb_set_error("pvb_fk_tree: out_xforms must be 16-byte aligned");
+        return PVB_ERR_INVALID;
+    }
+    FkTreePlanMax plan;
+    memset(&plan, 0, sizeof(plan));
+    plan.n_frames = n_frames;
+    plan.n_links = n_links;
+    memcpy(plan.frame, frames, sizeof(pvb_fk_frame) * (size_t)n_frames);
+    memcpy(plan.link, links, sizeof(pvb_fk_link) * (size_t)n_links);
+    const int bad = fk_tree_slots(parents, n_frames, plan.load, plan.save, &plan.n_saves);
+    if (bad >= 0) {
+        pvb_set_error("pvb_fk_tree: frame %d has parent %d: parents must be a depth-first pre-order (parents[0] = -1, "
+                      "and parents[f] is f - 1 or an ancestor of f - 1)", bad, parents[bad]);
+        return PVB_ERR_INVALID;
+    }
+    if (fk_check_links("pvb_fk_tree", plan.frame, n_frames, plan.link, n_links, n_joints, true) != PVB_OK)
+        return PVB_ERR_INVALID;
+    if (n_cfg == 0) return PVB_OK;
+    const size_t smem = sizeof(float) * 12 * kFkThreads * (size_t)plan.n_saves;
+    if (smem > 48 * 1024)
+        PVB_CUDA_TRY(cudaFuncSetAttribute(fk_tree_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                     "pvb_fk_tree");
+    fk_tree_kernel<<<(n_cfg + kFkThreads - 1) / kFkThreads, kFkThreads, smem, (cudaStream_t)stream>>>(plan, q, n_cfg,
+                                                                                                      n_joints, out_xforms);
+    PVB_CHECK_LAUNCH("pvb_fk_tree");
     return PVB_OK;
 }
 

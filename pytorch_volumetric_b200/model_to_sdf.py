@@ -126,16 +126,20 @@ class RobotSDF(sdf.ObjectFrameSDF):
     native_fk = True
 
     def _make_fk_plan(self):
-        """(pvb_fk_frame[], pvb_fk_link[]) for pvb_fk_serial when the chain is this package's SerialChain in
-        float32 on a CUDA device; None otherwise (duck-typed pytorch_kinematics chains keep their own FK)."""
+        """(pvb_fk_frame[], pvb_fk_link[], parents) for the native forward kinematics when the chain is this package's
+        SerialChain (pvb_fk_serial, parents None) or Chain (pvb_fk_tree, its int32 parents) in float32 on a CUDA device
+        and within the entry point's limits; None otherwise (duck-typed pytorch_kinematics chains keep their own FK)."""
         from . import _native as nat
-        from .kinematics import SerialChain
-        if not isinstance(self.chain, SerialChain) or self.dtype != torch.float32 or \
-                torch.device(self.device).type != "cuda" or not (1 <= len(self.sdf_to_link_name) <= nat.FK_MAX_LINKS):
+        from .kinematics import Chain, SerialChain
+        tree = isinstance(self.chain, Chain)
+        max_links = nat.FK_TREE_MAX_LINKS if tree else nat.FK_MAX_LINKS
+        if not (tree or isinstance(self.chain, SerialChain)) or self.dtype != torch.float32 or \
+                torch.device(self.device).type != "cuda" or not (1 <= len(self.sdf_to_link_name) <= max_links):
             return None
-        frames = self.chain.native_fk_frames()
-        if frames is None:
+        packed = self.chain.native_fk_frames()
+        if packed is None:
             return None
+        frames, parents = packed if tree else (packed, None)
         frame_of = {f.link.name: i for i, f in enumerate(self.chain._frames)}
         inv = self._mesh_from_link.detach().to("cpu", torch.float32)
         if not bool((inv[:, 3] == torch.tensor([0.0, 0.0, 0.0, 1.0])).all()):
@@ -148,7 +152,7 @@ class RobotSDF(sdf.ObjectFrameSDF):
                     links[k].mesh_from_link[4 * r + c] = float(inv[s_idx, r, c])
             links[k].frame = frame_of[self.sdf_to_link_name[s_idx]]
             links[k].slot = s_idx
-        return frames, links
+        return frames, links, parents
 
     # ------------------------------------------------------------------ state
     def set_joint_configuration(self, joint_config=None):
@@ -164,18 +168,24 @@ class RobotSDF(sdf.ObjectFrameSDF):
         flat_q = joint_config.reshape(-1, n_joints) if batched else joint_config
         self.q = flat_q
         if self.native_fk and self._fk_plan is not None:
-            # one kernel: FK along the chain + (FK @ visual_offset)^-1 per mesh link, written link-major
+            # one kernel: FK along the chain or tree + (FK @ visual_offset)^-1 per mesh link, written link-major
             from . import _native as nat
             import ctypes
-            frames, links = self._fk_plan
+            frames, links, parents = self._fk_plan
             dev = nat.compute_device(self.device)
             with torch.cuda.device(dev):
                 qd = flat_q.detach().reshape(-1, n_joints).to(device=dev, dtype=torch.float32).contiguous()
                 n_cfg = qd.shape[0]
                 out = torch.empty(len(links) * n_cfg, 4, 4, dtype=torch.float32, device=dev)
-                nat.check(nat.lib().pvb_fk_serial(ctypes.cast(frames, ctypes.c_void_p), len(frames),
-                                                  ctypes.cast(links, ctypes.c_void_p), len(links), nat.ptr(qd), n_cfg,
-                                                  n_joints, nat.ptr(out), nat.stream_ptr(dev)), "pvb_fk_serial")
+                tail = (ctypes.cast(links, ctypes.c_void_p), len(links), nat.ptr(qd), n_cfg, n_joints, nat.ptr(out),
+                        nat.stream_ptr(dev))
+                if parents is None:
+                    nat.check(nat.lib().pvb_fk_serial(ctypes.cast(frames, ctypes.c_void_p), len(frames), *tail),
+                              "pvb_fk_serial")
+                else:
+                    nat.check(nat.lib().pvb_fk_tree(ctypes.cast(frames, ctypes.c_void_p),
+                                                    ctypes.cast(parents, ctypes.c_void_p), len(frames), *tail),
+                              "pvb_fk_tree")
             self.object_to_link_frames = Transform3d(matrix=out)
             if self.sdf is not None:
                 self.sdf.set_transforms(self.object_to_link_frames, batch_dim=self.configuration_batch)
@@ -239,19 +249,45 @@ class RobotSDF(sdf.ObjectFrameSDF):
             hit = self._surface_points[(num_points, seed)] = torch.stack(per_link)
         return hit
 
+    def _link_paths(self):
+        """(parents, paths): the parent of every frame of `frame_names` (-1 for the root), and for every link of
+        `sdf_to_link_name` the frames from its own (a link's first frame) up to the root.  The parents are
+        Chain.frame_parents(), or for any other chain the frame before (its frame order read as a serial chain)."""
+        parents = getattr(self.chain, "frame_parents", None)
+        parents = parents() if parents is not None else list(range(-1, len(self.frame_names) - 1))
+        pos = {}
+        for k, fname in enumerate(self.frame_names):
+            pos.setdefault(self.chain.find_frame(fname).link.name, k)
+        paths = []
+        for name in self.sdf_to_link_name:
+            f, path = pos[name], []
+            while f >= 0:
+                path.append(f)
+                f = parents[f]
+            paths.append(path)
+        return parents, paths
+
     def self_collision_pairs(self):
-        """The default `allowed` matrix of self_clearance, [S, S] bool: with m(s) the number of movable joints from the
-        root up to link s's frame, the pair (i, j) is tested when |m(i) - m(j)| >= 2.  That leaves out links on the same
-        rigid body (one frame, or frames joined by fixed joints) and links one joint apart, which touch by design.
-        Defined for serial chains; other structures pass `allowed` explicitly."""
-        movable, m_of = 0, {}
-        for fname in self.frame_names:
-            frame = self.chain.find_frame(fname)
-            if frame.joint.joint_type != "fixed":
-                movable += 1
-            m_of.setdefault(frame.link.name, movable)
-        m = torch.tensor([m_of[name] for name in self.sdf_to_link_name])
-        return (m[:, None] - m[None, :]).abs() >= 2
+        """The default `allowed` matrix of self_clearance, [S, S] bool: the pair (i, j) is tested when at least two
+        movable joints lie on the tree path between the two links' frames, m(i) + m(j) - 2 m(lca(i, j)) >= 2, with m(f)
+        the number of movable joints from the root up to frame f and lca the deepest frame both descend from.  That
+        leaves out links on the same rigid body (one frame, or frames joined by fixed joints) and links one joint apart,
+        which touch by design.  On a serial chain the lca is the shallower frame: |m(i) - m(j)| >= 2.  The structure is
+        Chain.frame_parents(); any other chain is read as serial in frame order.  Other rules pass `allowed`
+        explicitly."""
+        parents, paths = self._link_paths()
+        m = []
+        for k, fname in enumerate(self.frame_names):
+            movable = self.chain.find_frame(fname).joint.joint_type != "fixed"
+            m.append((m[parents[k]] if parents[k] >= 0 else 0) + (1 if movable else 0))
+        above = [set(p) for p in paths]
+        S = len(paths)
+        out = torch.zeros(S, S, dtype=torch.bool)
+        for i in range(S):
+            for j in range(S):
+                lca = next(f for f in paths[j] if f in above[i])
+                out[i, j] = m[paths[i][0]] + m[paths[j][0]] - 2 * m[lca] >= 2
+        return out
 
     def self_clearance(self, link_points=None, allowed=None, return_argmin=False):
         """For every installed joint configuration, the smallest distance between the robot's own links: link_points
@@ -274,12 +310,13 @@ class RobotSDF(sdf.ObjectFrameSDF):
         if self._twists is None:
             q = self.q.reshape(-1, len(self.joint_names))
             poses = self.chain.forward_kinematics(q, end_only=False)
-            rows = []
+            rows, names = [], []
             for fname in self.frame_names:
                 frame = self.chain.find_frame(fname)
                 jt = frame.joint.joint_type
                 if jt == "fixed":
                     continue
+                names.append(frame.joint.name)
                 pose = matrix_of(poses[frame.link.name]).to(torch.float64)
                 axis = torch.as_tensor(frame.joint.axis, dtype=torch.float64, device=pose.device)
                 d = pose[:, :3, :3] @ (axis / axis.norm())
@@ -287,20 +324,20 @@ class RobotSDF(sdf.ObjectFrameSDF):
                     rows.append(torch.cat([d, torch.zeros_like(d)], dim=-1))
                 else:
                     rows.append(torch.cat([-torch.linalg.cross(d, pose[:, :3, 3], dim=-1), d], dim=-1))
+            assert names == list(self.joint_names), "joint twists must follow joint_names"
             self._twists = torch.stack(rows, dim=1) if rows else torch.zeros(q.shape[0], 0, 6, dtype=torch.float64)
         return self._twists
 
     def joint_moves_link(self):
-        """[J, S] bool: joint j moves link s when j's frame comes at or before s's frame in the chain's frame order
-        (get_frame_names(exclude_fixed=False)) -- a serial chain, as self_collision_pairs assumes."""
-        pos = {}
-        for k, fname in enumerate(self.frame_names):
-            pos.setdefault(self.chain.find_frame(fname).link.name, k)
+        """[J, S] bool: joint j moves link s when j's frame is s's frame or one of its ancestors.  The structure is
+        Chain.frame_parents(); any other chain is read as serial in frame order, where the ancestors of a frame are
+        the frames before it (get_frame_names(exclude_fixed=False))."""
+        _, paths = self._link_paths()
         joints = [k for k, fname in enumerate(self.frame_names)
                   if self.chain.find_frame(fname).joint.joint_type != "fixed"]
-        links = [pos[name] for name in self.sdf_to_link_name]
-        return torch.tensor([[j <= s for s in links] for j in joints], dtype=torch.bool).reshape(len(joints),
-                                                                                                  len(links))
+        above = [set(p) for p in paths]
+        return torch.tensor([[j in up for up in above] for j in joints], dtype=torch.bool).reshape(len(joints),
+                                                                                                   len(above))
 
     def collision_cost(self, points_in_object_frame, margin):
         """For every installed joint configuration and every segment of points [*B, N, 3] in the robot frame, the soft
@@ -341,8 +378,9 @@ class RobotSDF(sdf.ObjectFrameSDF):
 
     @staticmethod
     def joint_gradient(twist, joint_twists, moves):
-        """The Jacobian transpose of a serial chain: twist gradients [A, *B, S, 6] (configuration-major, A flat or
-        not), joint twists [A, J, 6] and the [J, S] move mask give [A, *B, J] in fp64, dC/dq_j = sum_s moves[j, s]
+        """The Jacobian transpose of the robot's structure, which the [J, S] move mask encodes (joint_moves_link: joint
+        j moves link s when j lies on s's path from the root): twist gradients [A, *B, S, 6] (configuration-major, A
+        flat or not) and joint twists [A, J, 6] give [A, *B, J] in fp64, dC/dq_j = sum_s moves[j, s]
         twist[..., s, :] . joint_twists[a, j, :]."""
         jt = joint_twists.to(device=twist.device, dtype=torch.float64)
         tw = twist.to(torch.float64)

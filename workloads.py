@@ -178,3 +178,118 @@ def arm_configurations(n, seed=3, dtype=torch.float32):
 
 
 ARM_QUERY_RANGE = ((-1.0, 0.5), (-0.5, 0.5), (-0.2, 0.8))     # README.md:86-90 of the reference
+
+
+# --------------------------------------------------------------------------- kinematic trees
+# Two branching robots for RobotSDF's tree path (build_chain_from_urdf).  Every joint carries a <limit>, which
+# tree_configurations samples within.  Joints are written in depth-first pre-order, so the document order of the
+# movable joints is the column order of q.
+def _tree_urdf(dirname, name, links, joints, meshes):
+    """Writes <name>.urdf (+ link.obj, the probe mesh, with `meshes`): links [(name, [(kind, dims, xyz, rpy)])],
+    joints [(name, type, parent, child, xyz, rpy, axis, (lower, upper))].  With `meshes` every visual is the probe mesh
+    scaled to the primitive's extents.  Returns the URDF path."""
+    from pytorch_volumetric_b200.meshio import write_obj
+    os.makedirs(dirname, exist_ok=True)
+    if meshes:
+        v, f = fixture_mesh("probe")
+        write_obj(os.path.join(dirname, "link.obj"), v, f)
+        span = v.max(0) - v.min(0)
+
+    def geometry(kind, dims):
+        if meshes:
+            size = dims if kind == "box" else (2 * dims[0], 2 * dims[0], dims[1] if kind == "cylinder" else 2 * dims[0])
+            return f'<mesh filename="link.obj" scale="{" ".join(f"{s / e:.6f}" for s, e in zip(size, span))}"/>'
+        if kind == "box":
+            return f'<box size="{dims[0]} {dims[1]} {dims[2]}"/>'
+        if kind == "cylinder":
+            return f'<cylinder radius="{dims[0]}" length="{dims[1]}"/>'
+        return f'<sphere radius="{dims[0]}"/>'
+
+    parts = [f'<robot name="{name}">']
+    for link, visuals in links:
+        vis = "".join(f'<visual><origin xyz="{xyz}" rpy="{rpy}"/><geometry>{geometry(k, d)}</geometry></visual>'
+                      for k, d, xyz, rpy in visuals)
+        parts.append(f'<link name="{link}">{vis}</link>')
+    for jn, jt, parent, child, xyz, rpy, axis, (lo, hi) in joints:
+        ax = f'<axis xyz="{axis}"/>' if axis else ""
+        parts.append(f'<joint name="{jn}" type="{jt}"><parent link="{parent}"/><child link="{child}"/>'
+                     f'<origin xyz="{xyz}" rpy="{rpy}"/>{ax}<limit lower="{lo}" upper="{hi}"/></joint>')
+    parts.append("</robot>")
+    path = os.path.join(dirname, name + ".urdf")
+    with open(path, "w") as fh:
+        fh.write("\n".join(parts))
+    return path
+
+
+HAND_FINGERS = 4
+
+
+def write_hand(dirname, meshes=False):
+    """A hand on a two-joint wrist: forearm (root) -> wrist -> palm; four fingers off the palm, each an abduction joint
+    and three flexion joints (knuckle without a visual, then proximal, middle and distal segments); a thumb mounted
+    through a fixed joint with a rotated origin, then three revolute joints.  23 links, 18 of them with a box,
+    cylinder or sphere visual (the probe mesh with `meshes`), 21 movable joints.  Returns the URDF path."""
+    links = [("forearm", [("cylinder", (0.035, 0.2), "0 0 -0.1", "0 0 0")]), ("wrist", []),
+             ("palm", [("box", (0.09, 0.03, 0.1), "0 0 0.05", "0 0 0")])]
+    joints = [("wrist_pitch", "revolute", "forearm", "wrist", "0 0 0.02", "0 0 0", "0 1 0", (-1.0, 1.0)),
+              ("wrist_roll", "revolute", "wrist", "palm", "0 0 0.03", "0 0 0", "1 0 0", (-1.0, 1.0))]
+    for i in range(HAND_FINGERS):
+        f, k = f"finger{i}", 1.0 - 0.08 * abs(i - 1.5)           # the middle fingers are the longest
+        x = -0.033 + 0.022 * i
+        links += [(f"{f}_knuckle", []),
+                  (f"{f}_proximal", [("cylinder", (0.009, 0.045 * k), f"0 0 {0.0225 * k:.5f}", "0 0 0")]),
+                  (f"{f}_middle", [("cylinder", (0.008, 0.03 * k), f"0 0 {0.015 * k:.5f}", "0 0 0")]),
+                  (f"{f}_distal", [("box", (0.014, 0.013, 0.025 * k), f"0 0 {0.0125 * k:.5f}", "0 0 0.1")])]
+        joints += [(f"{f}_abduct", "revolute", "palm", f"{f}_knuckle", f"{x:.3f} 0 0.1", "0 0 0", "0 1 0", (-0.3, 0.3)),
+                   (f"{f}_flex1", "revolute", f"{f}_knuckle", f"{f}_proximal", "0 0 0.002", "0 0 0", "1 0 0",
+                    (-0.2, 1.5)),
+                   (f"{f}_flex2", "revolute", f"{f}_proximal", f"{f}_middle", f"0 0 {0.045 * k:.5f}", "0 0 0",
+                    "1 0 0", (0.0, 1.6)),
+                   (f"{f}_flex3", "revolute", f"{f}_middle", f"{f}_distal", f"0 0 {0.03 * k:.5f}", "0 0 0", "1 0 0",
+                    (0.0, 1.4))]
+    links += [("thumb_base", [("sphere", (0.013,), "0 0 0", "0 0 0")]),
+              ("thumb_proximal", [("cylinder", (0.01, 0.035), "0 0 0.0175", "0 0 0")]),
+              ("thumb_middle", [("cylinder", (0.009, 0.03), "0 0 0.015", "0 0 0")]),
+              ("thumb_distal", [("sphere", (0.01,), "0 0 0.01", "0 0 0")])]
+    joints += [("thumb_mount", "fixed", "palm", "thumb_base", "0.05 0 0.03", "0.2 0.9 0.3", None, (0.0, 0.0)),
+               ("thumb_flex1", "revolute", "thumb_base", "thumb_proximal", "0 0 0.012", "0 0 0", "1 0 0", (-0.5, 1.2)),
+               ("thumb_flex2", "revolute", "thumb_proximal", "thumb_middle", "0 0 0.035", "0 0 0", "1 0 0",
+                (0.0, 1.2)),
+               ("thumb_flex3", "revolute", "thumb_middle", "thumb_distal", "0 0 0.03", "0 0 0", "1 0 0", (0.0, 1.2))]
+    return _tree_urdf(dirname, "hand_mesh" if meshes else "hand", links, joints, meshes)
+
+
+def write_gripper_tree(dirname):
+    """A short arm with a two-finger gripper: base (root) -> three revolute joints -> palm, then one prismatic finger
+    (with a fingertip through a fixed joint with a rotated origin) and one revolute finger of two segments.  8 links,
+    every one with a box, cylinder or sphere visual, so the fused cost and self-clearance kernels run on it; 6 movable
+    joints.  Returns the URDF path."""
+    links = [("base", [("box", (0.12, 0.12, 0.06), "0 0 0.03", "0 0 0.2")]),
+             ("link1", [("cylinder", (0.04, 0.2), "0 0 0.1", "0 0 0")]),
+             ("link2", [("cylinder", (0.035, 0.18), "0 0 0.09", "0.1 0 0")]),
+             ("palm", [("box", (0.1, 0.04, 0.04), "0 0 0.02", "0 0 0")]),
+             ("finger_a", [("box", (0.015, 0.02, 0.06), "0 0 0.03", "0 0 0")]),
+             ("finger_a_tip", [("sphere", (0.01,), "0 0 0.005", "0 0 0")]),
+             ("finger_b1", [("box", (0.015, 0.02, 0.05), "0 0 0.025", "0 0 0")]),
+             ("finger_b2", [("cylinder", (0.008, 0.04), "0 0 0.02", "0 0 0")])]
+    joints = [("j1", "revolute", "base", "link1", "0 0 0.06", "0 0 0", "0 0 1", (-3.0, 3.0)),
+              ("j2", "revolute", "link1", "link2", "0 0 0.2", "0 0 0", "0 1 0", (-1.5, 1.5)),
+              ("j3", "revolute", "link2", "palm", "0 0 0.18", "0 0 0", "0 0 1", (-3.0, 3.0)),
+              ("finger_a_slide", "prismatic", "palm", "finger_a", "-0.03 0 0.04", "0 0 0", "1 0 0", (-0.025, 0.0)),
+              ("finger_a_tip_mount", "fixed", "finger_a", "finger_a_tip", "0 0 0.06", "0 0.3 0", None, (0.0, 0.0)),
+              ("finger_b_base", "revolute", "palm", "finger_b1", "0.03 0 0.04", "0 0 0", "0 1 0", (-0.6, 0.3)),
+              ("finger_b_tip", "revolute", "finger_b1", "finger_b2", "0 0 0.05", "0 0 0", "0 1 0", (-0.8, 0.8))]
+    return _tree_urdf(dirname, "gripper_tree", links, joints, False)
+
+
+def tree_configurations(urdf_path, n, seed=5, dtype=torch.float32):
+    """[n, J] joint values of a URDF written by write_hand / write_gripper_tree: configuration 0 all zeros (clamped
+    into the limits), the others uniform within every movable joint's <limit>; J in document order."""
+    import xml.etree.ElementTree as ET
+    joints = [j for j in ET.parse(urdf_path).getroot().findall("joint") if j.get("type") != "fixed"]
+    lo = torch.tensor([float(j.find("limit").get("lower")) for j in joints], dtype=torch.float64)
+    hi = torch.tensor([float(j.find("limit").get("upper")) for j in joints], dtype=torch.float64)
+    g = torch.Generator().manual_seed(seed)
+    q = lo + (hi - lo) * torch.rand(n, len(joints), generator=g, dtype=torch.float64)
+    q[0] = torch.zeros(len(joints), dtype=torch.float64).clamp(lo, hi)
+    return q.to(dtype)
