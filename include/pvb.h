@@ -368,6 +368,39 @@ int pvb_composed_query_self_collision_cost(const pvb_sdf_desc *descs, int32_t n_
                                            const uint8_t *allowed, float margin, float *out_cost, float *out_twist,
                                            void *stream);
 
+/* ---- EXTENSION: scene queries, every configuration's link points against one static scene SDF ----
+ * The reference has no such operator.  The robot: a composition of n_sdf <= 255 sub-SDFs whose inverse transforms
+ * W_s(a) = _affine_inverse(M_s(a)) are inv_xforms [n_sdf][n_cfg][4][4] (device); link_pts [n_sdf][K][3] (device), each
+ * row in its own sub-SDF's frame, 1 <= K < 2^24; links [n_sdf] (HOST memory), nonzero for the sources tested.  The
+ * robot's own sub-SDFs are never evaluated, so they may be of any kind.  The scene: n_scene <= 128 descriptors (host
+ * array, device tables) with their one configuration of object->sub-frame transforms scene_xforms [n_scene][4][4]
+ * (device), in the robot's object frame; a bare SDF is one descriptor under the identity.  For configuration a, every
+ * tested source i and point k: x = W_i(a) . link_pts[i][k] (posed as pvb_transform_points_paired poses), and (d, g)
+ * the scene's value and object-frame gradient at x, evaluated with the scene composition's one-point sequence
+ * (pvb_composed_query at x gives the same bits).
+ * Clearance: out_val / out_grad [cfg_count] / [cfg_count * 3] hold the minimum over (d, i, k) lexicographically (-0 ==
+ * +0, NaN above every number) and its gradient; out_link / out_point (each may be null) its i and k.  A configuration
+ * without a tested source gets +inf, a zero gradient and -1, -1.
+ * Collision cost with margin m: when d < m, h = m - d and tau = 2h (g, x x g): cost[a] += h^2 and twist[a, i] -= tau
+ * (the source moves, its point with it; the static scene takes no term).  out_cost [cfg_count], out_twist
+ * [cfg_count * n_sdf * 6] (k = 0..5 of source s at (c * n_sdf + s) * 6 + k); a configuration with nothing inside the
+ * margin costs exactly 0, and every untested source's row is 0.  The sums are deterministic, without atomics or
+ * workspace; their order depends on K, n_sdf and links alone (pvb_device.cuh), so a slab reproduces the rows of a
+ * larger call bit for bit.
+ * Both serve scenes of GRID sub-SDFs with the bounding-box rule (nearest or trilinear) and primitives.
+ * PVB_ERR_INVALID for mesh or LOOKUP_GT_SDF scene sub-SDFs (callers query the scene at the posed points), more than
+ * 128 scene or 255 robot sub-SDFs, K < 1 or K >= 2^24, null inv_xforms, links or outputs, an empty or invalid slab,
+ * a margin that is not finite, and the descriptor checks of pvb_composed_query. */
+int pvb_composed_query_scene_clearance(const pvb_sdf_desc *scene, int32_t n_scene, const float *scene_xforms,
+                                       const float *inv_xforms, int32_t n_sdf, int32_t n_cfg, int32_t cfg_begin,
+                                       int32_t cfg_count, const float *link_pts, int64_t K, const uint8_t *links,
+                                       float *out_val, float *out_grad, int32_t *out_link, int32_t *out_point,
+                                       void *stream);
+int pvb_composed_query_scene_collision_cost(const pvb_sdf_desc *scene, int32_t n_scene, const float *scene_xforms,
+                                            const float *inv_xforms, int32_t n_sdf, int32_t n_cfg, int32_t cfg_begin,
+                                            int32_t cfg_count, const float *link_pts, int64_t K, const uint8_t *links,
+                                            float margin, float *out_cost, float *out_twist, void *stream);
+
 /* ---- the same query with the result slab stored to several destinations from the kernel epilogue ----
  * Multi-GPU re-assembly of a configuration-sharded RobotSDF result (model_to_sdf.py:117-125 returns the full
  * (|A|, N) tensors): every rank evaluates its slab [cfg_begin, cfg_begin + cfg_count) and writes it straight into

@@ -172,6 +172,18 @@ _SIGNATURES = {
                                                               ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p,
                                                               ctypes.c_int64, ctypes.c_void_p, ctypes.c_float,
                                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "pvb_composed_query_scene_clearance": (ctypes.c_int, [ctypes.POINTER(SdfDesc), ctypes.c_int32, ctypes.c_void_p,
+                                                          ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                                          ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p,
+                                                          ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
+                                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                                          ctypes.c_void_p]),
+    "pvb_composed_query_scene_collision_cost": (ctypes.c_int, [ctypes.POINTER(SdfDesc), ctypes.c_int32,
+                                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                                                               ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                                               ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
+                                                               ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p,
+                                                               ctypes.c_void_p]),
     "pvb_composed_query_multi":(ctypes.c_int, [ctypes.POINTER(SdfDesc), ctypes.c_int32, ctypes.c_int32,
                                                 ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                                 ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint32, ctypes.c_void_p,

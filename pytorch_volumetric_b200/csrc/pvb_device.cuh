@@ -1306,6 +1306,60 @@ __device__ __forceinline__ bool collision_cost_near(const float (&lb)[8], float 
 // count, so repeated calls give identical bits and a slab reproduces the rows of the full call.
 constexpr int kSccLanes = 32;                     // lanes of a configuration's warp: its accumulators
 
+// collision_cost_term added into running sums, every product fused into its sum: cost += h^2 and tw[k] += t x_k as
+// one fmaf each.  That is what robot_collision_cost_kernel's compiled code does with `cost += t.cost` and
+// `a[k] += t.tw[k]` (nvcc contracts each product with its sum; the PTX of both kExt shows the seven fma.rn).  In the
+// sub-step loop of robot_paired_collision_cost_kernel the compiler would otherwise hoist h * h out of the loop and
+// round it twice.  The host builds of the robot kernels (-ffp-contract=off) keep collision_cost_term and plain sums:
+// they check the summation order.  fmaf rounds once in both builds, so the host build of scene_collision_cost_kernel
+// calls this function itself.
+__device__ __forceinline__ void collision_cost_add(float m, float d, f3 g, f3 p, float *cost, float *tw, int stride) {
+    const float h = m - d, t = 2.f * h;
+    const float x[6] = {g.x, g.y, g.z, cc_diff_of_products(p.y, g.z, p.z, g.y),
+                        cc_diff_of_products(p.z, g.x, p.x, g.z), cc_diff_of_products(p.x, g.y, p.y, g.x)};
+    *cost = fmaf(h, h, *cost);
+#pragma unroll
+    for (int k = 0; k < 6; ++k) tw[k * stride] = fmaf(t, x[k], tw[k * stride]);
+}
+
+// ----------------------------------------------------------------------------
+// Scene queries (scene_clearance_kernel / scene_collision_cost_kernel, pvb_composed_query_scene_clearance /
+// pvb_composed_query_scene_collision_cost; ComposedSDF.scene_clearance / scene_collision_cost): the robot's own link
+// points, posed by every configuration, against one static scene SDF.
+// Inputs: a composition of S <= 255 sub-SDFs with transforms M_s(a), and W_s = _affine_inverse(M_s); link_points
+// [S, K, 3], each row in its own sub-SDF's frame; links [S], the sources tested; a scene of grid (bounding-box rule)
+// or primitive sub-SDFs with its one set of transforms, in the composition's object frame.  For configuration a,
+// every tested source i and every point k:
+//   * x = W_i(a) . link_points[i, k], posed with composed_xform (the point pvb_transform_points_paired gives);
+//   * (d, g) = composed_point<false, kExt> of the scene at x: the scene's own one-point sequence.
+// Clearance: the smallest self_clearance_key(d, i, k) -- (d, i, k) lexicographically, -0 == +0, NaN above every
+// number -- with its (d, g), i and k; +inf, a zero gradient and -1, -1 without a tested source.
+// Collision cost with margin m: when d < m, h = m - d and tau = 2h (g, x x g): cost[a] += h^2 and twist[a, i] -= tau
+// (the source moves and its point with it, so d changes by +g . (v + w x x)); the scene is static and gets no term.
+// Summation order (scene_collision_cost_kernel): lane l takes the points k = l, l + 32, l + 64, ... of a source in
+// order into its own fp32 accumulators through collision_cost_add; the 32 lanes' sums are added in lane order in fp64,
+// the source's twist row rounded to fp32 once and its cost kept in fp64; the sources' costs are then added in source
+// order in fp64.  The order depends on K, S and links alone.
+constexpr int kSceneLanes = 32;
+constexpr int kSceneMaxSources = 255;             // the 8 bits of the source in self_clearance_key
+
+// Whether the scene may be below m at x: false only when every sub-SDF has the pruning bound
+// (value >= dist(q, box) - prune_margin, PVB_GRID_PRUNE_OK) and it puts that sub-SDF at m or above -- the test
+// composed_consider skips a sub-SDF by, with m in place of the running minimum.  A NaN point is always near.
+template <class LoadXf>
+__device__ __forceinline__ bool scene_near(const pvb_sdf_desc *descs, int n_scene, const LoadXf &load_xf, f3 x,
+                                           float m) {
+    for (int s = 0; s < n_scene; ++s) {
+        const pvb_sdf_desc &d = descs[s];
+        if (!(d.flags & PVB_GRID_PRUNE_OK)) return true;
+        float4 r0, r1, r2;
+        load_xf(s, r0, r1, r2);
+        const float thr = m + d.prune_margin;
+        if (!(thr < 0.f || composed_aabb_lb2(d, composed_xform(r0, r1, r2, x)) > thr * thr)) return true;
+    }
+    return false;
+}
+
 // ----------------------------------------------------------------------------
 // Forward kinematics (fk_serial_kernel, fk_tree_kernel; RobotSDF.set_joint_configuration, model_to_sdf.py:82-115):
 // for every joint configuration a and every mesh link s, the object->mesh-frame transform

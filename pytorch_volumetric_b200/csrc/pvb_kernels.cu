@@ -2312,21 +2312,6 @@ collision_cost_finish_kernel(const float *__restrict__ partial, long long n_rows
     }
 }
 
-// collision_cost_term added into running sums, every product fused into its sum: cost += h^2 and tw[k] += t x_k as
-// one fmaf each.  That is what robot_collision_cost_kernel's compiled code does with `cost += t.cost` and
-// `a[k] += t.tw[k]` (nvcc contracts each product with its sum; the PTX of both kExt shows the seven fma.rn).  In the
-// sub-step loop of robot_paired_collision_cost_kernel the compiler would otherwise hoist h * h out of the loop and
-// round it twice.  The host build (-ffp-contract=off) of both kernels keeps collision_cost_term and plain sums: it
-// checks the summation order.
-__device__ __forceinline__ void collision_cost_add(float m, float d, f3 g, f3 p, float *cost, float *tw, int stride) {
-    const float h = m - d, t = 2.f * h;
-    const float x[6] = {g.x, g.y, g.z, cc_diff_of_products(p.y, g.z, p.z, g.y),
-                        cc_diff_of_products(p.z, g.x, p.x, g.z), cc_diff_of_products(p.x, g.y, p.y, g.x)};
-    *cost = __fmaf_rn(h, h, *cost);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) tw[k * stride] = __fmaf_rn(t, x[k], tw[k * stride]);
-}
-
 // ------------------------------------------------------------------------------------------------------------
 // Paired collision-cost query on the sets robot_collision_cost_kernel takes: configuration c against its OWN points,
 // pts [cfg_count][n_seg][seg_len][3].  The same partials as robot_collision_cost_kernel, in the same layout and with
@@ -2521,6 +2506,151 @@ robot_self_collision_cost_kernel(const __grid_constant__ RobotPack<kRsMaxS> pk, 
             if (e == 0) out_cost[c] = (float)s;
             else out_twist[(size_t)c * (E - 1) + (e - 1)] = (float)s;
         }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Scene queries (pvb_device.cuh: the definition and the summation order): every configuration's link points, posed by
+// its W_i, against one static scene of grid (bounding-box rule) or primitive sub-SDFs, evaluated with composed_point
+// -- the scene's own one-point sequence.  The robot's sub-SDFs are never evaluated, so their kinds and their number
+// (up to kSceneMaxSources) do not matter.
+//   * Work unit: one configuration, owned by one block of kSceneWarps warps; the blocks of a 1-D grid stride over the
+//     slab.  Warp w takes the sources w, w + kSceneWarps, ... (a source not tested is skipped, or for the cost given
+//     a zero row); lane l the points k = l, l + 32, ... of a source, in order.  W_i's three rows are read once per
+//     source (the same address for every lane).
+//   * The scene's transform rows are the same for every configuration: staged once per block in shared memory.
+//   * No atomics, no workspace and no finish kernel: the block's reductions go through shared memory.
+constexpr int kSceneWarps = 8;
+struct SceneLinks {
+    unsigned char on[kSceneMaxSources + 1];     // by source index: tested
+};
+
+// Clearance: per-lane running self_clearance_key, the warp minimum, the block minimum in shared memory; thread 0 then
+// poses the winning (i, k) again and evaluates the scene there once for the gradient.
+template <bool kExt, int MAXS>
+__global__ void __launch_bounds__(kSceneLanes * kSceneWarps)
+scene_clearance_kernel(const __grid_constant__ DescPack<MAXS> scene, int n_scene, const float *__restrict__ scene_xforms,
+                       const float *__restrict__ inv_xforms, int n_sdf, int n_cfg, int cfg_begin, int cfg_count,
+                       const float *__restrict__ link_pts, int K, const __grid_constant__ SceneLinks links,
+                       float *__restrict__ out_val, float *__restrict__ out_grad, int *__restrict__ out_link,
+                       int *__restrict__ out_point) {
+    __shared__ float4 sxf[3 * MAXS];
+    __shared__ unsigned long long wkey[kSceneWarps];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int t = threadIdx.x; t < 3 * n_scene; t += blockDim.x) sxf[t] = __ldg(xf_rows(scene_xforms, 1, t / 3, 0) + t % 3);
+    __syncthreads();
+    NodeStage st; st.smem = nullptr; st.n = 0;
+    auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) { r0 = sxf[3 * s]; r1 = sxf[3 * s + 1]; r2 = sxf[3 * s + 2]; };
+    for (int c = blockIdx.x; c < cfg_count; c += gridDim.x) {
+        const int cfg = cfg_begin + c;
+        unsigned long long run = ~0ull;
+        for (int i = warp; i < n_sdf; i += kSceneWarps) {
+            if (!links.on[i]) continue;
+            const float4 *w = xf_rows(inv_xforms, n_cfg, i, cfg);
+            const float4 w0 = __ldg(w), w1 = __ldg(w + 1), w2 = __ldg(w + 2);
+#pragma unroll 1
+            for (int k = lane; k < K; k += 32) {
+                const f3 x = composed_xform(w0, w1, w2, load_point(link_pts, (long long)i * K + k));
+                const ComposedOut o = composed_point<false, kExt>(scene.d, scene.order, n_scene, load_xf, st, x, 0u,
+                                                                  0ull, 0, 0.f);
+                const unsigned long long kk = self_clearance_key(o.val, i, k);
+                run = kk < run ? kk : run;
+            }
+        }
+        run = warp_min_key(run, 1);
+        if (lane == 0) wkey[warp] = run;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            unsigned long long best = wkey[0];
+            for (int v = 1; v < kSceneWarps; ++v) best = wkey[v] < best ? wkey[v] : best;
+            float val = PVB_INF;
+            f3 g = mk3(0.f, 0.f, 0.f);
+            int li = -1, pk = -1;
+            if (best != ~0ull) {
+                li = (int)((uint32_t)best >> 24); pk = (int)((uint32_t)best & 0xffffffu);
+                const float4 *w = xf_rows(inv_xforms, n_cfg, li, cfg);
+                const f3 x = composed_xform(__ldg(w), __ldg(w + 1), __ldg(w + 2),
+                                            load_point(link_pts, (long long)li * K + pk));
+                const ComposedOut o = composed_point<false, kExt>(scene.d, scene.order, n_scene, load_xf, st, x, 0u,
+                                                                  0ull, 0, 0.f);
+                val = o.val; g = o.grad;
+            }
+            out_val[c] = val;
+            out_grad[3 * c] = g.x; out_grad[3 * c + 1] = g.y; out_grad[3 * c + 2] = g.z;
+            if (out_link) out_link[c] = li;
+            if (out_point) out_point[c] = pk;
+        }
+        __syncthreads();                                     // wkey is free for the next configuration
+    }
+}
+
+// Collision cost: per-lane fp32 accumulators (collision_cost_add), a 32-point step skipped by the whole warp when
+// scene_near clears every lane's point; at the end of a source the lanes' sums in lane order in fp64 (acc[warp] in
+// shared memory, lane e adding row e), the twist row stored and the cost kept in shared memory by source; thread 0
+// then adds the sources' costs in order in fp64.
+struct __align__(16) SceneCostSmem {
+    float acc[kSceneWarps][7][kSceneLanes + 1];
+    double cost[kSceneMaxSources + 1];
+};
+
+template <bool kExt, int MAXS>
+__global__ void __launch_bounds__(kSceneLanes * kSceneWarps)
+scene_collision_cost_kernel(const __grid_constant__ DescPack<MAXS> scene, int n_scene,
+                            const float *__restrict__ scene_xforms, const float *__restrict__ inv_xforms, int n_sdf,
+                            int n_cfg, int cfg_begin, int cfg_count, const float *__restrict__ link_pts, int K,
+                            const __grid_constant__ SceneLinks links, float margin, float *__restrict__ out_cost,
+                            float *__restrict__ out_twist) {
+    __shared__ float4 sxf[3 * MAXS];
+    __shared__ SceneCostSmem sm;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const float m = margin;
+    for (int t = threadIdx.x; t < 3 * n_scene; t += blockDim.x) sxf[t] = __ldg(xf_rows(scene_xforms, 1, t / 3, 0) + t % 3);
+    __syncthreads();
+    NodeStage st; st.smem = nullptr; st.n = 0;
+    auto load_xf = [&](int s, float4 &r0, float4 &r1, float4 &r2) { r0 = sxf[3 * s]; r1 = sxf[3 * s + 1]; r2 = sxf[3 * s + 2]; };
+    for (int c = blockIdx.x; c < cfg_count; c += gridDim.x) {
+        const int cfg = cfg_begin + c;
+        // uniform per warp: every lane takes part in the votes and __syncwarp
+        for (int i = warp; i < n_sdf; i += kSceneWarps) {
+            float *const row = out_twist + ((size_t)c * n_sdf + i) * 6;
+            if (!links.on[i]) {
+                if (lane < 6) row[lane] = 0.f;
+                if (lane == 0) sm.cost[i] = 0.0;
+                continue;
+            }
+            const float4 *w = xf_rows(inv_xforms, n_cfg, i, cfg);
+            const float4 w0 = __ldg(w), w1 = __ldg(w + 1), w2 = __ldg(w + 2);
+            float acc[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll 1
+            for (int j0 = 0; j0 < K; j0 += 32) {
+                const int k = j0 + lane;
+                const bool on = k < K;
+                const f3 x = composed_xform(w0, w1, w2,
+                                            on ? load_point(link_pts, (long long)i * K + k) : mk3(0.f, 0.f, 0.f));
+                if (!__any_sync(0xffffffffu, on && scene_near(scene.d, n_scene, load_xf, x, m))) continue;
+                if (!on) continue;
+                const ComposedOut o = composed_point<false, kExt>(scene.d, scene.order, n_scene, load_xf, st, x, 0u,
+                                                                  0ull, 0, 0.f);
+                if (o.val < m) collision_cost_add(m, o.val, o.grad, x, acc, acc + 1, 1);
+            }
+#pragma unroll
+            for (int e = 0; e < 7; ++e) sm.acc[warp][e][lane] = acc[e];
+            __syncwarp();
+            if (lane < 7) {
+                double s = 0.0;
+                for (int l = 0; l < kSceneLanes; ++l) s += (double)sm.acc[warp][lane][l];
+                if (lane == 0) sm.cost[i] = s;
+                else row[lane - 1] = (float)(0.0 - s);     // twist[a, i] -= tau; +0 when nothing contributed
+            }
+            __syncwarp();                                    // acc[warp] is free for the warp's next source
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double s = 0.0;
+            for (int i = 0; i < n_sdf; ++i) s += sm.cost[i];
+            out_cost[c] = (float)s;
+        }
+        __syncthreads();                                     // sm.cost is free for the next configuration
     }
 }
 
@@ -4001,6 +4131,84 @@ extern "C" int pvb_composed_query_self_collision_cost(const pvb_sdf_desc *descs,
     timing_mark(1, s);
     PVB_CHECK_LAUNCH("pvb_composed_query_self_collision_cost");
     return PVB_OK;
+}
+
+// The checks of both scene entry points, in order (`fn` names the entry point): K, inv_xforms and links
+// (check_link_points), the scene as the composed entry points check their sub-SDFs (one configuration), the robot's
+// sub-SDF count and slab, then no mesh and no LOOKUP_GT_SDF grid in the scene; the tested sources into `on`.
+static int scene_check_args(const char *fn, const pvb_sdf_desc *scene, int32_t n_scene, const float *scene_xforms,
+                            const float *inv_xforms, int32_t n_sdf, int32_t n_cfg, int32_t cfg_begin,
+                            int32_t cfg_count, const float *link_pts, int64_t K, const uint8_t *links,
+                            const float *out_a, const float *out_b, SceneLinks &on, bool &any_ext) {
+    if (int rc = check_link_points(fn, K, inv_xforms, links)) return rc;
+    if (int rc = composed_check_args(fn, scene, n_scene, scene_xforms, 1, 0, 1, link_pts,
+                                     n_sdf > 0 ? (int64_t)n_sdf * K : 0, out_a, out_b, any_ext))
+        return rc;
+    if (n_sdf < 1 || n_sdf > kSceneMaxSources || n_cfg < 1 || cfg_begin < 0 || cfg_count < 1 ||
+        cfg_begin > n_cfg - cfg_count) {
+        pvb_set_error("%s: invalid argument (n_sdf=%d n_cfg=%d cfg=[%d,+%d); 1 <= n_sdf <= %d and a non-empty slab)",
+                      fn, n_sdf, n_cfg, cfg_begin, cfg_count, kSceneMaxSources);
+        return PVB_ERR_INVALID;
+    }
+    if (!rs_links_ok(scene, n_scene)) {
+        pvb_set_error("%s: the fused scene query takes grid (bounding-box rule) or primitive scene sub-SDFs, no mesh or "
+                      "LOOKUP_GT_SDF grid; query the scene at the posed link points instead", fn);
+        return PVB_ERR_INVALID;
+    }
+    memset(&on, 0, sizeof(on));
+    for (int i = 0; i < n_sdf; ++i) on.on[i] = links[i] ? 1 : 0;
+    return PVB_OK;
+}
+
+extern "C" int pvb_composed_query_scene_clearance(const pvb_sdf_desc *scene, int32_t n_scene,
+                                                  const float *scene_xforms, const float *inv_xforms, int32_t n_sdf,
+                                                  int32_t n_cfg, int32_t cfg_begin, int32_t cfg_count,
+                                                  const float *link_pts, int64_t K, const uint8_t *links,
+                                                  float *out_val, float *out_grad, int32_t *out_link,
+                                                  int32_t *out_point, void *stream) {
+    const char *fn = "pvb_composed_query_scene_clearance";
+    SceneLinks on;
+    bool any_ext;
+    if (int rc = scene_check_args(fn, scene, n_scene, scene_xforms, inv_xforms, n_sdf, n_cfg, cfg_begin, cfg_count,
+                                  link_pts, K, links, out_val, out_grad, on, any_ext))
+        return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    return comp_variant(false, any_ext, n_scene, [&](auto, auto kExt, auto kMaxS) {
+        const DescPack<kMaxS> pack = desc_pack<kMaxS>(scene, n_scene);
+        timing_mark(0, s);
+        scene_clearance_kernel<kExt, kMaxS><<<(unsigned)cfg_count, kSceneLanes * kSceneWarps, 0, s>>>(
+            pack, n_scene, scene_xforms, inv_xforms, n_sdf, n_cfg, cfg_begin, cfg_count, link_pts, (int)K, on, out_val,
+            out_grad, out_link, out_point);
+        timing_mark(1, s);
+        PVB_CHECK_LAUNCH("pvb_composed_query_scene_clearance");
+        return PVB_OK;
+    });
+}
+
+extern "C" int pvb_composed_query_scene_collision_cost(const pvb_sdf_desc *scene, int32_t n_scene,
+                                                       const float *scene_xforms, const float *inv_xforms,
+                                                       int32_t n_sdf, int32_t n_cfg, int32_t cfg_begin,
+                                                       int32_t cfg_count, const float *link_pts, int64_t K,
+                                                       const uint8_t *links, float margin, float *out_cost,
+                                                       float *out_twist, void *stream) {
+    const char *fn = "pvb_composed_query_scene_collision_cost";
+    if (int rc = check_margin(fn, margin)) return rc;
+    SceneLinks on;
+    bool any_ext;
+    if (int rc = scene_check_args(fn, scene, n_scene, scene_xforms, inv_xforms, n_sdf, n_cfg, cfg_begin, cfg_count,
+                                  link_pts, K, links, out_cost, out_twist, on, any_ext))
+        return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    return comp_variant(false, any_ext, n_scene, [&](auto, auto kExt, auto kMaxS) {
+        const DescPack<kMaxS> pack = desc_pack<kMaxS>(scene, n_scene);
+        timing_mark(0, s);
+        scene_collision_cost_kernel<kExt, kMaxS><<<(unsigned)cfg_count, kSceneLanes * kSceneWarps, 0, s>>>(
+            pack, n_scene, scene_xforms, inv_xforms, n_sdf, n_cfg, cfg_begin, cfg_count, link_pts, (int)K, on, margin,
+            out_cost, out_twist);
+        timing_mark(1, s);
+        PVB_CHECK_LAUNCH("pvb_composed_query_scene_collision_cost");
+        return PVB_OK;
+    });
 }
 
 extern "C" int pvb_composed_query_multi(const pvb_sdf_desc *descs, int32_t n_sdf, int32_t needs_mesh,

@@ -376,6 +376,31 @@ class RobotSDF(sdf.ObjectFrameSDF):
         grad = self.joint_gradient(twist, self.joint_twists(), self.joint_moves_link())
         return cost, grad.to(cost.dtype)
 
+    def scene_clearance(self, scene, link_points=None, links=None, return_argmin=False):
+        """For every installed joint configuration, the smallest distance from the robot's tested links to a static
+        scene SDF in the robot frame (a CachedSDF of a scene mesh, primitives, or a ComposedSDF of them; place one
+        with ComposedSDF([scene], T)): link_points [S, K, 3] (default: link_surface_points()) are posed with their
+        links, and links [S] bool leaves out links not tested (a base resting on the table, say; default: all).
+        Returns (values [*A], robot-frame scene gradients [*A, 3]) and, with return_argmin, the link (a position in
+        `sdf_to_link_name`) and point, int64 [*A]; a negative value is a penetration.  See
+        ComposedSDF.scene_clearance."""
+        if link_points is None:
+            link_points = self.link_surface_points()
+        return self.sdf.scene_clearance(scene, link_points, links, return_argmin=return_argmin)
+
+    def scene_collision_cost(self, scene, margin, link_points=None, links=None):
+        """For every installed joint configuration, the soft collision cost of the robot's tested links against a
+        static scene SDF and its derivative with respect to the joint values: link_points and links as in
+        scene_clearance, and every posed point within `margin` of the scene adds max(0, margin - d)^2.  Returns
+        (cost [*A], joint_grad [*A, J]), J in `joint_names` order: ComposedSDF.scene_collision_cost's twist gradient
+        through joint_gradient(twist, joint_twists(), joint_moves_link()).  Not autograd: the gradient is an output of
+        the query."""
+        if link_points is None:
+            link_points = self.link_surface_points()
+        cost, twist = self.sdf.scene_collision_cost(scene, link_points, margin, links)
+        grad = self.joint_gradient(twist, self.joint_twists(), self.joint_moves_link())
+        return cost, grad.to(cost.dtype)
+
     @staticmethod
     def joint_gradient(twist, joint_twists, moves):
         """The Jacobian transpose of the robot's structure, which the [J, S] move mask encodes (joint_moves_link: joint

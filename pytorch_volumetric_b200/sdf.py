@@ -1474,6 +1474,199 @@ class ComposedSDF(ObjectFrameSDF):
         out = self.query_self_collision_cost(link_points, allowed, margin)
         return self._deliver(link_points, out, shape, device=matrix_of(self.obj_frame_to_link_frame).device)
 
+    #: most sub-SDFs a composition may hold on the fused scene route (the 8 bits of the source in its key)
+    max_scene_sources = 255
+
+    def _scene_args(self, scene, link_points, links, form):
+        """(K, links as S bools) of a scene query; ValueError when link_points is not [S, K, 3] with 1 <= K < 2^24,
+        links is not an [S] bool mask, or the scene is not an ObjectFrameSDF with one pose."""
+        S = len(self.sdfs)
+        shape = tuple(link_points.shape)
+        if len(shape) != 3 or shape[0] != S or shape[2] != 3 or not 1 <= shape[1] < (1 << 24):
+            raise ValueError(f"{form}: link_points {shape} must be [S, K, 3] with S = {S} sub-SDFs and 1 <= K < 2^24")
+        if links is None:
+            mask = [True] * S
+        else:
+            lk = links if torch.is_tensor(links) else torch.as_tensor(np.asarray(links))
+            if lk.dtype != torch.bool or tuple(lk.shape) != (S,):
+                raise ValueError(f"{form}: links must be an [S] = [{S}] bool mask, got {tuple(lk.shape)} {lk.dtype}")
+            mask = lk.detach().cpu().tolist()
+        if not isinstance(scene, ObjectFrameSDF):
+            raise ValueError(f"{form}: the scene must be an ObjectFrameSDF, got {type(scene).__name__}")
+        if isinstance(scene, ComposedSDF) and _config_count(scene.tsf_batch) != 1:
+            raise ValueError(f"{form}: the scene ComposedSDF holds {_config_count(scene.tsf_batch)} configurations; a "
+                             f"static scene has one pose")
+        return shape[1], mask
+
+    def _scene_fused(self, scene, device):
+        """(descriptor array, n_scene, scene transforms [n_scene, 4, 4] fp32 on `device`) when the fused scene kernels
+        take this composition and scene, else None: at most `max_scene_sources` sub-SDFs here, and a scene of grid
+        (bounding-box rule) or primitive SDFs -- a CachedSDF, SphereSDF, BoxSDF or CylinderSDF, or a one-configuration
+        ComposedSDF of at most 128 of them.  A bare scene is one sub-SDF under the identity."""
+        if len(self.sdfs) > self.max_scene_sources:
+            return None
+        if isinstance(scene, ComposedSDF):
+            descs_arr, needs_mesh = scene._native_descs(device)
+            if descs_arr is None or needs_mesh:
+                return None
+            return descs_arr, len(scene.sdfs), scene._xforms_on(device)
+        d = scene.native_desc(device)
+        if d is None or d.kind == nat.PVB_KIND_MESH or (d.flags & nat.PVB_GRID_OOB_GT):
+            return None
+        return nat.desc_array([d]), 1, torch.eye(4, dtype=torch.float32, device=device)
+
+    def _scene_slab(self, cfg_begin, cfg_count, form):
+        n_cfg, cfg_count = self._slab(cfg_begin, cfg_count)
+        if cfg_count < 1 or cfg_begin < 0 or cfg_begin + cfg_count > n_cfg:
+            raise ValueError(f"{form}: empty or invalid configuration slab [{cfg_begin}, +{cfg_count}) of {n_cfg}")
+        return n_cfg, cfg_count
+
+    def query_scene_clearance(self, scene, link_points, links=None, cfg_begin=0, cfg_count=None, return_which=False):
+        """Scene clearance of configurations [cfg_begin, cfg_begin + cfg_count): for configuration a, the smallest
+        value of the static `scene` over every source sub-SDF i that `links[i]` tests (default: all) and every point
+        x = W_i(a) link_points[i, k], W_i = _affine_inverse(M_i) -- points that belong to sub-SDF i, given in its own
+        frame, posed with it (pvb_transform_points_paired).  The scene is any ObjectFrameSDF in this composition's
+        object frame (place one with ComposedSDF([scene], T)); (d, g) is its value and gradient at x.  The minimum is
+        taken over (d, i, k) lexicographically, -0 == +0 and a NaN value above every number.  A configuration without
+        a tested source gets +inf, a zero gradient and indices -1.
+
+        The definition is the composition route (`_composed_scene_clearance`: the posed points and scene(x)).  Scenes
+        of grid (bounding-box rule) or primitive SDFs -- CachedSDF, SphereSDF, BoxSDF, CylinderSDF, or a
+        one-configuration ComposedSDF of at most 128 of them -- run fused in one kernel
+        (pvb_composed_query_scene_clearance) for any kind of sub-SDF here, up to 255 of them, bit-identical to that
+        route; every other scene takes the route itself.
+
+        link_points [S, K, 3], 1 <= K < 2^24; links [S] bool.  Returns flat (cfg_count,) / (cfg_count, 3) fp32
+        tensors on the GPU, and with return_which also the int32 source i and point k.  Raises ValueError before any
+        device work on wrong shapes, a scene with more than one pose, or an empty slab."""
+        form = "scene-clearance query"
+        K, mask = self._scene_args(scene, link_points, links, form)
+        n_cfg, cfg_count = self._scene_slab(cfg_begin, cfg_count, form)
+        S = len(self.sdfs)
+        with _query_points(link_points) as (device, p):
+            fused = self._scene_fused(scene, device)
+            if fused is None:
+                return self._composed_scene_clearance(scene, p, K, mask, cfg_begin, cfg_count, return_which)
+            descs_arr, n_scene, sxf = fused
+            inv = self._inv_xforms_on(device)
+            val = torch.empty(cfg_count, dtype=torch.float32, device=device)
+            grad = torch.empty(cfg_count, 3, dtype=torch.float32, device=device)
+            link, point = (torch.empty(cfg_count, dtype=torch.int32, device=device) if return_which else None
+                           for _ in range(2))
+            nat.check(nat.lib().pvb_composed_query_scene_clearance(
+                descs_arr, n_scene, nat.ptr(sxf), nat.ptr(inv), S, n_cfg, cfg_begin, cfg_count, nat.ptr(p), K,
+                (ctypes.c_uint8 * S)(*mask), nat.ptr(val), nat.ptr(grad), nat.ptr(link), nat.ptr(point),
+                nat.stream_ptr(device)), "pvb_composed_query_scene_clearance")
+        return (val, grad, link, point) if return_which else (val, grad)
+
+    def _scene_chunks(self, scene, p, K, srcs, cfg_begin, cfg_count):
+        """The walk of the scene composition routes: (c0, cc, x, v, g) for every chunk of `composition_chunk`
+        configurations, ascending, with x [cc, n_src, K, 3] the tested sources' points posed (`_posed_link_points`)
+        and (v [cc, n_src, K], g [..., 3]) = scene(x) as fp32."""
+        lp = p.reshape(len(self.sdfs), K, 3)
+        for c0 in range(cfg_begin, cfg_begin + cfg_count, self.composition_chunk):
+            cc = min(self.composition_chunk, cfg_begin + cfg_count - c0)
+            x = torch.stack([self._posed_link_points(lp, i, c0, cc) for i in srcs], dim=1)
+            v, g = scene(x)
+            yield (c0, cc, x, v.to(device=p.device, dtype=torch.float32).reshape(cc, len(srcs), K),
+                   g.to(device=p.device, dtype=torch.float32).reshape(cc, len(srcs), K, 3))
+
+    def _composed_scene_clearance(self, scene, p, K, mask, cfg_begin, cfg_count, return_which):
+        """query_scene_clearance by composition, the definition of its result: `_scene_chunks`, then the first
+        minimum over (source, point) in clearance-key order."""
+        device = p.device
+        srcs = [i for i, on in enumerate(mask) if on]
+        val = torch.full((cfg_count,), float("inf"), dtype=torch.float32, device=device)
+        grad = torch.zeros(cfg_count, 3, dtype=torch.float32, device=device)
+        link, point = (torch.full((cfg_count,), -1, dtype=torch.int32, device=device) for _ in range(2))
+        src_t = torch.tensor(srcs, dtype=torch.int64, device=device)
+        for c0, cc, _, v, g in (self._scene_chunks(scene, p, K, srcs, cfg_begin, cfg_count) if srcs else ()):
+            j = self._first_minimum(v.reshape(cc, -1))[:, None]                      # pos * K + k: (i, k) order
+            out = slice(c0 - cfg_begin, c0 - cfg_begin + cc)
+            val[out] = v.reshape(cc, -1).gather(1, j).reshape(-1)
+            grad[out] = g.reshape(cc, -1, 3).gather(1, j[..., None].expand(cc, 1, 3)).reshape(-1, 3)
+            link[out] = src_t[j.reshape(-1) // K].to(torch.int32)
+            point[out] = (j.reshape(-1) % K).to(torch.int32)
+        return (val, grad, link, point) if return_which else (val, grad)
+
+    def scene_clearance(self, scene, link_points, links=None, return_argmin=False):
+        """For every installed configuration, the smallest distance from its tested links to a static scene:
+        link_points [S, K, 3] holds K points of every sub-SDF in its own frame (its surface, say), links [S] bool says
+        which sub-SDFs are tested (default: all), and `scene` is any ObjectFrameSDF in this composition's object frame.
+        Returns (values [*A], scene gradients [*A, 3]) in link_points' dtype on the composition's device -- 0-d / [3]
+        without a configuration batch -- and with return_argmin also the source sub-SDF i and point k, int64 [*A].
+        Negative values mean a link penetrates the scene.  The semantics, tie rule and routes are those of
+        `query_scene_clearance`.  Not a reference operator (an extension); raises ValueError before any device work on
+        wrong shapes or a scene with more than one pose."""
+        shape = () if self.tsf_batch is None else tuple(int(a) for a in self.tsf_batch)
+        out = self.query_scene_clearance(scene, link_points, links, return_which=return_argmin)
+        return self._deliver(link_points, out, shape, device=matrix_of(self.obj_frame_to_link_frame).device)
+
+    def query_scene_collision_cost(self, scene, link_points, margin, links=None, cfg_begin=0, cfg_count=None):
+        """Scene collision cost of configurations [cfg_begin, cfg_begin + cfg_count) and its twist gradient per
+        sub-SDF.  The posed points x and the scene's (d, g) at them are those of `query_scene_clearance`; the margin m
+        is rounded to fp32 as _collision_cost_margin does.  When d < m, with h = m - d and tau = 2h (g, x x g):
+          - cost[a] += h^2
+          - twist[a, i] -= tau.  The source moves and its point with it, so d changes by +g . (v + w x x); the scene
+            is static and takes no term, so every other twist entry is 0.
+        twist[a, s] is the derivative of the cost when sub-SDF s alone moves by an object-frame twist (v, w) about the
+        origin: the convention of collision_cost, so RobotSDF.joint_gradient applies unchanged.  A configuration with
+        nothing inside the margin costs exactly 0.
+
+        The routes are those of `query_scene_clearance`; the composition route (`_composed_scene_collision_cost`) is
+        the definition the fused one is checked against.  Both are deterministic, and the fused route's rows do not
+        depend on the slab: a configuration split reproduces the full call bit for bit.  Returns flat (cfg_count,) /
+        (cfg_count, S, 6) fp32 tensors on the GPU.  Raises ValueError before any device work on wrong shapes, a
+        margin that is not finite, a scene with more than one pose, or an empty slab."""
+        form = "scene-collision-cost query"
+        K, mask = self._scene_args(scene, link_points, links, form)
+        m = self._collision_cost_margin(margin)
+        n_cfg, cfg_count = self._scene_slab(cfg_begin, cfg_count, form)
+        S = len(self.sdfs)
+        with _query_points(link_points) as (device, p):
+            fused = self._scene_fused(scene, device)
+            if fused is None:
+                return self._composed_scene_collision_cost(scene, p, K, mask, m, cfg_begin, cfg_count)
+            descs_arr, n_scene, sxf = fused
+            inv = self._inv_xforms_on(device)
+            cost = torch.empty(cfg_count, dtype=torch.float32, device=device)
+            twist = torch.empty(cfg_count, S, 6, dtype=torch.float32, device=device)
+            nat.check(nat.lib().pvb_composed_query_scene_collision_cost(
+                descs_arr, n_scene, nat.ptr(sxf), nat.ptr(inv), S, n_cfg, cfg_begin, cfg_count, nat.ptr(p), K,
+                (ctypes.c_uint8 * S)(*mask), m, nat.ptr(cost), nat.ptr(twist), nat.stream_ptr(device)),
+                "pvb_composed_query_scene_collision_cost")
+        return cost, twist
+
+    def _composed_scene_collision_cost(self, scene, p, K, mask, m, cfg_begin, cfg_count):
+        """query_scene_collision_cost by composition, the definition of its result: `_scene_chunks`, the
+        `_hinge_terms`, and one sum per tested source (torch's sums are deterministic; scatter_add / index_add on
+        CUDA are not)."""
+        device = p.device
+        srcs = [i for i, on in enumerate(mask) if on]
+        cost = torch.zeros(cfg_count, dtype=torch.float64, device=device)
+        twist = torch.zeros(cfg_count, len(self.sdfs), 6, dtype=torch.float64, device=device)
+        for c0, cc, x, v, g in (self._scene_chunks(scene, p, K, srcs, cfg_begin, cfg_count) if srcs else ()):
+            h, tau = self._hinge_terms(v, g, x, m)
+            rs = slice(c0 - cfg_begin, c0 - cfg_begin + cc)
+            cost[rs] = (h * h).sum(dim=(-2, -1))
+            for pos, i in enumerate(srcs):
+                twist[rs, i] = 0.0 - tau[:, pos].sum(dim=-2)       # +0, as the fused kernel, without terms
+        return cost.float(), twist.float()
+
+    def scene_collision_cost(self, scene, link_points, margin, links=None):
+        """For every installed configuration, the soft collision cost of its tested links against a static scene and
+        its twist gradient per sub-SDF: link_points [S, K, 3] holds K points of every sub-SDF in its own frame, links
+        [S] bool says which sub-SDFs are tested (default: all), and every posed point within `margin` of `scene` (any
+        ObjectFrameSDF in this composition's object frame) adds max(0, margin - d)^2.  Returns (cost [*A],
+        twist_grad [*A, S, 6]) in link_points' dtype on the composition's device -- 0-d / [S, 6] without a
+        configuration batch.  twist_grad[..., s, :] is the derivative of the cost when sub-SDF s alone moves by an
+        object-frame twist (v, w) about the origin.  The definition and routes are those of
+        `query_scene_collision_cost`.  Not a reference operator (an extension), and not autograd; raises ValueError
+        before any device work on wrong shapes, a margin that is not finite or a scene with more than one pose."""
+        shape = () if self.tsf_batch is None else tuple(int(a) for a in self.tsf_batch)
+        out = self.query_scene_collision_cost(scene, link_points, margin, links)
+        return self._deliver(link_points, out, shape, device=matrix_of(self.obj_frame_to_link_frame).device)
+
     def query_into(self, points_in_object_frame, targets, cfg_begin=0, cfg_count=None):
         """`query` whose result slab is stored by the kernel epilogue into several full-size result buffers at once
         (pvb_composed_query_multi): `targets` is a list of (val, grad) pairs, each a float32 tensor or a raw device
