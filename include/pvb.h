@@ -523,6 +523,25 @@ int64_t pvb_compact_workspace(int64_t n);
 int pvb_compact_nonempty(const void *data, int64_t n, int32_t elem_bytes, double empty, void *workspace,
                          int64_t capacity, int64_t *out_index, int64_t *out_count, void *stream);
 
+/* ---- occupancy distance transform: OccupancySDF (sdf.py) ----
+ * occ DEVICE uint8 [nx][ny][nz] (C order, z fastest; nonzero = occupied), dims HOST int32[3] = {nx, ny, nz}, each
+ * 2..1024.  For every voxel c: its site s(c), the voxel of the OTHER state (occupied for a free c, free for an occupied
+ * c) at the smallest squared distance D(c) = |c - s|^2 in integer cell units, ties to the smallest flat C-order index
+ * (exact: integer arithmetic throughout).  Outputs, each DEVICE and each optional (not all NULL):
+ *   out_sqdist int32 [n_vox]  D(c)
+ *   out_site   int32 [n_vox]  flat index of s(c)
+ *   out_table  float [n_vox][4], 16-byte aligned: the CachedSDF record {val, gx, gy, gz} with sigma = +1 for a free
+ *              voxel and -1 for an occupied one, r32 = resolution and q = sqrt_rn(float(D)), every operation rounded to
+ *              nearest once: val = sigma (r32 * (q - 0.5)), g_k = sigma (float(c_k - s_k) / q).  The zero level lies
+ *              on the faces between occupied and free voxels.
+ * A grid without an occupied or without a free voxel has no field: D = -1, site = -1, val = sigma inf, gradient 0.
+ * workspace DEVICE, pvb_occupancy_sdf_workspace(dims) bytes (48 per voxel), 8-byte aligned; nothing is allocated.
+ * PVB_ERR_INVALID before any device work: dims outside 2..1024, a resolution that is not finite and positive, a
+ * missing or short workspace, occ NULL, every output NULL.  pvb_occupancy_sdf_workspace returns -1 for such dims. */
+int64_t pvb_occupancy_sdf_workspace(const int32_t *dims);
+int pvb_occupancy_sdf(const uint8_t *occ, const int32_t *dims, float resolution, void *workspace,
+                      int64_t workspace_bytes, int32_t *out_sqdist, int32_t *out_site, float *out_table, void *stream);
+
 /* ---- rigid transform helpers used by the generic (unfused) composition path ---- */
 /* out[b][i] = xforms[b] applied to pts[i] (pts DEVICE [n_pts][3], out DEVICE [n_tf][n_pts][3]), the FMA chain of the
  * composed kernels' transform; any n_tf >= 0, PVB_ERR_INVALID when n_tf * n_pts * 3 overflows int64 */

@@ -221,6 +221,10 @@ _SIGNATURES = {
     "pvb_mesh_sample": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
                                        ctypes.c_int64, ctypes.c_uint64, ctypes.c_void_p, ctypes.c_void_p,
                                        ctypes.c_void_p]),
+    "pvb_occupancy_sdf_workspace": (ctypes.c_int64, [ctypes.c_void_p]),
+    "pvb_occupancy_sdf": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p,
+                                         ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                         ctypes.c_void_p]),
     "pvb_transform_points": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,
                                             ctypes.c_void_p, ctypes.c_void_p]),
     "pvb_transform_points_paired": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,

@@ -1505,4 +1505,132 @@ __host__ __device__ __forceinline__ void fk_walk(const Plan &plan, const float *
     }
 }
 
+// ---------------------------------------------------------------- occupancy distance transform (pvb_occupancy_sdf)
+// The exact squared Euclidean distance transform of an occupancy grid, carrying each voxel's site: for the sites of
+// one state (occupied, or free), every voxel's nearest site in integer cell units.  Three separable passes, along z,
+// then y, then x; each 1-D pass breaks ties toward the smaller coordinate, so the site of a voxel is the nearest one
+// with the smallest flat C-order index.  Every decision is made in integer arithmetic.
+
+constexpr int kEdtMaxDim = 1024;      // voxels per axis: d <= 3 * 1023^2 is exact in int32 and in fp32
+
+// A voxel's squared distance d to its site and the site's flat index s; {-1, -1}: no site on the (sub-)line.
+struct alignas(8) EdtPair { int d, s; };
+
+__device__ __forceinline__ int edt_hibit(uint32_t w) {      // index of the highest set bit of w != 0
+#ifdef __CUDA_ARCH__
+    return 31 - __clz((int)w);
+#else
+    return 31 - __builtin_clz(w);
+#endif
+}
+
+__device__ __forceinline__ int edt_lobit(uint32_t w) {      // index of the lowest set bit of w != 0
+#ifdef __CUDA_ARCH__
+    return __ffs((int)w) - 1;
+#else
+    return __builtin_ctz(w);
+#endif
+}
+
+// Pass 1 (z): the site nearest to position p of a line whose sites are the set bits of `words` (bit b of word w is
+// position 32 w + b), the left one on a tie; -1 when the line has none.
+__device__ __forceinline__ int edt_line_nearest(const uint32_t *words, int n_words, int p) {
+    const int w0 = p >> 5, b = p & 31;
+    int left = -1, right = -1;
+    const uint32_t lo = words[w0] & (0xffffffffu >> (31 - b)), hi = words[w0] & (0xffffffffu << b);
+    if (lo) {
+        left = 32 * w0 + edt_hibit(lo);
+    } else {
+        for (int w = w0 - 1; w >= 0; --w)
+            if (words[w]) { left = 32 * w + edt_hibit(words[w]); break; }
+    }
+    if (hi) {
+        right = 32 * w0 + edt_lobit(hi);
+    } else {
+        for (int w = w0 + 1; w < n_words; ++w) {
+            if (left >= 0 && 32 * w - p >= p - left) break;       // nothing further right can win
+            if (words[w]) { right = 32 * w + edt_lobit(words[w]); break; }
+        }
+    }
+    if (left < 0 || (right >= 0 && right - p < p - left)) return right;
+    return left;
+}
+
+// Passes 2 and 3 (y, x): one line of n <= 1024 voxels, element i at in[i * stride] / out[i * stride], through the
+// lower envelope of the parabolas (i - v)^2 + f(v) over the line's sites v (Felzenszwalb & Huttenlocher).  The
+// envelope lives in `stk` (entry k at stk[k * stk_stride]: {f << 10 | v, site}; f < 2^21 for the inputs of these two
+// passes); its top entry stays in registers.  The breakpoint between parabolas p < q is
+// ((f_q + q^2) - (f_p + p^2)) / (2 (q - p)): numerator and denominator are exact int32, and two breakpoints are
+// compared by int64 cross-multiplication.  A new parabola removes the top when it takes over at or before the top's
+// own breakpoint, and a voxel on a breakpoint keeps the left parabola: ties go to the smaller coordinate.
+__device__ __forceinline__ void edt_envelope(const EdtPair *in, EdtPair *out, long long stride, int n,
+                                                      EdtPair *stk, long long stk_stride) {
+    int top = -1;                        // index of the register entry (pv, pf, ps); entries below it are in stk
+    int pv = 0, pf = 0, ps = 0;
+    int zn = 0, zd = 1;                  // the top's breakpoint zn / zd (top >= 1)
+    for (int q = 0; q < n; ++q) {
+        const EdtPair e = in[q * stride];
+        if (e.d < 0) continue;
+        int qn = 0, qd = 1;
+        while (top >= 0) {
+            qn = e.d + q * q - pf - pv * pv;
+            qd = 2 * (q - pv);
+            if (top == 0 || (long long)qn * zd > (long long)zn * qd) break;
+            --top;
+            const EdtPair t = stk[top * stk_stride];
+            pv = t.d & 1023; pf = t.d >> 10; ps = t.s;
+            if (top >= 1) {
+                const EdtPair u = stk[(top - 1) * stk_stride];
+                const int uv = u.d & 1023;
+                zn = pf + pv * pv - (u.d >> 10) - uv * uv;
+                zd = 2 * (pv - uv);
+            }
+        }
+        if (top >= 0) {
+            stk[top * stk_stride] = EdtPair{(pf << 10) | pv, ps};
+            zn = qn; zd = qd;
+        }
+        ++top;
+        pv = q; pf = e.d; ps = e.s;
+    }
+    if (top < 0) {
+        for (int i = 0; i < n; ++i) out[i * stride] = EdtPair{-1, -1};
+        return;
+    }
+    stk[top * stk_stride] = EdtPair{(pf << 10) | pv, ps};
+    int k = 0;
+    EdtPair cur = stk[0];
+    int cv = cur.d & 1023, cf = cur.d >> 10;
+    for (int i = 0; i < n; ++i) {
+        while (k < top) {
+            const EdtPair nx = stk[(k + 1) * stk_stride];
+            const int nv = nx.d & 1023, nf = nx.d >> 10;
+            if (nf + nv * nv - cf - cv * cv >= i * 2 * (nv - cv)) break;    // breakpoint >= i: keep the left one
+            ++k; cur = nx; cv = nv; cf = nf;
+        }
+        out[i * stride] = EdtPair{(i - cv) * (i - cv) + cf, cur.s};
+    }
+}
+
+__device__ __forceinline__ float edt_sqrt_rn(float x) {
+#ifdef __CUDA_ARCH__
+    return __fsqrt_rn(x);
+#else
+    return sqrtf(x);                     // IEEE square root, correctly rounded like sqrt.rn.f32
+#endif
+}
+
+// The table record {val, gx, gy, gz} of voxel c (occupied when occ) whose nearest opposite-state voxel s lies at
+// squared distance d: sigma (r (sqrt(d) - 1/2)) and sigma (c - s) / sqrt(d), sigma = -1 for an occupied voxel.  Each
+// operation rounds to nearest once.  d < 0 (no voxel of the other state): sigma inf and a zero gradient.
+__device__ __forceinline__ float4 edt_record(int d, bool occ, int cx, int cy, int cz, int sx, int sy, int sz,
+                                                      float r32) {
+    if (d < 0) return make_float4(occ ? -PVB_INF : PVB_INF, 0.f, 0.f, 0.f);
+    const float q = edt_sqrt_rn((float)d);
+    const float val = __fmul_rn(r32, __fsub_rn(q, 0.5f));
+    const float gx = __fdiv_rn((float)(cx - sx), q), gy = __fdiv_rn((float)(cy - sy), q),
+                gz = __fdiv_rn((float)(cz - sz), q);
+    return occ ? make_float4(-val, -gx, -gy, -gz) : make_float4(val, gx, gy, gz);
+}
+
 }  // namespace pvb

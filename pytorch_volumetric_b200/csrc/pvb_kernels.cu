@@ -4615,3 +4615,132 @@ extern "C" int pvb_transform_points(const float *xforms, int32_t n_tf, const flo
     PVB_CHECK_LAUNCH("pvb_transform_points");
     return PVB_OK;
 }
+
+// ---------------------------------------------------------------- occupancy distance transform (OccupancySDF)
+// Two transforms run side by side, blockIdx.y (or the word set) picking the state: 0 takes the occupied voxels as
+// sites, 1 the free ones.  Each pass writes its EdtPairs for state t at [t * n_vox, (t + 1) * n_vox).
+constexpr int kEdtWarps = 8;            // edt_z_kernel: one line per warp
+constexpr int kEdtLineThreads = 128;    // edt_envelope_kernel: one line per thread
+
+// Pass 1, along the contiguous z axis: a warp reads a line with coalesced byte loads, packs its occupancy into bit
+// words with ballots (shared memory), then every lane looks up the nearest site of each state for its positions.
+__global__ void __launch_bounds__(32 * kEdtWarps) edt_z_kernel(const unsigned char *__restrict__ occ, int nz,
+                                                               long long n_lines, long long n_vox,
+                                                               EdtPair *__restrict__ out) {
+    __shared__ uint32_t words[kEdtWarps][2][kEdtMaxDim / 32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int n_words = (nz + 31) >> 5;
+    for (long long line = (long long)blockIdx.x * kEdtWarps + w; line < n_lines; line += (long long)gridDim.x * kEdtWarps) {
+        const long long base = line * nz;
+        for (int j = 0; j < n_words; ++j) {
+            const int p = 32 * j + lane;
+            const bool in = p < nz;
+            const uint32_t mo = __ballot_sync(0xffffffffu, in && occ[base + p] != 0);
+            const uint32_t mv = __ballot_sync(0xffffffffu, in);
+            if (lane == 0) { words[w][0][j] = mo; words[w][1][j] = mv & ~mo; }
+        }
+        __syncwarp();
+        for (int p = lane; p < nz; p += 32) {
+#pragma unroll
+            for (int t = 0; t < 2; ++t) {
+                const int r = edt_line_nearest(words[w][t], n_words, p);
+                out[t * n_vox + base + p] = r < 0 ? EdtPair{-1, -1} : EdtPair{(p - r) * (p - r), (int)(base + r)};
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// Passes 2 and 3: one thread per line of n voxels spaced `stride` apart (y: stride nz; x: stride ny nz), threads laid
+// along the contiguous z coordinate so that every step's warp accesses are coalesced; the envelope stack of line t
+// is stk[k * n_lines + t], coalesced the same way.
+__global__ void __launch_bounds__(kEdtLineThreads) edt_envelope_kernel(const EdtPair *__restrict__ in,
+                                                                       EdtPair *__restrict__ out,
+                                                                       EdtPair *__restrict__ stk, int n,
+                                                                       long long stride, long long n_lines,
+                                                                       long long n_vox) {
+    const long long t = (long long)blockIdx.x * kEdtLineThreads + threadIdx.x;
+    if (t >= n_lines) return;
+    const long long base = (t / stride) * (stride * n) + t % stride, off = (long long)blockIdx.y * n_vox;
+    edt_envelope(in + off + base, out + off + base, stride, n, stk + off + t, n_lines);
+}
+
+// The outputs of voxel c from the transform of the other state: squared distance, site and table record.
+__global__ void edt_record_kernel(const unsigned char *__restrict__ occ, const EdtPair *__restrict__ edt, int ny,
+                                  int nz, long long n_vox, float r32, int32_t *__restrict__ out_sqdist,
+                                  int32_t *__restrict__ out_site, float4 *__restrict__ out_table) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < n_vox; c += stride) {
+        const bool o = occ[c] != 0;
+        const EdtPair e = edt[(o ? n_vox : 0) + c];
+        if (out_sqdist) out_sqdist[c] = e.d;
+        if (out_site) out_site[c] = e.s;
+        if (out_table) {
+            const int ci = (int)c, cz = ci % nz, cy = (ci / nz) % ny, cx = ci / nz / ny;
+            const int s = e.s < 0 ? 0 : e.s, sz = s % nz, sy = (s / nz) % ny, sx = s / nz / ny;
+            out_table[c] = edt_record(e.d, o, cx, cy, cz, sx, sy, sz, r32);
+        }
+    }
+}
+
+static int edt_check_dims(const char *fn, const int32_t *dims) {
+    if (!dims) { pvb_set_error("%s: invalid argument (dims is null)", fn); return PVB_ERR_INVALID; }
+    for (int k = 0; k < 3; ++k) {
+        if (dims[k] < 2 || dims[k] > kEdtMaxDim) {
+            pvb_set_error("%s: every axis must hold 2..%d voxels (dims=[%d, %d, %d])", fn, kEdtMaxDim, dims[0],
+                          dims[1], dims[2]);
+            return PVB_ERR_INVALID;
+        }
+    }
+    return PVB_OK;
+}
+
+extern "C" int64_t pvb_occupancy_sdf_workspace(const int32_t *dims) {
+    if (edt_check_dims("pvb_occupancy_sdf_workspace", dims)) return -1;
+    // two transforms x (pass buffer A, pass buffer B, envelope stacks), one EdtPair per voxel each
+    return (int64_t)6 * (int64_t)sizeof(EdtPair) * dims[0] * dims[1] * dims[2];
+}
+
+extern "C" int pvb_occupancy_sdf(const uint8_t *occ, const int32_t *dims, float resolution, void *workspace,
+                                 int64_t workspace_bytes, int32_t *out_sqdist, int32_t *out_site, float *out_table,
+                                 void *stream) {
+    const char *fn = "pvb_occupancy_sdf";
+    if (int rc = edt_check_dims(fn, dims)) return rc;
+    if (!(resolution > 0.f) || !isfinite(resolution)) {
+        pvb_set_error("%s: the resolution must be finite and positive (resolution=%g)", fn, (double)resolution);
+        return PVB_ERR_INVALID;
+    }
+    const int64_t need = pvb_occupancy_sdf_workspace(dims);
+    if (!workspace || workspace_bytes < need || (uintptr_t)workspace % alignof(EdtPair)) {
+        pvb_set_error("%s: the workspace must hold pvb_occupancy_sdf_workspace() = %lld bytes, 8-byte aligned "
+                      "(got %lld bytes at %p)", fn, (long long)need, (long long)workspace_bytes, workspace);
+        return PVB_ERR_INVALID;
+    }
+    if (!occ) { pvb_set_error("%s: invalid argument (occ is null)", fn); return PVB_ERR_INVALID; }
+    if (!out_sqdist && !out_site && !out_table) {
+        pvb_set_error("%s: invalid argument (out_sqdist, out_site and out_table are all null)", fn);
+        return PVB_ERR_INVALID;
+    }
+    if ((uintptr_t)out_table % 16) {
+        pvb_set_error("%s: out_table must be 16-byte aligned", fn);
+        return PVB_ERR_INVALID;
+    }
+    const int nx = dims[0], ny = dims[1], nz = dims[2];
+    const long long n_vox = (long long)nx * ny * nz;
+    EdtPair *a = static_cast<EdtPair *>(workspace), *b = a + 2 * n_vox, *stk = b + 2 * n_vox;
+    cudaStream_t s = (cudaStream_t)stream;
+    timing_mark(0, s);
+    const long long z_lines = (long long)nx * ny;
+    edt_z_kernel<<<grid_for((z_lines + kEdtWarps - 1) / kEdtWarps, 1, 8), 32 * kEdtWarps, 0, s>>>(occ, nz, z_lines,
+                                                                                                  n_vox, a);
+    const long long y_lines = n_vox / ny, x_lines = n_vox / nx;
+    edt_envelope_kernel<<<dim3((unsigned)((y_lines + kEdtLineThreads - 1) / kEdtLineThreads), 2), kEdtLineThreads, 0,
+                          s>>>(a, b, stk, ny, nz, y_lines, n_vox);
+    edt_envelope_kernel<<<dim3((unsigned)((x_lines + kEdtLineThreads - 1) / kEdtLineThreads), 2), kEdtLineThreads, 0,
+                          s>>>(b, a, stk, nx, (long long)ny * nz, x_lines, n_vox);
+    edt_record_kernel<<<grid_for(n_vox, 256, 8), 256, 0, s>>>(occ, a, ny, nz, n_vox, resolution, out_sqdist,
+                                                              out_site, reinterpret_cast<float4 *>(out_table));
+    timing_mark(1, s);
+    PVB_CHECK_LAUNCH(fn);
+    return PVB_OK;
+}

@@ -1953,10 +1953,16 @@ class CachedSDF(ObjectFrameSDF):
 
         val = cached_underlying_sdf.to(device=self._cdev, dtype=torch.float32)
         grad = cached_underlying_sdf_grad.to(device=self._cdev, dtype=torch.float32).reshape(-1, 3)
-        self.voxels = GridView(val, range_per_dim, invalid_value=self._fallback_sdf_value_func)
+        self._install_tables(val, grad)
+
+    def _install_tables(self, val, grad, table=None):
+        """Make val [nx, ny, nz] and grad [Nvox, 3] (fp32, on the compute device) the lookup tables over self.ranges,
+        with surface_bounding_box() the box of the bounding-box rule, and build the fused kernels' descriptor.
+        table: the [Nvox, 4] records of val and grad when the caller already holds them."""
+        self.voxels = GridView(val, self.ranges, invalid_value=self._fallback_sdf_value_func)
         self.voxels_grad = grad
         # one 16-byte record {val, gx, gy, gz} per voxel: each lookup is a single 128-bit load
-        self._table = torch.cat([val.reshape(-1, 1), grad], dim=1).contiguous()
+        self._table = torch.cat([val.reshape(-1, 1), grad], dim=1).contiguous() if table is None else table
         self.bb = self.surface_bounding_box().to(device=self._cdev)
         self._desc = self._make_desc()
 
@@ -2149,6 +2155,139 @@ class CachedSDF(ObjectFrameSDF):
         sdf_val = sdf_val.to(device=self._cdev)
         cached_underlying_sdf = sdf_val.reshape([len(coord) for coord in voxels.coords])
         return GridView(cached_underlying_sdf, voxels.range_per_dim, invalid_value=self._fallback_sdf_value_func)
+
+
+def _occupancy_u8(occupancy):
+    """occupancy (bool / uint8 tensor or array [nx, ny, nz]) as a contiguous uint8 tensor on its own device, checked
+    for the shape and the two states pvb_occupancy_sdf needs."""
+    occ = occupancy if torch.is_tensor(occupancy) else torch.as_tensor(np.asarray(occupancy))
+    if occ.dtype not in (torch.bool, torch.uint8):
+        raise ValueError(f"occupancy must be bool or uint8, got {occ.dtype}")
+    if occ.dim() != 3 or not all(2 <= n <= 1024 for n in occ.shape):
+        raise ValueError(f"occupancy must be [nx, ny, nz] with 2..1024 voxels per axis, got {tuple(occ.shape)}")
+    occ = occ.contiguous()
+    occ = occ.view(torch.uint8) if occ.dtype == torch.bool else occ
+    n_occ = int(torch.count_nonzero(occ))
+    if n_occ == 0 or n_occ == occ.numel():
+        raise ValueError("occupancy needs at least one occupied and one free voxel: a grid of one state has no "
+                         "distance field")
+    return occ
+
+
+def _occupancy_sdf(occ, resolution, sqdist=False, site=False, table=False):
+    """pvb_occupancy_sdf over the uint8 grid `occ` (on its CUDA device): the requested outputs, in the order
+    (sqdist int32 [nx, ny, nz], site int32 [nx, ny, nz], table fp32 [Nvox, 4])."""
+    dev = occ.device
+    dims = (ctypes.c_int32 * 3)(*occ.shape)
+    L = nat.lib()
+    with nat.on_device(dev):
+        ws = torch.empty(int(L.pvb_occupancy_sdf_workspace(dims)), dtype=torch.uint8, device=dev)
+        outs = [torch.empty(occ.shape, dtype=torch.int32, device=dev) if sqdist else None,
+                torch.empty(occ.shape, dtype=torch.int32, device=dev) if site else None,
+                torch.empty(occ.numel(), 4, dtype=torch.float32, device=dev) if table else None]
+        nat.check(L.pvb_occupancy_sdf(nat.ptr(occ), dims, float(resolution), nat.ptr(ws), ws.numel(),
+                                      *[nat.ptr(t) for t in outs], nat.stream_ptr(dev)), "pvb_occupancy_sdf")
+    return tuple(t for t in outs if t is not None)
+
+
+def occupancy_distance_transform(occupancy):
+    """Exact squared Euclidean distance transform of an occupancy grid, with the site of every voxel.
+
+    occupancy: bool / uint8 [nx, ny, nz] (nonzero = occupied), 2..1024 voxels per axis, with both states present.
+    Returns (D, site) on the occupancy's device: D int32 [nx, ny, nz] is the squared distance, in cell units, from each
+    voxel to the nearest voxel of the other state (free voxels measure to occupied ones and occupied voxels to free
+    ones); site int64 [nx, ny, nz] is that voxel's flat C-order index, the smallest index among equally near ones --
+    the role of scipy.ndimage.distance_transform_edt's return_indices.  Computed on the GPU, in integer arithmetic."""
+    src = occupancy.device if torch.is_tensor(occupancy) else torch.device("cpu")
+    occ = _occupancy_u8(occupancy)
+    d, site = _occupancy_sdf(occ.to(nat.compute_device(src)), 1.0, sqdist=True, site=True)
+    return nat.deliver(d, src), nat.deliver(site.long(), src)
+
+
+class OccupancySDF(CachedSDF):
+    """Signed distance table of an occupancy grid, built on the GPU by an exact Euclidean distance transform.
+
+    Each voxel's value is its distance to the nearest voxel of the other state, minus half a cell, negative inside:
+    val = sigma r (sqrt(D) - 1/2) with sigma = -1 for an occupied voxel, so the zero level lies on the faces between
+    occupied and free voxels, and the gradient is sigma (c - site) / sqrt(D).  The table is a CachedSDF table on the
+    same lattice (range snapped by get_divisible_range_by_resolution, voxel i at lo + i r), looked up with the
+    bounding-box rule outside the range, the box being that of the occupied voxel centres widened by r / 2.  So an
+    OccupancySDF serves everywhere a CachedSDF does: as a scene (RobotSDF.scene_clearance), as a ComposedSDF
+    sub-SDF and as batch_chamfer_dist's obj_sdf, on the fused kernels.
+
+    A cloud sampled on surfaces marks only the surfaces occupied: the inside of a solid stays free and its values are
+    positive there.  A signed interior needs filled occupancy.
+
+    :param occupancy: VoxelGrid (its resolution and range are used), or a bool / uint8 tensor [nx, ny, nz] together
+        with resolution and range_per_dim; its shape must be the lattice those imply.  Both states must be present.
+    :param interpolation: "nearest" or "trilinear", as for CachedSDF
+    :param device: device results are returned on (the tables always live on the GPU)
+    There is no ground-truth SDF and no cache file; the bounding-box rule is the only out-of-range rule."""
+
+    def __init__(self, occupancy, resolution=None, range_per_dim=None, interpolation="nearest", device="cpu"):
+        if interpolation not in ("nearest", "trilinear"):
+            raise ValueError(f"interpolation must be 'nearest' or 'trilinear', got {interpolation!r}")
+        if isinstance(occupancy, VoxelGrid):
+            if resolution is not None or range_per_dim is not None:
+                raise ValueError("a VoxelGrid carries its own resolution and range; pass neither")
+            resolution, range_per_dim, occupancy = occupancy.resolution, occupancy.range_per_dim, \
+                occupancy.get_voxel_values()
+        elif resolution is None or range_per_dim is None:
+            raise ValueError("an occupancy tensor needs resolution and range_per_dim")
+        if not (math.isfinite(float(resolution)) and float(resolution) > 0):
+            raise ValueError(f"resolution must be finite and positive, got {resolution}")
+        self.interpolation = interpolation
+        self.device = device
+        self.out_of_bounds_strategy = OutOfBoundsStrategy.BOUNDING_BOX
+        self.gt_sdf = None
+        self.resolution = resolution
+        self.debug_check_sdf = False
+        self.ranges = get_divisible_range_by_resolution(resolution, range_per_dim)
+        self.name = f"occupancy {resolution} {tuple(self.ranges)}"
+        coords, _ = get_coordinates_and_points_in_grid(resolution, self.ranges, get_points=False)
+        shape = tuple(len(c) for c in coords)
+        if tuple(occupancy.shape) != shape:
+            raise ValueError(f"occupancy of shape {tuple(occupancy.shape)} does not match the lattice of resolution "
+                             f"{resolution} over {self.ranges}, {shape}")
+        occ = _occupancy_u8(occupancy)
+        self._cdev = nat.compute_device(device)
+        occ = occ.to(self._cdev)
+        self.occupancy = occ.view(torch.bool)
+        (table,) = _occupancy_sdf(occ, resolution, table=True)
+        box = np.empty((3, 2))
+        for k in range(3):
+            idx = torch.nonzero(self.occupancy.any(dim=tuple(a for a in range(3) if a != k))).reshape(-1)
+            lo = float(min(self.ranges[k]))
+            box[k] = (lo + int(idx[0]) * resolution - 0.5 * resolution, lo + int(idx[-1]) * resolution + 0.5 * resolution)
+        self._surface_box = box
+        self._install_tables(table[:, 0].reshape(shape).contiguous(), table[:, 1:].contiguous(), table=table)
+
+    @classmethod
+    def from_points(cls, points, resolution, range_per_dim, interpolation="nearest", device="cpu"):
+        """OccupancySDF of the voxels the points [N, 3] fall into (pvb_voxel_scatter, as
+        VoxelGrid(resolution, range_per_dim, dtype=torch.bool)[points] = True); points outside the range are dropped."""
+        cdev = nat.compute_device(device)
+        grid = VoxelGrid(resolution, range_per_dim, dtype=torch.bool, device=cdev)
+        grid[nat.as_f32_points(points, cdev)] = True
+        return cls(grid, interpolation=interpolation, device=device)
+
+    def surface_bounding_box(self, padding=0., padding_ratio=0.):
+        """The box of the occupied voxel centres widened by half a cell, inflated by padding + padding_ratio * extent
+        (fp64)."""
+        box = self._surface_box.copy()
+        grow = padding + padding_ratio * (box[:, 1] - box[:, 0])
+        box[:, 0] -= grow
+        box[:, 1] += grow
+        return torch.from_numpy(box)
+
+    def _fallback_sdf_value_func(self, points, *args, **kwargs):
+        """Values outside the range (GridView lookups of self.voxels): the bounding-box rule of __call__."""
+        return self._lookup(points)[1]
+
+    def get_voxel_view(self, voxels: VoxelGrid = None, dtype=torch.float, device='cpu') -> GridView:
+        if voxels is None:
+            return self.voxels
+        return ObjectFrameSDF.get_voxel_view(self, voxels, dtype=dtype, device=device)
 
 
 def sample_mesh_points(obj_factory: ObjectFactory = None, num_points=100, seed=0, name="",
