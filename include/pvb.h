@@ -542,6 +542,37 @@ int64_t pvb_occupancy_sdf_workspace(const int32_t *dims);
 int pvb_occupancy_sdf(const uint8_t *occ, const int32_t *dims, float resolution, void *workspace,
                       int64_t workspace_bytes, int32_t *out_sqdist, int32_t *out_site, float *out_table, void *stream);
 
+/* ---- depth images: depth_to_points, depth_occupancy, OccupancySDF.from_depth (sdf.py) ----
+ * depth DEVICE float [V][H][W], z-depth in metres, row-major; V 1..64, H and W 1..32768.  A pixel is valid when its
+ * depth d is finite, d > 0 and d <= max_depth (+inf allowed); any other pixel carries no information.
+ * intrinsics HOST float [V][4] = {fx, fy, cx, cy}: fx, fy finite and positive, cx, cy finite.  The camera follows the
+ * OpenCV convention (x right, y down, z forward); pixel (row i, column j) is centred at u = j, v = i.
+ * cam_to_world / world_to_cam HOST float [V][12]: the rows [R | t] of a rigid transform, finite.
+ * Every fp32 operation rounds to nearest once, in the order written; (float)i is exact.
+ *
+ * pvb_depth_points: out_points DEVICE float [V][H][W][3].  A valid pixel (i, j) of depth d gives
+ *   x = ((float)j - cx) * d / fx,  y = ((float)i - cy) * d / fy  (subtract, multiply, divide), p_cam = (x, y, d),
+ *   world = R p_cam + t, row k as fma(R_k0, x, fma(R_k1, y, fma(R_k2, d, t_k))) (composed_xform);
+ * an invalid pixel gives (NaN, NaN, NaN).
+ *
+ * pvb_depth_carve: out_state DEVICE uint8 [nx][ny][nz] (C order, z fastest), dims HOST int32[3] each 2..1024, lo HOST
+ * float[3] finite.  Voxel (ix, iy, iz) has its centre c_k = lo_k + (float)i_k * resolution (multiply, then add).  Per
+ * view, p = world_to_cam c (the same FMA chain); the view says nothing when p.z <= 0, when the pixel
+ *   (row floor(fy * p.y / p.z + cy + 0.5), column floor(fx * p.x / p.z + cx + 0.5))  (multiply, divide, add, add)
+ * lies outside the image, or when that pixel is invalid; otherwise it says free when p.z < d - free_margin.  The
+ * voxel's state is 0 (free) when any view says free and 2 (unknown) otherwise; the order of the views does not
+ * matter.  Occupied voxels (1) are written afterwards by pvb_voxel_scatter of the valid points: hits win over free.
+ *
+ * PVB_ERR_INVALID before any device work: V, H or W out of range, null pointers, a focal length that is not finite
+ * and positive, a principal point or transform entry that is not finite, max_depth <= 0 or NaN; for the carve also
+ * dims outside 2..1024, a resolution that is not finite and positive, a free_margin that is negative or not finite
+ * and a lo that is not finite. */
+int pvb_depth_points(const float *depth, int32_t V, int32_t H, int32_t W, const float *intrinsics,
+                     const float *cam_to_world, float max_depth, float *out_points, void *stream);
+int pvb_depth_carve(const float *depth, int32_t V, int32_t H, int32_t W, const float *intrinsics,
+                    const float *world_to_cam, float max_depth, float free_margin, const float *lo, float resolution,
+                    const int32_t *dims, uint8_t *out_state, void *stream);
+
 /* ---- rigid transform helpers used by the generic (unfused) composition path ---- */
 /* out[b][i] = xforms[b] applied to pts[i] (pts DEVICE [n_pts][3], out DEVICE [n_tf][n_pts][3]), the FMA chain of the
  * composed kernels' transform; any n_tf >= 0, PVB_ERR_INVALID when n_tf * n_pts * 3 overflows int64 */

@@ -225,6 +225,13 @@ _SIGNATURES = {
     "pvb_occupancy_sdf": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p,
                                          ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                          ctypes.c_void_p]),
+    "pvb_depth_points": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p,
+                                        ctypes.c_void_p]),
+    "pvb_depth_carve": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                       ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_float,
+                                       ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p,
+                                       ctypes.c_void_p]),
     "pvb_transform_points": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,
                                             ctypes.c_void_p, ctypes.c_void_p]),
     "pvb_transform_points_paired": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,

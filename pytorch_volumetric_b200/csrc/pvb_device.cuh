@@ -1633,4 +1633,47 @@ __device__ __forceinline__ float4 edt_record(int d, bool occ, int cx, int cy, in
     return occ ? make_float4(-val, -gx, -gy, -gz) : make_float4(val, gx, gy, gz);
 }
 
+// ---------------------------------------------------------------- depth images (pvb_depth_points, pvb_depth_carve)
+// OpenCV pinhole camera: x right, y down, z forward; pixel (row i, column j) centred at u = j, v = i.  `cam` holds
+// {fx, fy, cx, cy}; r0..r2 are the rows [R | t] of a rigid transform.  Every fp32 operation rounds to nearest once,
+// in the order written (include/pvb.h states it).
+
+constexpr int kDepthMaxViews = 64;
+
+// A depth reading carries information when it is finite, positive and at most max_depth (NaN fails every test).
+__device__ __forceinline__ bool depth_valid(float d, float max_depth) {
+    return d > 0.f && d <= max_depth && d < PVB_INF;
+}
+
+// The world point of pixel (i, j) at valid z-depth d: p_cam = ((j - cx) d / fx, (i - cy) d / fy, d), then
+// world = [R | t] p_cam with composed_xform's FMA chain.
+__device__ __forceinline__ f3 depth_point(int i, int j, float d, const float4 &cam, const float4 &r0,
+                                          const float4 &r1, const float4 &r2) {
+    const float x = __fdiv_rn(__fmul_rn(__fsub_rn((float)j, cam.z), d), cam.x);
+    const float y = __fdiv_rn(__fmul_rn(__fsub_rn((float)i, cam.w), d), cam.y);
+    return composed_xform(r0, r1, r2, mk3(x, y, d));
+}
+
+// The centre of voxel (ix, iy, iz) of the lattice lo + i r: c_k = lo_k + float(i_k) * r, product then sum.
+__device__ __forceinline__ f3 depth_voxel_centre(const float *lo, float r, int ix, int iy, int iz) {
+    return mk3(__fadd_rn(lo[0], __fmul_rn((float)ix, r)), __fadd_rn(lo[1], __fmul_rn((float)iy, r)),
+               __fadd_rn(lo[2], __fmul_rn((float)iz, r)));
+}
+
+// Whether one view says the voxel with centre c is free.  r0..r2 map the world to the camera.  The view says nothing
+// when the centre is not in front of the camera (z <= 0), when its pixel (floor(fy y / z + cy + 0.5),
+// floor(fx x / z + cx + 0.5)) lies outside the H x W image, or when that pixel is invalid; otherwise it says free
+// when z < d - margin (and unseen when not).
+__device__ __forceinline__ bool depth_says_free(const float *depth, int H, int W, const float4 &cam,
+                                                const float4 &r0, const float4 &r1, const float4 &r2, f3 c,
+                                                float max_depth, float margin) {
+    const f3 p = composed_xform(r0, r1, r2, c);
+    if (!(p.z > 0.f)) return false;
+    const float u = floorf(__fadd_rn(__fadd_rn(__fdiv_rn(__fmul_rn(cam.x, p.x), p.z), cam.z), 0.5f));
+    const float v = floorf(__fadd_rn(__fadd_rn(__fdiv_rn(__fmul_rn(cam.y, p.y), p.z), cam.w), 0.5f));
+    if (!(u >= 0.f && u < (float)W && v >= 0.f && v < (float)H)) return false;
+    const float d = depth[(long long)(int)v * W + (int)u];
+    return depth_valid(d, max_depth) && p.z < __fsub_rn(d, margin);
+}
+
 }  // namespace pvb

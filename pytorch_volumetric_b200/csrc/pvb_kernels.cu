@@ -4744,3 +4744,146 @@ extern "C" int pvb_occupancy_sdf(const uint8_t *occ, const int32_t *dims, float 
     PVB_CHECK_LAUNCH(fn);
     return PVB_OK;
 }
+
+// ---------------------------------------------------------------- depth images (depth_to_points, depth_occupancy)
+// The view parameters travel as one __grid_constant__ parameter: per view {fx, fy, cx, cy} and the three rows of a
+// rigid transform (camera -> world for the points, world -> camera for the carve).
+struct DepthViews {
+    float4 cam[kDepthMaxViews];
+    float4 rows[kDepthMaxViews][3];
+};
+constexpr int kDepthMaxSide = 32768;
+constexpr int kDepthThreads = 256;
+
+// One thread per pixel, pixels in row-major order (the depth image's own layout).
+__global__ void __launch_bounds__(kDepthThreads) depth_points_kernel(const float *__restrict__ depth, int H, int W,
+                                                                    long long n_px,
+                                                                    const __grid_constant__ DepthViews views,
+                                                                    float max_depth, float *__restrict__ out) {
+    const long long stride = (long long)gridDim.x * blockDim.x, hw = (long long)H * W;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n_px; t += stride) {
+        const int v = (int)(t / hw), pix = (int)(t - v * hw), i = pix / W, j = pix - i * W;
+        const float d = depth[t];
+        f3 p = mk3(__int_as_float(0x7fc00000), __int_as_float(0x7fc00000), __int_as_float(0x7fc00000));
+        if (depth_valid(d, max_depth))
+            p = depth_point(i, j, d, views.cam[v], views.rows[v][0], views.rows[v][1], views.rows[v][2]);
+        out[3 * t] = p.x; out[3 * t + 1] = p.y; out[3 * t + 2] = p.z;
+    }
+}
+
+// One thread per voxel, z fastest, so that neighbouring threads gather neighbouring pixels.  The view parameters are
+// staged in shared memory once per block.  A voxel stops at its first free view: the result is an OR over the views.
+__global__ void __launch_bounds__(kDepthThreads) depth_carve_kernel(const float *__restrict__ depth, int n_views,
+                                                                   int H, int W,
+                                                                   const __grid_constant__ DepthViews views,
+                                                                   float max_depth, float margin, float lo_x,
+                                                                   float lo_y, float lo_z, float r, int ny, int nz,
+                                                                   long long n_vox, uint8_t *__restrict__ out) {
+    __shared__ float4 s_cam[kDepthMaxViews], s_rows[kDepthMaxViews][3];
+    for (int k = threadIdx.x; k < n_views; k += blockDim.x) {
+        s_cam[k] = views.cam[k];
+        s_rows[k][0] = views.rows[k][0]; s_rows[k][1] = views.rows[k][1]; s_rows[k][2] = views.rows[k][2];
+    }
+    __syncthreads();
+    const float lo[3] = {lo_x, lo_y, lo_z};
+    const long long stride = (long long)gridDim.x * blockDim.x, hw = (long long)H * W;
+    for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < n_vox; c += stride) {
+        const int ci = (int)c, iz = ci % nz, iy = (ci / nz) % ny, ix = ci / nz / ny;
+        const f3 x = depth_voxel_centre(lo, r, ix, iy, iz);
+        uint8_t state = 2;
+        for (int v = 0; v < n_views; ++v) {
+            if (depth_says_free(depth + v * hw, H, W, s_cam[v], s_rows[v][0], s_rows[v][1], s_rows[v][2], x,
+                                max_depth, margin)) {
+                state = 0;
+                break;
+            }
+        }
+        out[c] = state;
+    }
+}
+
+// The checks both entry points share; fills `views` from the HOST intrinsics and rows.
+static int depth_check_views(const char *fn, const float *depth, int32_t V, int32_t H, int32_t W,
+                             const float *intrinsics, const float *rows, float max_depth, DepthViews &views) {
+    if (V < 1 || V > kDepthMaxViews || H < 1 || H > kDepthMaxSide || W < 1 || W > kDepthMaxSide) {
+        pvb_set_error("%s: V must be 1..%d and H, W 1..%d (V=%d, H=%d, W=%d)", fn, kDepthMaxViews, kDepthMaxSide, V,
+                      H, W);
+        return PVB_ERR_INVALID;
+    }
+    if (!depth || !intrinsics || !rows) {
+        pvb_set_error("%s: invalid argument (depth, intrinsics or the transforms are null)", fn);
+        return PVB_ERR_INVALID;
+    }
+    if (!(max_depth > 0.f)) {
+        pvb_set_error("%s: max_depth must be positive (max_depth=%g)", fn, (double)max_depth);
+        return PVB_ERR_INVALID;
+    }
+    for (int v = 0; v < V; ++v) {
+        const float *k = intrinsics + 4 * v;
+        if (!(k[0] > 0.f && k[1] > 0.f) || !isfinite(k[0]) || !isfinite(k[1]) || !isfinite(k[2]) || !isfinite(k[3])) {
+            pvb_set_error("%s: view %d: the focal lengths must be finite and positive and the principal point finite "
+                          "(fx=%g, fy=%g, cx=%g, cy=%g)", fn, v, (double)k[0], (double)k[1], (double)k[2],
+                          (double)k[3]);
+            return PVB_ERR_INVALID;
+        }
+        for (int e = 0; e < 12; ++e) {
+            if (!isfinite(rows[12 * v + e])) {
+                pvb_set_error("%s: view %d: the transform is not finite", fn, v);
+                return PVB_ERR_INVALID;
+            }
+        }
+        views.cam[v] = make_float4(k[0], k[1], k[2], k[3]);
+        for (int q = 0; q < 3; ++q) {
+            const float *m = rows + 12 * v + 4 * q;
+            views.rows[v][q] = make_float4(m[0], m[1], m[2], m[3]);
+        }
+    }
+    return PVB_OK;
+}
+
+extern "C" int pvb_depth_points(const float *depth, int32_t V, int32_t H, int32_t W, const float *intrinsics,
+                                const float *cam_to_world, float max_depth, float *out_points, void *stream) {
+    const char *fn = "pvb_depth_points";
+    DepthViews views = {};
+    if (int rc = depth_check_views(fn, depth, V, H, W, intrinsics, cam_to_world, max_depth, views)) return rc;
+    if (!out_points) { pvb_set_error("%s: invalid argument (out_points is null)", fn); return PVB_ERR_INVALID; }
+    const long long n_px = (long long)V * H * W;
+    cudaStream_t s = (cudaStream_t)stream;
+    timing_mark(0, s);
+    depth_points_kernel<<<grid_for(n_px, kDepthThreads, 8), kDepthThreads, 0, s>>>(depth, H, W, n_px, views,
+                                                                                   max_depth, out_points);
+    timing_mark(1, s);
+    PVB_CHECK_LAUNCH(fn);
+    return PVB_OK;
+}
+
+extern "C" int pvb_depth_carve(const float *depth, int32_t V, int32_t H, int32_t W, const float *intrinsics,
+                               const float *world_to_cam, float max_depth, float free_margin, const float *lo,
+                               float resolution, const int32_t *dims, uint8_t *out_state, void *stream) {
+    const char *fn = "pvb_depth_carve";
+    DepthViews views = {};
+    if (int rc = depth_check_views(fn, depth, V, H, W, intrinsics, world_to_cam, max_depth, views)) return rc;
+    if (int rc = edt_check_dims(fn, dims)) return rc;
+    if (!(resolution > 0.f) || !isfinite(resolution)) {
+        pvb_set_error("%s: the resolution must be finite and positive (resolution=%g)", fn, (double)resolution);
+        return PVB_ERR_INVALID;
+    }
+    if (!(free_margin >= 0.f) || !isfinite(free_margin)) {
+        pvb_set_error("%s: free_margin must be finite and non-negative (free_margin=%g)", fn, (double)free_margin);
+        return PVB_ERR_INVALID;
+    }
+    if (!lo || !out_state) { pvb_set_error("%s: invalid argument (lo or out_state is null)", fn); return PVB_ERR_INVALID; }
+    if (!isfinite(lo[0]) || !isfinite(lo[1]) || !isfinite(lo[2])) {
+        pvb_set_error("%s: the lattice origin lo must be finite", fn);
+        return PVB_ERR_INVALID;
+    }
+    const long long n_vox = (long long)dims[0] * dims[1] * dims[2];
+    cudaStream_t s = (cudaStream_t)stream;
+    timing_mark(0, s);
+    depth_carve_kernel<<<grid_for(n_vox, kDepthThreads, 8), kDepthThreads, 0, s>>>(
+        depth, V, H, W, views, max_depth, free_margin, lo[0], lo[1], lo[2], resolution, dims[1], dims[2], n_vox,
+        out_state);
+    timing_mark(1, s);
+    PVB_CHECK_LAUNCH(fn);
+    return PVB_OK;
+}

@@ -31,7 +31,7 @@ import torch
 
 from . import _native as nat
 from . import meshio
-from .transforms import Transform3d, matrix_of
+from .transforms import Transform3d, invert_rigid, matrix_of
 from .voxel import (GridView, VoxelGrid, get_coordinates_and_points_in_grid, get_divisible_range_by_resolution,
                     nonempty_indices, range_dtype)
 
@@ -2271,6 +2271,27 @@ class OccupancySDF(CachedSDF):
         grid[nat.as_f32_points(points, cdev)] = True
         return cls(grid, interpolation=interpolation, device=device)
 
+    @classmethod
+    def from_depth(cls, depth, K, cam_to_world, resolution, range_per_dim, unknown="occupied", max_depth=math.inf,
+                   free_margin=None, interpolation="nearest", device="cpu"):
+        """OccupancySDF of the scene that depth images see (depth_occupancy's state grid).
+
+        unknown="occupied" (the default) counts the voxels no view saw as occupied, as planners do: solids are
+        negative inside.  unknown="free" counts only the voxels a valid pixel's point falls into as occupied, which
+        gives the same occupancy and table as from_points(points[valid]) with the same resolution and range.
+        The other arguments are depth_occupancy's, plus interpolation and device as for OccupancySDF."""
+        if unknown not in ("occupied", "free"):
+            raise ValueError(f"unknown must be 'occupied' or 'free', got {unknown!r}")
+        if interpolation not in ("nearest", "trilinear"):
+            raise ValueError(f"interpolation must be 'nearest' or 'trilinear', got {interpolation!r}")
+        views = _depth_views(depth, K, cam_to_world, max_depth)
+        lattice = _depth_lattice(resolution, range_per_dim, free_margin)
+        cdev = nat.compute_device(device)
+        state = _depth_state(views, lattice, cdev)
+        grid = VoxelGrid(resolution, range_per_dim, dtype=torch.bool, device=cdev)
+        grid.get_voxel_values().copy_(state == 1 if unknown == "free" else state != 0)
+        return cls(grid, interpolation=interpolation, device=device)
+
     def surface_bounding_box(self, padding=0., padding_ratio=0.):
         """The box of the occupied voxel centres widened by half a cell, inflated by padding + padding_ratio * extent
         (fp64)."""
@@ -2288,6 +2309,142 @@ class OccupancySDF(CachedSDF):
         if voxels is None:
             return self.voxels
         return ObjectFrameSDF.get_voxel_view(self, voxels, dtype=dtype, device=device)
+
+
+# ---------------------------------------------------------------- depth images
+class _DepthViews(NamedTuple):
+    depth: torch.Tensor         # fp32 [V, H, W], on the caller's device
+    intrinsics: np.ndarray      # fp32 [V, 4] = fx, fy, cx, cy
+    cam_to_world: torch.Tensor  # fp64 [V, 4, 4], host
+    max_depth: float
+
+
+def _depth_views(depth, K, cam_to_world, max_depth):
+    """Check depth_to_points' / depth_occupancy's view arguments (ValueError, before any device work)."""
+    d = depth if torch.is_tensor(depth) else torch.as_tensor(np.asarray(depth))
+    if d.dtype != torch.float32:
+        raise ValueError(f"depth must be float32 metres, got {d.dtype}")
+    if d.dim() != 3 or not (1 <= d.shape[0] <= 64 and 1 <= d.shape[1] <= 32768 and 1 <= d.shape[2] <= 32768):
+        raise ValueError(f"depth must be [V, H, W] with V in 1..64 and H, W in 1..32768, got {tuple(d.shape)}")
+    V = d.shape[0]
+    k = torch.as_tensor(np.asarray(K.detach().cpu() if torch.is_tensor(K) else K, dtype=np.float64))
+    if k.shape == (3, 3):
+        k = k.expand(V, 3, 3)
+    if k.shape != (V, 3, 3):
+        raise ValueError(f"K must be [3, 3] or [V, 3, 3] with V = {V}, got {tuple(k.shape)}")
+    if (k[:, 0, 1] != 0).any() or (k[:, 1, 0] != 0).any() or (k[:, 2] != torch.tensor([0., 0., 1.],
+                                                                                         dtype=k.dtype)).any():
+        raise ValueError("K must be a pinhole matrix [[fx, 0, cx], [0, fy, cy], [0, 0, 1]]: no skew, bottom row 0 0 1")
+    fx, fy, cx, cy = k[:, 0, 0], k[:, 1, 1], k[:, 0, 2], k[:, 1, 2]
+    if not (torch.isfinite(k).all() and (fx > 0).all() and (fy > 0).all()):
+        raise ValueError("K must be finite, with positive focal lengths")
+    intr = torch.stack([fx, fy, cx, cy], 1).numpy().astype(np.float32)
+    if not (np.isfinite(intr).all() and (intr[:, :2] > 0).all()):
+        raise ValueError("K's entries must be finite and its focal lengths positive in float32")
+    m = matrix_of(cam_to_world) if isinstance(cam_to_world, Transform3d) else cam_to_world
+    m = torch.as_tensor(np.asarray(m.detach().cpu() if torch.is_tensor(m) else m, dtype=np.float64))
+    if m.shape != (V, 4, 4):
+        raise ValueError(f"cam_to_world must hold one 4x4 transform per view, [{V}, 4, 4], got {tuple(m.shape)}")
+    R = m[:, :3, :3]
+    if not (torch.isfinite(m).all() and (m[:, 3] == torch.tensor([0., 0., 0., 1.], dtype=m.dtype)).all()
+            and (R @ R.transpose(1, 2) - torch.eye(3, dtype=m.dtype)).abs().max() < 1e-5
+            and (torch.linalg.det(R) > 0).all()):
+        raise ValueError("cam_to_world must be finite rigid transforms: a rotation, a translation, bottom row 0 0 0 1")
+    max_depth = float(max_depth)
+    if not max_depth > 0:
+        raise ValueError(f"max_depth must be positive (+inf allowed), got {max_depth}")
+    return _DepthViews(d, intr, m, max_depth)
+
+
+def _depth_lattice(resolution, range_per_dim, free_margin):
+    """(resolution, free_margin) checked, free_margin defaulting to half a cell diagonal, sqrt(3) r / 2; the lattice
+    must hold 2..1024 voxels per axis."""
+    resolution = float(resolution)
+    if not (math.isfinite(resolution) and resolution > 0):
+        raise ValueError(f"resolution must be finite and positive, got {resolution}")
+    margin = math.sqrt(3.0) * resolution / 2 if free_margin is None else float(free_margin)
+    if not (math.isfinite(margin) and margin >= 0):
+        raise ValueError(f"free_margin must be finite and non-negative, got {free_margin}")
+    coords, _ = get_coordinates_and_points_in_grid(resolution, get_divisible_range_by_resolution(resolution,
+                                                                                                 range_per_dim),
+                                                   get_points=False)
+    shape = tuple(len(c) for c in coords)
+    if len(shape) != 3 or not all(2 <= n <= 1024 for n in shape):
+        raise ValueError(f"the lattice of resolution {resolution} over {range_per_dim} must hold 2..1024 voxels per "
+                         f"axis, got {shape}")
+    return resolution, range_per_dim, margin
+
+
+def _depth_points(views, d, cdev):
+    """pvb_depth_points of the depth images d (views.depth on cdev): (points fp32 [V, H, W, 3], valid bool
+    [V, H, W]), both on cdev."""
+    V, H, W = d.shape
+    c2w = (ctypes.c_float * (12 * V))(*views.cam_to_world[:, :3].to(torch.float32).reshape(-1).tolist())
+    intr = (ctypes.c_float * (4 * V))(*views.intrinsics.reshape(-1).tolist())
+    with nat.on_device(cdev):
+        out = torch.empty(V, H, W, 3, dtype=torch.float32, device=cdev)
+        nat.check(nat.lib().pvb_depth_points(nat.ptr(d), V, H, W, intr, c2w, views.max_depth, nat.ptr(out),
+                                             nat.stream_ptr(cdev)), "pvb_depth_points")
+    valid = (d > 0) & (d <= views.max_depth) & torch.isfinite(d)
+    return out, valid
+
+
+def _depth_state(views, lattice, cdev):
+    """The uint8 state grid [nx, ny, nz] on cdev: pvb_depth_carve writes 0 (free) or 2 (unknown), then the scatter of
+    the valid points (VoxelGrid(...)[points] = True, pvb_voxel_scatter) writes 1 (occupied)."""
+    resolution, range_per_dim, margin = lattice
+    d = views.depth.to(cdev).contiguous()
+    points, valid = _depth_points(views, d, cdev)
+    V, H, W = d.shape
+    grid = VoxelGrid(resolution, range_per_dim, dtype=torch.bool, device=cdev)
+    state = grid.get_voxel_values().view(torch.uint8)
+    w2c = (ctypes.c_float * (12 * V))(*invert_rigid(views.cam_to_world)[:, :3].to(torch.float32).reshape(-1).tolist())
+    intr = (ctypes.c_float * (4 * V))(*views.intrinsics.reshape(-1).tolist())
+    lo = (ctypes.c_float * 3)(*[float(min(r)) for r in grid.range_per_dim])
+    dims = (ctypes.c_int32 * 3)(*state.shape)
+    with nat.on_device(cdev):
+        nat.check(nat.lib().pvb_depth_carve(nat.ptr(d), V, H, W, intr, w2c, views.max_depth, margin, lo, resolution,
+                                            dims, nat.ptr(state), nat.stream_ptr(cdev)), "pvb_depth_carve")
+    grid[points[valid]] = True
+    return state
+
+
+def depth_to_points(depth, K, cam_to_world, max_depth=math.inf):
+    """Back-project depth images to world points on the GPU (pvb_depth_points).
+
+    depth: float32 [V, H, W], z-depth in metres, row-major; V up to 64.  K: [3, 3] or [V, 3, 3] pinhole intrinsics
+    (fx = K[0, 0], fy = K[1, 1], cx = K[0, 2], cy = K[1, 2]; any skew or a bottom row other than 0 0 1 is refused).
+    cam_to_world: Transform3d or [V, 4, 4] rigid camera-to-world transforms.  The camera follows the OpenCV
+    convention (x right, y down, z forward) with pixel (row i, column j) centred at u = j, v = i.
+    A pixel is valid when its depth d is finite, d > 0 and d <= max_depth; write 0 where a pixel should be ignored
+    (the robot's own body, say).  A valid pixel gives p_cam = ((j - cx) d / fx, (i - cy) d / fy, d) and the point
+    cam_to_world p_cam, in fp32 (the operation order is in include/pvb.h); an invalid one gives NaN.
+    Returns (points float32 [V, H, W, 3], valid bool [V, H, W]) on depth's device."""
+    views = _depth_views(depth, K, cam_to_world, max_depth)
+    src = views.depth.device
+    cdev = nat.compute_device(src)
+    points, valid = _depth_points(views, views.depth.to(cdev).contiguous(), cdev)
+    return nat.deliver(points, src), nat.deliver(valid, src)
+
+
+def depth_occupancy(depth, K, cam_to_world, resolution, range_per_dim, max_depth=math.inf, free_margin=None):
+    """Fuse depth images into an occupancy state grid on the GPU (pvb_depth_carve, then pvb_voxel_scatter).
+
+    The grid is the lattice OccupancySDF uses (range snapped by get_divisible_range_by_resolution, voxel i centred at
+    lo + i r in fp32), 2..1024 voxels per axis.  The depth, K, cam_to_world and max_depth arguments are
+    depth_to_points'.  Each voxel is
+      1 occupied  when a valid pixel's back-projected point falls into it (the VoxelGrid scatter from_points uses);
+      0 free      otherwise, when any view says free: the voxel centre c is in front of the camera, its pixel
+                  (floor(fy y / z + cy + 0.5), floor(fx x / z + cx + 0.5)) of c's camera coordinates (x, y, z) lies in
+                  the image and is valid, and z < d - free_margin;
+      2 unknown   otherwise: no view saw it.
+    free_margin defaults to sqrt(3) r / 2, half a cell diagonal, so that a voxel is carved only when its whole cube
+    lies in front of the surface along that pixel's ray.  The result depends on neither the view order nor the thread
+    order.  Returns uint8 [nx, ny, nz] on depth's device."""
+    views = _depth_views(depth, K, cam_to_world, max_depth)
+    lattice = _depth_lattice(resolution, range_per_dim, free_margin)
+    src = views.depth.device
+    return nat.deliver(_depth_state(views, lattice, nat.compute_device(src)), src)
 
 
 def sample_mesh_points(obj_factory: ObjectFactory = None, num_points=100, seed=0, name="",

@@ -41,9 +41,7 @@ def _boxes(boxes, spheres=()):
     return pv.ComposedSDF(sdfs, pv.Transform3d(matrix=torch.stack(mats).cuda()))
 
 
-TABLE = [(-1.0, -0.5, -0.25, 1.5, 1.0, 0.05), (-0.9, -0.45, -0.2, 0.3, 0.25, 0.35), (0.2, -0.45, -0.2, 0.25, 0.2, 0.6),
-         (-0.4, 0.3, -0.2, 0.5, 0.15, 0.25), (0.3, 0.25, -0.2, 0.15, 0.2, 0.9), (-0.95, 0.2, 0.4, 0.2, 0.25, 0.3),
-         (-0.3, -0.5, 0.5, 0.6, 0.05, 0.3)]
+TABLE = list(workloads.TABLETOP_BOXES)
 HAND_OBJECTS = [(-0.05, -0.12, 0.2, 0.1, 0.04, 0.1), (0.06, -0.03, 0.22, 0.04, 0.08, 0.12),
                 (-0.08, 0.05, 0.3, 0.16, 0.05, 0.03)]
 

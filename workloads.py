@@ -293,3 +293,79 @@ def tree_configurations(urdf_path, n, seed=5, dtype=torch.float32):
     q = lo + (hi - lo) * torch.rand(n, len(joints), generator=g, dtype=torch.float64)
     q[0] = torch.zeros(len(joints), dtype=torch.float64).clamp(lo, hi)
     return q.to(dtype)
+
+
+# ---------------------------------------------------------------- depth images of box scenes (depth_occupancy)
+# The tabletop scene of scripts/c4bench.scene_points as solid boxes (lo_x, lo_y, lo_z, size_x, size_y, size_z): the
+# table, 5 cm thick with its top at z = -0.2, and the six boxes standing on it or above it.
+TABLETOP_BOXES = ((-1.0, -0.5, -0.25, 1.5, 1.0, 0.05), (-0.9, -0.45, -0.2, 0.3, 0.25, 0.35),
+                  (0.2, -0.45, -0.2, 0.25, 0.2, 0.6), (-0.4, 0.3, -0.2, 0.5, 0.15, 0.25),
+                  (0.3, 0.25, -0.2, 0.15, 0.2, 0.9), (-0.95, 0.2, 0.4, 0.2, 0.25, 0.3),
+                  (-0.3, -0.5, 0.5, 0.6, 0.05, 0.3))
+TABLETOP_RANGE = ((-1.1, 0.7), (-0.6, 0.6), (-0.35, 1.0))
+
+
+def look_at(eye, target, up=(0.0, 0.0, 1.0)):
+    """fp64 [4, 4] camera-to-world transform of an OpenCV camera (x right, y down, z forward) at eye looking at
+    target."""
+    eye, target = np.asarray(eye, np.float64), np.asarray(target, np.float64)
+    z = target - eye
+    z /= np.linalg.norm(z)
+    x = np.cross(z, np.asarray(up, np.float64))
+    x /= np.linalg.norm(x)
+    m = np.eye(4)
+    m[:3, :3] = np.stack([x, np.cross(z, x), z], axis=1)
+    m[:3, 3] = eye
+    return m
+
+
+def camera_ring(n, target, radius, height, f, H=480, W=640, seed=0):
+    """(K fp64 [3, 3], cam_to_world fp64 [n, 4, 4]): n pinhole cameras of focal length f pixels (principal point at
+    the image centre) evenly spaced on a horizontal circle of the given radius about target, `height` above it, all
+    looking at target; the seed turns the ring by a random angle."""
+    K = np.array([[f, 0.0, (W - 1) / 2], [0.0, f, (H - 1) / 2], [0.0, 0.0, 1.0]])
+    phase = np.random.default_rng(seed).uniform(0.0, 2 * math.pi)
+    target = np.asarray(target, np.float64)
+    poses = []
+    for k in range(n):
+        a = phase + 2 * math.pi * k / n
+        poses.append(look_at(target + [radius * math.cos(a), radius * math.sin(a), height], target))
+    return K, np.stack(poses)
+
+
+def render_depth(boxes, K, cam_to_world, H=480, W=640, noise=0.0, seed=0):
+    """float32 [V, H, W] z-depth images of solid axis-aligned boxes (lo_x, lo_y, lo_z, size_x, size_y, size_z), in
+    fp64 by ray-slab intersection: pixel (i, j) looks along ((j - cx) / fx, (i - cy) / fy, 1) in the camera, so the
+    ray parameter of the first hit is its z-depth.  A pixel that hits nothing reads 0 (no return); noise > 0 adds
+    seeded Gaussian noise of that standard deviation (metres) to every hit."""
+    K = np.asarray(K, np.float64)
+    poses = np.asarray(cam_to_world, np.float64)
+    K = np.broadcast_to(K, (len(poses), 3, 3))
+    b = np.asarray(boxes, np.float64)
+    lo, hi = b[:, :3], b[:, :3] + b[:, 3:]
+    i, j = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
+    g = np.random.default_rng(seed)
+    out = np.zeros((len(poses), H, W), np.float32)
+    for v, (k, m) in enumerate(zip(K, poses)):
+        d_cam = np.stack([(j - k[0, 2]) / k[0, 0], (i - k[1, 2]) / k[1, 1], np.ones_like(i)], -1).reshape(-1, 3)
+        d = d_cam @ m[:3, :3].T
+        o = m[:3, 3]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            t0 = (lo[None] - o) / d[:, None]                    # [rays, boxes, 3]
+            t1 = (hi[None] - o) / d[:, None]
+        near = np.fmax.reduce(np.minimum(t0, t1), axis=2)
+        far = np.fmin.reduce(np.maximum(t0, t1), axis=2)
+        hit = (near <= far) & (near > 0)
+        t = np.where(hit, near, np.inf).min(axis=1)
+        depth = np.where(np.isfinite(t), t, 0.0)
+        if noise > 0:
+            depth = np.where(depth > 0, depth + g.normal(0.0, noise, depth.shape), 0.0)
+        out[v] = depth.reshape(H, W)
+    return out
+
+
+def tabletop_views(n, H=480, W=640, f=800.0, seed=0):
+    """(depth float32 [n, H, W], K fp64 [3, 3], cam_to_world fp64 [n, 4, 4]): the tabletop boxes seen by a ring of n
+    cameras 2.2 m from the scene's centre and 1.3 m above it (about 2.5 m away)."""
+    K, poses = camera_ring(n, (-0.25, 0.0, 0.2), 2.2, 1.3, f, H, W, seed)
+    return render_depth(TABLETOP_BOXES, K, poses, H, W), K, poses
