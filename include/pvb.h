@@ -573,6 +573,28 @@ int pvb_depth_carve(const float *depth, int32_t V, int32_t H, int32_t W, const f
                     const float *world_to_cam, float max_depth, float free_margin, const float *lo, float resolution,
                     const int32_t *dims, uint8_t *out_state, void *stream);
 
+/* ---- occupancy maps: OccupancyMap.integrate (sdf.py) ----
+ * pvb_depth_integrate: one observation of the V views of one call, fused into a log-odds occupancy grid on the
+ * lattice, depth images, views and checks of pvb_depth_carve.
+ * log_odds DEVICE int16 [nx][ny][nz]: log-odds in units of 1/1024; -32768 marks a voxel never observed.
+ * hits DEVICE uint8 [nx][ny][nz]: nonzero where a valid pixel's point falls into the voxel.  The caller writes it
+ *   with pvb_voxel_scatter (value 1) of all V*H*W points of pvb_depth_points (an invalid pixel's NaN point falls into
+ *   no voxel); the kernel reads it and writes 0 back, so it is all zero when the call returns.
+ * params HOST int32[4] = {hit, miss, clamp_lo, clamp_hi} in 1/1024 units, with
+ *   -32767 <= clamp_lo <= miss < 0 < hit <= clamp_hi <= 32767.
+ * Per voxel, in int32 arithmetic, with L = 0 for a voxel never observed:
+ *   hit (hits nonzero):                                  L = min(L + hit, clamp_hi)
+ *   else free (some view says free, as pvb_depth_carve):  L = max(L + miss, clamp_lo)
+ *   else:                                                the stored value is unchanged (-32768 stays -32768).
+ * Each voxel receives at most one update per call; the result depends on neither the view order nor the thread
+ * order.  Frames taken at different times go in separate calls.
+ * PVB_ERR_INVALID before any device work: pvb_depth_carve's cases, null hits, log_odds or params, and parameters
+ * outside the order above. */
+int pvb_depth_integrate(const float *depth, int32_t V, int32_t H, int32_t W, const float *intrinsics,
+                        const float *world_to_cam, float max_depth, float free_margin, const float *lo,
+                        float resolution, const int32_t *dims, uint8_t *hits, int16_t *log_odds,
+                        const int32_t *params, void *stream);
+
 /* ---- rigid transform helpers used by the generic (unfused) composition path ---- */
 /* out[b][i] = xforms[b] applied to pts[i] (pts DEVICE [n_pts][3], out DEVICE [n_tf][n_pts][3]), the FMA chain of the
  * composed kernels' transform; any n_tf >= 0, PVB_ERR_INVALID when n_tf * n_pts * 3 overflows int64 */

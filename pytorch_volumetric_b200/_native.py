@@ -232,6 +232,10 @@ _SIGNATURES = {
                                        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_float,
                                        ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p,
                                        ctypes.c_void_p]),
+    "pvb_depth_integrate": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_float,
+                                           ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p,
+                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "pvb_transform_points": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,
                                             ctypes.c_void_p, ctypes.c_void_p]),
     "pvb_transform_points_paired": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,

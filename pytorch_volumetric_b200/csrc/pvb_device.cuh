@@ -1676,4 +1676,22 @@ __device__ __forceinline__ bool depth_says_free(const float *depth, int H, int W
     return depth_valid(d, max_depth) && p.z < __fsub_rn(d, margin);
 }
 
+// ---------------------------------------------------------------- occupancy maps (pvb_depth_integrate)
+// Log-odds are int16 in units of 1/1024; kOccUnobserved marks a voxel no call has observed.
+constexpr int kOccUnobserved = -32768;
+
+// {hit, miss, clamp_lo, clamp_hi} in 1/1024 units, with -32767 <= clamp_lo <= miss < 0 < hit <= clamp_hi <= 32767:
+// no int32 sum below overflows and every result fits an int16 other than kOccUnobserved.
+struct OccupancyParams {
+    int hit, miss, clamp_lo, clamp_hi;
+};
+
+// One call's update of a voxel holding L: a voxel never observed starts from 0; a hit adds `hit` up to clamp_hi,
+// otherwise a free observation adds `miss` down to clamp_lo, otherwise L stays.
+__device__ __forceinline__ int occupancy_update(int L, bool hit, bool free, const OccupancyParams &p) {
+    if (!hit && !free) return L;
+    const int base = L == kOccUnobserved ? 0 : L;
+    return hit ? min(base + p.hit, p.clamp_hi) : max(base + p.miss, p.clamp_lo);
+}
+
 }  // namespace pvb

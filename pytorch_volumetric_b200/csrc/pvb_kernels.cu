@@ -4887,3 +4887,81 @@ extern "C" int pvb_depth_carve(const float *depth, int32_t V, int32_t H, int32_t
     PVB_CHECK_LAUNCH(fn);
     return PVB_OK;
 }
+
+// ---------------------------------------------------------------- occupancy maps (OccupancyMap.integrate)
+// depth_carve_kernel's layout: one thread per voxel, z fastest, the views staged in shared memory once per block.  A
+// voxel a valid pixel's point fell into (its hit byte, set by pvb_voxel_scatter) is a hit and skips the views; any
+// other voxel runs the views up to the first that says free.  The update is applied in place, and the hit byte is
+// cleared, so the scratch grid is zero again for the next call without a memset.
+__global__ void __launch_bounds__(kDepthThreads) depth_integrate_kernel(const float *__restrict__ depth, int n_views,
+                                                                       int H, int W,
+                                                                       const __grid_constant__ DepthViews views,
+                                                                       float max_depth, float margin, float lo_x,
+                                                                       float lo_y, float lo_z, float r, int ny, int nz,
+                                                                       long long n_vox, OccupancyParams params,
+                                                                       uint8_t *__restrict__ hits,
+                                                                       int16_t *__restrict__ log_odds) {
+    __shared__ float4 s_cam[kDepthMaxViews], s_rows[kDepthMaxViews][3];
+    for (int k = threadIdx.x; k < n_views; k += blockDim.x) {
+        s_cam[k] = views.cam[k];
+        s_rows[k][0] = views.rows[k][0]; s_rows[k][1] = views.rows[k][1]; s_rows[k][2] = views.rows[k][2];
+    }
+    __syncthreads();
+    const float lo[3] = {lo_x, lo_y, lo_z};
+    const long long stride = (long long)gridDim.x * blockDim.x, hw = (long long)H * W;
+    for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < n_vox; c += stride) {
+        const bool hit = hits[c] != 0;
+        bool free = false;
+        if (!hit) {
+            const int ci = (int)c, iz = ci % nz, iy = (ci / nz) % ny, ix = ci / nz / ny;
+            const f3 x = depth_voxel_centre(lo, r, ix, iy, iz);
+            for (int v = 0; v < n_views && !free; ++v)
+                free = depth_says_free(depth + v * hw, H, W, s_cam[v], s_rows[v][0], s_rows[v][1], s_rows[v][2], x,
+                                       max_depth, margin);
+        }
+        if (hit || free) log_odds[c] = (int16_t)occupancy_update(log_odds[c], hit, free, params);
+        if (hit) hits[c] = 0;
+    }
+}
+
+extern "C" int pvb_depth_integrate(const float *depth, int32_t V, int32_t H, int32_t W, const float *intrinsics,
+                                   const float *world_to_cam, float max_depth, float free_margin, const float *lo,
+                                   float resolution, const int32_t *dims, uint8_t *hits, int16_t *log_odds,
+                                   const int32_t *params, void *stream) {
+    const char *fn = "pvb_depth_integrate";
+    DepthViews views = {};
+    if (int rc = depth_check_views(fn, depth, V, H, W, intrinsics, world_to_cam, max_depth, views)) return rc;
+    if (int rc = edt_check_dims(fn, dims)) return rc;
+    if (!(resolution > 0.f) || !isfinite(resolution)) {
+        pvb_set_error("%s: the resolution must be finite and positive (resolution=%g)", fn, (double)resolution);
+        return PVB_ERR_INVALID;
+    }
+    if (!(free_margin >= 0.f) || !isfinite(free_margin)) {
+        pvb_set_error("%s: free_margin must be finite and non-negative (free_margin=%g)", fn, (double)free_margin);
+        return PVB_ERR_INVALID;
+    }
+    if (!lo || !hits || !log_odds || !params) {
+        pvb_set_error("%s: invalid argument (lo, hits, log_odds or params is null)", fn);
+        return PVB_ERR_INVALID;
+    }
+    if (!isfinite(lo[0]) || !isfinite(lo[1]) || !isfinite(lo[2])) {
+        pvb_set_error("%s: the lattice origin lo must be finite", fn);
+        return PVB_ERR_INVALID;
+    }
+    const OccupancyParams p = {params[0], params[1], params[2], params[3]};
+    if (!(-32767 <= p.clamp_lo && p.clamp_lo <= p.miss && p.miss < 0 && 0 < p.hit && p.hit <= p.clamp_hi &&
+          p.clamp_hi <= 32767)) {
+        pvb_set_error("%s: the parameters must satisfy -32767 <= clamp_lo <= miss < 0 < hit <= clamp_hi <= 32767 "
+                      "(hit=%d, miss=%d, clamp_lo=%d, clamp_hi=%d)", fn, p.hit, p.miss, p.clamp_lo, p.clamp_hi);
+        return PVB_ERR_INVALID;
+    }
+    const long long n_vox = (long long)dims[0] * dims[1] * dims[2];
+    cudaStream_t s = (cudaStream_t)stream;
+    timing_mark(0, s);
+    depth_integrate_kernel<<<grid_for(n_vox, kDepthThreads, 8), kDepthThreads, 0, s>>>(
+        depth, V, H, W, views, max_depth, free_margin, lo[0], lo[1], lo[2], resolution, dims[1], dims[2], n_vox, p,
+        hits, log_odds);
+    timing_mark(1, s);
+    PVB_CHECK_LAUNCH(fn);
+    return PVB_OK;
+}

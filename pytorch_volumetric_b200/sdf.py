@@ -2447,6 +2447,129 @@ def depth_occupancy(depth, K, cam_to_world, resolution, range_per_dim, max_depth
     return nat.deliver(_depth_state(views, lattice, nat.compute_device(src)), src)
 
 
+# ---------------------------------------------------------------- occupancy maps
+LOG_ODDS_UNIT = 1024         # log-odds are stored as int16 in units of 1 / LOG_ODDS_UNIT
+LOG_ODDS_UNOBSERVED = -32768
+
+
+class OccupancyParams(NamedTuple):
+    """OccupancyMap's update parameters in units of 1 / LOG_ODDS_UNIT."""
+    hit: int
+    miss: int
+    clamp_lo: int
+    clamp_hi: int
+    threshold: int
+
+
+def _occupancy_params(hit, miss, clamp, threshold):
+    """Each parameter quantized once as round(x * 1024) (Python's round: nearest, ties to even), then checked:
+    -32767 <= clamp_lo <= miss < 0 < hit <= clamp_hi <= 32767 and miss < threshold <= hit."""
+    if len(clamp) != 2:
+        raise ValueError(f"clamp must be (lo, hi), got {clamp!r}")
+    raw = dict(hit=hit, miss=miss, clamp_lo=clamp[0], clamp_hi=clamp[1], threshold=threshold)
+    for name, x in raw.items():
+        if not math.isfinite(float(x)):
+            raise ValueError(f"{name} must be finite, got {x}")
+    p = OccupancyParams(**{name: round(float(x) * LOG_ODDS_UNIT) for name, x in raw.items()})
+    if not (-32767 <= p.clamp_lo <= p.miss < 0 < p.hit <= p.clamp_hi <= 32767 and p.miss < p.threshold <= p.hit):
+        raise ValueError(f"in units of 1/{LOG_ODDS_UNIT} the parameters must satisfy -32767 <= clamp_lo <= miss < 0 "
+                         f"< hit <= clamp_hi <= 32767 and miss < threshold <= hit, got {p}")
+    return p
+
+
+class OccupancyMap:
+    """A log-odds occupancy grid that fuses depth frames over time on the GPU (pvb_depth_integrate).
+
+    The lattice is depth_occupancy's: the range snapped by get_divisible_range_by_resolution, voxel i centred at
+    lo + i r, 2..1024 voxels per axis.  Each voxel holds a log-odds L, stored as an int16 in units of 1/1024, or
+    "never observed".  Every parameter is quantized once as round(x * 1024), and after that they must satisfy
+    -32767 <= clamp_lo <= miss < 0 < hit <= clamp_hi <= 32767 and miss < threshold <= hit (ValueError otherwise), so
+    that a single observation decides a fresh voxel.  The defaults approximate OctoMap's (p_hit 0.7, p_miss 0.4,
+    clamping at 0.12 / 0.97, threshold 0.5).
+
+    integrate() adds one observation of the views of one call.  In int32 arithmetic, a voxel never observed starting
+    from 0, each voxel receives at most one update per call:
+      hit   a valid pixel's point of any view falls into it:  L = min(L + hit, clamp_hi);
+      free  otherwise, when some view says free (depth_occupancy's rule, free_margin included):  L = max(L + miss,
+            clamp_lo);
+      otherwise L is unchanged.
+    The result depends on neither the view order nor the thread order; frames taken at different times go in separate
+    calls.  Because the evidence is bounded by the clamps, old evidence can be overturned: a voxel holding L turns free
+    after ceil((L - threshold + 1) / -miss) free observations in a row, 9 from the upper clamp with the defaults, so an
+    object that has moved leaves no ghost where later frames see free space.  After one call on a fresh map, state()
+    equals depth_occupancy of the same views.  integrate does not synchronise with the host when the depth images are
+    on the GPU.
+
+    :param free_margin: depth_occupancy's, for every call; defaults to sqrt(3) r / 2
+    :param device: device state() and log_odds() return on, and sdf()'s default device (the grid lives on the GPU)"""
+
+    def __init__(self, resolution, range_per_dim, hit=0.85, miss=-0.4, clamp=(-2.0, 3.5), threshold=0.0,
+                 free_margin=None, device="cpu"):
+        self.params = _occupancy_params(hit, miss, clamp, threshold)
+        self.resolution, self.range_per_dim, self.free_margin = _depth_lattice(resolution, range_per_dim, free_margin)
+        self.device = device
+        self._cdev = nat.compute_device(device)
+        self._hits = VoxelGrid(self.resolution, self.range_per_dim, dtype=torch.bool, device=self._cdev)
+        self._hits.voxels._geom()            # reads the lattice from the device once, so integrate never synchronises
+        self.shape = tuple(self._hits.get_voxel_values().shape)
+        self._log_odds = torch.full(self.shape, LOG_ODDS_UNOBSERVED, dtype=torch.int16, device=self._cdev)
+        self._lo = (ctypes.c_float * 3)(*[float(min(r)) for r in self._hits.range_per_dim])
+        self._dims = (ctypes.c_int32 * 3)(*self.shape)
+        self._update = (ctypes.c_int32 * 4)(*self.params[:4])
+
+    def integrate(self, depth, K, cam_to_world, max_depth=math.inf):
+        """Add one observation of depth images [V, H, W] (V up to 64) to the map; the arguments are
+        depth_to_points'.  Write 0 on pixels that should say nothing (the robot's own body, say)."""
+        views = _depth_views(depth, K, cam_to_world, max_depth)
+        d = views.depth.to(self._cdev).contiguous()
+        V, H, W = d.shape
+        intr = (ctypes.c_float * (4 * V))(*views.intrinsics.reshape(-1).tolist())
+        c2w = (ctypes.c_float * (12 * V))(*views.cam_to_world[:, :3].to(torch.float32).reshape(-1).tolist())
+        w2c = (ctypes.c_float * (12 * V))(
+            *invert_rigid(views.cam_to_world)[:, :3].to(torch.float32).reshape(-1).tolist())
+        L = nat.lib()
+        with nat.on_device(self._cdev):
+            points = torch.empty(V * H * W, 3, dtype=torch.float32, device=self._cdev)
+            nat.check(L.pvb_depth_points(nat.ptr(d), V, H, W, intr, c2w, views.max_depth, nat.ptr(points),
+                                         nat.stream_ptr(self._cdev)), "pvb_depth_points")
+            self._hits[points] = True           # the NaN point of an invalid pixel falls into no voxel
+            nat.check(L.pvb_depth_integrate(nat.ptr(d), V, H, W, intr, w2c, views.max_depth, self.free_margin,
+                                            self._lo, self.resolution, self._dims,
+                                            nat.ptr(self._hits.get_voxel_values()), nat.ptr(self._log_odds),
+                                            self._update, nat.stream_ptr(self._cdev)), "pvb_depth_integrate")
+
+    def _state(self):
+        L = self._log_odds
+        return (L >= self.params.threshold).to(torch.uint8).masked_fill_(L == LOG_ODDS_UNOBSERVED, 2)
+
+    def state(self):
+        """uint8 [nx, ny, nz] on the map's device: 1 occupied (L >= threshold), 0 free, 2 never observed --
+        depth_occupancy's encoding."""
+        return nat.deliver(self._state(), self.device)
+
+    def log_odds(self):
+        """float32 [nx, ny, nz] on the map's device: the stored value / 1024 (exact), NaN where never observed."""
+        L = self._log_odds
+        return nat.deliver((L.to(torch.float32) / LOG_ODDS_UNIT).masked_fill_(L == LOG_ODDS_UNOBSERVED, math.nan),
+                           self.device)
+
+    def sdf(self, unknown="occupied", interpolation="nearest", device=None):
+        """OccupancySDF of state() on the map's lattice: voxels never observed count as occupied
+        (unknown="occupied") or free ("free"), OccupancySDF.from_depth's rule.  ValueError unless both states are
+        present.  device defaults to the map's."""
+        if unknown not in ("occupied", "free"):
+            raise ValueError(f"unknown must be 'occupied' or 'free', got {unknown!r}")
+        state = self._state()
+        grid = VoxelGrid(self.resolution, self.range_per_dim, dtype=torch.bool, device=self._cdev)
+        grid.get_voxel_values().copy_(state == 1 if unknown == "free" else state != 0)
+        return OccupancySDF(grid, interpolation=interpolation, device=self.device if device is None else device)
+
+    def reset(self):
+        """Every voxel back to "never observed"."""
+        self._log_odds.fill_(LOG_ODDS_UNOBSERVED)
+        self._hits.get_voxel_values().zero_()
+
+
 def sample_mesh_points(obj_factory: ObjectFactory = None, num_points=100, seed=0, name="",
                        clean_cache=False, dtype=torch.float, min_init_sample_points=200,
                        dbpath='model_points_cache.pkl', device="cpu", cache=None):
