@@ -595,6 +595,48 @@ int pvb_depth_integrate(const float *depth, int32_t V, int32_t H, int32_t W, con
                         float resolution, const int32_t *dims, uint8_t *hits, int16_t *log_odds,
                         const int32_t *params, void *stream);
 
+/* ---- ray-cast point clouds: ray_occupancy, OccupancySDF.from_rays, OccupancyMap.integrate_points (sdf.py) ----
+ * A ray is a sensor origin o and a return p, fp32 world points on pvb_depth_carve's lattice (voxel i centred at
+ * lo + i * resolution, dims HOST int32[3] each 2..1024, lo HOST float[3] finite).  Every fp32 operation rounds to
+ * nearest once, in the order written; fma, sqrt, min, max and floor are the IEEE operations, (float)i is exact.
+ *
+ * Valid ray: d = p - o per axis, l = sqrt(fma(dz, dz, fma(dy, dy, dx * dx))); the ray is valid when all six
+ * coordinates of o and p are finite and 0 < l <= max_range with l finite (+inf max_range allowed).  An invalid ray
+ * (a NaN row pads a ragged scan; l = 0 is a LiDAR's "no return" in the sensor frame) says nothing: no hit, no free
+ * voxel.  Returns beyond max_range are dropped.
+ * Free voxels: the face-connected (6-connected) walk of the segment o + t d, 0 <= t <= t_end, t_end = (l - m) / l with
+ * m = free_margin; nothing when l <= m.  In lattice coordinates a_k = (o_k - lo_k) / resolution + 0.5 and
+ * u_k = d_k / resolution, voxel i covers [i, i + 1).
+ *   clip: t_lo = 0, t_hi = t_end; per axis with u_k != 0, t0 = -a_k / u_k and t1 = (n_k - a_k) / u_k give
+ *     t_lo = max(t_lo, min(t0, t1)), t_hi = min(t_hi, max(t0, t1)); an axis with u_k == 0 needs 0 <= a_k < n_k.  No
+ *     voxel unless t_lo < t_hi.
+ *   start: i_k = floor(fma(t_lo, u_k, a_k)) clamped to 0..n_k - 1.
+ *   boundaries: tb_k = ((float)(i_k + (u_k > 0)) - a_k) / u_k (subtract, divide), recomputed from the index after
+ *     every step, +inf when u_k == 0; no step accumulates rounding.
+ *   step: visit the voxel; take the axis of the smallest tb (ties: x, then y, then z); stop when that tb >= t_end;
+ *     move its index one voxel towards u_k's sign; stop when it leaves 0..n_k - 1.
+ *   Every index moves one way only: no voxel twice, at most n_x + n_y + n_z voxels per ray (also a hard loop bound).
+ *
+ * pvb_ray_carve: points DEVICE float [n_rays][3]; origins DEVICE float [n_rays / rays_per_origin][3], ray t taking
+ * origin t / rays_per_origin.  Writes 2 into marks DEVICE uint8 [nx][ny][nz] (C order) on every free voxel of every
+ * valid ray and leaves every other byte as it is; writes out_points DEVICE float [n_rays][3]: p for a valid ray and
+ * (NaN, NaN, NaN) otherwise.  The caller then scatters out_points with pvb_voxel_scatter (value 1), so hits win over
+ * free.  Every carve write stores the same value: the result depends on neither the ray order nor the thread order.
+ * The origins are not read on the host (a non-finite origin makes its rays invalid), so the call does not
+ * synchronise.
+ * pvb_occupancy_apply: one observation from such marks into pvb_depth_integrate's log_odds grid: per voxel, mark 1
+ * applies the hit update, mark 2 the free update and 0 nothing (any other mark nothing), then every mark is set to 0,
+ * so marks is all zero when the call returns.  params as pvb_depth_integrate's.
+ *
+ * PVB_ERR_INVALID before any device work: null pointers, n_rays < 1, n_rays >= 2^31, a rays_per_origin < 1 or one
+ * that does not divide n_rays, max_range <= 0 or NaN, dims outside 2..1024, a resolution that is not finite and
+ * positive, a free_margin that is negative or not finite, a lo that is not finite; for the apply, null pointers, dims
+ * outside 2..1024 and parameters outside pvb_depth_integrate's order. */
+int pvb_ray_carve(const float *points, int64_t n_rays, int64_t rays_per_origin, const float *origins,
+                  float max_range, float free_margin, const float *lo, float resolution, const int32_t *dims,
+                  uint8_t *marks, float *out_points, void *stream);
+int pvb_occupancy_apply(uint8_t *marks, int16_t *log_odds, const int32_t *dims, const int32_t *params, void *stream);
+
 /* ---- rigid transform helpers used by the generic (unfused) composition path ---- */
 /* out[b][i] = xforms[b] applied to pts[i] (pts DEVICE [n_pts][3], out DEVICE [n_tf][n_pts][3]), the FMA chain of the
  * composed kernels' transform; any n_tf >= 0, PVB_ERR_INVALID when n_tf * n_pts * 3 overflows int64 */

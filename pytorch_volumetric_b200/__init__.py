@@ -9,7 +9,7 @@ from . import chamfer as _chamfer, distributed, kinematics as _kin, model_to_sdf
 _EXPORTS = {
     _sdf: ("BoxSDF", "CachedSDF", "ComposedSDF", "CylinderSDF", "MeshObjectFactory", "MeshSDF", "ObjectFactory",
            "ObjectFrameSDF", "OccupancyMap", "OccupancySDF", "OutOfBoundsStrategy", "SDFQuery", "SphereSDF", "depth_occupancy",
-           "depth_to_points", "occupancy_distance_transform", "sample_mesh_points"),
+           "depth_to_points", "occupancy_distance_transform", "ray_occupancy", "sample_mesh_points"),
     _robot: ("RobotSDF", "aabb_to_ordered_end_points", "cache_link_sdf_factory"),
     _chamfer: ("PlausibleDiversity", "batch_chamfer_dist", "pairwise_distance", "pairwise_distance_chamfer"),
     _voxel: ("ExpandingVoxelGrid", "VoxelGrid", "VoxelSet", "Voxels", "get_coordinates_and_points_in_grid",

@@ -1694,4 +1694,79 @@ __device__ __forceinline__ int occupancy_update(int L, bool hit, bool free, cons
     return hit ? min(base + p.hit, p.clamp_hi) : max(base + p.miss, p.clamp_lo);
 }
 
+// ---------------------------------------------------------------- ray-cast point clouds (pvb_ray_carve)
+// A ray runs from a sensor origin o to its return p.  Every fp32 operation rounds to nearest once, in the order
+// written (include/pvb.h states it); fmaf, sqrtf, fminf, fmaxf and floorf are the IEEE operations on both builds.
+
+// d = p - o and l = |d| = sqrt(fma(dz, dz, fma(dy, dy, dx * dx))).  The ray is valid when all six coordinates are
+// finite and 0 < l <= max_range with l finite; an invalid ray says nothing.
+__device__ __forceinline__ bool ray_valid(f3 o, f3 p, float max_range, f3 &d, float &len) {
+    d = mk3(__fsub_rn(p.x, o.x), __fsub_rn(p.y, o.y), __fsub_rn(p.z, o.z));
+    len = sqrtf(fmaf(d.z, d.z, fmaf(d.y, d.y, __fmul_rn(d.x, d.x))));
+    const bool finite = fabsf(o.x) < PVB_INF && fabsf(o.y) < PVB_INF && fabsf(o.z) < PVB_INF &&
+                        fabsf(p.x) < PVB_INF && fabsf(p.y) < PVB_INF && fabsf(p.z) < PVB_INF;
+    return finite && len > 0.f && len <= max_range && len < PVB_INF;
+}
+
+// One step of ray_walk along an axis: the index moves towards u's sign; false when it leaves 0..n - 1, otherwise
+// the axis' next boundary parameter from the new index.
+__device__ __forceinline__ bool ray_step(int &i, float &tb, float a, float u, int n) {
+    i += u > 0.f ? 1 : -1;
+    if (i < 0 || i >= n) return false;
+    tb = __fdiv_rn(__fsub_rn((float)(i + (u > 0.f)), a), u);
+    return true;
+}
+
+// The face-connected walk of a valid ray's free segment, o + t d for t in [0, t_end] with
+// t_end = (len - margin) / len, through the lattice of n[k] voxels per axis centred at lo + i r.  In lattice
+// coordinates a_k = (o_k - lo_k) / r + 0.5 and u_k = d_k / r, voxel i covers [i, i + 1).  The segment is clipped to
+// the box [0, n_k) of every axis with u_k != 0 (entry t0 = -a_k / u_k, exit t1 = (n_k - a_k) / u_k, the smaller one
+// entering); an axis with u_k == 0 must have 0 <= a_k < n_k.  Nothing is visited unless t_lo < t_hi.  The walk starts
+// at i_k = floor(fma(t_lo, u_k, a_k)) clamped to 0..n_k - 1; the next boundary of axis k is
+// tb_k = ((float)(i_k + (u_k > 0)) - a_k) / u_k, recomputed from the index after every step (+inf when u_k == 0).  It
+// visits the current voxel, then moves along the axis of the smallest tb (ties: x, then y, then z), and stops when that
+// tb >= t_end or when the index leaves the grid.  Every index moves one way only, so no voxel is visited twice and at
+// most n_x + n_y + n_z voxels are visited, a bound the loop also enforces.  Returns the number of voxels visited.
+template <class Visit>
+__device__ __forceinline__ int ray_walk(f3 o, f3 d, float len, float margin, const float *lo, float r, const int *n,
+                                        Visit &&visit) {
+    if (!(len > margin)) return 0;
+    const float t_end = __fdiv_rn(__fsub_rn(len, margin), len);
+    const float oc[3] = {o.x, o.y, o.z}, dc[3] = {d.x, d.y, d.z};
+    float a[3], u[3], tb[3];
+    int i[3];
+    float t_lo = 0.f, t_hi = t_end;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        a[k] = __fadd_rn(__fdiv_rn(__fsub_rn(oc[k], lo[k]), r), 0.5f);
+        u[k] = __fdiv_rn(dc[k], r);
+        if (u[k] == 0.f) {
+            if (!(a[k] >= 0.f && a[k] < (float)n[k])) return 0;
+        } else {
+            const float t0 = __fdiv_rn(-a[k], u[k]), t1 = __fdiv_rn(__fsub_rn((float)n[k], a[k]), u[k]);
+            t_lo = fmaxf(t_lo, fminf(t0, t1));
+            t_hi = fminf(t_hi, fmaxf(t0, t1));
+        }
+    }
+    if (!(t_lo < t_hi)) return 0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        i[k] = (int)fminf(fmaxf(floorf(fmaf(t_lo, u[k], a[k])), 0.f), (float)(n[k] - 1));
+        tb[k] = u[k] == 0.f ? PVB_INF : __fdiv_rn(__fsub_rn((float)(i[k] + (u[k] > 0.f)), a[k]), u[k]);
+    }
+    // The axis is chosen by selects rather than an index, so that the per-axis state stays in registers.
+    const int max_visits = n[0] + n[1] + n[2];
+    int visits = 0;
+    for (;;) {
+        visit(i[0], i[1], i[2]);
+        if (++visits >= max_visits) break;
+        const bool sx = tb[0] <= tb[1] && tb[0] <= tb[2], sy = !sx && tb[1] <= tb[2];
+        if (!((sx ? tb[0] : sy ? tb[1] : tb[2]) < t_end)) break;
+        if (!(sx ? ray_step(i[0], tb[0], a[0], u[0], n[0])
+                 : sy ? ray_step(i[1], tb[1], a[1], u[1], n[1]) : ray_step(i[2], tb[2], a[2], u[2], n[2])))
+            break;
+    }
+    return visits;
+}
+
 }  // namespace pvb

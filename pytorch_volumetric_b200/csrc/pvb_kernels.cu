@@ -4965,3 +4965,110 @@ extern "C" int pvb_depth_integrate(const float *depth, int32_t V, int32_t H, int
     PVB_CHECK_LAUNCH(fn);
     return PVB_OK;
 }
+
+// ---------------------------------------------------------------- ray-cast point clouds (OccupancyMap.integrate_points)
+constexpr int kRayThreads = 256;
+
+// One thread per ray on a grid-stride loop: ray_valid, then out_points, then ray_walk writes 2 on every voxel of the
+// free segment.  Every write stores the same value, so the marks depend on neither the ray order nor the thread order.
+__global__ void __launch_bounds__(kRayThreads) ray_carve_kernel(const float *__restrict__ points, long long n_rays,
+                                                                long long per_origin,
+                                                                const float *__restrict__ origins, float max_range,
+                                                                float margin, float lo_x, float lo_y, float lo_z,
+                                                                float r, int nx, int ny, int nz,
+                                                                uint8_t *__restrict__ marks, float *__restrict__ out) {
+    const float lo[3] = {lo_x, lo_y, lo_z};
+    const int n[3] = {nx, ny, nz};
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n_rays; t += stride) {
+        const float *q = origins + 3 * (t / per_origin);
+        const f3 o = mk3(__ldg(q), __ldg(q + 1), __ldg(q + 2));
+        const f3 p = mk3(points[3 * t], points[3 * t + 1], points[3 * t + 2]);
+        f3 d;
+        float len;
+        const bool valid = ray_valid(o, p, max_range, d, len);
+        const float nan = __int_as_float(0x7fc00000);
+        out[3 * t] = valid ? p.x : nan; out[3 * t + 1] = valid ? p.y : nan; out[3 * t + 2] = valid ? p.z : nan;
+        if (valid)
+            ray_walk(o, d, len, margin, lo, r, n, [&](int ix, int iy, int iz) {
+                marks[((long long)ix * ny + iy) * nz + iz] = 2;
+            });
+    }
+}
+
+// One thread per voxel: mark 1 is a hit, 2 a free observation, 0 nothing (occupancy_update); every mark is cleared.
+__global__ void __launch_bounds__(256) occupancy_apply_kernel(uint8_t *__restrict__ marks,
+                                                              int16_t *__restrict__ log_odds, long long n_vox,
+                                                              OccupancyParams params) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < n_vox; c += stride) {
+        const uint8_t m = marks[c];
+        if (m == 0) continue;
+        log_odds[c] = (int16_t)occupancy_update(log_odds[c], m == 1, m == 2, params);
+        marks[c] = 0;
+    }
+}
+
+extern "C" int pvb_ray_carve(const float *points, int64_t n_rays, int64_t rays_per_origin, const float *origins,
+                             float max_range, float free_margin, const float *lo, float resolution,
+                             const int32_t *dims, uint8_t *marks, float *out_points, void *stream) {
+    const char *fn = "pvb_ray_carve";
+    if (!points || !origins || !lo || !marks || !out_points) {
+        pvb_set_error("%s: invalid argument (points, origins, lo, marks or out_points is null)", fn);
+        return PVB_ERR_INVALID;
+    }
+    if (n_rays < 1 || n_rays >= ((int64_t)1 << 31) || rays_per_origin < 1 || n_rays % rays_per_origin) {
+        pvb_set_error("%s: n_rays must be 1..2^31 - 1 and a multiple of rays_per_origin >= 1 (n_rays=%lld, "
+                      "rays_per_origin=%lld)", fn, (long long)n_rays, (long long)rays_per_origin);
+        return PVB_ERR_INVALID;
+    }
+    if (!(max_range > 0.f)) {
+        pvb_set_error("%s: max_range must be positive (max_range=%g)", fn, (double)max_range);
+        return PVB_ERR_INVALID;
+    }
+    if (int rc = edt_check_dims(fn, dims)) return rc;
+    if (!(resolution > 0.f) || !isfinite(resolution)) {
+        pvb_set_error("%s: the resolution must be finite and positive (resolution=%g)", fn, (double)resolution);
+        return PVB_ERR_INVALID;
+    }
+    if (!(free_margin >= 0.f) || !isfinite(free_margin)) {
+        pvb_set_error("%s: free_margin must be finite and non-negative (free_margin=%g)", fn, (double)free_margin);
+        return PVB_ERR_INVALID;
+    }
+    if (!isfinite(lo[0]) || !isfinite(lo[1]) || !isfinite(lo[2])) {
+        pvb_set_error("%s: the lattice origin lo must be finite", fn);
+        return PVB_ERR_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    timing_mark(0, s);
+    ray_carve_kernel<<<grid_for(n_rays, kRayThreads, 8), kRayThreads, 0, s>>>(
+        points, n_rays, rays_per_origin, origins, max_range, free_margin, lo[0], lo[1], lo[2], resolution, dims[0],
+        dims[1], dims[2], marks, out_points);
+    timing_mark(1, s);
+    PVB_CHECK_LAUNCH(fn);
+    return PVB_OK;
+}
+
+extern "C" int pvb_occupancy_apply(uint8_t *marks, int16_t *log_odds, const int32_t *dims, const int32_t *params,
+                                   void *stream) {
+    const char *fn = "pvb_occupancy_apply";
+    if (int rc = edt_check_dims(fn, dims)) return rc;
+    if (!marks || !log_odds || !params) {
+        pvb_set_error("%s: invalid argument (marks, log_odds or params is null)", fn);
+        return PVB_ERR_INVALID;
+    }
+    const OccupancyParams p = {params[0], params[1], params[2], params[3]};
+    if (!(-32767 <= p.clamp_lo && p.clamp_lo <= p.miss && p.miss < 0 && 0 < p.hit && p.hit <= p.clamp_hi &&
+          p.clamp_hi <= 32767)) {
+        pvb_set_error("%s: the parameters must satisfy -32767 <= clamp_lo <= miss < 0 < hit <= clamp_hi <= 32767 "
+                      "(hit=%d, miss=%d, clamp_lo=%d, clamp_hi=%d)", fn, p.hit, p.miss, p.clamp_lo, p.clamp_hi);
+        return PVB_ERR_INVALID;
+    }
+    const long long n_vox = (long long)dims[0] * dims[1] * dims[2];
+    cudaStream_t s = (cudaStream_t)stream;
+    timing_mark(0, s);
+    occupancy_apply_kernel<<<grid_for(n_vox, 256, 8), 256, 0, s>>>(marks, log_odds, n_vox, p);
+    timing_mark(1, s);
+    PVB_CHECK_LAUNCH(fn);
+    return PVB_OK;
+}

@@ -2292,6 +2292,26 @@ class OccupancySDF(CachedSDF):
         grid.get_voxel_values().copy_(state == 1 if unknown == "free" else state != 0)
         return cls(grid, interpolation=interpolation, device=device)
 
+    @classmethod
+    def from_rays(cls, points, origins, resolution, range_per_dim, unknown="occupied", max_range=math.inf,
+                  free_margin=None, interpolation="nearest", device="cpu"):
+        """OccupancySDF of the scene that point clouds taken from known sensor origins see (ray_occupancy's state
+        grid), under from_depth's rules: unknown="occupied" (the default) counts the voxels no ray passed through as
+        occupied; unknown="free" counts only the voxels a valid ray's return falls into, which gives the occupancy
+        and table of from_points(the returns of the valid rays).  The other arguments are ray_occupancy's, plus
+        interpolation and device as for OccupancySDF."""
+        if unknown not in ("occupied", "free"):
+            raise ValueError(f"unknown must be 'occupied' or 'free', got {unknown!r}")
+        if interpolation not in ("nearest", "trilinear"):
+            raise ValueError(f"interpolation must be 'nearest' or 'trilinear', got {interpolation!r}")
+        rays = _rays(points, origins, max_range)
+        lattice = _depth_lattice(resolution, range_per_dim, free_margin)
+        cdev = nat.compute_device(device)
+        state = _ray_state(rays, lattice, cdev)
+        grid = VoxelGrid(resolution, range_per_dim, dtype=torch.bool, device=cdev)
+        grid.get_voxel_values().copy_(state == 1 if unknown == "free" else state != 0)
+        return cls(grid, interpolation=interpolation, device=device)
+
     def surface_bounding_box(self, padding=0., padding_ratio=0.):
         """The box of the occupied voxel centres widened by half a cell, inflated by padding + padding_ratio * extent
         (fp64)."""
@@ -2447,6 +2467,81 @@ def depth_occupancy(depth, K, cam_to_world, resolution, range_per_dim, max_depth
     return nat.deliver(_depth_state(views, lattice, nat.compute_device(src)), src)
 
 
+# ---------------------------------------------------------------- ray-cast point clouds
+class _Rays(NamedTuple):
+    points: torch.Tensor        # fp32 [n_rays, 3], on the caller's device
+    origins: torch.Tensor       # fp32 [V, 3], on points' device
+    per_origin: int             # rays per origin: N
+    max_range: float
+
+
+def _rays(points, origins, max_range):
+    """Check ray_occupancy's / integrate_points' ray arguments (ValueError, before any device work): float32 points
+    [N, 3] with origins [3], or [V, N, 3] with origins [V, 3]."""
+    p = points if torch.is_tensor(points) else torch.as_tensor(np.asarray(points))
+    o = origins if torch.is_tensor(origins) else torch.as_tensor(np.asarray(origins))
+    if p.dtype != torch.float32 or o.dtype != torch.float32:
+        raise ValueError(f"points and origins must be float32, got {p.dtype} and {o.dtype}")
+    shapes = tuple(p.shape), tuple(o.shape)
+    if p.dim() == 2 and o.dim() == 1:
+        p, o = p.unsqueeze(0), o.unsqueeze(0)
+    if p.dim() != 3 or p.shape[2] != 3 or p.shape[0] < 1 or p.shape[1] < 1 or tuple(o.shape) != (p.shape[0], 3):
+        raise ValueError(f"points must be [N, 3] with origins [3], or [V, N, 3] with origins [V, 3], N, V >= 1; got "
+                         f"{shapes[0]} and {shapes[1]}")
+    if p.shape[0] * p.shape[1] >= 2 ** 31:
+        raise ValueError(f"at most 2^31 - 1 rays per call, got {p.shape[0] * p.shape[1]}")
+    max_range = float(max_range)
+    if not max_range > 0:
+        raise ValueError(f"max_range must be positive (+inf allowed), got {max_range}")
+    return _Rays(p.reshape(-1, 3), o.to(p.device), int(p.shape[1]), max_range)
+
+
+def _ray_carve(rays, margin, lo, resolution, dims, marks, cdev):
+    """pvb_ray_carve of the rays into the uint8 marks on cdev; returns out_points (NaN for an invalid ray)."""
+    pts = rays.points.to(cdev).contiguous()
+    org = rays.origins.to(cdev).contiguous()
+    with nat.on_device(cdev):
+        out = torch.empty_like(pts)
+        nat.check(nat.lib().pvb_ray_carve(nat.ptr(pts), pts.shape[0], rays.per_origin, nat.ptr(org), rays.max_range,
+                                          margin, lo, resolution, dims, nat.ptr(marks), nat.ptr(out),
+                                          nat.stream_ptr(cdev)), "pvb_ray_carve")
+    return out
+
+
+def _ray_state(rays, lattice, cdev):
+    """The uint8 state grid [nx, ny, nz] on cdev: 2 - marks after pvb_ray_carve writes 2 on the free voxels and the
+    scatter of the valid returns (VoxelGrid(...)[points] = True, pvb_voxel_scatter) writes 1."""
+    resolution, range_per_dim, margin = lattice
+    grid = VoxelGrid(resolution, range_per_dim, dtype=torch.bool, device=cdev)
+    marks = grid.get_voxel_values().view(torch.uint8)
+    lo = (ctypes.c_float * 3)(*[float(min(r)) for r in grid.range_per_dim])
+    out = _ray_carve(rays, margin, lo, resolution, (ctypes.c_int32 * 3)(*marks.shape), marks, cdev)
+    grid[out] = True                    # an invalid ray's NaN point falls into no voxel
+    return 2 - marks
+
+
+def ray_occupancy(points, origins, resolution, range_per_dim, max_range=math.inf, free_margin=None):
+    """Fuse point clouds taken from known sensor origins into an occupancy state grid on the GPU (pvb_ray_carve, then
+    pvb_voxel_scatter), as OctoMap's insertPointCloud does: each ray is walked from its origin towards its return.
+
+    points: float32 [N, 3] with origins [3] (one scan), or [V, N, 3] with origins [V, 3] (V scans), world frame; any
+    other dtype or shape raises ValueError.  A ray is valid when its six coordinates are finite and its length l
+    satisfies 0 < l <= max_range: NaN rows pad ragged scans, l = 0 is a "no return", and returns beyond max_range are
+    dropped.  An invalid ray says nothing.  The grid is depth_occupancy's lattice (range snapped by
+    get_divisible_range_by_resolution, voxel i centred at lo + i r), 2..1024 voxels per axis.  Each voxel is
+      1 occupied  when the return of a valid ray falls into it (the VoxelGrid scatter from_points uses);
+      0 free      otherwise, when the face-connected walk of some valid ray's segment from its origin to
+                  (l - free_margin) / l of the way to its return passes through it (nothing when l <= free_margin);
+      2 unknown   otherwise.
+    free_margin defaults to sqrt(3) r / 2, half a cell diagonal.  The walk's fp32 rules (clipping, start voxel,
+    boundary parameters, ties x then y then z) are in include/pvb.h.  The result depends on neither the ray order nor
+    the thread order.  Returns uint8 [nx, ny, nz] on points' device."""
+    rays = _rays(points, origins, max_range)
+    lattice = _depth_lattice(resolution, range_per_dim, free_margin)
+    src = rays.points.device
+    return nat.deliver(_ray_state(rays, lattice, nat.compute_device(src)), src)
+
+
 # ---------------------------------------------------------------- occupancy maps
 LOG_ODDS_UNIT = 1024         # log-odds are stored as int16 in units of 1 / LOG_ODDS_UNIT
 LOG_ODDS_UNOBSERVED = -32768
@@ -2498,9 +2593,10 @@ class OccupancyMap:
     after ceil((L - threshold + 1) / -miss) free observations in a row, 9 from the upper clamp with the defaults, so an
     object that has moved leaves no ghost where later frames see free space.  After one call on a fresh map, state()
     equals depth_occupancy of the same views.  integrate does not synchronise with the host when the depth images are
-    on the GPU.
+    on the GPU.  integrate_points() adds one observation of point clouds with their sensor origins by the same update,
+    ray_occupancy's rules deciding hit and free, and after one call on a fresh map state() equals ray_occupancy.
 
-    :param free_margin: depth_occupancy's, for every call; defaults to sqrt(3) r / 2
+    :param free_margin: depth_occupancy's and ray_occupancy's, for every call; defaults to sqrt(3) r / 2
     :param device: device state() and log_odds() return on, and sdf()'s default device (the grid lives on the GPU)"""
 
     def __init__(self, resolution, range_per_dim, hit=0.85, miss=-0.4, clamp=(-2.0, 3.5), threshold=0.0,
@@ -2537,6 +2633,21 @@ class OccupancyMap:
                                             self._lo, self.resolution, self._dims,
                                             nat.ptr(self._hits.get_voxel_values()), nat.ptr(self._log_odds),
                                             self._update, nat.stream_ptr(self._cdev)), "pvb_depth_integrate")
+
+    def integrate_points(self, points, origins, max_range=math.inf):
+        """Add one observation of point clouds taken from known sensor origins to the map; the arguments are
+        ray_occupancy's, with the map's free_margin.  Per voxel, a valid ray's return falling into it is a hit, and
+        otherwise a valid ray's walk passing through it is a free observation (ray_occupancy's rules), each updating L
+        as integrate's do; the call is one observation, so depth frames and point clouds can be fused into the same
+        map in any interleaving.  With points and origins on the GPU it does not synchronise with the host.  Write NaN
+        on points that should say nothing (the robot's own body, say)."""
+        rays = _rays(points, origins, max_range)
+        marks = self._hits.get_voxel_values().view(torch.uint8)
+        out = _ray_carve(rays, self.free_margin, self._lo, self.resolution, self._dims, marks, self._cdev)
+        with nat.on_device(self._cdev):
+            self._hits[out] = True              # an invalid ray's NaN point falls into no voxel: hits win over free
+            nat.check(nat.lib().pvb_occupancy_apply(nat.ptr(marks), nat.ptr(self._log_odds), self._dims,
+                                                    self._update, nat.stream_ptr(self._cdev)), "pvb_occupancy_apply")
 
     def _state(self):
         L = self._log_odds

@@ -369,3 +369,58 @@ def tabletop_views(n, H=480, W=640, f=800.0, seed=0):
     cameras 2.2 m from the scene's centre and 1.3 m above it (about 2.5 m away)."""
     K, poses = camera_ring(n, (-0.25, 0.0, 0.2), 2.2, 1.3, f, H, W, seed)
     return render_depth(TABLETOP_BOXES, K, poses, H, W), K, poses
+
+
+# ---------------------------------------------------------------- LiDAR scans of box scenes (ray_occupancy)
+def render_lidar(boxes, origin, beams, columns, elevation=(-0.4, 0.4), max_range=10.0, noise=0.0, seed=0):
+    """float32 [beams * columns, 3] world returns of a spinning LiDAR at `origin` among solid axis-aligned boxes
+    (lo_x, lo_y, lo_z, size_x, size_y, size_z), in fp64 by ray-slab intersection as render_depth does.  Beam b looks
+    at elevation lo + (hi - lo) b / (beams - 1) radians, column c at azimuth 2 pi c / columns, rows beam-major.  The
+    first hit along a ray at range t <= max_range gives o + t d; a ray that hits nothing within max_range reads NaN
+    (no return).  noise > 0 adds seeded Gaussian noise of that standard deviation (metres) to every hit's range."""
+    o = np.asarray(origin, np.float64)
+    b = np.asarray(boxes, np.float64)
+    lo, hi = b[:, :3], b[:, :3] + b[:, 3:]
+    el = np.linspace(elevation[0], elevation[1], beams) if beams > 1 else np.array([elevation[0]], np.float64)
+    az = 2 * math.pi * np.arange(columns, dtype=np.float64) / columns
+    e, a = np.meshgrid(el, az, indexing="ij")
+    d = np.stack([np.cos(e) * np.cos(a), np.cos(e) * np.sin(a), np.sin(e)], -1).reshape(-1, 3)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        t0 = (lo[None] - o) / d[:, None]
+        t1 = (hi[None] - o) / d[:, None]
+    near = np.fmax.reduce(np.minimum(t0, t1), axis=2)
+    far = np.fmin.reduce(np.maximum(t0, t1), axis=2)
+    t = np.where((near <= far) & (near > 0), near, np.inf).min(axis=1)
+    if noise > 0:
+        t = t + np.random.default_rng(seed).normal(0.0, noise, t.shape)
+    hit = np.isfinite(t) & (t <= max_range)
+    return np.where(hit[:, None], o + np.where(hit, t, 0.0)[:, None] * d, np.nan).astype(np.float32)
+
+
+# The tabletop boxes in a room: a floor 0.45 m below the table's top and four walls 3 m from the scene's centre.
+TABLETOP_ROOM = TABLETOP_BOXES + ((-3.25, -3.0, -0.75, 6.0, 6.0, 0.1), (-3.35, -3.0, -0.75, 0.1, 6.0, 3.0),
+                                  (2.75, -3.0, -0.75, 0.1, 6.0, 3.0), (-3.25, -3.1, -0.75, 6.0, 0.1, 3.0),
+                                  (-3.25, 3.0, -0.75, 6.0, 0.1, 3.0))
+
+# Sensor positions about the tabletop: even ones inside TABLETOP_RANGE (above the table, clear of every box), odd
+# ones outside it on a ring, so that rays both start inside the grid and enter it from outside.
+TABLETOP_LIDAR_INSIDE = ((-0.25, 0.0, 0.3), (-0.5, 0.1, 0.25), (0.0, -0.1, 0.45), (-0.6, -0.2, 0.35))
+
+
+def tabletop_lidar(n, beams=64, columns=1024, max_range=6.0, noise=0.0, seed=0, boxes=TABLETOP_ROOM):
+    """(points float32 [n, beams * columns, 3], origins float32 [n, 3]): n LiDAR scans of the tabletop room, the
+    sensors alternately inside TABLETOP_RANGE (TABLETOP_LIDAR_INSIDE in turn) and outside it (on a circle 1.8 m from
+    the scene's centre, 1.2 m above it, at seeded angles), elevations -0.6..0.3 rad inside and -0.7..0.1 outside."""
+    g = np.random.default_rng(seed)
+    pts, origins = [], []
+    for k in range(n):
+        if k % 2 == 0:
+            o = np.asarray(TABLETOP_LIDAR_INSIDE[(k // 2) % len(TABLETOP_LIDAR_INSIDE)], np.float64)
+            elevation = (-0.6, 0.3)
+        else:
+            a = g.uniform(0.0, 2 * math.pi)
+            o = np.array([-0.25 + 1.8 * math.cos(a), 1.8 * math.sin(a), 1.4])
+            elevation = (-0.7, 0.1)
+        pts.append(render_lidar(boxes, o, beams, columns, elevation, max_range, noise, seed + k))
+        origins.append(o)
+    return np.stack(pts), np.asarray(origins, np.float32)
